@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """bench.py — BASELINE.json headline: queries/s (+ GB/s scanned) of single-query brute-force cosine search over
-10M x 768 f32 vectors, sharded over N B200s, next to the reference's CPU path on the same box.
+10M x 768 f32 vectors, sharded over N H100s, next to the reference's CPU path on the same box.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config all|c2|c3|c4|c5]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config all|c2|c3|c4|c5] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 A step = one query (BASELINE configs[1]: single-query streaming scan) answered over the WHOLE data set: every rank
@@ -15,7 +15,7 @@ kernel (qb_comm.cu; consecutive steps are pipelined across GPUs), every rank end
   roofline: the dominant kernel timed live with CUDA events on its stream (qb_profile_enable).  Shards of >= 2^19 rows are
            scanned through the int8 shadow plane (dense_q8_filter_kernel, qb_prefilter.cu) with exact rescoring — results
            bit-identical to the f32 scan, asserted inside the run; achieved = ALGORITHMIC bytes (rows_per_rank*768*4, SURVEY 8d)
-           / avg launch time against MEASURED_PEAKS.json hbm_gbs, so it exceeds the peak; bytes_moved_per_launch /
+           / avg launch time against MEASURED_PEAKS.json hbm_gbs (else the H100 SXM data sheet's 3.35 TB/s), so it exceeds the peak; bytes_moved_per_launch /
            hbm_frac_of_bytes_moved describe the kernel's own traffic.  QB_DISABLE_PREFILTER=1 measures the f32 scan itself.
   cpu_baseline: the oracle's restatement of the reference's AVX2+FMA path (peek_top_iter loop) on this box's cores: the FULL
            10M rows per query when RAM allows (pinned threads, one first-touched segment each, oracle/mt.c).
@@ -24,7 +24,12 @@ kernel (qb_comm.cu; consecutive steps are pipelined across GPUs), every rank end
 The default run (`--config all`) prints ONE JSON line: the C2 headline fields above plus `configs.{c3,c4,c5}` — the other
 BASELINE configs measured in the same process (each with value / e2e / roofline / parity / cpu_baseline): C3 10Mx768 SQ8 batch
 1024 on the int8 tensor cores, C4 one 6.25M-row PQ shard per GPU, C5 HNSW M=16 ef=128 with the traversal on the device.
-At N > 1 only the sharded configs (C2, C4) run.
+At N > 1 only the sharded configs (C2, C4) run.  Every config times exactly --steps steps.
+
+--dump-outputs DIR writes, after the timed steps, the result lists of the last timed step of every config as DIR/<config>_idx.npy
+(float64 point ids, -1 past a query's count) and DIR/<config>_score.npy (float32, -inf past the count), [queries, top] each.
+Inputs are seeded, so two builds can be compared output for output.  C5 is left out: its graph comes from a multi-threaded
+host builder whose links differ from run to run.
 """
 from __future__ import annotations
 
@@ -66,25 +71,29 @@ def parse():
     ap.add_argument("--c5-rows", type=int, default=1_000_000, help="points of the HNSW index (BASELINE says 10M; the graph is built on the host cores inside the run)")
     ap.add_argument("--c5-queries", type=int, default=4096)
     ap.add_argument("--batch", type=int, default=1024, help="queries per batch (c3)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's result lists as DIR/<config>_{idx,score}.npy")
     return ap.parse_args()
 
 
-def ncu_traffic(name):
-    """(bytes per launch, source) of the largest launch in a profiles/ summary: dram read + write."""
-    try:
-        best = None
-        rd = None
-        for ln in open(os.path.join(ROOT, "profiles", name)):
-            f = ln.split()
-            if len(f) >= 3 and f[0] == "dram__bytes_read.sum":
-                rd = float(f[1]) * {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}[f[2]]
-            elif len(f) >= 3 and f[0] == "dram__bytes_write.sum" and rd is not None:
-                tot = rd + float(f[1]) * {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}[f[2]]
-                best = tot if best is None or tot > best else best
-                rd = None
-        return best, ("profiles/" + name if best else None)
-    except Exception:
-        return None, None
+def dump_topk(args, name, lists, top):
+    """Result lists (structured arrays with idx / score, descending) -> DIR/<name>_idx.npy, DIR/<name>_score.npy, [len(lists), top]."""
+    if not args.dump_outputs:
+        return
+    idx = np.full((len(lists), top), -1.0, np.float64)
+    score = np.full((len(lists), top), -np.inf, np.float32)
+    for i, r in enumerate(lists):
+        idx[i, : r.size] = r["idx"]
+        score[i, : r.size] = r["score"]
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    np.save(os.path.join(args.dump_outputs, name + "_idx.npy"), idx)
+    np.save(os.path.join(args.dump_outputs, name + "_score.npy"), score)
+
+
+def device_lists(d_out, d_cnt):
+    """qb_scored_point [nq, top] + counts in HBM -> host result lists."""
+    rec = d_out.cpu().numpy().view(np.dtype([("idx", np.uint32), ("score", np.float32)])).reshape(d_out.shape[0], -1)
+    cnt = d_cnt.cpu().numpy()
+    return [rec[i, : cnt[i]].copy() for i in range(rec.shape[0])]
 
 
 def peaks():
@@ -95,7 +104,7 @@ def peaks():
             return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -332,6 +341,8 @@ def main_ours(args):
     # sanity: the result of the last step must be a valid top-k
     last = searcher.results_host(1)[0]
     assert last.size == TOP and np.all(last["score"][:-1] >= last["score"][1:]), "invalid top-k from the timed region"
+    if rank == 0:
+        dump_topk(args, "c2", [last], TOP)
 
     # ---- timed region 2: end to end through the public host API (H2D query, D2H results inside)
     for i in range(3):
@@ -407,16 +418,14 @@ def main_ours(args):
         algo_bytes = n_local * args.dim * 4
         kern_ms = prof_ms / max(n_prof, 1)
         achieved = algo_bytes / (kern_ms / 1e3) / 1e9 if n_prof else None
-        # dram__bytes_read.sum + dram__bytes_write.sum of this kernel's main pass from the committed `ncu --set full` capture; it
-        # was taken on the 10M x 768 single-GPU workload, so it is only quoted for that shape
-        traffic, traffic_src = ncu_traffic(("ncu_q8_filter_kernel_r02.txt" if plane_q8 else "ncu_bf16_filter_kernel_r02.txt") if prefilter else "ncu_stream_kernel_r01_localk.txt") if (n_local == 10_000_000 and args.dim == 768) else (None, None)
+        traffic, traffic_src = None, None
         line = {
             "metric": METRIC, "value": qps, "unit": "queries/s", "n_gpus": world, "steps": K, "warmup": W, "ms_per_step": dev_ms / K,
             "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
             "dtype": ("f32 results (exact reference arithmetic); the scan itself runs on an " + ("int8" if plane_q8 else "bf16") + " shadow plane and re-scores the survivors in f32") if prefilter else "f32",
             "data": "synthetic",
             "config": dict(c2_config(args.rows, args.dim), rows_per_gpu=n_local, parallelism=f"row-sharded x{world}, top-k exchange ({exchange}) + device merge",
-                           l2="inputs larger than L2 (shard = %.1f GB >> 126 MB), no flush needed" % (algo_bytes / 1e9)),
+                           l2="inputs larger than L2 (shard = %.1f GB >> 50 MB), no flush needed" % (algo_bytes / 1e9)),
             "gb_per_s_scanned": qps * args.rows * args.dim * 4 / 1e9,
             "e2e": {"value": K / (e2e_ms / 1e3), "unit": "queries/s", "h2d_bytes_per_step": args.dim * 4, "d2h_bytes_per_step": TOP * 8 + 4,
                     "ms_per_step": e2e_ms / K},
@@ -435,12 +444,12 @@ def main_ours(args):
             line["roofline"]["bytes_moved_per_launch"] = moved
             line["roofline"]["hbm_frac_of_bytes_moved"] = moved / (kern_ms / 1e3) / 1e9 / peak
             line["roofline"]["note"] = ("achieved = algorithmic f32 bytes / kernel time; the kernel itself streams the shadow plane (bytes_moved_per_launch) at "
-                                        "hbm_frac_of_bytes_moved of the measured copy peak; results are bit-identical to the f32 scan (parity.prefilter_equals_exact_scan)")
+                                        "hbm_frac_of_bytes_moved of the peak named in peak_source; results are bit-identical to the f32 scan (parity.prefilter_equals_exact_scan)")
         line["parity"] = parity
         line["fallback_reruns"] = reruns
         if cpu is not None:
             line["cpu_baseline"] = cpu
-    # ---- the same storage, 1024 f32 queries at once (north_star: "batched multi-query x segment scoring on tensor cores"): bf16 tcgen05
+    # ---- the same storage, 1024 f32 queries at once (north_star: "batched multi-query x segment scoring on tensor cores"): bf16 wgmma
     # prefilter + exact rescoring.  Reported as configs.f32_batch of the default line.
     if rank == 0 and world == 1 and getattr(args, "with_f32_batch", False):
         line["_f32_batch"] = f32_batch_on(st, args, dev)
@@ -474,7 +483,7 @@ def f32_batch_on(st, args, dev):
     torch.cuda.synchronize()
     st.search_stats(reset=True); st.profile_read(reset=True); st.profile(True)
     launches0 = int(lib().qb_kernel_launch_count())
-    K = 5
+    K = args.steps
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     ev0.record(stream)
     for _ in range(K):
@@ -482,6 +491,7 @@ def f32_batch_on(st, args, dev):
     ev1.record(stream)
     torch.cuda.synchronize()
     dev_ms = ev0.elapsed_time(ev1)
+    dump_topk(args, "f32_batch", device_lists(d_out, d_cnt), top)
     launches = int(lib().qb_kernel_launch_count()) - launches0
     n_prof, prof_ms = st.profile_read(reset=True)
     st.profile(False)
@@ -501,7 +511,7 @@ def f32_batch_on(st, args, dev):
     try:
         peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops"]); peak_src = "measured (MEASURED_PEAKS.json bf16_tflops)"
     except Exception:
-        peak, peak_src = 2250.0, "fallback (nominal dense bf16)"
+        peak, peak_src = 989.0, "H100 SXM data sheet (dense bf16), not measured"
     n = st.count
     flops = 2.0 * nq * n * args.dim
     kern_ms = prof_ms / max(n_prof, 1)
@@ -511,7 +521,7 @@ def f32_batch_on(st, args, dev):
             "data": "synthetic", "config": {"workload": f"{n}x{args.dim} f32 cosine, batch={nq}", "rows": n, "dim": args.dim, "batch": nq},
             "e2e": {"value": nq / (e2e_ms / 1e3), "unit": "queries/s", "h2d_bytes_per_step": nq * args.dim * 4, "d2h_bytes_per_step": nq * top * 8 + nq * 4, "ms_per_step": e2e_ms},
             "gpu_launches": launches,
-            "roofline": {"bound": "tensor", "kernel": "sq8_mma_kernel<1,1> (tcgen05.mma kind::f16 prefilter) + f32_rescore_kernel, main pass", "achieved": ach, "peak": peak, "unit": "TFLOP/s",
+            "roofline": {"bound": "tensor", "kernel": "sq8_mma_kernel<.,true> (wgmma bf16 prefilter) + f32_rescore_kernel, main pass", "achieved": ach, "peak": peak, "unit": "TFLOP/s",
                          "frac": (ach / peak) if ach else None, "traffic": None, "peak_source": peak_src, "avg_launch_ms": kern_ms, "launches_timed": n_prof,
                          "algorithmic_flops_per_launch": flops},
             "parity": {"checked": True, "tensor_core_equals_cuda_core": "bit-exact on 32 queries x all rows", "fallback_reruns": reruns}}
@@ -529,7 +539,6 @@ def main_c3(args):
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(0)
     n, dim, nq, top = args.rows, args.dim, args.batch, TOP
-    args = argparse.Namespace(**dict(vars(args), steps=min(args.steps, 10)))   # a step is a 1024-query batch (~6 ms); 10 is plenty
     ad = dim + (16 - dim % 16) % 16
     chunk = 500_000
 
@@ -598,6 +607,7 @@ def main_c3(args):
     ev1.record(stream)
     torch.cuda.synchronize()
     dev_ms = ev0.elapsed_time(ev1)
+    dump_topk(args, "c3", device_lists(d_out, d_cnt), top)
     launches = int(lib().qb_kernel_launch_count()) - launches0
     n_prof, prof_ms = st.profile_read(reset=True)
     st.profile(False)
@@ -646,30 +656,19 @@ def main_c3(args):
         cpu = {"value": nq / (dt * n / sample_rows), "unit": "queries/s", "cores": threads, "kind": "reference+port",
                "sample": f"{sample_rows} of {n} rows x {nq} queries: impl_score_dot_avx arithmetic + postprocess + heap (oracle qo_scan_sq8), {threads} pinned threads over row "
                          f"segments (oracle/mt.c), {dt*1e3:.0f} ms per sample batch, extrapolated linearly to {n} rows (compute-bound: every row meets every query)"}
-    # MEASURED_PEAKS.json has no int8 figure (its tensor number is cuBLAS bf16, 1645.8 TF/s); the denominator here is the stricter
-    # one: the tcgen05.mma kind::i8 issue rate measured on this pool by tools/mma_rate.cu (8190 MAC/clk/SM x 148 SMs x 1.965 GHz)
-    peak_i8 = 4539.0
-    try:
-        for ln in open(os.path.join(ROOT, "profiles", "mma_rate_r01.jsonl")):
-            r = json.loads(ln)
-            if r.get("kind") == "i8" and r.get("n") == 256:
-                peak_i8 = float(r["chip_tera_ops_per_s"])
-                break
-    except Exception:
-        pass
+    peak_i8 = 1979.0   # H100 SXM data sheet, dense int8 TOP/s at up to 700 W
     ops = 2.0 * nq * n * ad
     kern_ms = prof_ms / max(n_prof, 1)
     achieved = ops / (kern_ms / 1e3) / 1e12 if n_prof else None
     line = {"metric": f"queries/sec, {n}x{dim} SQ8 cosine brute-force top-{top}, batch={nq} (BASELINE configs[2])", "value": nq * K / (dev_ms / 1e3), "unit": "queries/s",
             "n_gpus": 1, "steps": K, "warmup": W, "ms_per_step": dev_ms / K, "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "u8 (s32 accumulate)",
             "data": "synthetic", "config": {"workload": f"{n}x{dim} SQ8 cosine, batch={nq}, int8 tensor-core GEMM scorer + fused top-{top}", "rows": n, "dim": dim, "batch": nq,
-                                            "l2": "code plane 7.68 GB >> 126 MB L2"},
+                                            "l2": "code plane 7.68 GB >> 50 MB L2"},
             "e2e": {"value": nq * K / (e2e_ms / 1e3), "unit": "queries/s", "h2d_bytes_per_step": nq * dim * 4, "d2h_bytes_per_step": nq * top * 8 + nq * 4, "ms_per_step": e2e_ms / K},
             "gpu_launches": launches, "clocks": clk,
-            "roofline": {"bound": "tensor", "kernel": "sq8_mma_kernel (tcgen05.mma kind::i8, main pass)", "achieved": achieved, "peak": peak_i8, "unit": "TOP/s",
+            "roofline": {"bound": "tensor", "kernel": "sq8_mma_kernel (wgmma u8, main pass)", "achieved": achieved, "peak": peak_i8, "unit": "TOP/s",
                          "frac": (achieved / peak_i8) if achieved else None, "traffic": None,
-                         "peak_source": "measured tcgen05.mma kind::i8 issue rate (profiles/mma_rate_r01.jsonl, tools/mma_rate.cu); MEASURED_PEAKS.json holds no int8 figure "
-                                        "(2 x its cuBLAS bf16 number would be 3291.6)", "avg_launch_ms": kern_ms,
+                         "peak_source": "H100 SXM data sheet (dense int8), not measured", "avg_launch_ms": kern_ms,
                          "launches_timed": n_prof, "algorithmic_ops_per_launch": ops}}
     line["parity"] = parity
     if cpu:
@@ -693,7 +692,6 @@ def main_c4(args):
     from qdrant_b200.sharded import ShardedSegmentSearcher
 
     world, rank, local_rank, dev = dist_ctx()
-    args = argparse.Namespace(**dict(vars(args), steps=min(args.steps, 5)))   # a step is a 256-query batch over the shard
     total_rows, dim, chunk, nq, top = 50_000_000, 1536, 16, 256, TOP
     if args.rows != N_ROWS:
         total_rows = args.rows
@@ -736,6 +734,9 @@ def main_c4(args):
     ev1.record(searcher.stream)
     barrier()
     dev_ms = ev0.elapsed_time(ev1)
+    last = searcher.results_host(nq)
+    if rank == 0:
+        dump_topk(args, "c4", last, top)
     launches = int(lib().qb_kernel_launch_count()) - launches0
     n_prof, prof_ms = st.profile_read(reset=True)
     st.profile(False)
@@ -788,23 +789,25 @@ def main_c4(args):
     if rank == 0:
         lookups = float(nq) * n_local * m
         kern_ms = prof_ms / max(n_prof, 1)
-        # shared-memory gather peak: 148 SMs x 32 banks x 4 B per clock at clocks.max.sm
-        smem_peak_glookups = 148 * 32 * 1.965
+        # shared-memory gather peak: SMs x 32 banks x 4 B per clock at clocks.max.sm
+        n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
+        sm_ghz = (clk or {}).get("sm_max_mhz") or 1980.0
+        sm_ghz /= 1e3
+        smem_peak_glookups = n_sm * 32 * sm_ghz
         line = {"metric": f"queries/sec, {total_rows}x{dim} PQ(m={m},256) LUT scorer top-{top}, batch={nq}, {world} of 8 shards resident (BASELINE configs[3])",
                 "value": nq * K / (dev_ms / 1e3), "unit": "queries/s", "n_gpus": world, "steps": K, "warmup": W, "ms_per_step": dev_ms / K, "higher_is_better": True,
                 "scaling": "weak", "vs_baseline": None, "dtype": "u8 codes, f32 LUT sums", "data": "synthetic (random codes / centroids)",
                 "config": {"workload": f"PQ m={m} chunk={chunk}, {n_local} rows per GPU (= 50M/8), batch={nq}", "rows_per_gpu": n_local, "dim": dim, "m": m, "batch": nq,
-                           "l2": "code plane 600 MB per GPU > 126 MB L2"},
+                           "l2": "code plane 600 MB per GPU > 50 MB L2"},
                 "e2e": {"value": nq * K / (e2e_ms / 1e3), "unit": "queries/s", "h2d_bytes_per_step": nq * dim * 4, "d2h_bytes_per_step": nq * top * 8 + nq * 4, "ms_per_step": e2e_ms / K},
                 "gpu_launches": launches, "clocks": clk,
                 "roofline": {"bound": "smem-gather", "kernel": "pq16_prep_kernel + pq_scan16_kernel (sixteen queries per 16-byte gather through u8 tables, integer thresholds) + "
                                                                "pq_rescore_kernel (exact f32 sums of the survivors)", "achieved": (lookups / (kern_ms / 1e3) / 1e9) if n_prof else None,
                              "peak": smem_peak_glookups, "unit": "Glookup/s", "frac": (lookups / (kern_ms / 1e3) / 1e9 / smem_peak_glookups) if n_prof else None, "traffic": None,
-                             "peak_source": "148 SMs x 32 banks x clocks.max.sm = one 4-byte table entry per bank per clock (the exact kernels' conflict-free gather rate, the "
-                                            "denominator of rounds 1-2; no such figure in MEASURED_PEAKS.json).  A (row, query, chunk) lookup of the batched kernel moves ONE byte "
-                                            "(sixteen queries share a 16-byte gather), so frac > 1 is possible; see frac_of_16B_gather_peak and profiles/ncu_pq16_kernel_r02.txt "
-                                            "(shared-memory pipe 88 % busy, 9.6 wavefronts per LDS.128 on random codes where 4 is conflict-free)",
-                             "frac_of_16B_gather_peak": (lookups / (kern_ms / 1e3) / 1e9 / (148 * 8 * 16 * 1.965)) if n_prof else None,
+                             "peak_source": f"{n_sm} SMs x 32 banks x clocks.max.sm = one 4-byte table entry per bank per clock (the exact kernels' conflict-free gather rate).  "
+                                            "A (row, query, chunk) lookup of the batched kernel moves ONE byte (sixteen queries share a 16-byte gather), so frac > 1 is possible; "
+                                            "see frac_of_16B_gather_peak",
+                             "frac_of_16B_gather_peak": (lookups / (kern_ms / 1e3) / 1e9 / (n_sm * 8 * 16 * sm_ghz)) if n_prof else None,
                              "avg_launch_ms": kern_ms, "launches_timed": n_prof, "hbm_gb_per_s": (float(nq) * n_local * m / (kern_ms / 1e3) / 1e9) if n_prof else None}}
         line["parity"] = parity
         if cpu:
@@ -868,7 +871,7 @@ def main_c5(args):
     def step_device():
         check(lib().qb_hnsw_search_batch_device(hg._h, vp(d_q.data_ptr()), nq, top, ef, entry, entry_level, vp(d_out.data_ptr()), vp(d_cnt.data_ptr())))
 
-    W, K = 3, max(3, min(args.steps, 10))
+    W, K = 3, args.steps
     for _ in range(W):
         step_device()
     torch.cuda.synchronize()
@@ -922,7 +925,7 @@ def main_c5(args):
             "value": nq * K / (dev_ms / 1e3), "unit": "queries/s", "n_gpus": 1, "steps": K, "warmup": W, "ms_per_step": dev_ms / K, "higher_is_better": True, "scaling": "strong",
             "vs_baseline": None, "dtype": "f32", "data": "synthetic (1024 Gaussian clusters)",
             "config": {"workload": f"HNSW graph search, {nq} concurrent queries per batch, {hops:.0f} hops / {evals:.0f} scored points per query", "rows": n, "dim": dim, "ef": ef, "m": m,
-                       "batch": nq, "graph_build_s": build_s, "graph_build_threads": threads, "l2": f"vectors {n * dim * 4 / 1e9:.1f} GB >> 126 MB L2"},
+                       "batch": nq, "graph_build_s": build_s, "graph_build_threads": threads, "l2": f"vectors {n * dim * 4 / 1e9:.1f} GB >> 50 MB L2"},
             "e2e": {"value": nq * K / (e2e_ms / 1e3), "unit": "queries/s", "h2d_bytes_per_step": nq * dim * 4, "d2h_bytes_per_step": nq * top * 8 + nq * 4, "ms_per_step": e2e_ms / K},
             "gpu_launches": launches, "clocks": clk,
             "roofline": {"bound": "hbm", "kernel": "hnsw_search_kernel (random 3-KB row reads)", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": (achieved / peak) if achieved else None,

@@ -1,5 +1,5 @@
 /*
- * qb200.h — C ABI of libqdrant_b200.so: Qdrant's vector-scoring hot path on NVIDIA B200 (sm_100a).
+ * qb200.h — C ABI of libqdrant_b200.so: Qdrant's vector-scoring hot path on NVIDIA H100 (sm_90a).
  *
  * This is the drop-in boundary.  The reference has no FFI seam for scorers; its seam is the Rust trait
  * object `RawScorer` (lib/segment/src/vector_storage/raw_scorer.rs:39-54) built by `RawScorerBuilder`

@@ -115,7 +115,7 @@ def lib() -> C.CDLL:
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise ImportError(
-                f"{LIB_PATH} is missing: build it with `python -m qdrant_b200.build` (nvcc, sm_100a). "
+                f"{LIB_PATH} is missing: build it with `python -m qdrant_b200.build` (nvcc, sm_90a). "
                 "qdrant_b200 has no CPU fallback.")
         L = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():

@@ -1,8 +1,8 @@
-"""Builds libqdrant_b200.so in-tree with nvcc for sm_100a (no torch, no cmake).
+"""Builds libqdrant_b200.so in-tree with nvcc for sm_90a / H100 (no torch, no cmake).
 
     python -m qdrant_b200.build [--force] [--verbose]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The .so and the objects are build products (git-ignored).
 """
 from __future__ import annotations
 
@@ -16,9 +16,10 @@ CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "lib")
 OUT = os.path.join(OUT_DIR, "libqdrant_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]   # H100: wgmma, TMA, clusters
 
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *ARCH,
     "-O3", "-lineinfo", "-std=c++17",
     "--fmad=false",            # never contract a*b+c: every FMA in the kernels is an explicit __fmaf_rn
     "-Xcompiler", "-fPIC,-fvisibility=hidden,-O3",
@@ -36,7 +37,7 @@ def stale() -> bool:
         return True
     t = os.path.getmtime(OUT)
     deps = sources() + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.h")) + [
-        os.path.join(HERE, "..", "include", "qb200.h")] + glob.glob(os.path.join(HERE, "host", "*"))
+        os.path.join(HERE, "..", "include", "qb200.h"), os.path.abspath(__file__)] + glob.glob(os.path.join(HERE, "host", "*"))   # build.py: flags
     if not os.path.exists(os.path.join(OUT_DIR, "host_selftest")):
         return True
     return any(os.path.getmtime(d) > t for d in deps)
@@ -60,7 +61,7 @@ def build_variant(name: str, defines: list[str]) -> str:
         if p.returncode != 0:
             sys.stderr.write(o)
             raise RuntimeError("nvcc failed")
-    r = subprocess.run([NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-cudart", "static", "-o", out] + objs + ["-lpthread", "-ldl", "-lrt"],
+    r = subprocess.run([NVCC, *ARCH, "-shared", "-cudart", "static", "-o", out] + objs + ["-lpthread", "-ldl", "-lrt"],
                        stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout)
@@ -94,7 +95,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         raise RuntimeError("nvcc failed")
     if verbose:
         print("\n".join(log))
-    link = [NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-cudart", "static", "-o", OUT] + objs + ["-lpthread", "-ldl", "-lrt"]
+    link = [NVCC, *ARCH, "-shared", "-cudart", "static", "-o", OUT] + objs + ["-lpthread", "-ldl", "-lrt"]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout)

@@ -34,7 +34,7 @@ qb_status qb_sq8_mma_scan(const qb_storage* s, const uint8_t* d_q_codes, uint32_
                           void* d_scratch, size_t scratch_bytes, cudaStream_t stream);
 uint32_t qb_f32_mma_block(qb_storage* s, uint32_t nq, cudaStream_t stream);
 size_t qb_f32_mma_scratch_bytes(const qb_storage* s, uint32_t nq_pad);
-qb_status qb_f32_mma_scan(qb_storage* s, const float* d_q_pre, uint32_t q_stride_f, uint32_t nq, uint32_t nq_pad, uint32_t n_blk_flag, uint64_t row_end, const QbEmit& emit,
+qb_status qb_f32_mma_scan(qb_storage* s, const float* d_q_pre, uint32_t q_stride_f, uint32_t nq, uint32_t nq_pad, uint32_t n_blk, uint64_t row_end, const QbEmit& emit,
                           unsigned int* d_flags, void* d_scratch, size_t scratch_bytes, cudaStream_t stream);
 qb_status qb_bq_encode_queries(const qb_storage* s, const float* d_q_pre, uint32_t q_stride_f, uint32_t nq, int force_binary, void* d_out, cudaStream_t stream);
 qb_status qb_bq_scan(const qb_storage* s, const QbScanArgs& a, cudaStream_t stream);
@@ -62,7 +62,6 @@ QbOptions& qb_opt() {
         v.prefilter_plane = (int)num("QB_PREFILTER_PLANE", 0);
         v.prefilter_slot_bytes = (uint32_t)num("QB_PREFILTER_SLOT_BYTES", 0);
         v.disable_mma = getenv("QB_DISABLE_MMA") != nullptr;
-        v.mma_1cta = getenv("QB_MMA_1CTA") != nullptr;
         v.mma_no_segments = getenv("QB_MMA_NO_SEGMENTS") != nullptr;
         v.mma_debug = (int)num("QB_MMA_DEBUG", 0);
         v.sample_rows = (uint64_t)num("QB_SAMPLE_ROWS", 0);
@@ -85,7 +84,6 @@ extern "C" qb_status qb_set_option(const char* name, int64_t value) {
     else if (n == "prefilter_slot_bytes") o.prefilter_slot_bytes = (uint32_t)value;
     else if (n == "prefilter_producers") o.prefilter_producers = (int)value;
     else if (n == "disable_mma") o.disable_mma = value != 0;
-    else if (n == "mma_1cta") o.mma_1cta = value != 0;
     else if (n == "mma_no_segments") o.mma_no_segments = value != 0;
     else if (n == "mma_debug") o.mma_debug = (int)value;
     else if (n == "sample_rows") o.sample_rows = (uint64_t)value;
@@ -728,7 +726,7 @@ static qb_status run_search(qb_storage* s, QbSearchCtx* c, uint32_t nq, uint32_t
             a.emit.dense = 1; a.emit.dense_base = 0;
             const bool f32b = f32_mma && qb_f32_mma_block(s, qn, stream) != 0;   // this chunk of the batch is wide enough for the tensor-core prefilter
             const uint32_t mma_blk = mma_ok ? (f32b ? qb_f32_mma_block(s, qn, stream) : qb_sq8_mma_block(s, qn)) : 0;
-            const uint32_t nq_pad = mma_blk ? (uint32_t)round_up_u64(qn, mma_blk & 0x7FFFFFFFu) : 0;
+            const uint32_t nq_pad = mma_blk ? (uint32_t)round_up_u64(qn, mma_blk) : 0;
             const uint32_t q_stride_f = s->row_stride / 4;              // dense f32: encoded queries = preprocessed f32 rows
             if (mma_blk && !f32b) {
                 QB_TRY(qb_sq8_mma_scan(s, reinterpret_cast<const uint8_t*>(a.d_q_enc), nq_pad, a.d_q_off, qn, mma_blk, 0, plan.sample, a.emit, d_overflow, nullptr,

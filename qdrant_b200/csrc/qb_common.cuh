@@ -1,4 +1,4 @@
-// qb_common.cuh — shared device/host helpers for libqdrant_b200 (sm_100a only).
+// qb_common.cuh — shared device/host helpers for libqdrant_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -42,7 +42,7 @@ extern std::atomic<uint64_t> g_qb_launches;
     } while (0)
 
 struct QbOptions {
-    bool disable_localk = false, disable_mma = false, mma_1cta = false, mma_no_segments = false, verbose = false;
+    bool disable_localk = false, disable_mma = false, mma_no_segments = false, verbose = false;
     int mma_debug = 0;
     int pq_queries_per_pass = 0;   // 0 = automatic
     int hnsw_threads = 0;          // 0 / 128 (default) or 256 threads per traversal CTA

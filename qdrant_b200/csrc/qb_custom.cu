@@ -69,7 +69,7 @@ qb_status qb_launch_custom_combine(int kind, uint32_t n_a, uint32_t n_b, const f
     if (n == 0) return QB_OK;
     QbEmit e{};
     if (emit) e = *emit;
-    const unsigned grid = (unsigned)std::min<uint64_t>(ceil_div_u64(n, 256), 148ull * 16);
+    const unsigned grid = (unsigned)std::min<uint64_t>(ceil_div_u64(n, 256), 132ull * 16);
     custom_combine_kernel<<<grid, 256, 0, stream>>>(kind, n_a, n_b, d_coef, d_sims, stride, n, d_scores, d_ids, e, emit ? 1 : 0);
     QB_LAUNCHED();
     QB_CUDA(cudaGetLastError());
@@ -82,7 +82,7 @@ qb_status qb_launch_maxsim_fold(const float* d_sims, uint64_t stride, uint32_t n
     if (n_points == 0) return QB_OK;
     QbEmit e{};
     if (emit) e = *emit;
-    const unsigned grid = (unsigned)std::min<uint64_t>(ceil_div_u64(n_points, 128), 148ull * 16);
+    const unsigned grid = (unsigned)std::min<uint64_t>(ceil_div_u64(n_points, 128), 132ull * 16);
     maxsim_fold_kernel<<<grid, 128, 0, stream>>>(d_sims, stride, n_query_tokens, d_row_offsets, d_point_ids, n_points, d_scores, e, emit ? 1 : 0);
     QB_LAUNCHED();
     QB_CUDA(cudaGetLastError());
@@ -91,7 +91,7 @@ qb_status qb_launch_maxsim_fold(const float* d_sims, uint64_t stride, uint32_t n
 
 qb_status qb_launch_iota(uint32_t* d, uint64_t n, cudaStream_t stream) {
     if (n == 0) return QB_OK;
-    iota_kernel<<<(unsigned)std::min<uint64_t>(ceil_div_u64(n, 256), 148ull * 16), 256, 0, stream>>>(d, n);
+    iota_kernel<<<(unsigned)std::min<uint64_t>(ceil_div_u64(n, 256), 132ull * 16), 256, 0, stream>>>(d, n);
     QB_LAUNCHED();
     QB_CUDA(cudaGetLastError());
     return QB_OK;

@@ -1,4 +1,4 @@
-// qb_dense.cu — f32 dense metrics (dot / cosine / euclid / manhattan) on B200.
+// qb_dense.cu — f32 dense metrics (dot / cosine / euclid / manhattan) on H100.
 //
 // Replaces: Metric<f32>::similarity / preprocess (lib/segment/src/spaces/simple.rs:36-206) as dispatched on an
 // AVX2+FMA host — dot_similarity_avx / euclid_similarity_avx / manhattan_similarity_avx / cosine_preprocess_avx
@@ -212,8 +212,7 @@ __global__ void __launch_bounds__(STREAM_THREADS, 1) dense_f32_stream_kernel(con
         }
         if (LOCALK) {
             // CTA merge of the eight lists.  Only the consumer warps meet at a NAMED barrier: with __syncthreads() the 31 idle lanes of the
-            // producer warp would sit in the barrier from the first cycle on and share issue slots with the one lane that feeds the ring
-            // (measured: 10 % less bandwidth).
+            // producer warp would sit in the barrier from the first cycle on and share issue slots with the one lane that feeds the ring.
             unsigned long long* lists = reinterpret_cast<unsigned long long*>(empty + p.n_slots);
             if (lane < QB_LOCALK_SLOTS) lists[cw * QB_LOCALK_SLOTS + lane] = (my_key == ~0ull) ? 0ull : my_key;
             asm volatile("bar.sync 1, %0;" ::"n"(STREAM_CONSUMER_WARPS * 32) : "memory");
@@ -573,7 +572,7 @@ qb_status qb_launch_preprocess_rows(qb_distance distance, uint32_t dim, uint64_t
                                     uint64_t out_stride_f, cudaStream_t stream) {
     if (n == 0) return QB_OK;
     uint64_t blocks = ceil_div_u64(n, 256 / 8);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     preprocess_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(distance == QB_DIST_COSINE ? 1 : 0, dim, n, in, in_stride_f, out, out_stride_f);
     QB_LAUNCHED();
     QB_CUDA(cudaGetLastError());

@@ -191,7 +191,7 @@ extern "C" qb_status qb_sq8_find_alpha_offset_device(int32_t device, uint32_t di
     if (row_stride_bytes == 0) row_stride_bytes = (uint64_t)dim * 4;
     QB_CHECK(row_stride_bytes % 4 == 0 && row_stride_bytes >= (uint64_t)dim * 4, QB_ERR_INVALID, "sq8_find_alpha_offset: bad row stride");
     QB_TRY(use_dev(device));
-    const unsigned grid = 148 * 8;
+    const unsigned grid = 132 * 8;
     float* d_part = nullptr;
     QB_CUDA(cudaMalloc(&d_part, grid * 2 * sizeof(float)));
     minmax_kernel<<<grid, 256>>>(dev_rows, row_stride_bytes / 4, dim, count, d_part);
@@ -223,10 +223,10 @@ extern "C" qb_status qb_sq8_encode_rows_device(int32_t device, uint32_t dim, uin
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const bool exact_window = is_dot ? ((uint64_t)ad * 127ull < (1ull << 24)) : (is_l1 || (uint64_t)ad * 127ull * 127ull < (1ull << 24));
     if (exact_window) {
-        const unsigned grid = (unsigned)std::min<uint64_t>(ceil_div_u64(count, 8), 148ull * 32);
+        const unsigned grid = (unsigned)std::min<uint64_t>(ceil_div_u64(count, 8), 132ull * 32);
         sq8_encode_rows_kernel<<<grid, 256, 0, st>>>(dev_rows, row_stride_bytes / 4, dim, ad, count, alpha, offset, is_dot, is_l1, invert, shift, dev_out);
     } else {
-        const unsigned grid = (unsigned)std::min<uint64_t>(count, 148ull * 32);
+        const unsigned grid = (unsigned)std::min<uint64_t>(count, 132ull * 32);
         sq8_encode_rows_seq_kernel<<<grid, 256, 0, st>>>(dev_rows, row_stride_bytes / 4, dim, ad, count, alpha, offset, is_dot, is_l1, invert, shift, dev_out);
     }
     QB_LAUNCHED();
@@ -259,7 +259,7 @@ extern "C" qb_status qb_bq_encode_rows_device(int32_t device, uint32_t dim, uint
     }
     const uint32_t row_bytes = qb_bq_row_bytes(dim, encoding);
     const uint64_t total_words = count * (uint64_t)(row_bytes / 4);
-    const unsigned grid = (unsigned)std::min<uint64_t>(ceil_div_u64(total_words, 8), 148ull * 32);
+    const unsigned grid = (unsigned)std::min<uint64_t>(ceil_div_u64(total_words, 8), 132ull * 32);
     bq_encode_rows_kernel<<<grid, 256, 0, st>>>(dev_rows, row_stride_bytes / 4, dim, count, (int)encoding, d_ms, row_bytes, dev_out);
     QB_LAUNCHED();
     cudaError_t e = cudaGetLastError();
@@ -284,7 +284,7 @@ extern "C" qb_status qb_pq_encode_rows_device(int32_t device, uint32_t dim, uint
     cudaError_t e = cudaMemcpyAsync(d_c, centroids, (size_t)n_centroids * dim * sizeof(float), cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) {
         const size_t smem = (size_t)n_centroids * chunk * sizeof(float);  // <= 64 KB
-        const unsigned gx = (unsigned)std::min<uint64_t>(ceil_div_u64(count, 256), 148ull * 4);
+        const unsigned gx = (unsigned)std::min<uint64_t>(ceil_div_u64(count, 256), 132ull * 4);
         auto launch = [&](auto kernel) {
             e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             if (e != cudaSuccess) return;

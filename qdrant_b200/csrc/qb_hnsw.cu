@@ -425,7 +425,7 @@ extern "C" qb_status qb_hnsw_create_plain(qb_storage* s, const uint8_t* links_bi
     if (ce == cudaSuccess) ce = cudaMemcpy(g->d_offsets, p_of, 8 * n_off, cudaMemcpyHostToDevice);
     if (ce == cudaSuccess) ce = cudaMemset(g->d_stats, 0, 256);
     if (ce == cudaSuccess && n) {
-        hnsw_links0_kernel<<<(unsigned)std::min<uint64_t>(ceil_div_u64(n * m0, 256), 148 * 16), 256>>>(g->d_neighbors, g->d_offsets, (uint32_t)n, m0, g->d_links0);
+        hnsw_links0_kernel<<<(unsigned)std::min<uint64_t>(ceil_div_u64(n * m0, 256), 132 * 16), 256>>>(g->d_neighbors, g->d_offsets, (uint32_t)n, m0, g->d_links0);
         QB_LAUNCHED();
         ce = cudaDeviceSynchronize();
     }
@@ -477,8 +477,7 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
     const size_t smem = hnsw_smem_bytes(p.q_bytes, ef);
     QB_CHECK(smem <= 200 * 1024, QB_ERR_UNSUPPORTED, "hnsw_search: query (%u B) + ef %u need %zu B of shared memory", p.q_bytes, ef, smem);
     // threads per CTA: 256 = one 8-lane group per level-0 link (m0 = 32), fewer queries in flight per SM; 128 (default) = two scoring rounds
-    // per hop, twice the resident queries.  The traversal is a chain of dependent memory round trips, so queries in flight is what hides
-    // them: measured 519 K vs 276-423 K q/s (500K x 768, ef 128, 8192-query batch, through the host API).
+    // per hop, twice the resident queries.  The traversal is a chain of dependent memory round trips, so queries in flight is what hides them.
     const int nt = qb_opt().hnsw_threads == 256 ? 256 : (qb_opt().hnsw_threads == 64 ? 64 : 128);
     const int per_sm = nt == 128 ? occupancy_dispatch<128>(kind, metric, smem) : (nt == 64 ? occupancy_dispatch<64>(kind, metric, smem) : occupancy_dispatch<256>(kind, metric, smem));
     p.prefetch = qb_opt().hnsw_no_prefetch ? 0 : 1;

@@ -99,7 +99,7 @@ struct qb_storage {
     uint64_t prof_launches = 0;
     double prof_ms = 0.0;
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_pending;
-    int sm_count = 148;
+    int sm_count = 132;
 };
 
 struct qb_scorer {
@@ -148,7 +148,7 @@ qb_status qb_hnsw_read_stats(qb_hnsw* g, cudaStream_t stream);
 constexpr uint32_t QB_MAX_WORLD = 16;
 constexpr uint32_t QB_XCHG_SLOTS = 4;     // ring of exchange slots (window of 2 pipelined steps, see qb_comm.cu)
 struct qb_comm {
-    int device = 0, rank = 0, world = 1, sm_count = 148;
+    int device = 0, rank = 0, world = 1, sm_count = 132;
     uint32_t max_q = 0, max_top = 0;
     void* d_buf = nullptr; uint64_t bytes = 0;
     uint8_t* peers[QB_MAX_WORLD] = {};

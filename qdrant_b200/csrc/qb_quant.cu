@@ -1,4 +1,4 @@
-// qb_quant.cu — quantized scorers on B200: SQ8 (scalar), PQ (product, LUT) and BQ (binary).
+// qb_quant.cu — quantized scorers on H100: SQ8 (scalar), PQ (product, LUT) and BQ (binary).
 //
 // Replaces quantization::EncodedVectors::{encode_query, score, score_point, score_internal}
 // (lib/quantization/src/encoded_vectors.rs:41-117) for
@@ -912,7 +912,7 @@ qb_status qb_sq8_repack(const qb_storage* s, const uint8_t* d_rows_in, uint32_t 
     if (n == 0) return QB_OK;
     uint64_t total = n * (uint64_t)(s->actual_dim >> 2);
     uint64_t blocks = ceil_div_u64(total, 256);
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > 132 * 32) blocks = 132 * 32;
     sq8_repack_kernel<<<(unsigned)blocks, 256, 0, stream>>>(d_rows_in, row_bytes, s->actual_dim, n, s->d_codes + first * s->actual_dim,
                                                             s->d_voff + first);
     QB_LAUNCHED();

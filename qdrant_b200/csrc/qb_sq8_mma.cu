@@ -1,35 +1,33 @@
-// qb_sq8_mma.cu — batched SQ8 scoring on the 5th-gen tensor cores (tcgen05.mma kind::i8, TMEM accumulators, TMA).
+// qb_sq8_mma.cu — batched SQ8 scoring on the Hopper tensor cores (wgmma.mma_async, register accumulators, TMA, mbarriers).
 //
 // The one dense contraction on the path (north_star): many queries x one segment.  In the reference every
 // (query, vector) pair is a separate impl_score_dot_avx call (lib/quantization/cpp/avx2.c:25-63) made from
 // QuantizedQueryScorer::score_stored_batch (quantized_query_scorer.rs:81-93) inside the peek_top_iter loop
 // (point_scorer.rs:453-462), i.e. the batch re-reads each 64-vector chunk once per query.  Here it is
-//      D[vectors x N queries] (s32, TMEM)  +=  A[vectors x K] (u8 codes, smem via TMA)  x  B[N x K]^T (u8 query codes)
+//      D[vectors x N queries] (s32, registers)  +=  A[vectors x K] (u8 codes, smem via TMA)  x  B[N x K]^T (u8 query codes)
 // with the integer dot exact by construction, followed by the reference's epilogue
 //      score = multiplier * f32(dot) + q_off[q] + v_off[v]              (encoded_vectors_u8.rs:101-103)
 // and the fused threshold filter that feeds the top-k selection (the N x 10M score matrix is never materialised).
 //
-// One persistent CTA per SM, 18 warps:
-//   warps 0-15 epilogue: tcgen05.ld (lane = vector row, 16 columns = 16 queries per load, software-pipelined), an integer
-//              prefilter of 8 min/max instructions per 16 dot products, exact scoring only for the rare survivors.
-//   warp 16   TMA producer: the CTA's query block B stays resident in shared memory (128-B-swizzled K-blocks); vector-code
-//              tiles A (128 rows x 128 B) stream through a ring; tiles are L2-prefetched three tiles ahead.
-//   warp 17   allocates 512 TMEM columns (two N-column s32 accumulators) and issues the MMAs from one elected lane;
-//              tcgen05.commit releases smem stages and publishes finished accumulators.
-// Two variants of the same kernel:
-//   TWO = false  cta_group::1, M = 128, N <= 208 (K = 768), 4-stage ring; CTAs of one worker group walk the same tiles.
-//   TWO = true   cta_group::2: a CTA pair computes 256 rows x N <= 256; each SM supplies its own 128 A rows and HALF of B,
-//                which halves the tensor-side shared-memory operand traffic and leaves room for a 7-stage ring.
+// One persistent CTA per SM, 9 warps:
+//   warps 0-7  two consumer warpgroups: each owns 64 rows of every 128-row tile and all n_blk <= 128 columns, issues
+//              wgmma.m64n32k32 (u8) per 32-column chunk straight from the shared-memory ring, and filters its accumulators
+//              in registers: an integer prefilter of min/max instructions per 16 dot products, exact scoring only for the
+//              rare survivors.
+//   warp 8     TMA producer: the CTA's query block B stays resident in shared memory (128-B-swizzled K-blocks); vector-code
+//              tiles A (128 rows x 128 B) stream through a ring of as many stages as shared memory leaves (4..8); tiles are
+//              L2-prefetched three tiles ahead.
+// A consumer keeps one wgmma group in flight: the stage of K-block k is released once the MMAs of K-block k + 1 are issued
+// and those of k have retired.
 //
-// What the epilogue must NOT do (measured, profiles/README_r01.md): touch shared memory or branch per element.  The tensor
-// core streams its operands from shared memory at close to the port's bandwidth, and 16 uniform LDS.128 per 16 columns for
-// per-query thresholds cost more than the MMAs.  So the per-query part of the threshold is moved INTO the accumulator: one
-// extra K = 32 MMA per tile multiplies a constant A tile (fifteen 127s and a 1 per 16 bytes) with a per-query "bias" row
+// The per-query part of the threshold is moved INTO the accumulator, so that the filter needs no shared-memory load per
+// element: one extra K = 32 MMA per tile multiplies a constant A tile (fifteen 127s and a 1 per 16 bytes) with a per-query
+// "bias" row
 //      D' = dot + bias_q,   bias_q = 2 * ceil((T - t_q) / 2),   t_q = (thr_q - q_off_q) / multiplier - slack
 // after which ONE integer threshold serves every query of the batch and a row only needs
-//      max(D'[0..15]) >= T - row_term
-// with both sides in registers (8 VIMNMX3 per 16 dot products).  Survivors of that test are re-scored exactly
-// (dot = D' - bias_q) against their own query's threshold.
+//      max(D'[...]) >= T - row_term
+// with both sides in registers.  Survivors of that test are re-scored exactly (dot = D' - bias_q) against their own
+// query's threshold.
 //
 // Exactness: codes are <= 127, so dot <= 127^2 * K.  While dot < 2^24 the CPU's lane-wise f32 tree equals f32(dot)
 // exactly (all partial sums are non-negative integers <= dot).  If any dot >= 2^24 (possible only for K > 1040) the
@@ -37,7 +35,7 @@
 //
 // F16 = true: the same pipeline for DENSE f32 storages (dot / cosine) — "batched multi-query x segment scoring on tensor cores" for
 // full-precision vectors.  bf16 inputs cannot reproduce the reference's f32 FMA chains, so the tensor cores only PREFILTER:
-//      approx = bf16(row) . bf16(query)   (tcgen05.mma kind::f16, f32 accumulators; a bf16 shadow plane of the rows lives beside the f32 plane)
+//      approx = bf16(row) . bf16(query)   (wgmma.m64n32k16 bf16, f32 accumulators; a bf16 shadow plane of the rows lives beside the f32 plane)
 //      |approx - exact| <= eps_q = (2^-8 + 2^-18 + K 2^-22) |q| max|row|  (RN-even input rounding of both operands + f32 accumulation) + slack
 // a row survives when approx >= thr_q - eps_q, and every survivor is re-scored by the bit-exact AVX-order kernel before the
 // selection sees it (f32_rescore_kernel).  thr_q comes from exactly scored samples, so it never exceeds the final k-th score:
@@ -50,38 +48,32 @@
 
 namespace {
 
-constexpr int MMA_M = 128;
+constexpr int MMA_M = 128;                   // rows per tile: 64 per consumer warpgroup
+constexpr int WG_M = 64;                     // rows of one wgmma
 constexpr int KB = 128;                      // K bytes per smem block (one 128-B swizzle atom wide), for A stages and B blocks
 constexpr int A_STAGE_BYTES = MMA_M * KB;    // 16 KB
-constexpr int STAGES_1 = 4;                  // cta_group::1 ring
-constexpr int STAGES_2 = 7;                  // cta_group::2 ring
-constexpr int N_MAX = 256;
-#ifndef QB_EPI_WARPS
-#define QB_EPI_WARPS 16
-#endif
+constexpr int MIN_STAGES = 4;
+constexpr int MAX_STAGES = 8;
+constexpr int NC = 32;                       // columns (queries) per wgmma
+constexpr int N_MAX = 128;                   // columns per CTA: 4 chunks x 16 accumulator registers per thread
 #ifndef QB_MMA_PF
 #define QB_MMA_PF 3
 #endif
-constexpr int EPI_WARPS = QB_EPI_WARPS;      // a multiple of 4: EPI_WARPS / 4 per TMEM lane quarter (build-time experiment knob)
-constexpr int EPI_PARTS = EPI_WARPS / 4;     // 16-column chunks are dealt round-robin to the warps of a quarter
-constexpr uint32_t MAX_CHUNKS_PER_WARP = (N_MAX / 16 + EPI_PARTS - 1) / EPI_PARTS;
-constexpr int THREADS = 32 * (2 + EPI_WARPS);
-constexpr int WARP_TMA = EPI_WARPS;
-constexpr int WARP_MMA = EPI_WARPS + 1;
-constexpr uint32_t TMEM_COLS = 512;
-constexpr uint32_t PEER_BIT_MASK = 0xFEFFFFFFu;  // clears the CTA-rank bit of a shared::cluster address -> the leader's copy
+constexpr int CONSUMER_WARPS = 8;
+constexpr int THREADS = 32 * (CONSUMER_WARPS + 1);
+constexpr int WARP_TMA = CONSUMER_WARPS;
 constexpr int T_CLAMP = 1 << 29;
-constexpr int BIAS_KB = 32;                  // K bytes of the bias MMA (one kind::i8 instruction)
+constexpr int BIAS_KB = 32;                  // K bytes of the bias MMA (one u8 k32 / bf16 k16 instruction)
 constexpr int BIAS_HALF_MAX = 127 * 127 * 15 + 126;  // largest representable bias / 2
 
 struct MmaParams {
     const float* voff;
     uint64_t n_rows;
     uint32_t ad;             // K bytes
-    uint32_t n_blk;          // queries per block (multiple of 16 / 32)
     uint32_t n_qblocks;
     uint32_t nq;             // real number of queries
-    uint32_t n_workers;      // CTAs (pairs) per query block
+    uint32_t n_workers;      // CTAs per query block
+    uint32_t stages;         // A ring depth, MIN_STAGES..MAX_STAGES
     float multiplier;
     const float* q_off;      // [nq]
     const uint8_t* bias_rows;  // [nq_pad][32] per-query B rows of the bias MMA; null = no bias / no prefilter (sample pass)
@@ -94,7 +86,7 @@ struct MmaParams {
 };
 
 // Everything the survivor path needs, in shared memory: the out-of-line slow path takes ONE pointer, and nothing it reads sits
-// in per-thread local memory (18 warps x a 200-byte parameter copy do not fit the L1 that 227 KB of shared memory leave).
+// in per-thread local memory.
 struct EpiShared {
     float thr[N_MAX];          // exact per-query thresholds (+inf for padding)
     float qoff[N_MAX];
@@ -109,64 +101,31 @@ struct EpiShared {
     uint32_t seg_cap, seg_index, q_base, nq, id_base;
     int dense, check_exact;
 };
-constexpr size_t SMALL_SMEM = sizeof(EpiShared) + 32 * 8 + 16;  // + barriers, tmem ptr
+constexpr size_t SMALL_SMEM = sizeof(EpiShared) + (2 * MAX_STAGES + 1) * 8 + 16;  // + barriers
 
 // ---------------------------------------------------------------------------------------------- PTX helpers
-__device__ __forceinline__ bool elect_one() {  // one lane of a converged warp; keeps UTC*/UTMA* operands in uniform registers
+__device__ __forceinline__ bool elect_one() {  // one lane of a converged warp
     uint32_t pred;
     asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
     return pred != 0;
 }
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive_on_cta(uint64_t* bar, uint32_t cta_rank) {
-    uint32_t remote;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(qb_smem_u32(bar)), "r"(cta_rank));
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-template <bool TWO>
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* smem_dst, int32_t c0, int32_t c1, uint64_t policy) {
-    if (TWO)  // both CTAs of the pair execute this; the transaction bytes are credited to the LEADER's barrier
-        asm volatile(
-            "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(
-                qb_smem_u32(smem_dst)),
-            "l"(reinterpret_cast<uint64_t>(map)), "r"(qb_smem_u32(bar) & PEER_BIT_MASK), "r"(c0), "r"(c1), "l"(policy)
-            : "memory");
-    else
-        asm volatile(
-            "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(
-                qb_smem_u32(smem_dst)),
-            "l"(reinterpret_cast<uint64_t>(map)), "r"(qb_smem_u32(bar)), "r"(c0), "r"(c1), "l"(policy)
-            : "memory");
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(
+            qb_smem_u32(smem_dst)),
+        "l"(reinterpret_cast<uint64_t>(map)), "r"(qb_smem_u32(bar)), "r"(c0), "r"(c1), "l"(policy)
+        : "memory");
 }
 __device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int32_t c0, int32_t c1) {  // into L2 only
     asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-template <bool TWO>
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    if (TWO)  // arrives on `bar` in BOTH CTAs of the pair
-        asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(qb_smem_u32(bar)),
-                     "h"((uint16_t)3)
-                     : "memory");
-    else
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(qb_smem_u32(bar)) : "memory");
-}
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): K-major, 128-B swizzle, version 1 (sm_100)
+// wgmma shared-memory matrix descriptor (sm_90): K-major, 128-B swizzle, 8 rows x 128 B between swizzle atoms
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFFu);     // start address  [0,14)
-    d |= (uint64_t)((8 * KB) >> 4) << 32;            // stride byte offset [32,46): 8 rows x 128 B between swizzle atoms
-    d |= (uint64_t)1 << 46;                          // version = 1
-    d |= (uint64_t)2 << 61;                          // SWIZZLE_128B
+    d |= (uint64_t)1 << 16;                          // leading byte offset: unused for swizzled K-major, canonical value 1
+    d |= (uint64_t)((8 * KB) >> 4) << 32;            // stride byte offset [32,46)
+    d |= (uint64_t)1 << 62;                          // layout [62,64): 1 = SWIZZLE_128B
     return d;
 }
 // 32-B swizzle, rows of 32 B, 8-row groups 256 B apart (the bias MMA's operands; both 16-B halves of every row are identical,
@@ -174,59 +133,42 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
 __device__ __forceinline__ uint64_t make_smem_desc_sw32(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFFu);
-    d |= (uint64_t)1 << 16;                          // leading byte offset: unused for swizzled K-major, canonical value 1
+    d |= (uint64_t)1 << 16;
     d |= (uint64_t)((8 * BIAS_KB) >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)6 << 61;                          // SWIZZLE_32B
+    d |= (uint64_t)3 << 62;                          // 3 = SWIZZLE_32B
     return d;
 }
-template <bool TWO>
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    if (TWO)
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+__device__ __forceinline__ void acc_fence(uint32_t (&d)[16]) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
+// D[64 x 32] (+)= A[64 x 32 B] . B[32 x 32 B]^T; u8 x u8 -> s32, or (F16) bf16 x bf16 -> f32 held as raw bits
+template <bool F16>
+__device__ __forceinline__ void wgmma_n32(uint32_t (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    if (F16)
         asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d), "l"(a_desc),
-            "l"(b_desc), "r"(idesc), "r"(accumulate)
-            : "memory");
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+            : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]),
+              "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+            : "l"(a_desc), "l"(b_desc), "r"(accumulate));
     else
         asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d), "l"(a_desc),
-            "l"(b_desc), "r"(idesc), "r"(accumulate)
-            : "memory");
-}
-template <bool TWO>
-__device__ __forceinline__ void mma_i8(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    if (TWO)
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::2.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d), "l"(a_desc),
-            "l"(b_desc), "r"(idesc), "r"(accumulate)
-            : "memory");
-    else
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d), "l"(a_desc),
-            "l"(b_desc), "r"(idesc), "r"(accumulate)
-            : "memory");
-}
-// asynchronous TMEM -> register load of 16 columns for the warp's 32 lanes; results are valid only after tmem_ld_wait(r)
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-// the "+r" operands tie the registers to the wait so that no use of them can be scheduled above it
-__device__ __forceinline__ void tmem_ld_wait(uint32_t (&r)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]), "+r"(r[9]), "+r"(r[10]),
-                   "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-                 :
-                 : "memory");
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n32k32.s32.u8.u8 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p;\n\t}"
+            : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]),
+              "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+            : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
 
 // ---------------------------------------------------------------------------------------------- epilogue
 // Exact epilogue of one (vector, query) pair: int -> f32 (exact), three roundings (encoded_vectors_u8.rs:101-103), emit.
-// Survivors go to a segment private to (query, CTA): the slot comes from a SHARED-memory counter, the store is fire-and-forget
-// (a global atomicAdd per survivor puts ~1 us on the slowest epilogue warp, and the accumulator is released by the last warp).
+// Survivors go to a segment private to (query, CTA): the slot comes from a SHARED-memory counter, the store is fire-and-forget.
 __device__ __forceinline__ void epilogue_exact(EpiShared* es, uint32_t acc, uint32_t n, uint64_t row, bool valid_row, bool dead, float v_off) {
     const uint32_t q = es->q_base + n;
     if (q >= es->nq) return;
@@ -268,41 +210,26 @@ __device__ __forceinline__ void epilogue_approx(EpiShared* es, float val, uint32
         if (pos < es->cap) es->cand[(unsigned long long)q * es->cap + pos] = qb_pack_key(approx, (uint32_t)row);
     }
 }
-__device__ __noinline__ void epilogue_hits_f16(EpiShared* es, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3, uint32_t r4, uint32_t r5, uint32_t r6, uint32_t r7,
-                                               uint32_t r8, uint32_t r9, uint32_t r10, uint32_t r11, uint32_t r12, uint32_t r13, uint32_t r14, uint32_t r15, uint32_t c,
-                                               float t_row, uint64_t row, uint32_t row_flags) {
-    uint32_t mask = 0;
-#define QB_HIT(j) mask |= (__uint_as_float(r##j) >= t_row) ? (1u << j) : 0u;
-    QB_HIT(0) QB_HIT(1) QB_HIT(2) QB_HIT(3) QB_HIT(4) QB_HIT(5) QB_HIT(6) QB_HIT(7) QB_HIT(8) QB_HIT(9) QB_HIT(10) QB_HIT(11) QB_HIT(12) QB_HIT(13) QB_HIT(14) QB_HIT(15)
-#undef QB_HIT
-    while (mask) {
-        const uint32_t j = (uint32_t)__ffs((int)mask) - 1u;
-        mask &= mask - 1u;
-        const bool b0 = j & 1u, b1 = j & 2u, b2 = j & 4u, b3 = j & 8u;
-        const uint32_t s0 = b0 ? r1 : r0, s1 = b0 ? r3 : r2, s2 = b0 ? r5 : r4, s3 = b0 ? r7 : r6, s4 = b0 ? r9 : r8, s5 = b0 ? r11 : r10, s6 = b0 ? r13 : r12,
-                       s7 = b0 ? r15 : r14;
-        const uint32_t u0 = b1 ? s1 : s0, u1 = b1 ? s3 : s2, u2 = b1 ? s5 : s4, u3 = b1 ? s7 : s6;
-        const uint32_t w0 = b2 ? u1 : u0, w1 = b2 ? u3 : u2;
-        epilogue_approx(es, __uint_as_float(b3 ? w1 : w0), c * 16 + j, row, (row_flags & 1u) != 0, (row_flags & 2u) != 0);
-    }
-}
-__device__ __forceinline__ void epilogue_chunk_f16(EpiShared* es, uint32_t (&r)[16], uint32_t c, float t_row, uint64_t row, uint32_t row_flags) {
-    float mx = __uint_as_float(r[0]);
-#pragma unroll
-    for (int j = 1; j < 16; ++j) mx = fmaxf(mx, __uint_as_float(r[j]));
-    if (__any_sync(0xFFFFFFFFu, mx >= t_row))
-        epilogue_hits_f16(es, r[0], r[1], r[2], r[3], r[4], r[5], r[6], r[7], r[8], r[9], r[10], r[11], r[12], r[13], r[14], r[15], c, t_row, row, row_flags);
-}
 
-// Slow path of a chunk: at least one lane of the warp has a column at or above the threshold.  ONE out-of-line copy for the
-// whole kernel (the 16 accumulator values travel in registers): the hot loop stays a few hundred bytes of straight-line code.
+// Slow path of a 32-column chunk: at least one lane of the warp holds a value at or above its row's threshold.  ONE out-of-line copy
+// per variant (the 16 accumulator values travel in registers): the hot loop stays straight-line code.
+// wgmma accumulator layout (m64nN): value j of a thread sits in row  row_lo + 8 * ((j >> 1) & 1)  and column
+// 8 * (j >> 2) + 2 * (lane & 3) + (j & 1) of the chunk, row_lo = 16 * (warp in warpgroup) + lane / 4.
+// row_flags: bit 0 / 1 = valid / deleted for row_lo, bits 2 / 3 the same for row_lo + 8.
+template <bool F16>
 __device__ __noinline__ void epilogue_hits(EpiShared* es, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3, uint32_t r4, uint32_t r5, uint32_t r6, uint32_t r7,
                                            uint32_t r8, uint32_t r9, uint32_t r10, uint32_t r11, uint32_t r12, uint32_t r13, uint32_t r14, uint32_t r15, uint32_t c,
-                                           int t_row, uint64_t row, uint32_t row_flags, float v_off) {
+                                           uint32_t t_lo, uint32_t t_hi, uint64_t row_lo, uint32_t row_flags, float voff_lo, float voff_hi) {
     uint32_t mask = 0;
-#define QB_HIT(j) mask |= ((int)r##j >= t_row) ? (1u << j) : 0u;
+#define QB_HIT(j)                                                                                                          \
+    {                                                                                                                      \
+        const uint32_t t = ((j) & 2) ? t_hi : t_lo;                                                                        \
+        const bool hit = F16 ? (__uint_as_float(r##j) >= __uint_as_float(t)) : ((int)r##j >= (int)t);                    \
+        mask |= hit ? (1u << (j)) : 0u;                                                                                    \
+    }
     QB_HIT(0) QB_HIT(1) QB_HIT(2) QB_HIT(3) QB_HIT(4) QB_HIT(5) QB_HIT(6) QB_HIT(7) QB_HIT(8) QB_HIT(9) QB_HIT(10) QB_HIT(11) QB_HIT(12) QB_HIT(13) QB_HIT(14) QB_HIT(15)
 #undef QB_HIT
+    const uint32_t lane_col = 2u * (threadIdx.x & 3u);
     while (mask) {  // divergent: usually one lane, one column
         const uint32_t j = (uint32_t)__ffs((int)mask) - 1u;
         mask &= mask - 1u;
@@ -312,64 +239,100 @@ __device__ __noinline__ void epilogue_hits(EpiShared* es, uint32_t r0, uint32_t 
                        s7 = b0 ? r15 : r14;
         const uint32_t u0 = b1 ? s1 : s0, u1 = b1 ? s3 : s2, u2 = b1 ? s5 : s4, u3 = b1 ? s7 : s6;
         const uint32_t w0 = b2 ? u1 : u0, w1 = b2 ? u3 : u2;
-        epilogue_exact(es, b3 ? w1 : w0, c * 16 + j, row, (row_flags & 1u) != 0, (row_flags & 2u) != 0, v_off);
+        const uint32_t v = b3 ? w1 : w0;
+        const uint32_t n = c * NC + 8u * (j >> 2) + lane_col + (j & 1u);
+        const uint64_t row = row_lo + (b1 ? 8u : 0u);
+        const uint32_t fl = b1 ? (row_flags >> 2) : row_flags;
+        if (F16) epilogue_approx(es, __uint_as_float(v), n, row, (fl & 1u) != 0, (fl & 2u) != 0);
+        else epilogue_exact(es, v, n, row, (fl & 1u) != 0, (fl & 2u) != 0, b1 ? voff_hi : voff_lo);
     }
 }
 
-// Filter one 16-column chunk of the accumulator row held by this lane.  t_row = batch threshold - row term (registers only).
-__device__ __forceinline__ void epilogue_chunk(EpiShared* es, uint32_t (&r)[16], uint32_t c, int t_row, uint64_t row, uint32_t row_flags, float v_off) {
-    int mx = (int)r[0];
+// Filter one 32-column chunk held by this thread (two rows x 8 columns).  t_lo / t_hi = batch threshold - row term (registers only).
+template <bool F16>
+__device__ __forceinline__ void epilogue_chunk(EpiShared* es, const uint32_t (&r)[16], uint32_t c, uint32_t t_lo, uint32_t t_hi, uint64_t row_lo, uint32_t row_flags,
+                                               float voff_lo, float voff_hi) {
+    bool hit;
+    if (F16) {
+        float m_lo = __uint_as_float(r[0]), m_hi = __uint_as_float(r[2]);
 #pragma unroll
-    for (int j = 1; j < 16; ++j) mx = max(mx, (int)r[j]);
-    if (__any_sync(0xFFFFFFFFu, mx >= t_row))
-        epilogue_hits(es, r[0], r[1], r[2], r[3], r[4], r[5], r[6], r[7], r[8], r[9], r[10], r[11], r[12], r[13], r[14], r[15], c, t_row, row, row_flags, v_off);
+        for (int j = 0; j < 16; ++j) {
+            if (j & 2) m_hi = fmaxf(m_hi, __uint_as_float(r[j]));
+            else m_lo = fmaxf(m_lo, __uint_as_float(r[j]));
+        }
+        hit = m_lo >= __uint_as_float(t_lo) || m_hi >= __uint_as_float(t_hi);
+    } else {
+        int m_lo = (int)r[0], m_hi = (int)r[2];
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            if (j & 2) m_hi = max(m_hi, (int)r[j]);
+            else m_lo = max(m_lo, (int)r[j]);
+        }
+        hit = m_lo >= (int)t_lo || m_hi >= (int)t_hi;
+    }
+    if (__any_sync(0xFFFFFFFFu, hit))
+        epilogue_hits<F16>(es, r[0], r[1], r[2], r[3], r[4], r[5], r[6], r[7], r[8], r[9], r[10], r[11], r[12], r[13], r[14], r[15], c, t_lo, t_hi, row_lo, row_flags,
+                           voff_lo, voff_hi);
+}
+
+// per-row inputs of the epilogue: validity, delete bit, v_off and the row term of the prefilter
+struct RowIn {
+    bool valid, dead;
+    float v_off;
+    int vi;
+};
+template <bool F16>
+__device__ __forceinline__ RowIn row_in(const MmaParams& p, const QbEmit& emit, uint64_t row, bool pre) {
+    RowIn r;
+    r.valid = row < p.n_rows;
+    r.v_off = (r.valid && !F16) ? p.voff[row] : 0.0f;
+    r.dead = !r.valid || qb_is_deleted(emit, (uint32_t)(r.valid ? row : 0));
+    r.vi = 0;
+    if (pre && !F16) {  // score >= thr  <=>  dot >= t_query - v_off/mult; everything is rounded towards "pass"
+        const float vm = r.v_off / p.multiplier;
+        const float up = ceilf(vm + 1.0e-5f * fabsf(vm)) + 2.0f;
+        r.vi = (int)fminf(fmaxf(up, (float)-T_CLAMP), (float)T_CLAMP);
+    }
+    return r;
 }
 
 // ---------------------------------------------------------------------------------------------- the kernel
-template <bool TWO, bool F16 = false>
+template <int NCH, bool F16>
 __global__ void __launch_bounds__(THREADS, 1)
 sq8_mma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const MmaParams p, const QbEmit emit) {
-    constexpr int STAGES = TWO ? STAGES_2 : STAGES_1;
-    constexpr uint32_t TILE_M = TWO ? 2 * MMA_M : MMA_M;  // rows per tile of the CTA (pair)
+    constexpr uint32_t n_blk = NCH * NC;
     extern __shared__ __align__(1024) uint8_t smem[];
     if ((qb_smem_u32(smem) & 1023u) != 0u) __trap();      // 128-B swizzle atoms need 1024-B alignment (no static smem precedes)
-    const uint32_t rank = TWO ? cluster_ctarank() : 0u;
-    const uint32_t n_mine = TWO ? (p.n_blk >> 1) : p.n_blk;  // query rows of B held by this CTA
     const uint32_t n_kb = (p.ad + KB - 1) / KB;
-    const uint32_t b_block_bytes = n_mine * KB;
+    const uint32_t b_block_bytes = n_blk * KB;
+    const uint32_t stages = p.stages;
     uint8_t* b_s = smem;
     uint8_t* a_s = b_s + (size_t)n_kb * b_block_bytes;
-    uint8_t* a_const = a_s + STAGES * A_STAGE_BYTES;            // [128 rows][32 B] constant A operand of the bias MMA
-    uint8_t* b_bias = a_const + MMA_M * BIAS_KB;                // [n_mine rows][32 B] per-query bias rows
-    EpiShared* es = reinterpret_cast<EpiShared*>(b_bias + (size_t)n_mine * BIAS_KB);
-    uint64_t* full_a = reinterpret_cast<uint64_t*>(es + 1);     // [STAGES]   (TWO: only the leader's copy is used)
-    uint64_t* empty_a = full_a + STAGES;                        // [STAGES]
-    uint64_t* b_full = empty_a + STAGES;                        // [1]
-    uint64_t* tm_full = b_full + 1;                             // [2]
-    uint64_t* tm_empty = tm_full + 2;                           // [2]        (TWO: only the leader's copy is used)
-    uint32_t* tmem_ptr_s = reinterpret_cast<uint32_t*>(tm_empty + 2);
+    uint8_t* a_const = a_s + (size_t)stages * A_STAGE_BYTES;    // [128 rows][32 B] constant A operand of the bias MMA
+    uint8_t* b_bias = a_const + MMA_M * BIAS_KB;                // [n_blk rows][32 B] per-query bias rows
+    EpiShared* es = reinterpret_cast<EpiShared*>(b_bias + (size_t)n_blk * BIAS_KB);
+    uint64_t* full_a = reinterpret_cast<uint64_t*>(es + 1);     // [stages]
+    uint64_t* empty_a = full_a + MAX_STAGES;                    // [stages]
+    uint64_t* b_full = empty_a + MAX_STAGES;                    // [1]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t group = TWO ? (blockIdx.x >> 1) : blockIdx.x;  // CTA (pair) index
-    const uint32_t qblock = group % p.n_qblocks;
-    const uint32_t worker = group / p.n_qblocks;
-    const uint64_t n_tiles = (p.n_rows + TILE_M - 1) / TILE_M;
+    const uint32_t qblock = blockIdx.x % p.n_qblocks;
+    const uint32_t worker = blockIdx.x / p.n_qblocks;
+    const uint64_t n_tiles = (p.n_rows + MMA_M - 1) / MMA_M;
     const uint64_t my_tiles = (worker < n_tiles) ? (n_tiles - worker + p.n_workers - 1) / p.n_workers : 0;
-    const uint32_t q_base = qblock * p.n_blk;
-    const uint32_t row_in_tile0 = rank * MMA_M;
+    const uint32_t q_base = qblock * n_blk;
     const bool use_bias = p.bias_rows != nullptr;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { qb_mbar_init(&full_a[s], 1); qb_mbar_init(&empty_a[s], 1); }
+        for (uint32_t s = 0; s < stages; ++s) { qb_mbar_init(&full_a[s], 1); qb_mbar_init(&empty_a[s], CONSUMER_WARPS); }
         qb_mbar_init(b_full, 1);
-        for (int a = 0; a < 2; ++a) { qb_mbar_init(&tm_full[a], 1); qb_mbar_init(&tm_empty[a], (TWO ? 2 : 1) * EPI_WARPS); }
         es->cand = emit.cand; es->cap = emit.cap; es->dense_base = emit.dense_base; es->gcnt = emit.cnt; es->flags = p.flags;
-        es->multiplier = p.multiplier; es->seg_cap = p.seg_cap; es->seg_index = TWO ? worker * 2 + rank : worker; es->q_base = q_base; es->nq = p.nq;
+        es->multiplier = p.multiplier; es->seg_cap = p.seg_cap; es->seg_index = worker; es->q_base = q_base; es->nq = p.nq;
         es->id_base = emit.id_base; es->dense = emit.dense; es->check_exact = p.check_exact;
     }
     for (uint32_t i = threadIdx.x; i < N_MAX; i += blockDim.x) {
         const uint32_t q = q_base + i;
-        const bool real = i < p.n_blk && q < p.nq;
+        const bool real = i < n_blk && q < p.nq;
         es->thr[i] = real ? (emit.dense ? __int_as_float(0xff800000) : emit.thr[q]) : __int_as_float(0x7f800000);  // +inf: padding never emits
         es->qoff[i] = (real && !F16) ? p.q_off[q] : 0.0f;
         es->bias[i] = (real && use_bias) ? p.bias_i[q] : 0;
@@ -380,181 +343,107 @@ sq8_mma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         reinterpret_cast<uint4*>(a_const)[i] = F16 ? make_uint4(0x3F803F80u, 0u, 0u, 0u)                          // bf16 (1, 1, 0, 0, 0, 0, 0, 0)
                                                    : make_uint4(0x7F7F7F7Fu, 0x7F7F7F7Fu, 0x7F7F7F7Fu, 0x017F7F7Fu);  // bytes 0-14 = 127, byte 15 = 1
     if (use_bias)
-        for (uint32_t i = threadIdx.x; i < n_mine * BIAS_KB / 16; i += blockDim.x)
-            reinterpret_cast<uint4*>(b_bias)[i] = reinterpret_cast<const uint4*>(p.bias_rows + (size_t)(q_base + rank * n_mine) * BIAS_KB)[i];
-    qb_fence_barrier_init();  // mbarrier inits + the generic-proxy stores above become visible to the async proxy (TMA / UMMA)
-    if (warp == WARP_MMA) {  // TWO: the same warp of both CTAs allocates (Allocator2Sm contract)
-        if (TWO) {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(qb_smem_u32(tmem_ptr_s)), "r"(TMEM_COLS) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(qb_smem_u32(tmem_ptr_s)), "r"(TMEM_COLS) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-    }
-    tc_fence_before();
+        for (uint32_t i = threadIdx.x; i < n_blk * BIAS_KB / 16; i += blockDim.x)
+            reinterpret_cast<uint4*>(b_bias)[i] = reinterpret_cast<const uint4*>(p.bias_rows + (size_t)q_base * BIAS_KB)[i];
+    qb_fence_barrier_init();  // mbarrier inits + the generic-proxy stores above become visible to the async proxy (TMA / wgmma)
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_s;
-    // resident query block: every CTA loads its own rows and waits for them; for a pair the cluster barrier then tells the leader
-    // that the peer's half is in place (and that the peer's barriers exist before any remote arrive / multicast commit)
-    if (warp == WARP_TMA && elect_one()) {
-        const uint64_t pol_keep = qb_policy_evict_last();
-        qb_mbar_arrive_expect_tx(b_full, n_kb * b_block_bytes);
-        for (uint32_t kb = 0; kb < n_kb; ++kb)
-            tma_load_2d<false>(&map_b, b_full, b_s + (size_t)kb * b_block_bytes, (int32_t)(kb * KB), (int32_t)(q_base + rank * n_mine), pol_keep);
-    }
-    qb_mbar_wait(b_full, 0);
-    if (TWO) cluster_sync_all();
 
     if (warp == WARP_TMA) {
         // ------------------------------------------------------------ TMA producer (warp-uniform loop, one elected lane issues)
         const uint64_t pol_keep = qb_policy_evict_last();
         const uint64_t pol_stream = qb_policy_evict_first();
-        uint64_t it = 0;
+        if (elect_one()) {  // resident query block
+            qb_mbar_arrive_expect_tx(b_full, n_kb * b_block_bytes);
+            for (uint32_t kb = 0; kb < n_kb; ++kb) tma_load_2d(&map_b, b_full, b_s + (size_t)kb * b_block_bytes, (int32_t)(kb * KB), (int32_t)q_base, pol_keep);
+        }
+        __syncwarp();
+        uint32_t s = 0, ph = 0;
         constexpr uint64_t PF = QB_MMA_PF;  // L2 prefetch distance in tiles: hides the HBM latency that the smem ring cannot
         for (uint64_t ti = 0; ti < my_tiles; ++ti) {
-            const int32_t row0 = (int32_t)((worker + ti * p.n_workers) * TILE_M + row_in_tile0);
+            const int32_t row0 = (int32_t)((worker + ti * p.n_workers) * MMA_M);
             if (!(p.debug & 16) && elect_one()) {  // the n_qblocks groups of a worker walk the same tiles: each prefetches its share of the K-blocks
                 for (uint64_t d = (ti == 0) ? 0 : PF; d <= PF; ++d)
                     if (ti + d < my_tiles)
                         for (uint32_t ka = qblock; ka < n_kb; ka += p.n_qblocks)
-                            tma_prefetch_2d(&map_a, (int32_t)(ka * KB), (int32_t)((worker + (ti + d) * p.n_workers) * TILE_M + row_in_tile0));
+                            tma_prefetch_2d(&map_a, (int32_t)(ka * KB), (int32_t)((worker + (ti + d) * p.n_workers) * MMA_M));
             }
             __syncwarp();
-            for (uint32_t ka = 0; ka < n_kb; ++ka, ++it) {
-                const uint32_t s = (uint32_t)(it % STAGES), ph = (uint32_t)((it / STAGES) & 1);
+            for (uint32_t ka = 0; ka < n_kb; ++ka) {
                 qb_mbar_wait(&empty_a[s], ph ^ 1u);
-                if (p.debug & 8) {  // timing experiment: stages are "filled" without moving data
-                    if (rank == 0 && elect_one()) qb_mbar_arrive(&full_a[s]);
-                } else if (elect_one()) {
-                    if (rank == 0) qb_mbar_arrive_expect_tx(&full_a[s], (TWO ? 2 : 1) * A_STAGE_BYTES);  // TWO: both CTAs' boxes land on the leader's barrier
-                    tma_load_2d<TWO>(&map_a, &full_a[s], a_s + (size_t)s * A_STAGE_BYTES, (int32_t)(ka * KB), row0, p.n_qblocks > 1 ? pol_keep : pol_stream);
+                if (elect_one()) {
+                    if (p.debug & 8) qb_mbar_arrive(&full_a[s]);  // timing experiment: stages are "filled" without moving data
+                    else {
+                        qb_mbar_arrive_expect_tx(&full_a[s], A_STAGE_BYTES);
+                        tma_load_2d(&map_a, &full_a[s], a_s + (size_t)s * A_STAGE_BYTES, (int32_t)(ka * KB), row0, p.n_qblocks > 1 ? pol_keep : pol_stream);
+                    }
                 }
                 __syncwarp();
-            }
-        }
-    } else if (warp == WARP_MMA) {
-        // ------------------------------------------------------------ MMA issuer (leader CTA of a pair; warp-uniform loop, one elected lane issues)
-        if (rank == 0) {
-            // instruction descriptor (cute::UMMA::InstrDescriptor): D = s32, A/B = u8, both K-major, M = 128 / 256, N = n_blk
-            // (F16: D = f32, A/B = bf16)
-            const uint32_t idesc = (F16 ? ((1u << 4) | (1u << 7) | (1u << 10)) : ((2u << 4) | (0u << 7) | (0u << 10))) | ((p.n_blk >> 3) << 17) |
-                                   ((uint32_t)(TILE_M >> 4) << 24);
-            // one lane issues every MMA and an int8 MMA lasts ~100 cycles: descriptors differ only in their 14-bit start-address
-            // field (low word), everything else is hoisted out of the loop
-            const uint64_t a_desc0 = make_smem_desc(qb_smem_u32(a_s)), b_desc0 = make_smem_desc(qb_smem_u32(b_s));
-            const uint32_t a_hi = (uint32_t)(a_desc0 >> 32), a_lo0 = (uint32_t)a_desc0;
-            const uint32_t b_hi = (uint32_t)(b_desc0 >> 32), b_lo0 = (uint32_t)b_desc0;
-            const uint32_t b_blk16 = b_block_bytes >> 4;
-            const uint64_t bias_a_desc = make_smem_desc_sw32(qb_smem_u32(a_const)), bias_b_desc = make_smem_desc_sw32(qb_smem_u32(b_bias));
-            const uint32_t n_k32 = (p.ad + 31) / 32;  // MMAs (K = 32 B) per tile
-            uint64_t it = 0;
-            for (uint64_t ti = 0; ti < my_tiles; ++ti) {
-                const uint32_t acc = (uint32_t)(ti & 1), acc_ph = (uint32_t)((ti >> 1) & 1);
-                qb_mbar_wait(&tm_empty[acc], acc_ph ^ 1u);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * p.n_blk;
-                for (uint32_t ka = 0; ka < n_kb; ++ka, ++it) {
-                    const uint32_t s = (uint32_t)(it % STAGES), ph = (uint32_t)((it / STAGES) & 1);
-                    qb_mbar_wait(&full_a[s], ph);
-                    tc_fence_after();
-                    const uint32_t a_lo = a_lo0 + s * (A_STAGE_BYTES >> 4);
-                    const uint32_t b_lo = b_lo0 + ka * b_blk16;  // stage ka pairs with K-block ka
-                    const uint32_t k32 = ka * (KB / 32);
-                    if (elect_one()) {
-#pragma unroll
-                        for (uint32_t j = 0; j < KB / 32; ++j)
-                            if (k32 + j < n_k32) {  // +32 B inside the swizzled row per K-step (32 u8 codes, or 16 bf16 values)
-                                if (F16) mma_f16<TWO>(d_tmem, ((uint64_t)a_hi << 32) | (a_lo + 2 * j), ((uint64_t)b_hi << 32) | (b_lo + 2 * j), idesc, (k32 + j) != 0 ? 1u : 0u);
-                                else mma_i8<TWO>(d_tmem, ((uint64_t)a_hi << 32) | (a_lo + 2 * j), ((uint64_t)b_hi << 32) | (b_lo + 2 * j), idesc, (k32 + j) != 0 ? 1u : 0u);
-                            }
-                        tc_commit<TWO>(&empty_a[s]);                      // frees the smem stage once the MMAs above have read it
-                        if (ka + 1 == n_kb) {
-                            if (use_bias) {                                                          // D += bias_q in every row
-                                if (F16) mma_f16<TWO>(d_tmem, bias_a_desc, bias_b_desc, idesc, 1u);
-                                else mma_i8<TWO>(d_tmem, bias_a_desc, bias_b_desc, idesc, 1u);
-                            }
-                            tc_commit<TWO>(&tm_full[acc]);                                        // accumulator complete -> epilogue
-                        }
-                    }
-                    __syncwarp();
-                }
+                if (++s == stages) { s = 0; ph ^= 1u; }
             }
         }
     } else {
-        // ------------------------------------------------------------ epilogue warps (own 128 rows, all n_blk columns)
-        const uint32_t quarter = (uint32_t)(warp & 3);  // TMEM lanes this warp may read: [32*quarter, 32*quarter+32)
-        const uint32_t part = (uint32_t)(warp >> 2);    // which of every EPI_PARTS 16-column chunks
-        const uint32_t n_chunks = p.n_blk >> 4;
+        // ------------------------------------------------------------ consumer warpgroups: MMAs, then the epilogue on the accumulators
+        const uint32_t wg = (uint32_t)warp >> 2;
+        const uint32_t row_off = wg * WG_M + (uint32_t)(warp & 3) * 16 + ((uint32_t)lane >> 2);  // row_lo within the tile
         const bool pre = use_bias && (F16 || p.multiplier > 0.0f);
         const int t_int = pre ? ((p.debug & 4) ? 0x7fffffff - T_CLAMP : *p.t_int) : -T_CLAMP;  // one threshold for the whole batch, in a register
         const float t_f16 = (F16 && pre) ? __int_as_float(*p.t_int) : __int_as_float(0xff800000);  // F16: the same word holds the f32 threshold
-        // the per-row offset (and delete bit) of the NEXT tile is fetched one tile ahead, off the critical path
-        uint64_t row_n = (uint64_t)worker * TILE_M + row_in_tile0 + quarter * 32 + lane;
-        bool valid_n = my_tiles > 0 && row_n < p.n_rows;
-        float voff_n = (valid_n && !F16) ? p.voff[row_n] : 0.0f;
-        bool dead_n = !valid_n || qb_is_deleted(emit, (uint32_t)(valid_n ? row_n : 0));
-        for (uint64_t ti = 0; ti < my_tiles; ++ti) {
-            const uint32_t acc = (uint32_t)(ti & 1), acc_ph = (uint32_t)((ti >> 1) & 1);
-            const uint64_t row = row_n;
-            const bool valid_row = valid_n, dead = dead_n;
-            const float v_off = voff_n;
-            if (ti + 1 < my_tiles) {
-                row_n = (worker + (ti + 1) * p.n_workers) * TILE_M + row_in_tile0 + quarter * 32 + lane;
-                valid_n = row_n < p.n_rows;
-                voff_n = (valid_n && !F16) ? p.voff[row_n] : 0.0f;
-                dead_n = !valid_n || qb_is_deleted(emit, (uint32_t)(valid_n ? row_n : 0));
-            }
-            // row term of the prefilter: score >= thr  <=>  dot >= t_query - v_off/mult; everything is rounded towards "pass"
-            int vi = 0;
-            if (pre && !F16) {
-                const float vm = v_off / p.multiplier;
-                const float up = ceilf(vm + 1.0e-5f * fabsf(vm)) + 2.0f;
-                vi = (int)fminf(fmaxf(up, (float)-T_CLAMP), (float)T_CLAMP);
-            }
-            qb_mbar_wait(&tm_full[acc], acc_ph);
-            tc_fence_after();
-            // software pipeline: the TMEM load of the next chunk is in flight while the current one is filtered.  (Pulling all four
-            // chunks into registers at once and releasing the accumulator before filtering was measured 30 % SLOWER: bursts of
-            // tcgen05.ld from 16 warps collide with the accumulator traffic of the running MMAs.)
-            const uint32_t t_addr = tmem_base + ((quarter * 32u) << 16) + acc * p.n_blk;
-            uint32_t ra[16], rb[16];
-            const bool skip = (p.debug & 1) != 0;
-            const uint32_t row_flags = (valid_row ? 1u : 0u) | (dead ? 2u : 0u);
-            const int t_row = t_int - vi;
-            if (!skip && part < n_chunks) tmem_ld16_issue(t_addr + part * 16, ra);
+        // descriptors differ only in their 14-bit start-address field (low word): the high word is hoisted out of the loop
+        const uint64_t a_desc0 = make_smem_desc(qb_smem_u32(a_s + wg * WG_M * KB)), b_desc0 = make_smem_desc(qb_smem_u32(b_s));
+        const uint32_t a_hi = (uint32_t)(a_desc0 >> 32), a_lo0 = (uint32_t)a_desc0;
+        const uint32_t b_hi = (uint32_t)(b_desc0 >> 32), b_lo0 = (uint32_t)b_desc0;
+        const uint64_t bias_a_desc = make_smem_desc_sw32(qb_smem_u32(a_const + wg * WG_M * BIAS_KB)), bias_b_desc = make_smem_desc_sw32(qb_smem_u32(b_bias));
+        uint32_t acc[NCH][16];
 #pragma unroll
-            for (uint32_t i = 0; i < MAX_CHUNKS_PER_WARP; ++i) {
-                const uint32_t c = part + i * EPI_PARTS;
-                if (skip || c >= n_chunks) break;
-                if (i & 1) {
-                    tmem_ld_wait(rb);
-                    if (c + EPI_PARTS < n_chunks) tmem_ld16_issue(t_addr + (c + EPI_PARTS) * 16, ra);
-                    if (F16) epilogue_chunk_f16(es, rb, c, t_f16, row, row_flags);
-                    else epilogue_chunk(es, rb, c, t_row, row, row_flags, v_off);
-                } else {
-                    tmem_ld_wait(ra);
-                    if (c + EPI_PARTS < n_chunks) tmem_ld16_issue(t_addr + (c + EPI_PARTS) * 16, rb);
-                    if (F16) epilogue_chunk_f16(es, ra, c, t_f16, row, row_flags);
-                    else epilogue_chunk(es, ra, c, t_row, row, row_flags, v_off);
+        for (int c = 0; c < NCH; ++c)
+#pragma unroll
+            for (int i = 0; i < 16; ++i) acc[c][i] = 0u;
+        qb_mbar_wait(b_full, 0);
+        uint32_t s = 0, ph = 0;
+        for (uint64_t ti = 0; ti < my_tiles; ++ti) {
+            const uint64_t row_lo = (worker + ti * p.n_workers) * MMA_M + row_off;
+            const RowIn lo = row_in<F16>(p, emit, row_lo, pre), hi = row_in<F16>(p, emit, row_lo + 8, pre);  // loads in flight under the MMAs
+            uint32_t s_prev = 0;
+            for (uint32_t ka = 0; ka < n_kb; ++ka) {
+                qb_mbar_wait(&full_a[s], ph);
+                wg_fence();
+#pragma unroll
+                for (int c = 0; c < NCH; ++c) acc_fence(acc[c]);
+                const uint32_t a_lo = a_lo0 + s * (A_STAGE_BYTES >> 4);
+                const uint32_t b_lo = b_lo0 + ka * (b_block_bytes >> 4);  // stage ka pairs with K-block ka
+#pragma unroll
+                for (uint32_t j = 0; j < KB / 32; ++j)  // +32 B inside the swizzled row per K-step (32 u8 codes, or 16 bf16 values); past ad the TMA boxes hold zeros
+#pragma unroll
+                    for (int c = 0; c < NCH; ++c)
+                        wgmma_n32<F16>(acc[c], ((uint64_t)a_hi << 32) | (a_lo + 2 * j), ((uint64_t)b_hi << 32) | (b_lo + c * (NC * KB >> 4) + 2 * j),
+                                       (ka | j) != 0 ? 1u : 0u);
+                wg_commit();
+                if (ka > 0) {  // the MMAs of K-block ka - 1 have retired: its stage goes back to the producer
+                    wg_wait<1>();
+                    __syncwarp();
+                    if (lane == 0) qb_mbar_arrive(&empty_a[s_prev]);
                 }
+                s_prev = s;
+                if (++s == stages) { s = 0; ph ^= 1u; }
             }
-            tc_fence_before();
+            if (use_bias) {  // D += bias_q in every row
+                wg_fence();
+#pragma unroll
+                for (int c = 0; c < NCH; ++c) wgmma_n32<F16>(acc[c], bias_a_desc, bias_b_desc + (uint64_t)(c * NC * BIAS_KB >> 4), 1u);
+                wg_commit();
+            }
+            wg_wait<0>();
+#pragma unroll
+            for (int c = 0; c < NCH; ++c) acc_fence(acc[c]);
             __syncwarp();
-            if (lane == 0) {
-                if (TWO) mbar_arrive_on_cta(&tm_empty[acc], 0);  // the leader's barrier counts the warps of both CTAs
-                else qb_mbar_arrive(&tm_empty[acc]);
-            }
+            if (lane == 0) qb_mbar_arrive(&empty_a[s_prev]);
+            if (p.debug & 1) continue;
+            const uint32_t row_flags = (lo.valid ? 1u : 0u) | (lo.dead ? 2u : 0u) | (hi.valid ? 4u : 0u) | (hi.dead ? 8u : 0u);
+            const uint32_t t_lo = F16 ? __float_as_uint(t_f16) : (uint32_t)(t_int - lo.vi);
+            const uint32_t t_hi = F16 ? __float_as_uint(t_f16) : (uint32_t)(t_int - hi.vi);
+#pragma unroll
+            for (int c = 0; c < NCH; ++c) epilogue_chunk<F16>(es, acc[c], (uint32_t)c, t_lo, t_hi, row_lo, row_flags, lo.v_off, hi.v_off);
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (TWO) cluster_sync_all();  // the leader's MMAs write the peer's TMEM: nobody deallocates before both CTAs are done
-    if (warp == WARP_MMA) {
-        tc_fence_after();
-        if (TWO) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-        else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
     }
 }
 
@@ -762,29 +651,50 @@ qb_status make_map_u8(CUtensorMap* m, const void* base, uint64_t inner_bytes, ui
     return QB_OK;
 }
 
-// query block width for a variant: resident B + A ring + small arrays must fit 227 KB; equal-width blocks
-uint32_t block_for_bytes(uint32_t k_bytes, uint32_t nq, bool two);
-uint32_t block_for(const qb_storage* s, uint32_t nq, bool two) { return block_for_bytes(s->actual_dim, nq, two); }
-uint32_t block_for_bytes(uint32_t k_bytes, uint32_t nq, bool two) {
-    const uint32_t n_kb = (k_bytes + KB - 1) / KB;
-    const size_t budget = 227 * 1024 - (size_t)(two ? STAGES_2 : STAGES_1) * A_STAGE_BYTES - MMA_M * BIAS_KB - SMALL_SMEM;
-    uint32_t n_blk = (uint32_t)(budget / ((size_t)n_kb * KB + BIAS_KB)) * (two ? 2u : 1u);
-    const uint32_t gran = two ? 32u : 16u;
-    n_blk = (n_blk > (uint32_t)N_MAX ? (uint32_t)N_MAX : n_blk) & ~(gran - 1);
-    if (n_blk < gran) return 0;
+constexpr size_t SMEM_MAX = 227 * 1024;
+// shared memory of everything but the A ring: resident query block and its bias rows, the bias MMA's constant A tile, small arrays
+size_t fixed_smem(uint32_t k_bytes, uint32_t n_blk) {
+    return (size_t)n_blk * ((size_t)((k_bytes + KB - 1) / KB) * KB + BIAS_KB) + MMA_M * BIAS_KB + SMALL_SMEM;
+}
+// query block width: the fixed part and a ring of MIN_STAGES must fit; equal-width blocks, multiples of one wgmma's N
+uint32_t block_for_bytes(uint32_t k_bytes, uint32_t nq) {
+    uint32_t n_blk = N_MAX;
+    while (n_blk >= NC && fixed_smem(k_bytes, n_blk) + MIN_STAGES * A_STAGE_BYTES > SMEM_MAX) n_blk -= NC;
+    if (n_blk < NC) return 0;
     const uint32_t n_qblocks = (nq + n_blk - 1) / n_blk;
-    return (((nq + n_qblocks - 1) / n_qblocks) + gran - 1) & ~(gran - 1);
+    return (((nq + n_qblocks - 1) / n_qblocks) + NC - 1) & ~(NC - 1);
+}
+uint32_t block_for(const qb_storage* s, uint32_t nq) { return block_for_bytes(s->actual_dim, nq); }
+
+// one CTA per (worker, query block); the ring takes what shared memory the fixed part leaves, up to MAX_STAGES
+template <bool F16>
+qb_status launch_mma(const CUtensorMap& map_a, const CUtensorMap& map_b, MmaParams p, const QbEmit& emit, uint32_t n_blk, cudaStream_t stream) {
+    QB_CHECK(n_blk % NC == 0 && n_blk >= NC && n_blk <= N_MAX, QB_ERR_INVALID, "mma scan: query block width %u", n_blk);
+    const size_t fixed = fixed_smem(p.ad, n_blk);
+    QB_CHECK(fixed + MIN_STAGES * A_STAGE_BYTES <= SMEM_MAX, QB_ERR_INVALID, "mma scan: shared memory %zu exceeds 227 KB", fixed + MIN_STAGES * A_STAGE_BYTES);
+    p.stages = (uint32_t)std::min<size_t>(MAX_STAGES, (SMEM_MAX - fixed) / A_STAGE_BYTES);
+    const size_t smem = fixed + (size_t)p.stages * A_STAGE_BYTES;
+    void (*k)(const CUtensorMap, const CUtensorMap, const MmaParams, const QbEmit) = nullptr;
+    switch (n_blk / NC) {
+        case 1: k = sq8_mma_kernel<1, F16>; break;
+        case 2: k = sq8_mma_kernel<2, F16>; break;
+        case 3: k = sq8_mma_kernel<3, F16>; break;
+        default: k = sq8_mma_kernel<4, F16>; break;
+    }
+    QB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k<<<p.n_workers * p.n_qblocks, THREADS, smem, stream>>>(map_a, map_b, p, emit);
+    QB_LAUNCHED();
+    QB_CUDA(cudaGetLastError());
+    return QB_OK;
 }
 
 }  // namespace
 
-// Can this (storage, batch) use the tensor-core path?  Returns the query block width (0 = no); bit 31 selects the cta_group::2 kernel.
+// Can this (storage, batch) use the tensor-core path?  Returns the query block width (0 = no).
 uint32_t qb_sq8_mma_block(const qb_storage* s, uint32_t nq) {
     if (s->kind != QB_KIND_SQ8 || s->qdist == QB_QD_L1) return 0;
     if (nq < 32 || s->count < 4 * 128) return 0;
-    if (!qb_opt().mma_1cta && !(s->sm_count & 1))
-        if (const uint32_t b2 = block_for(s, nq, true)) return b2 | 0x80000000u;
-    return block_for(s, nq, false);
+    return block_for(s, nq);
 }
 // scratch the filter-mode scan needs (bias rows, bias integers, the batch threshold)
 size_t qb_sq8_mma_scratch_bytes(const qb_storage*, uint32_t nq_pad) { return (size_t)nq_pad * (BIAS_KB + 4) + 256; }
@@ -792,11 +702,9 @@ size_t qb_sq8_mma_scratch_bytes(const qb_storage*, uint32_t nq_pad) { return (si
 // d_q_codes: [>= nq_pad][ad] u8 query codes (rows past nq are never scored).  Dense emit = sample pass (no thresholds yet);
 // filter emit = main pass: queries are sorted by threshold first, survivors land in per-(query, CTA) segments and *seg_len
 // (if given) returns the fixed length of each query's candidate row (zero = empty slot).
-qb_status qb_sq8_mma_scan(const qb_storage* s, const uint8_t* d_q_codes, uint32_t nq_pad, const float* d_q_off, uint32_t nq, uint32_t n_blk_flag,
+qb_status qb_sq8_mma_scan(const qb_storage* s, const uint8_t* d_q_codes, uint32_t nq_pad, const float* d_q_off, uint32_t nq, uint32_t n_blk,
                           uint64_t row_begin, uint64_t row_end, const QbEmit& emit, unsigned int* d_flags, unsigned long long* seg_len, void* d_scratch,
                           size_t scratch_bytes, cudaStream_t stream) {
-    const bool two = (n_blk_flag & 0x80000000u) != 0;
-    const uint32_t n_blk = n_blk_flag & 0x7FFFFFFFu;
     if (seg_len) *seg_len = 0;
     QB_CHECK(row_begin == 0, QB_ERR_INVALID, "sq8_mma_scan: scans start at row 0");
     QB_CHECK(emit.dense || (emit.thr && emit.cnt), QB_ERR_INVALID, "sq8_mma_scan: filter mode needs thresholds and counters");
@@ -804,7 +712,7 @@ qb_status qb_sq8_mma_scan(const qb_storage* s, const uint8_t* d_q_codes, uint32_
     const uint32_t n_qblocks = (nq + n_blk - 1) / n_blk;
     QB_CHECK(nq_pad >= n_qblocks * n_blk && nq_pad % 16 == 0, QB_ERR_INVALID, "sq8_mma_scan: query buffer not padded");
     MmaParams p{};
-    p.voff = s->d_voff; p.n_rows = row_end; p.ad = ad; p.n_blk = n_blk; p.n_qblocks = n_qblocks; p.nq = nq;
+    p.voff = s->d_voff; p.n_rows = row_end; p.ad = ad; p.n_qblocks = n_qblocks; p.nq = nq;
     p.multiplier = s->multiplier; p.q_off = d_q_off; p.flags = d_flags;
     p.check_exact = ((uint64_t)ad * 127ull * 127ull >= (1ull << 24)) ? 1 : 0;
     p.debug = qb_opt().mma_debug;
@@ -821,14 +729,13 @@ qb_status qb_sq8_mma_scan(const qb_storage* s, const uint8_t* d_q_codes, uint32_
     }
     CUtensorMap map_a, map_b;
     QB_TRY(make_map_u8(&map_a, s->d_codes, ad, row_end, KB, MMA_M));
-    QB_TRY(make_map_u8(&map_b, d_q_codes, ad, nq_pad, KB, two ? n_blk / 2 : n_blk));
-    const uint32_t tile_m = two ? 2 * MMA_M : MMA_M;
-    const uint64_t n_tiles = (row_end + tile_m - 1) / tile_m;
-    uint32_t workers = (two ? (uint32_t)s->sm_count / 2 : (uint32_t)s->sm_count) / n_qblocks;
+    QB_TRY(make_map_u8(&map_b, d_q_codes, ad, nq_pad, KB, n_blk));
+    const uint64_t n_tiles = (row_end + MMA_M - 1) / MMA_M;
+    uint32_t workers = (uint32_t)s->sm_count / n_qblocks;
     if (workers < 1) workers = 1;
     if (workers > n_tiles) workers = (uint32_t)n_tiles;
     p.n_workers = workers;
-    const uint32_t n_seg = two ? 2 * workers : workers;  // CTAs that ever see a given query
+    const uint32_t n_seg = workers;  // CTAs that ever see a given query
     if (!emit.dense && seg_len && !qb_opt().mma_no_segments) {
         uint64_t seg = (emit.cap / n_seg) & ~15ull;
         const uint64_t seg_max = qb_opt().mma_seg_cap ? qb_opt().mma_seg_cap : 256;   // slots per (query, CTA): the selection scans all of them
@@ -839,28 +746,7 @@ qb_status qb_sq8_mma_scan(const qb_storage* s, const uint8_t* d_q_codes, uint32_
             QB_CUDA(cudaMemset2DAsync(emit.cand, emit.cap * 8, 0, (size_t)n_seg * seg * 8, nq, stream));
         }
     }
-    const uint32_t n_kb = (ad + KB - 1) / KB;
-    const size_t smem = (size_t)(two ? n_blk / 2 : n_blk) * ((size_t)n_kb * KB + BIAS_KB) + (size_t)(two ? STAGES_2 : STAGES_1) * A_STAGE_BYTES + MMA_M * BIAS_KB + SMALL_SMEM;
-    QB_CHECK(smem <= 227 * 1024, QB_ERR_INVALID, "sq8_mma_scan: shared memory %zu exceeds 227 KB", smem);
-    if (two) {
-        QB_CUDA(cudaFuncSetAttribute(sq8_mma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(2 * workers * n_qblocks);
-        cfg.blockDim = dim3(THREADS);
-        cfg.dynamicSmemBytes = smem;
-        cfg.stream = stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        QB_CUDA(cudaLaunchKernelEx(&cfg, sq8_mma_kernel<true>, map_a, map_b, p, emit));
-    } else {
-        QB_CUDA(cudaFuncSetAttribute(sq8_mma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        sq8_mma_kernel<false><<<workers * n_qblocks, THREADS, smem, stream>>>(map_a, map_b, p, emit);
-    }
-    QB_LAUNCHED();
-    QB_CUDA(cudaGetLastError());
-    return QB_OK;
+    return launch_mma<false>(map_a, map_b, p, emit, n_blk, stream);
 }
 
 // ---------------------------------------------------------------------------------------------- dense f32 batches (F16 prefilter + exact rescoring)
@@ -890,7 +776,7 @@ qb_status qb_f32_shadow_ensure(qb_storage* s, cudaStream_t stream) {
     return QB_OK;
 }
 
-// Query block width of the tensor-core prefilter for a dense f32 storage (0 = not applicable); bit 31 = cta_group::2.
+// Query block width of the tensor-core prefilter for a dense f32 storage (0 = not applicable).
 uint32_t qb_f32_mma_block(qb_storage* s, uint32_t nq, cudaStream_t stream) {
     if (s->kind != QB_KIND_DENSE || s->dtype != QB_DT_F32) return 0;
     if (s->distance != QB_DIST_DOT && s->distance != QB_DIST_COSINE) return 0;   // the approximation bounds a dot product
@@ -898,19 +784,15 @@ uint32_t qb_f32_mma_block(qb_storage* s, uint32_t nq, cudaStream_t stream) {
     if (qb_f32_shadow_ensure(s, stream) != QB_OK) { cudaGetLastError(); return 0; }  // e.g. no room for the shadow plane: stay on the exact kernels
     if (!s->bf16_usable) return 0;                                                // NaN / inf rows: only the exact kernels honour OrderedFloat
     const uint32_t k_bytes = (uint32_t)round_up_u64(s->dim, 8) * 2;
-    if (!qb_opt().mma_1cta && !(s->sm_count & 1))
-        if (const uint32_t b2 = block_for_bytes(k_bytes, nq, true)) return b2 | 0x80000000u;
-    return block_for_bytes(k_bytes, nq, false);
+    return block_for_bytes(k_bytes, nq);
 }
 size_t qb_f32_mma_scratch_bytes(const qb_storage* s, uint32_t nq_pad) { return (size_t)nq_pad * ((size_t)round_up_u64(s->dim, 8) * 2 + BIAS_KB + 4) + 512; }
 
 // Filter pass over rows [0, row_end): survivors of the bf16 prefilter are re-scored exactly and land, with their exact scores, in the
 // counted candidate lists of `emit` (emit.thr = exact per-query thresholds).  d_q_pre = preprocessed f32 queries [nq][q_stride_f].
 // Returns QB_ERR_UNSUPPORTED (nothing launched) when the storage holds non-finite values: the caller takes the exact path.
-qb_status qb_f32_mma_scan(qb_storage* s, const float* d_q_pre, uint32_t q_stride_f, uint32_t nq, uint32_t nq_pad, uint32_t n_blk_flag, uint64_t row_end, const QbEmit& emit,
+qb_status qb_f32_mma_scan(qb_storage* s, const float* d_q_pre, uint32_t q_stride_f, uint32_t nq, uint32_t nq_pad, uint32_t n_blk, uint64_t row_end, const QbEmit& emit,
                           unsigned int* d_flags, void* d_scratch, size_t scratch_bytes, cudaStream_t stream) {
-    const bool two = (n_blk_flag & 0x80000000u) != 0;
-    const uint32_t n_blk = n_blk_flag & 0x7FFFFFFFu;
     QB_CHECK(!emit.dense && emit.thr && emit.cnt, QB_ERR_INVALID, "f32_mma_scan: filter mode only");
     QB_CHECK(s->bf16_ready && s->bf16_usable, QB_ERR_INVALID, "f32_mma_scan: no usable bf16 shadow (qb_f32_mma_block decides)");
     const uint32_t row_h = s->bf16_row_h, ad = row_h * 2;
@@ -926,39 +808,18 @@ qb_status qb_f32_mma_scan(qb_storage* s, const float* d_q_pre, uint32_t q_stride
     QB_LAUNCHED();
     QB_CUDA(cudaGetLastError());
     MmaParams p{};
-    p.voff = nullptr; p.n_rows = row_end; p.ad = ad; p.n_blk = n_blk; p.n_qblocks = n_qblocks; p.nq = nq;
+    p.voff = nullptr; p.n_rows = row_end; p.ad = ad; p.n_qblocks = n_qblocks; p.nq = nq;
     p.multiplier = 1.0f; p.q_off = nullptr; p.flags = d_flags; p.check_exact = 0; p.debug = qb_opt().mma_debug;
     p.bias_rows = bias_rows; p.bias_i = bias_f; p.t_int = t_word; p.seg_cap = 0;
     CUtensorMap map_a, map_b;
     QB_TRY(make_map_u8(&map_a, s->d_bf16, ad, row_end, KB, MMA_M));
-    QB_TRY(make_map_u8(&map_b, qb, ad, nq_pad, KB, two ? n_blk / 2 : n_blk));
-    const uint32_t tile_m = two ? 2 * MMA_M : MMA_M;
-    const uint64_t n_tiles = (row_end + tile_m - 1) / tile_m;
-    uint32_t workers = (two ? (uint32_t)s->sm_count / 2 : (uint32_t)s->sm_count) / n_qblocks;
+    QB_TRY(make_map_u8(&map_b, qb, ad, nq_pad, KB, n_blk));
+    const uint64_t n_tiles = (row_end + MMA_M - 1) / MMA_M;
+    uint32_t workers = (uint32_t)s->sm_count / n_qblocks;
     if (workers < 1) workers = 1;
     if (workers > n_tiles) workers = (uint32_t)n_tiles;
     p.n_workers = workers;
-    const uint32_t n_kb = (ad + KB - 1) / KB;
-    const size_t smem = (size_t)(two ? n_blk / 2 : n_blk) * ((size_t)n_kb * KB + BIAS_KB) + (size_t)(two ? STAGES_2 : STAGES_1) * A_STAGE_BYTES + MMA_M * BIAS_KB + SMALL_SMEM;
-    QB_CHECK(smem <= 227 * 1024, QB_ERR_INVALID, "f32_mma_scan: shared memory %zu exceeds 227 KB", smem);
-    if (two) {
-        QB_CUDA(cudaFuncSetAttribute(sq8_mma_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        cudaLaunchConfig_t cfg{};
-        cfg.gridDim = dim3(2 * workers * n_qblocks);
-        cfg.blockDim = dim3(THREADS);
-        cfg.dynamicSmemBytes = smem;
-        cfg.stream = stream;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        QB_CUDA(cudaLaunchKernelEx(&cfg, sq8_mma_kernel<true, true>, map_a, map_b, p, emit));
-    } else {
-        QB_CUDA(cudaFuncSetAttribute(sq8_mma_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        sq8_mma_kernel<false, true><<<workers * n_qblocks, THREADS, smem, stream>>>(map_a, map_b, p, emit);
-    }
-    QB_LAUNCHED();
-    QB_CUDA(cudaGetLastError());
+    QB_TRY(launch_mma<true>(map_a, map_b, p, emit, n_blk, stream));
     // exact scores for the survivors (and only them)
     const dim3 grid(8, std::min<uint32_t>(nq, (uint32_t)s->sm_count * 4));
     f32_rescore_kernel<<<grid, 256, 0, stream>>>(reinterpret_cast<const uint8_t*>(s->d_rows), s->row_stride, s->dim, d_q_pre, q_stride_f, nq, emit.cand, emit.cnt, emit.cap,

@@ -193,7 +193,7 @@ extern "C" qb_status qb_sq8_quantile_interval_device(int32_t device, uint32_t di
     if (cudaMalloc(&d_in, len * 4) != cudaSuccess || cudaMalloc(&d_out, len * 4) != cudaSuccess || cudaMalloc(&d_tmp, tmp_bytes + 256) != cudaSuccess) st = QB_ERR_OOM;
     uint32_t k2[2] = {0, 0};
     if (st == QB_OK) {
-        f32_to_sort_keys<<<(unsigned)std::min<uint64_t>((len + 255) / 256, 148 * 16), 256>>>(dev_sample_rows, row_stride_bytes / 4, dim, n_sample, d_in);
+        f32_to_sort_keys<<<(unsigned)std::min<uint64_t>((len + 255) / 256, 132 * 16), 256>>>(dev_sample_rows, row_stride_bytes / 4, dim, n_sample, d_in);
         QB_LAUNCHED();
         cub::DeviceRadixSort::SortKeys(d_tmp, tmp_bytes, d_in, d_out, (int)len);
         cudaError_t e = cudaMemcpy(&k2[0], d_out + cut + 1, 4, cudaMemcpyDeviceToHost);

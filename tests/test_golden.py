@@ -1,5 +1,5 @@
-"""Committed golden vectors = outputs of the reference's OWN C kernels (tests/golden/make_golden.py ran them from
-/root/reference; that tree does not exist on the GPU box).  CPU: the oracle's restatement reproduces them.  GPU: the CUDA path
+"""Committed golden vectors = outputs of the reference's OWN C kernels (tests/golden/make_golden.py ran them from a
+qdrant source tree, which is not part of this repository).  CPU: the oracle's restatement reproduces them.  GPU: the CUDA path
 reproduces them through the C ABI."""
 import ctypes as C
 import os

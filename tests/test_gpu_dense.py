@@ -196,7 +196,7 @@ def test_filtered_scorer_like_hnsw_hop(qb, oracle):
 # ------------------------------------------------------------------------------------------------ batched f32 on the tensor cores (J1)
 @pytest.mark.parametrize("dist,n,dim,nq", [("Cosine", 150_000, 768, 200), ("Dot", 140_000, 100, 64), ("Cosine", 200_000, 128, 300), ("Dot", 131_072, 1536, 33)])
 def test_f32_batch_tensor_core_prefilter_is_exact(qb, oracle, dist, n, dim, nq):
-    """Batches of >= 32 f32 queries: bf16 tcgen05 prefilter + exact rescoring of the survivors == oracle peek_top_iter, bit-exact
+    """Batches of >= 32 f32 queries: bf16 wgmma prefilter + exact rescoring of the survivors == oracle peek_top_iter, bit-exact
     scores, no fallback rerun, and == the CUDA-core path (option disable_mma)."""
     d = getattr(qb.Distance, dist)
     rng = np.random.default_rng(dim + nq)

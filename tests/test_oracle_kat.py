@@ -8,6 +8,7 @@ Each case re-types the fixed vectors of a reference unit test and asserts what t
   SQ8/BQ inner loops: the reference's C kernels compiled verbatim (oracle/_ref/libsimd_utils.so)
 """
 import ctypes as C
+import os
 
 import numpy as np
 import pytest
@@ -117,14 +118,19 @@ def test_topk_matches_sort(oracle):
     np.testing.assert_array_equal(res["idx"], order.astype(np.uint32))
 
 
+def _ref_golden():
+    """What the reference's own C kernels (lib/quantization/cpp/{avx2,sse}.c, compiled verbatim) return on the seeded inputs
+    below; recorded by tests/golden/make_golden.py kernel-tests."""
+    return np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_kernels_r03.npz"))
+
+
 def test_sq8_inner_loops_match_reference_c(oracle):
     """oracle restatement == the reference's own avx2.c / sse.c compiled verbatim, on random + extreme codes."""
-    R = oracle.ref()
-    if R is None:
-        pytest.skip("oracle/_ref/libsimd_utils.so not built (no /root/reference and no prebuilt)")
+    G = _ref_golden()
     L = oracle.lib()
     u8p = C.POINTER(C.c_uint8)
     rng = np.random.default_rng(42)
+    c = 0
     for dim in (16, 32, 48, 64, 80, 768, 784, 1536, 4096):
         for trial in range(20):
             q = rng.integers(0, 128, dim, dtype=np.uint8)
@@ -133,40 +139,37 @@ def test_sq8_inner_loops_match_reference_c(oracle):
                 q[:] = 127; v[:] = 127
             if trial == 1:
                 q[:] = 0
+            assert (int(q.astype(np.int64).sum()), int(v.astype(np.int64).sum())) == (G["kat_sq8_qsum"][c], G["kat_sq8_vsum"][c]), "input stream changed"
             qp, vp = q.ctypes.data_as(u8p), v.ctypes.data_as(u8p)
-            assert L.qo_sq8_dot_avx(qp, vp, dim) == R.impl_score_dot_avx(qp, vp, dim)
-            assert L.qo_sq8_l1_avx(qp, vp, dim) == R.impl_score_l1_avx(qp, vp, dim)
+            dot_avx, l1_avx, dot_sse = G["kat_sq8_dot_avx"][c], G["kat_sq8_l1_avx"][c], G["kat_sq8_dot_sse"][c]
+            assert L.qo_sq8_dot_avx(qp, vp, dim) == dot_avx
+            assert L.qo_sq8_l1_avx(qp, vp, dim) == l1_avx
             # the SSE tier is the same integers for dims whose sums stay < 2^24 (exactness window)
             if dim <= 1040:
-                assert R.impl_score_dot_sse(qp, vp, dim) == R.impl_score_dot_avx(qp, vp, dim)
-                assert R.impl_score_dot_avx(qp, vp, dim) == np.float32(int(np.dot(q.astype(np.int64), v.astype(np.int64))))
+                assert dot_sse == dot_avx
+                assert dot_avx == np.float32(int(np.dot(q.astype(np.int64), v.astype(np.int64))))
+            c += 1
+    assert c == G["kat_sq8_dot_avx"].size
 
 
 def test_bq_popcount_matches_reference_c(oracle):
-    R = oracle.ref()
-    if R is None:
-        pytest.skip("oracle/_ref/libsimd_utils.so not built")
+    G = _ref_golden()
     rng = np.random.default_rng(9)
-    u8p = C.POINTER(C.c_uint8)
-    for dim in (1, 127, 128, 129, 768, 1000, 1536):
+    for di, dim in enumerate((1, 127, 128, 129, 768, 1000, 1536)):
         data = rng.standard_normal((4, dim)).astype(np.float32)
         q = rng.standard_normal(dim).astype(np.float32)
-        for qenc, bits, fn in ((oracle.BQQ_SCALAR8, 8, R.impl_xor_popcnt_scalar8_avx_uint128),
-                               (oracle.BQQ_SCALAR4, 4, R.impl_xor_popcnt_scalar4_avx_uint128)):
+        for qenc, bits, tag in ((oracle.BQQ_SCALAR8, 8, "s8"), (oracle.BQQ_SCALAR4, 4, "s4")):
             bq = oracle.BQ.encode(data, oracle.BQ_ONE, qenc, oracle.QD_DOT, False)
             qe = bq.encode_query(q)
-            words = bq.rows.shape[1] // 16
             for i in range(data.shape[0]):
-                row = np.ascontiguousarray(bq.rows[i])
-                x = fn(qe.ctypes.data_as(u8p), row.ctypes.data_as(u8p), words)
+                x = G["kat_bq_" + tag][di, i]
                 xf = np.float32(x) / np.float32((1 << bits) - 1)
                 zeros = np.float32(dim) - xf
                 assert bq.score(qe, i) == zeros - xf
         bq = oracle.BQ.encode(data, oracle.BQ_ONE, oracle.BQQ_SAME, oracle.QD_DOT, False)
         qe = bq.encode_query(q)
         for i in range(data.shape[0]):
-            row = np.ascontiguousarray(bq.rows[i])
-            x = R.impl_xor_popcnt_sse_uint128(qe.ctypes.data_as(u8p), row.ctypes.data_as(u8p), bq.rows.shape[1] // 16)
+            x = int(G["kat_bq_sse"][di, i])
             assert bq.score(qe, i) == np.float32(dim - x) - np.float32(x)
             bits_q = (q > 0)
             bits_v = (data[i] > 0)

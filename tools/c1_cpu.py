@@ -5,7 +5,7 @@ The reference's own CPU-runnable case: the oracle's restatement of `dot_similari
 merge = how SegmentsSearcher parallelises.  With --gpu it also runs the same queries through the CUDA path on cuda:0 and
 checks the results against the CPU scan (C1 is a parity case, not a GPU bench line: the whole data set is 51 MB).
 
-    python tools/c1_cpu.py [--gpu] > profiles/c1_cpu_r01.json
+    python tools/c1_cpu.py [--gpu] > c1_cpu.json
 """
 import argparse
 import concurrent.futures as cf
