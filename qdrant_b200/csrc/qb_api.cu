@@ -265,6 +265,7 @@ extern "C" qb_status qb_storage_write_rows(qb_storage* s, uint64_t first_row, ui
                          cudaMemcpyHostToDevice));
     s->bf16_ready = false;   // the bf16 shadow (if any) no longer mirrors the rows
     s->q8_ready = false;
+    s->q6_ready = false;
     return QB_OK;
 }
 
@@ -279,6 +280,7 @@ extern "C" qb_status qb_storage_write_rows_device(qb_storage* s, uint64_t first_
                          cudaMemcpyDeviceToDevice));
     s->bf16_ready = false;
     s->q8_ready = false;
+    s->q6_ready = false;
     return QB_OK;
 }
 
@@ -438,7 +440,7 @@ extern "C" void qb_storage_destroy(qb_storage* s) {
     ctx_destroy(s->dev_ctx);
     for (auto& pr : s->prof_pending) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
     for (auto& pr : s->prof_free) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
-    cudaFree(s->d_rows); cudaFree(s->d_bf16); cudaFree(s->d_bf16_meta); cudaFree(s->d_q8); cudaFree(s->d_q8_meta); cudaFree(s->d_codes); cudaFree(s->d_voff); cudaFree(s->d_pq_div); cudaFree(s->d_centroids); cudaFree(s->d_pq_codes);
+    cudaFree(s->d_rows); cudaFree(s->d_bf16); cudaFree(s->d_bf16_meta); cudaFree(s->d_q8); cudaFree(s->d_q8_meta); cudaFree(s->d_q6); cudaFree(s->d_q6_meta); cudaFree(s->d_codes); cudaFree(s->d_voff); cudaFree(s->d_pq_div); cudaFree(s->d_centroids); cudaFree(s->d_pq_codes);
     cudaFree(s->d_bq_rows); cudaFree(s->d_mean_std); cudaFree(s->d_deleted); cudaFree(s->d_pf_fallbacks);
     cudaGetLastError();
     delete s;

@@ -1,4 +1,5 @@
-// qb_prefilter.cu — single-query dense f32 (dot / cosine) scans at half the HBM bytes, results unchanged.
+// qb_prefilter.cu — single-query dense f32 (dot / cosine) scans at a fraction of the HBM bytes, results unchanged.
+// (The default plane is the 6-bit one further down; the bf16 plane described first is the simplest case of the same scheme.)
 //
 // The single-query scan of qb_dense.cu runs at the HBM copy rate: every query reads dim * 4 bytes per row.  The only way to more
 // queries per second is fewer bytes per row — and the scan only has to FIND the rows whose exact score can reach the top-k; it does
@@ -13,8 +14,8 @@
 //   2. dense_bf16_filter_kernel: the whole bf16 plane streams through the same TMA-bulk ring (dim * 2 bytes per row); the query sits in
 //      REGISTERS (a lane always meets the same dimensions); rows with approx >= thr_q - eps_q are appended to a candidate list — a
 //      superset of the rows whose exact score reaches thr_q, hence of the true top-k;
-//   3. f32_prefilter_finish_kernel: exact AVX-order scores of the candidates (a few hundred rows, 32 CTAs), top-k by the usual keys in the
-//      last CTA to finish;
+//   3. f32_prefilter_finish_kernel: exact AVX-order scores of the candidates (one CTA per SM, each keeping its own top-k), the top-k of
+//      those by the usual keys in the last CTA to finish;
 //   4. if the list overflowed (mass ties, a NaN query, a sample without k live rows), step 3 raises a device flag and the exact scan of
 //      the whole storage — always enqueued, it exits at once while the flag is down — produces the answer instead.
 // (RawScorer results are bit-identical to the exact path: tests/test_gpu_dense.py::test_single_query_prefilter_*.)
@@ -33,7 +34,7 @@ constexpr int PF_PRODUCERS = 2;             // producer warps (one lane each): a
                                             // barrier, issue), so ONE producer caps a CTA at one 12-KB slot per ~500 clocks — below the HBM rate for these planes
 constexpr int PF_THREADS = 32 * (PF_CONSUMER_WARPS + PF_MAX_PRODUCERS);     // launch bound; the launch uses 32 * (consumers + producers)
 constexpr uint32_t PF_SLOT_BYTES = 12288;  // target bytes per ring slot (a consumer warp holds one slot while the others are in flight)
-constexpr uint32_t PF_CAP = 16384;         // candidate rows per query (a few hundred to a few thousand expected)
+constexpr uint32_t PF_CAP = 131072;        // candidate rows per query at most (a few thousand to a few tens of thousands expected on 10M rows)
 
 static int pf_producers() { const int o = qb_opt().prefilter_producers; return (o >= 1 && o <= PF_MAX_PRODUCERS) ? o : PF_PRODUCERS; }
 
@@ -47,7 +48,7 @@ struct PfParams {
     uint32_t rows_per_slot, n_slots, slot_bytes;
     const qb_scored_point* samp_out; const uint32_t* samp_cnt; uint32_t top;   // exact top-k of the sample prefix
     const unsigned int* max_norm_bits;                                         // max row norm of the storage (f32 bits)
-    uint32_t* cand; unsigned int* cnt;
+    uint32_t* cand; unsigned int* cnt; uint32_t cap;
     const uint32_t* deleted; const uint32_t* deleted2;
     int l2_keep;
 };
@@ -56,6 +57,27 @@ __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);
     return v;
+}
+
+// One producer lane of a filter kernel's ring: tiles blockIdx.x, blockIdx.x + gridDim.x, ... of `rows_per_slot` rows, every n_prod-th one.
+// A tile's copy is rounded up to 16 bytes; planes whose stride is not a multiple of 16 keep that much padding behind their last row.
+template <typename P>
+__device__ __forceinline__ void pf_produce(const P& p, uint8_t* slots, uint64_t* full, uint64_t* empty, int warp, int n_prod, uint64_t n_local) {
+    const uint64_t policy = p.l2_keep ? qb_policy_evict_last() : qb_policy_evict_first();
+    // slot / phase / first row advance incrementally: 64-bit divisions in this loop cost more than the copy they issue
+    uint32_t s = (uint32_t)warp, ph = 0;                 // n_slots is a multiple of 8, n_prod of 1 / 2 / 4: s wraps exactly
+    uint64_t r0 = ((uint64_t)blockIdx.x + (uint64_t)warp * gridDim.x) * p.rows_per_slot;
+    const uint64_t r_step = (uint64_t)n_prod * gridDim.x * p.rows_per_slot;
+    for (uint64_t i = warp; i < n_local; i += n_prod, r0 += r_step) {
+        qb_mbar_wait(&empty[s], ph ^ 1u);
+        const uint64_t left = p.n_rows - r0;
+        const uint32_t nr = (uint32_t)(left < p.rows_per_slot ? left : p.rows_per_slot);
+        const uint32_t bytes = (nr * p.stride + 15u) & ~15u;
+        qb_mbar_arrive_expect_tx(&full[s], bytes);
+        qb_bulk_g2s(slots + (size_t)s * p.slot_bytes, p.rows + r0 * p.stride, bytes, &full[s], policy);
+        s += (uint32_t)n_prod;
+        if (s >= p.n_slots) { s -= p.n_slots; ph ^= 1u; }
+    }
 }
 
 // NCH = 16-byte chunks of a row per lane (row_h <= NCH * 256)
@@ -75,23 +97,7 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_bf16_filter_kernel(const 
     __syncthreads();
     const int n_prod = (int)(blockDim.x >> 5) - PF_CONSUMER_WARPS;
     if (warp < n_prod) {
-        if (lane == 0) {
-            const uint64_t policy = p.l2_keep ? qb_policy_evict_last() : qb_policy_evict_first();
-            // slot / phase / first row advance incrementally: 64-bit divisions in this loop cost more than the copy they issue
-            uint32_t s = (uint32_t)warp, ph = 0;                 // n_slots is a multiple of 8, n_prod of 1 / 2 / 4: s wraps exactly
-            uint64_t r0 = ((uint64_t)blockIdx.x + (uint64_t)warp * gridDim.x) * p.rows_per_slot;
-            const uint64_t r_step = (uint64_t)n_prod * gridDim.x * p.rows_per_slot;
-            for (uint64_t i = warp; i < n_local; i += n_prod, r0 += r_step) {
-                qb_mbar_wait(&empty[s], ph ^ 1u);
-                const uint64_t left = p.n_rows - r0;
-                const uint32_t nr = (uint32_t)(left < p.rows_per_slot ? left : p.rows_per_slot);
-                const uint32_t bytes = nr * p.stride;
-                qb_mbar_arrive_expect_tx(&full[s], bytes);
-                qb_bulk_g2s(slots + (size_t)s * p.slot_bytes, p.rows + r0 * p.stride, bytes, &full[s], policy);
-                s += (uint32_t)n_prod;
-                if (s >= p.n_slots) { s -= p.n_slots; ph ^= 1u; }
-            }
-        }
+        if (lane == 0) pf_produce(p, slots, full, empty, warp, n_prod, n_local);
         return;
     }
     const int cw = warp - n_prod;
@@ -163,7 +169,7 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_bf16_filter_kernel(const 
                 if (p.deleted2) dead = dead || ((p.deleted2[id >> 5] >> (id & 31)) & 1u);
                 if (!dead) {
                     const unsigned int pos = atomicAdd(p.cnt, 1u);
-                    if (pos < PF_CAP) p.cand[pos] = id;
+                    if (pos < p.cap) p.cand[pos] = id;
                 }
             }
         }
@@ -230,7 +236,7 @@ struct Pf8Params {
     uint32_t rows_per_slot, n_slots, slot_bytes;
     const qb_scored_point* samp_out; const uint32_t* samp_cnt; uint32_t top;
     const unsigned int* max_norm_bits;
-    uint32_t* cand; unsigned int* cnt;
+    uint32_t* cand; unsigned int* cnt; uint32_t cap;
     const uint32_t* deleted; const uint32_t* deleted2;
     int l2_keep;
 };
@@ -255,23 +261,7 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q8_filter_kernel(const Pf
     __syncthreads();
     const int n_prod = (int)(blockDim.x >> 5) - PF_CONSUMER_WARPS;
     if (warp < n_prod) {
-        if (lane == 0) {
-            const uint64_t policy = p.l2_keep ? qb_policy_evict_last() : qb_policy_evict_first();
-            // slot / phase / first row advance incrementally: 64-bit divisions in this loop cost more than the copy they issue
-            uint32_t s = (uint32_t)warp, ph = 0;                 // n_slots is a multiple of 8, n_prod of 1 / 2 / 4: s wraps exactly
-            uint64_t r0 = ((uint64_t)blockIdx.x + (uint64_t)warp * gridDim.x) * p.rows_per_slot;
-            const uint64_t r_step = (uint64_t)n_prod * gridDim.x * p.rows_per_slot;
-            for (uint64_t i = warp; i < n_local; i += n_prod, r0 += r_step) {
-                qb_mbar_wait(&empty[s], ph ^ 1u);
-                const uint64_t left = p.n_rows - r0;
-                const uint32_t nr = (uint32_t)(left < p.rows_per_slot ? left : p.rows_per_slot);
-                const uint32_t bytes = nr * p.stride;
-                qb_mbar_arrive_expect_tx(&full[s], bytes);
-                qb_bulk_g2s(slots + (size_t)s * p.slot_bytes, p.rows + r0 * p.stride, bytes, &full[s], policy);
-                s += (uint32_t)n_prod;
-                if (s >= p.n_slots) { s -= p.n_slots; ph ^= 1u; }
-            }
-        }
+        if (lane == 0) pf_produce(p, slots, full, empty, warp, n_prod, n_local);
         return;
     }
     const int cw = warp - n_prod;
@@ -358,7 +348,7 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q8_filter_kernel(const Pf
                     if (p.deleted2) dead = dead || ((p.deleted2[id >> 5] >> (id & 31)) & 1u);
                     if (!dead) {
                         const unsigned int pos = atomicAdd(p.cnt, 1u);
-                        if (pos < PF_CAP) p.cand[pos] = id;
+                        if (pos < p.cap) p.cand[pos] = id;
                     }
                 }
             }
@@ -370,8 +360,232 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q8_filter_kernel(const Pf
     }
 }
 
+// ------------------------------------------------------------------------------------------------ 6-bit shadow plane (0.19 of the f32 bytes)
+// x_i = s_r c_i + r_i, c_i = rint(x_i / s_r) in [-31, 31], s_r = max_i |x_i| / 31; stored per row: u_i = c_i + 31 = 4 a_i + b_i as a 4-bit plane of
+// a (d_pad / 2 bytes) and a 2-bit plane of b (d_pad / 4 bytes), d_pad = dim rounded up to 32, then s_r and rho_r >= ||r||_2 (f32, rounded up).
+//   a-plane byte 8v + 4w + j: a of dim 16v + 8w + j (low nibble) and of dim 16v + 8w + 4 + j (high nibble)
+//   b-plane byte 4v + j:      b of dim 16v + 4k + j in bits [2k, 2k + 2)
+// so `word & 0x0F0F0F0F`, `(word >> 4) & 0x0F0F0F0F` and `(word >> 2k) & 0x03030303` are dp4a operands (bytes < 16) against the packed query
+// bytes of four consecutive dimensions.  The query is split into two int8 levels as for the int8 plane, q_i ~ s_q (h_i + l_i / 254), and
+//   H = sum_i h_i c_i = 4 sum h a + sum h b - 31 sum h,  L likewise   (exact: |H|, |L| <= 127 * 31 * dim < 2^24 and the partial sums < 2^24)
+//   exact - s_r s_q (H + L / 254) = sum_i (q_i - q^_i) s_r c_i + sum_i q_i r_i, bounded by the smaller of
+//     t1 = s_r E1,  E1 = (1/2 + 2^-13) ||q||_1 + s_q dim (31/508)(1 + 0.08)     (|r_i| <= s_r (1/2 + 2^-13), |c_i| <= 31, |q_i - q^_i| <= s_q (1/508 + 2.3e-5))
+//     t2 = ||q||_2 rho_r + e2 (max||x|| + rho_r),  e2 = s_q sqrt(dim)(1/508 + 2.3e-5)(1 + 0.01) >= ||q - q^||_2   (Cauchy-Schwarz; s_r ||c||_2 <= ||x|| + rho_r)
+//   + slack_q = 2 (dim 2^-22 + 2^-17) ||q|| max||x||: the exact f32 sum (<= dim 2^-24 ||q|| ||x||) and the kernel's f32 evaluation of
+//     s_r s_q (H + L / 254) (<= 2^-22 ||q|| (||x|| + rho_r), rho_r <= max(||x||, sqrt(dim) / 62 ||x||) <= max||x|| for dim <= 1024)
+// A row passes iff  s_r s_q (H + L / 254) + min(t1, t2) >= thr_q - slack_q, every bound term rounded towards "pass".
+// Zero and denormal-only rows (max < 1e-30) keep all-zero codes, s_r = 2 max and rho_r = ||x||: their bound is their norm.
+__global__ void __launch_bounds__(256) f32_to_q6_rows_kernel(const float* __restrict__ rows, uint64_t stride_f, uint32_t dim, uint32_t d_pad, uint64_t n,
+                                                              uint8_t* __restrict__ out, uint32_t out_stride_b, unsigned int* __restrict__ max_norm_bits,
+                                                              unsigned int* __restrict__ nonfinite) {
+    const int t = threadIdx.x & 7;
+    const uint64_t groups = (uint64_t)gridDim.x * (blockDim.x >> 3), g0 = (uint64_t)blockIdx.x * (blockDim.x >> 3) + (threadIdx.x >> 3);
+    const uint64_t n_iter = (n + groups - 1) / groups;
+    for (uint64_t it = 0; it < n_iter; ++it) {
+        const uint64_t r = g0 + it * groups;
+        const bool valid = r < n;
+        const float* src = rows + (valid ? r : 0) * stride_f;
+        uint8_t* dst = out + (valid ? r : 0) * out_stride_b;
+        double ss = 0.0;
+        float mx = 0.f;
+        bool bad = false;
+        for (uint32_t i = t; i < dim; i += 8) {
+            const float v = src[i];
+            bad |= !(fabsf(v) <= 3.0e38f);
+            ss += (double)v * (double)v;
+            mx = fmaxf(mx, fabsf(v));
+        }
+#pragma unroll
+        for (int o = 1; o < 8; o <<= 1) {
+            ss += __shfl_xor_sync(0xFFFFFFFFu, ss, o); mx = fmaxf(mx, __shfl_xor_sync(0xFFFFFFFFu, mx, o));
+            bad |= __shfl_xor_sync(0xFFFFFFFFu, (int)bad, o) != 0;
+        }
+        const bool tiny = !(mx >= 1.0e-30f);
+        const float sr = tiny ? __fmul_ru(mx, 2.0f) : __fdiv_rn(mx, 31.f);
+        const float inv = tiny ? 0.f : __fdiv_rn(31.f, mx);
+        auto code = [&](uint32_t d) -> int { return (d < dim) ? (int)fminf(fmaxf(rintf(__fmul_rn(src[d], inv)), -31.f), 31.f) : 0; };
+        // r_i = x_i - s_r c_i is exact in f64 up to one rounding of the difference (s_r c_i has <= 29 significant bits)
+        double rr = 0.0;
+        for (uint32_t i = t; i < dim; i += 8) {
+            const double e = (double)src[i] - (double)sr * (double)code(i);
+            rr += e * e;
+        }
+#pragma unroll
+        for (int o = 1; o < 8; o <<= 1) rr += __shfl_xor_sync(0xFFFFFFFFu, rr, o);
+        for (uint32_t ab = t; ab < d_pad / 2; ab += 8) {
+            const uint32_t d = (ab >> 3) * 16 + ((ab >> 2) & 1) * 8 + (ab & 3);
+            if (valid) dst[ab] = (uint8_t)(((code(d) + 31) >> 2) | (((code(d + 4) + 31) >> 2) << 4));
+        }
+        for (uint32_t bb = t; bb < d_pad / 4; bb += 8) {
+            const uint32_t d = (bb >> 2) * 16 + (bb & 3);
+            uint32_t v = 0;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) v |= (uint32_t)((code(d + 4 * k) + 31) & 3) << (2 * k);
+            if (valid) dst[d_pad / 2 + bb] = (uint8_t)v;
+        }
+        if (valid && t == 0) {
+            // f64 sums of <= 1024 squares and a square root: relative error < 2^-42, covered by the factor 1 + 2^-40 (then rounded up to f32)
+            const float rho = __double2float_ru(__dmul_ru(sqrt(rr), 1.0 + 0x1p-40));
+            *reinterpret_cast<float2*>(dst + out_stride_b - 8) = make_float2(sr, rho);
+            if (bad || !(ss <= 3.0e38)) atomicOr(nonfinite, 1u);
+            else atomicMax(max_norm_bits, __float_as_uint(__double2float_ru(__dmul_ru(sqrt(ss), 1.0 + 0x1p-40))));
+        }
+    }
+}
+
+struct Pf6Params {
+    const uint8_t* rows;        // 6-bit plane: per row d_pad / 2 bytes of a, d_pad / 4 bytes of b, then the row's f32 scale and residual bound
+    uint32_t stride;            // bytes per row = 3 d_pad / 4 + 8 (a multiple of 8; two rows are a multiple of 16)
+    uint32_t d_pad;             // dim rounded up to 32
+    uint32_t dim;
+    uint64_t n_rows;
+    const float* q;
+    uint32_t rows_per_slot, n_slots, slot_bytes;
+    const qb_scored_point* samp_out; const uint32_t* samp_cnt; uint32_t top;
+    const unsigned int* max_norm_bits;
+    uint32_t* cand; unsigned int* cnt; uint32_t cap;
+    const uint32_t* deleted; const uint32_t* deleted2;
+    int l2_keep;
+};
+
+// Half a warp per row, two rows per step.  NCH = 16-dimension chunks of a row per lane (d_pad <= NCH * 256)
 template <int NCH>
-qb_status launch_filter_q8(Pf8Params& p, int sm_count, cudaStream_t stream) {
+__global__ void __launch_bounds__(PF_THREADS, 1) dense_q6_filter_kernel(const Pf6Params p) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    uint8_t* slots = smem;                                       // [n_slots][slot_bytes]
+    uint64_t* full = reinterpret_cast<uint64_t*>(slots + (size_t)p.n_slots * p.slot_bytes);
+    uint64_t* empty = full + p.n_slots;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint64_t n_tiles = (p.n_rows + p.rows_per_slot - 1) / p.rows_per_slot;
+    const uint64_t n_local = (blockIdx.x < n_tiles) ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+    if (threadIdx.x == 0) {
+        for (uint32_t s = 0; s < p.n_slots; ++s) { qb_mbar_init(&full[s], 1); qb_mbar_init(&empty[s], 1); }
+        qb_fence_barrier_init();
+    }
+    __syncthreads();
+    const int n_prod = (int)(blockDim.x >> 5) - PF_CONSUMER_WARPS;
+    if (warp < n_prod) {
+        if (lane == 0) pf_produce(p, slots, full, empty, warp, n_prod, n_local);
+        return;
+    }
+    const int cw = warp - n_prod;
+    const int half = lane >> 4, hl = lane & 15;
+    const uint32_t n16 = p.d_pad / 16;
+    // query statistics over the whole vector (each half-warp holds all of it), then this lane's chunks quantised to two int8 levels
+    float qmax = 0.f, q1 = 0.f, q2 = 0.f;
+    bool qbad = false;
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+        const uint32_t v = (uint32_t)(c * 16 + hl);
+#pragma unroll
+        for (int k = 0; k < 16; ++k) {
+            const float x = (v < n16 && v * 16 + k < p.dim) ? p.q[v * 16 + k] : 0.f;
+            qbad |= !(fabsf(x) <= 3.0e38f);
+            qmax = fmaxf(qmax, fabsf(x)); q1 = __fadd_ru(q1, fabsf(x)); q2 = __fmaf_rn(x, x, q2);
+        }
+    }
+#pragma unroll
+    for (int o = 8; o; o >>= 1) {
+        qmax = fmaxf(qmax, __shfl_xor_sync(0xFFFFFFFFu, qmax, o)); q1 = __fadd_ru(q1, __shfl_xor_sync(0xFFFFFFFFu, q1, o)); q2 += __shfl_xor_sync(0xFFFFFFFFu, q2, o);
+        qbad |= __shfl_xor_sync(0xFFFFFFFFu, (int)qbad, o) != 0;
+    }
+    qbad |= (qmax > 0.f && qmax < 1.0e-30f);                     // 127 / qmax would overflow: leave such a query to the exact scan
+    const float sq = (qmax > 0.f) ? __fdiv_rn(qmax, 127.f) : 0.f;
+    const float inv_sq = (qmax > 0.f && !qbad) ? __fdiv_rn(127.f, qmax) : 0.f;
+    uint32_t hq[NCH][4], lq[NCH][4], aoff[NCH], boff[NCH];
+    int sum_h = 0, sum_l = 0;
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+        const uint32_t v = (uint32_t)(c * 16 + hl);
+        aoff[c] = (v < n16) ? v * 8 : 0;                          // past the row: any valid address, the query chunk is zero
+        boff[c] = p.d_pad / 2 + ((v < n16) ? v * 4 : 0);
+#pragma unroll
+        for (int m = 0; m < 4; ++m) {
+            int h[4], l[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const uint32_t d = v * 16 + 4 * m + j;
+                const float y = __fmul_rn((v < n16 && d < p.dim) ? p.q[d] : 0.f, inv_sq);
+                const float hf = fminf(fmaxf(rintf(y), -127.f), 127.f);
+                h[j] = (int)hf;
+                l[j] = (int)fminf(fmaxf(rintf(__fmul_rn(__fsub_rn(y, hf), 254.f)), -127.f), 127.f);
+                sum_h += h[j]; sum_l += l[j];
+            }
+            hq[c][m] = pack_s8x4(h[0], h[1], h[2], h[3]);
+            lq[c][m] = pack_s8x4(l[0], l[1], l[2], l[3]);
+        }
+    }
+#pragma unroll
+    for (int o = 8; o; o >>= 1) { sum_h += __shfl_xor_sync(0xFFFFFFFFu, sum_h, o); sum_l += __shfl_xor_sync(0xFFFFFFFFu, sum_l, o); }
+    // per-query constants of the bound, rounded towards "pass"; a non-finite query makes every row pass (-> fallback to the exact scan)
+    const float qn = __fmul_ru(__fsqrt_ru(q2), 1.0001f);
+    const float mxn = __uint_as_float(*p.max_norm_bits);
+    const float e1 = __fadd_ru(__fmul_ru(q1, 0x1.001p-1f), __fmul_ru(__fmul_ru(sq, (float)p.dim), 0.066f));
+    const float e2 = __fmul_ru(__fmul_ru(sq, __fsqrt_ru((float)p.dim)), 0.00202f);
+    const float t2a = __fadd_ru(qn, e2), t2b = __fmul_ru(e2, mxn);
+    const float slack = __fadd_ru(__fmul_ru(__fmul_ru(__fadd_ru(__fmul_ru((float)p.dim, 0x1p-21f), 0x1p-16f), qn), mxn), 1.0e-37f);
+    const float thr = (*p.samp_cnt >= p.top) ? p.samp_out[p.top - 1].score : __int_as_float(0xff800000);
+    const float thr_adj = qbad ? __int_as_float(0x7fc00000) : __fsub_rd(thr, slack);
+    const float k254 = 1.0f / 254.0f;
+    const float corr_h = (float)(31 * sum_h), corr_l = (float)(31 * sum_l);
+    uint32_t s = (uint32_t)cw, ph = 0;                            // as in the producers: no 64-bit division per slot
+    uint64_t r0 = ((uint64_t)blockIdx.x + (uint64_t)cw * gridDim.x) * p.rows_per_slot;
+    const uint64_t r_step = (uint64_t)PF_CONSUMER_WARPS * gridDim.x * p.rows_per_slot;
+    for (uint64_t i = cw; i < n_local; i += PF_CONSUMER_WARPS, r0 += r_step) {
+        const uint64_t left = p.n_rows - r0;
+        const uint32_t nr = (uint32_t)(left < p.rows_per_slot ? left : p.rows_per_slot);
+        qb_mbar_wait(&full[s], ph);
+        const uint8_t* slot = slots + (size_t)s * p.slot_bytes;
+        for (uint32_t r = 0; r < nr; r += 2) {
+            const uint32_t rr = r + (uint32_t)half;
+            const bool valid = rr < nr;
+            const uint8_t* row = slot + (size_t)(valid ? rr : r) * p.stride;
+            int ha = 0, hb = 0, la = 0, lb = 0;
+#pragma unroll
+            for (int c = 0; c < NCH; ++c) {
+                const uint2 wa = *reinterpret_cast<const uint2*>(row + aoff[c]);
+                const uint32_t wb = *reinterpret_cast<const uint32_t*>(row + boff[c]);
+                const uint32_t a[4] = {wa.x & 0x0F0F0F0Fu, (wa.x >> 4) & 0x0F0F0F0Fu, wa.y & 0x0F0F0F0Fu, (wa.y >> 4) & 0x0F0F0F0Fu};
+#pragma unroll
+                for (int m = 0; m < 4; ++m) {
+                    const uint32_t b = (wb >> (2 * m)) & 0x03030303u;
+                    ha = __dp4a((int)a[m], (int)hq[c][m], ha); la = __dp4a((int)a[m], (int)lq[c][m], la);
+                    hb = __dp4a((int)b, (int)hq[c][m], hb);    lb = __dp4a((int)b, (int)lq[c][m], lb);
+                }
+            }
+            const int hs = 4 * ha + hb, ls = 4 * la + lb;
+            // both half-warp sums in one butterfly: lanes 0-7 of a half end up with sum h u, lanes 8-15 with sum l u
+            int v = ((hl & 8) ? ls : hs) + __shfl_xor_sync(0xFFFFFFFFu, (hl & 8) ? hs : ls, 8);
+#pragma unroll
+            for (int o = 4; o; o >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);
+            const int lsum = __shfl_xor_sync(0xFFFFFFFFu, v, 8);
+            if (hl == 0 && valid) {
+                const float H = __fsub_rn((float)v, corr_h), L = __fsub_rn((float)lsum, corr_l);   // exact: integers below 2^24
+                const float2 sp = *reinterpret_cast<const float2*>(row + p.stride - 8);
+                const float app = __fmul_rn(sp.x, __fmul_rn(sq, __fmaf_rn(L, k254, H)));
+                const float up = __fadd_ru(app, fminf(__fmul_ru(sp.x, e1), __fmaf_ru(sp.y, t2a, t2b)));   // an upper bound of the exact score (up to slack_q)
+                if (!(up < thr_adj)) {
+                    const uint32_t id = (uint32_t)(r0 + rr);
+                    bool dead = false;
+                    if (p.deleted) dead = (p.deleted[id >> 5] >> (id & 31)) & 1u;
+                    if (p.deleted2) dead = dead || ((p.deleted2[id >> 5] >> (id & 31)) & 1u);
+                    if (!dead) {
+                        const unsigned int pos = atomicAdd(p.cnt, 1u);
+                        if (pos < p.cap) p.cand[pos] = id;
+                    }
+                }
+            }
+        }
+        __syncwarp();
+        if (lane == 0) qb_mbar_arrive(&empty[s]);
+        s += PF_CONSUMER_WARPS;
+        if (s >= p.n_slots) { s -= p.n_slots; ph ^= 1u; }
+    }
+}
+
+// the ring of any filter kernel above: slots of ~PF_SLOT_BYTES (an even number of rows), as many as fit, one CTA per SM
+template <typename P>
+qb_status launch_ring(void (*kernel)(P), P& p, int sm_count, cudaStream_t stream) {
     const uint32_t kMaxSmem = 227 * 1024;
     const uint32_t target = qb_opt().prefilter_slot_bytes ? qb_opt().prefilter_slot_bytes : PF_SLOT_BYTES;
     uint32_t rps = (target / p.stride) & ~1u;
@@ -384,36 +598,64 @@ qb_status launch_filter_q8(Pf8Params& p, int sm_count, cudaStream_t stream) {
     QB_CHECK(n_slots >= (uint32_t)PF_CONSUMER_WARPS, QB_ERR_INVALID, "prefilter: rows too wide for the ring");
     p.n_slots = n_slots;
     const size_t smem = (size_t)n_slots * p.slot_bytes + (size_t)n_slots * 16;
-    QB_CUDA(cudaFuncSetAttribute(dense_q8_filter_kernel<NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem));
+    QB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem));
     const uint64_t n_tiles = ceil_div_u64(p.n_rows, p.rows_per_slot);
     const unsigned grid = (unsigned)std::min<uint64_t>(n_tiles, (uint64_t)sm_count);
-    dense_q8_filter_kernel<NCH><<<grid, 32 * (PF_CONSUMER_WARPS + pf_producers()), smem, stream>>>(p);
+    kernel<<<grid, 32 * (PF_CONSUMER_WARPS + pf_producers()), smem, stream>>>(p);
     QB_LAUNCHED();
     QB_CUDA(cudaGetLastError());
     return QB_OK;
 }
 
-// exact scores of the candidates in score_avx_group8's order (all CTAs, one 8-lane group per candidate), then the LAST CTA to finish picks
-// the top-k by (score desc, id asc) — or raises the fallback flag when the list overflowed / the sample gave no threshold
-constexpr int PF_FINISH_CTAS = 32;
-__global__ void __launch_bounds__(256) f32_prefilter_finish_kernel(const uint8_t* __restrict__ rows, uint32_t stride, uint32_t dim, const float* __restrict__ q,
-                                                                   const uint32_t* __restrict__ cand, unsigned int* __restrict__ cnt, uint32_t top, uint32_t id_base,
+// the largest key below `prev` among k[0, n) (keys are unique: the id is part of the key), block-wide; 0 when there is none
+template <bool GLOBAL>
+__device__ unsigned long long block_next_key(const unsigned long long* k, uint32_t n, unsigned long long prev, unsigned long long* s_best) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    unsigned long long best = 0ull;
+    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+        const unsigned long long x = GLOBAL ? __ldcg(k + i) : k[i];
+        if (x < prev && x > best) best = x;
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) { const unsigned long long w = __shfl_xor_sync(0xFFFFFFFFu, best, o); best = w > best ? w : best; }
+    if (lane == 0) s_best[warp] = best;
+    __syncthreads();
+    best = s_best[0];
+    for (int w = 1; w < (int)(blockDim.x >> 5); ++w) best = s_best[w] > best ? s_best[w] : best;
+    __syncthreads();
+    return best;
+}
+
+// exact scores of the candidates in score_avx_group8's order, one contiguous share of the list per CTA (one 8-lane group per candidate); each
+// CTA writes its own top-k keys to keys[blockIdx.x * top, + top), and the LAST CTA to finish picks the top-k of those by (score desc, id asc)
+// — or raises the fallback flag when the list overflowed / the sample gave no threshold
+constexpr int PF_FINISH_THREADS = 256;
+__global__ void __launch_bounds__(PF_FINISH_THREADS) f32_prefilter_finish_kernel(const uint8_t* __restrict__ rows, uint32_t stride, uint32_t dim, const float* __restrict__ q,
+                                                                   const uint32_t* __restrict__ cand, unsigned int* __restrict__ cnt, uint32_t cap, uint32_t top, uint32_t id_base,
                                                                    unsigned long long* __restrict__ keys, unsigned int* __restrict__ ticket, qb_scored_point* __restrict__ out,
                                                                    uint32_t* __restrict__ out_cnt, unsigned int* __restrict__ fallback, unsigned int* __restrict__ n_fallbacks) {
-    __shared__ unsigned long long s_best[8];
+    extern __shared__ unsigned long long s_keys[];                // ceil(cap / gridDim.x)
+    __shared__ unsigned long long s_best[PF_FINISH_THREADS / 32];
     __shared__ unsigned int s_ticket;
     const unsigned int c = *cnt;                                  // nobody resets it before every CTA has drawn its ticket
-    const bool bad = c > PF_CAP || c < top;                       // overflow, or a sample that could not give a threshold
-    const int t = threadIdx.x & 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const bool bad = c > cap || c < top;                          // overflow, or a sample that could not give a threshold
+    const int t = threadIdx.x & 7;
     if (!bad) {
-        const uint32_t groups = gridDim.x * (blockDim.x >> 3), g = blockIdx.x * (blockDim.x >> 3) + (threadIdx.x >> 3);
-        const uint32_t n_iter = (c + groups - 1) / groups;        // uniform: the 8-lane scorer shuffles with the full warp mask
+        const uint32_t per = (c + gridDim.x - 1) / gridDim.x, begin = min(c, blockIdx.x * per), m = min(c, begin + per) - begin;
+        const uint32_t groups = blockDim.x >> 3, g = threadIdx.x >> 3;
+        const uint32_t n_iter = (m + groups - 1) / groups;        // uniform: the 8-lane scorer shuffles with the full warp mask
         for (uint32_t it = 0; it < n_iter; ++it) {
             const uint32_t i = g + it * groups;
-            const bool valid = i < c;
-            const uint32_t row = valid ? cand[i] : 0u;
+            const bool valid = i < m;
+            const uint32_t row = valid ? cand[begin + i] : 0u;
             const float sc = qbs::score_avx_group8<qbs::M_DOT>(reinterpret_cast<const float*>(rows + (size_t)row * stride), q, dim, t);
-            if (valid && t == 0) keys[i] = qb_pack_key(sc, row + id_base);
+            if (valid && t == 0) s_keys[i] = qb_pack_key(sc, row + id_base);
+        }
+        __syncthreads();
+        unsigned long long prev = ~0ull;
+        for (uint32_t r = 0; r < top; ++r) {
+            prev = block_next_key<false>(s_keys, m, prev, s_best);
+            if (threadIdx.x == 0) keys[(size_t)blockIdx.x * top + r] = prev;
         }
     }
     __threadfence();
@@ -424,46 +666,12 @@ __global__ void __launch_bounds__(256) f32_prefilter_finish_kernel(const uint8_t
     __threadfence();
     if (threadIdx.x == 0) { *cnt = 0u; *ticket = 0u; *fallback = bad ? 1u : 0u; if (bad) atomicAdd(n_fallbacks, 1u); }   // ready for the next query on this context
     if (bad) return;
-    // keys are unique (the id is part of the key): round r takes the largest key below round r-1's winner
     unsigned long long prev = ~0ull;
     for (uint32_t r = 0; r < top; ++r) {
-        unsigned long long best = 0ull;
-        for (uint32_t i = threadIdx.x; i < c; i += blockDim.x) { const unsigned long long k = __ldcg(keys + i); if (k < prev && k > best) best = k; }
-#pragma unroll
-        for (int o = 16; o; o >>= 1) { const unsigned long long w = __shfl_xor_sync(0xFFFFFFFFu, best, o); best = w > best ? w : best; }
-        if (lane == 0) s_best[warp] = best;
-        __syncthreads();
-        best = s_best[0];
-#pragma unroll
-        for (int w = 1; w < 8; ++w) best = s_best[w] > best ? s_best[w] : best;
-        __syncthreads();
-        if (threadIdx.x == 0) { qb_scored_point sp; sp.idx = qb_key_id(best); sp.score = qb_key_score(best); out[r] = sp; }
-        prev = best;
+        prev = block_next_key<true>(keys, gridDim.x * top, prev, s_best);
+        if (threadIdx.x == 0) { qb_scored_point sp; sp.idx = qb_key_id(prev); sp.score = qb_key_score(prev); out[r] = sp; }
     }
     if (threadIdx.x == 0) *out_cnt = top;
-}
-
-template <int NCH>
-qb_status launch_filter(PfParams& p, int sm_count, cudaStream_t stream) {
-    const uint32_t kMaxSmem = 227 * 1024;
-    const uint32_t target = qb_opt().prefilter_slot_bytes ? qb_opt().prefilter_slot_bytes : PF_SLOT_BYTES;
-    uint32_t rps = (target / p.stride) & ~1u;
-    if (rps < 2) rps = 2;
-    p.rows_per_slot = rps;
-    p.slot_bytes = rps * p.stride;
-    uint32_t n_slots = (kMaxSmem - 2048) / p.slot_bytes;
-    if (n_slots > 64) n_slots = 64;
-    n_slots = (n_slots / PF_CONSUMER_WARPS) * PF_CONSUMER_WARPS;
-    QB_CHECK(n_slots >= (uint32_t)PF_CONSUMER_WARPS, QB_ERR_INVALID, "prefilter: rows too wide for the ring");
-    p.n_slots = n_slots;
-    const size_t smem = (size_t)n_slots * p.slot_bytes + (size_t)n_slots * 16;
-    QB_CUDA(cudaFuncSetAttribute(dense_bf16_filter_kernel<NCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem));
-    const uint64_t n_tiles = ceil_div_u64(p.n_rows, p.rows_per_slot);
-    const unsigned grid = (unsigned)std::min<uint64_t>(n_tiles, (uint64_t)sm_count);
-    dense_bf16_filter_kernel<NCH><<<grid, 32 * (PF_CONSUMER_WARPS + pf_producers()), smem, stream>>>(p);
-    QB_LAUNCHED();
-    QB_CUDA(cudaGetLastError());
-    return QB_OK;
 }
 
 }  // namespace
@@ -492,16 +700,49 @@ static qb_status q8_shadow_ensure(qb_storage* s, cudaStream_t stream) {
     s->q8_usable = meta[1] == 0;
     return QB_OK;
 }
-static bool use_q8_plane(const qb_storage* s) { return qb_opt().prefilter_plane != 1 && s->dim <= 1024; }   // dim * 127^2 < 2^24 and <= 4 chunks per lane
+
+// 6-bit shadow plane (codes + the row's scale and residual bound), built like the int8 plane: +19 % HBM
+static qb_status q6_shadow_ensure(qb_storage* s, cudaStream_t stream) {
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (s->q6_ready) return QB_OK;
+    const uint32_t d_pad = (uint32_t)round_up_u64(s->dim, 32);
+    const uint32_t row_b = d_pad / 4 * 3 + 8;
+    const size_t bytes = (size_t)s->count * row_b + 16;                  // + 16: a tile's bulk copy is rounded up to 16 bytes (pf_produce)
+    if (!s->d_q6) {
+        QB_CUDA(cudaMalloc(&s->d_q6, std::max<size_t>(bytes, 256)));
+        QB_CUDA(cudaMalloc(&s->d_q6_meta, 256));
+        s->hbm_bytes += bytes;
+    }
+    s->q6_row_b = row_b;
+    QB_CUDA(cudaMemsetAsync(s->d_q6_meta, 0, 256, stream));
+    const uint64_t blocks = std::min<uint64_t>(ceil_div_u64(std::max<uint64_t>(s->count, 1), 32), (uint64_t)s->sm_count * 16);
+    f32_to_q6_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(reinterpret_cast<const float*>(s->d_rows), s->row_stride / 4, s->dim, d_pad, s->count, s->d_q6, row_b,
+                                                                s->d_q6_meta, s->d_q6_meta + 1);
+    QB_LAUNCHED();
+    QB_CUDA(cudaGetLastError());
+    unsigned int meta[2] = {0, 0};
+    QB_CUDA(cudaMemcpyAsync(meta, s->d_q6_meta, 8, cudaMemcpyDeviceToHost, stream));
+    QB_CUDA(cudaStreamSynchronize(stream));
+    s->q6_ready = true;
+    s->q6_usable = meta[1] == 0;
+    return QB_OK;
+}
+
+// option prefilter_plane: 0 = the 6-bit plane, 1 = bf16, 2 = int8 (the integer planes need dim * 127 * 62 < 2^24 and <= 4 chunks per lane: dim <= 1024,
+// which every prefiltered storage meets).  Only the selected plane is built; when it cannot be allocated, the bf16 plane is tried.
+static int pf_plane() { const int o = qb_opt().prefilter_plane; return (o == 1 || o == 2) ? o : 0; }
 
 // Can this storage answer single-query top-k searches through a shadow-plane prefilter?  Builds the plane on first use.
 bool qb_f32_prefilter_usable(qb_storage* s, uint64_t n_rows, uint32_t top, cudaStream_t stream) {
     if (s->kind != QB_KIND_DENSE || s->dtype != QB_DT_F32) return false;
     if (s->distance != QB_DIST_DOT && s->distance != QB_DIST_COSINE) return false;       // the bound is on a dot product
     if (qb_opt().disable_prefilter || n_rows != s->count || n_rows < (1ull << 19) || top > 16 || s->dim < 32 || round_up_u64(s->dim, 8) > 1024) return false;
-    if (use_q8_plane(s)) {
+    if (pf_plane() == 0) {
+        if (q6_shadow_ensure(s, stream) == QB_OK) return s->q6_usable;
+        cudaGetLastError();                                                               // e.g. no room for the plane: try the bf16 one / stay exact
+    } else if (pf_plane() == 2) {
         if (q8_shadow_ensure(s, stream) == QB_OK) return s->q8_usable;
-        cudaGetLastError();                                                               // e.g. no room for the plane: try the other one / stay exact
+        cudaGetLastError();
     }
     if (qb_f32_shadow_ensure(s, stream) != QB_OK) { cudaGetLastError(); return false; }
     return s->bf16_usable;
@@ -514,7 +755,7 @@ size_t qb_f32_prefilter_scratch_bytes() { return (size_t)PF_CAP * 12 + 16 * size
 qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t top, void* d_scratch, unsigned int* d_n_fallbacks, qb_scored_point* d_out, uint32_t* d_out_cnt,
                                   cudaEvent_t prof0, cudaEvent_t prof1, cudaStream_t stream) {
     uint8_t* sc = reinterpret_cast<uint8_t*>(d_scratch);
-    // scratch: [0,16) cnt | [16,32) fallback flag | [32,48) finish ticket | [48,64) sample count | [64, 64+16*8) sample top-k | candidate keys | candidate rows
+    // scratch: [0,16) cnt | [16,32) fallback flag | [32,48) finish ticket | [48,64) sample count | [64, 64+16*8) sample top-k | per-CTA top-k keys | candidate rows
     unsigned int* d_cnt = reinterpret_cast<unsigned int*>(sc);
     unsigned int* d_fallback = reinterpret_cast<unsigned int*>(sc + 16);
     uint32_t* d_samp_cnt = reinterpret_cast<uint32_t*>(sc + 48);
@@ -523,6 +764,9 @@ qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t t
     unsigned long long* d_keys = reinterpret_cast<unsigned long long*>(sc + 64 + 16 * sizeof(qb_scored_point));
     uint32_t* d_cand = reinterpret_cast<uint32_t*>(d_keys + PF_CAP);
     const uint64_t n = s->count;
+    // the candidate list holds n / 32 rows (at most PF_CAP): re-scoring reads a whole f32 row per candidate, and past 1/32 of the rows the
+    // exact scan that a longer list would save is no longer far off
+    const uint32_t cap = (uint32_t)std::min<uint64_t>(PF_CAP, n / 32);
     // 1. exact top-k of a prefix
     // 1/64 of the rows, 2^14..2^17: a shard of a sharded search (1.25M rows at N = 8) should not spend a fifth of its step on the sample
     uint64_t sample = std::min<uint64_t>(131072, std::max<uint64_t>(16384, (n / 64) & ~(uint64_t)3));
@@ -535,18 +779,33 @@ qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t t
     QB_CHECK(n_slots != 0 && n_slots <= 4096, QB_ERR_CUDA, "prefilter: the sample scan did not launch (%llu slots)", (unsigned long long)n_slots);
     // 2. filter pass over the whole shadow plane
     const float* d_q = reinterpret_cast<const float*>(a.d_q_enc);
-    if (use_q8_plane(s) && s->q8_ready && s->q8_usable) {
+    const int plane = pf_plane();
+    if (plane == 0 && s->q6_ready && s->q6_usable) {
+        Pf6Params p6{};
+        p6.rows = s->d_q6; p6.stride = s->q6_row_b; p6.d_pad = (uint32_t)round_up_u64(s->dim, 32); p6.dim = s->dim; p6.n_rows = n;
+        p6.q = d_q; p6.samp_out = d_samp; p6.samp_cnt = d_samp_cnt; p6.top = top; p6.max_norm_bits = s->d_q6_meta;
+        p6.cand = d_cand; p6.cnt = d_cnt; p6.cap = cap; p6.deleted = a.emit.deleted; p6.deleted2 = a.emit.deleted2;
+        p6.l2_keep = ((uint64_t)n * p6.stride <= (64ull << 20)) ? 1 : 0;
+        if (prof0) cudaEventRecord(prof0, stream);
+        switch ((p6.d_pad + 255) / 256) {
+            case 1: QB_TRY(launch_ring(dense_q6_filter_kernel<1>, p6, s->sm_count, stream)); break;
+            case 2: QB_TRY(launch_ring(dense_q6_filter_kernel<2>, p6, s->sm_count, stream)); break;
+            case 3: QB_TRY(launch_ring(dense_q6_filter_kernel<3>, p6, s->sm_count, stream)); break;
+            default: QB_TRY(launch_ring(dense_q6_filter_kernel<4>, p6, s->sm_count, stream)); break;
+        }
+        if (prof1) cudaEventRecord(prof1, stream);
+    } else if (plane == 2 && s->q8_ready && s->q8_usable) {
         Pf8Params p8{};
         p8.rows = reinterpret_cast<const uint8_t*>(s->d_q8); p8.stride = s->q8_row_b; p8.dim = s->dim; p8.n_rows = n;
         p8.q = d_q; p8.samp_out = d_samp; p8.samp_cnt = d_samp_cnt; p8.top = top; p8.max_norm_bits = s->d_q8_meta;
-        p8.cand = d_cand; p8.cnt = d_cnt; p8.deleted = a.emit.deleted; p8.deleted2 = a.emit.deleted2;
+        p8.cand = d_cand; p8.cnt = d_cnt; p8.cap = cap; p8.deleted = a.emit.deleted; p8.deleted2 = a.emit.deleted2;
         p8.l2_keep = ((uint64_t)n * p8.stride <= (64ull << 20)) ? 1 : 0;
         if (prof0) cudaEventRecord(prof0, stream);
         switch ((p8.stride - 16 + 255) / 256) {
-            case 1: QB_TRY(launch_filter_q8<1>(p8, s->sm_count, stream)); break;
-            case 2: QB_TRY(launch_filter_q8<2>(p8, s->sm_count, stream)); break;
-            case 3: QB_TRY(launch_filter_q8<3>(p8, s->sm_count, stream)); break;
-            default: QB_TRY(launch_filter_q8<4>(p8, s->sm_count, stream)); break;
+            case 1: QB_TRY(launch_ring(dense_q8_filter_kernel<1>, p8, s->sm_count, stream)); break;
+            case 2: QB_TRY(launch_ring(dense_q8_filter_kernel<2>, p8, s->sm_count, stream)); break;
+            case 3: QB_TRY(launch_ring(dense_q8_filter_kernel<3>, p8, s->sm_count, stream)); break;
+            default: QB_TRY(launch_ring(dense_q8_filter_kernel<4>, p8, s->sm_count, stream)); break;
         }
         if (prof1) cudaEventRecord(prof1, stream);
     } else {
@@ -554,21 +813,24 @@ qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t t
     p.rows = reinterpret_cast<const uint8_t*>(s->d_bf16); p.row_h = s->bf16_row_h; p.stride = s->bf16_row_h * 2; p.dim = s->dim; p.n_rows = n;
     p.q = reinterpret_cast<const float*>(a.d_q_enc);
     p.samp_out = d_samp; p.samp_cnt = d_samp_cnt; p.top = top; p.max_norm_bits = s->d_bf16_meta;
-    p.cand = d_cand; p.cnt = d_cnt; p.deleted = a.emit.deleted; p.deleted2 = a.emit.deleted2;
+    p.cand = d_cand; p.cnt = d_cnt; p.cap = cap; p.deleted = a.emit.deleted; p.deleted2 = a.emit.deleted2;
     p.l2_keep = ((uint64_t)n * p.stride <= (64ull << 20)) ? 1 : 0;
     if (prof0) cudaEventRecord(prof0, stream);
     const uint32_t nch = (p.row_h + 255) / 256;
     switch (nch) {
-        case 1: QB_TRY(launch_filter<1>(p, s->sm_count, stream)); break;
-        case 2: QB_TRY(launch_filter<2>(p, s->sm_count, stream)); break;
-        case 3: QB_TRY(launch_filter<3>(p, s->sm_count, stream)); break;
-        default: QB_TRY(launch_filter<4>(p, s->sm_count, stream)); break;
+        case 1: QB_TRY(launch_ring(dense_bf16_filter_kernel<1>, p, s->sm_count, stream)); break;
+        case 2: QB_TRY(launch_ring(dense_bf16_filter_kernel<2>, p, s->sm_count, stream)); break;
+        case 3: QB_TRY(launch_ring(dense_bf16_filter_kernel<3>, p, s->sm_count, stream)); break;
+        default: QB_TRY(launch_ring(dense_bf16_filter_kernel<4>, p, s->sm_count, stream)); break;
     }
     if (prof1) cudaEventRecord(prof1, stream);
     }
-    // 3. exact scores + top-k of the survivors (or the fallback flag)
-    f32_prefilter_finish_kernel<<<PF_FINISH_CTAS, 256, 0, stream>>>(reinterpret_cast<const uint8_t*>(s->d_rows), s->row_stride, s->dim, d_q, d_cand, d_cnt, top, a.emit.id_base,
-                                                                    d_keys, d_ticket, d_out, d_out_cnt, d_fallback, d_n_fallbacks);
+    // 3. exact scores + top-k of the survivors (or the fallback flag): one CTA per SM, enough of them that a CTA's share fits in 32 KB
+    const unsigned fin_grid = (unsigned)std::max<uint32_t>((uint32_t)s->sm_count, ceil_div_u64(PF_CAP, 4096));
+    const size_t fin_smem = (size_t)ceil_div_u64(cap, fin_grid) * sizeof(unsigned long long);
+    QB_CHECK((uint64_t)fin_grid * top <= PF_CAP, QB_ERR_INVALID, "prefilter: %u finish CTAs x top %u exceed the key buffer", fin_grid, top);
+    f32_prefilter_finish_kernel<<<fin_grid, PF_FINISH_THREADS, fin_smem, stream>>>(reinterpret_cast<const uint8_t*>(s->d_rows), s->row_stride, s->dim, d_q, d_cand, d_cnt, cap,
+                                                                                   top, a.emit.id_base, d_keys, d_ticket, d_out, d_out_cnt, d_fallback, d_n_fallbacks);
     QB_LAUNCHED();
     QB_CUDA(cudaGetLastError());
     // 4. the exact scan of everything: its CTAs return at once unless the flag is up
@@ -579,4 +841,3 @@ qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t t
     QB_CHECK(n_slots != 0 && n_slots <= 4096, QB_ERR_CUDA, "prefilter: the fallback scan did not launch (%llu slots)", (unsigned long long)n_slots);
     return QB_OK;
 }
-

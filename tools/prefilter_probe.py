@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """prefilter_probe.py [rows] [dim] — single-query searches over one synthetic cosine storage (generated on the device), device-timed, for several
-ring-slot sizes / producer-warp counts of the shadow-plane filter kernels and both planes; prints one JSON line.  Results of every variant are compared with the exact scan."""
+ring-slot sizes / producer-warp counts of the shadow-plane filter kernels and the three planes; prints one JSON line.  Results of every variant are compared with the exact scan.
+"candidates" counts, per query, the rows each integer plane's bound lets through (the kernels' bounds restated in torch on the same rows, f64 where they round up)."""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -48,7 +49,7 @@ qb.set_option("disable_prefilter", 1)
 exact = [st.search_batch(queries[i], 10)[0] for i in range(4)]
 out = {"rows": rows, "dim": dim, "exact_f32_scan": run(10)}
 qb.set_option("disable_prefilter", 0)
-for plane, name in ((0, "int8"), (1, "bf16")):
+for plane, name in ((0, "q6"), (2, "int8"), (1, "bf16")):
     qb.set_option("prefilter_plane", plane)
     for prod in (1, 2, 4):
         qb.set_option("prefilter_producers", prod)
@@ -62,4 +63,54 @@ for plane, name in ((0, "int8"), (1, "bf16")):
 qb.set_option("prefilter_producers", 0)
 qb.set_option("prefilter_slot_bytes", 0); qb.set_option("prefilter_plane", 0)
 out["fallbacks"] = int(st.search_stats()[1])
+
+
+def candidate_counts(nq=16, top=10):
+    """Rows with upper bound >= thr_q - slack_q on the 6-bit and int8 planes, thr_q = the exact top-`top` score of the sample prefix."""
+    qd = torch.from_numpy(queries[:nq]).to(dev).double()
+    qd = (qd / qd.norm(dim=1, keepdim=True)).float().double()          # cosine queries are normalised
+    qmax = qd.abs().amax(1, keepdim=True)
+    sq = (qmax / 127).float().double()
+    y = (qd * (127 / qmax)).float().double()
+    h = y.round().clamp(-127, 127)
+    l = ((y - h) * 254).round().clamp(-127, 127)
+    q1, qn = qd.abs().sum(1), qd.norm(dim=1)
+    sample = min(131072, max(16384, rows // 64))
+    e1 = q1 * (0.5 + 2.0 ** -13) + sq[:, 0] * dim * 0.066
+    e2 = sq[:, 0] * dim ** 0.5 * 0.00202
+    e8 = q1 * (0.5 + 2.0 ** -13) + sq[:, 0] * dim * 0.27
+    g = torch.Generator(device=dev); g.manual_seed(42)
+    chunks, mxn = [], 0.0
+    for r0 in range(0, rows, 500_000):
+        n = min(500_000, rows - r0)
+        x = torch.randn((n, dim), generator=g, device=dev, dtype=torch.float32)
+        check(lib().qb_metric_preprocess_device(0, int(qb.Distance.Cosine), dim, n, vp(x.data_ptr()), dim * 4))
+        mxn = max(mxn, float(x.double().norm(dim=1).max()))
+        chunks.append((r0, n))
+    slack6 = 2 * (dim * 2.0 ** -22 + 2.0 ** -17) * qn * mxn
+    slack8 = (dim * 2.0 ** -22 + 2.0 ** -17) * (1 + dim ** 0.5 / 127) * qn * mxn
+    g.manual_seed(42)
+    thr, c6, c8 = None, torch.zeros(nq, dtype=torch.int64, device=dev), torch.zeros(nq, dtype=torch.int64, device=dev)
+    for r0, n in chunks:
+        x = torch.randn((n, dim), generator=g, device=dev, dtype=torch.float32)
+        check(lib().qb_metric_preprocess_device(0, int(qb.Distance.Cosine), dim, n, vp(x.data_ptr()), dim * 4))
+        if thr is None:
+            thr = (x[:sample].double() @ qd.T).topk(top, dim=0).values[-1]
+        mx = x.abs().amax(1, keepdim=True)
+        sr = (mx / 31).double()
+        c = (x * (31 / mx)).round().clamp(-31, 31).double()
+        rho = (x.double() - sr * c).norm(dim=1, keepdim=True)
+        up6 = sr * sq.T * (c @ h.T + (c @ l.T) / 254) + torch.minimum(sr * e1, rho * (qn + e2) + e2 * mxn)
+        c6 += (up6 >= thr - slack6).sum(0)
+        s8 = (mx / 127).double()
+        c = (x * (127 / mx)).round().clamp(-127, 127).double()
+        up8 = s8 * (sq.T * (c @ h.T + (c @ l.T) / 254) + e8)
+        c8 += (up8 >= thr - slack8).sum(0)
+        del x, c, rho, up6, up8
+    return {"q6": c6.tolist(), "int8": c8.tolist(), "sample_rows": sample}
+
+
+st.close()
+torch.cuda.empty_cache()
+out["candidates"] = candidate_counts()
 print(json.dumps(out))
