@@ -440,7 +440,7 @@ extern "C" void qb_storage_destroy(qb_storage* s) {
     ctx_destroy(s->dev_ctx);
     for (auto& pr : s->prof_pending) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
     for (auto& pr : s->prof_free) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
-    cudaFree(s->d_rows); cudaFree(s->d_bf16); cudaFree(s->d_bf16_meta); cudaFree(s->d_q8); cudaFree(s->d_q8_meta); cudaFree(s->d_q6); cudaFree(s->d_q6_meta); cudaFree(s->d_codes); cudaFree(s->d_voff); cudaFree(s->d_pq_div); cudaFree(s->d_centroids); cudaFree(s->d_pq_codes);
+    cudaFree(s->d_rows); cudaFree(s->d_bf16); cudaFree(s->d_bf16_meta); cudaFree(s->d_q8); cudaFree(s->d_q8_meta); cudaFree(s->d_q6); cudaFree(s->d_q6_lo); cudaFree(s->d_q6_meta); cudaFree(s->d_codes); cudaFree(s->d_voff); cudaFree(s->d_pq_div); cudaFree(s->d_centroids); cudaFree(s->d_pq_codes);
     cudaFree(s->d_bq_rows); cudaFree(s->d_mean_std); cudaFree(s->d_deleted); cudaFree(s->d_pf_fallbacks);
     cudaGetLastError();
     delete s;

@@ -52,8 +52,10 @@ struct qb_storage {
     // int8 shadow (per-row scale) for single-query searches (qb_prefilter.cu): a quarter of the f32 bytes per scan; built on first use
     int8_t* d_q8 = nullptr;  uint32_t q8_row_b = 0;  unsigned int* d_q8_meta = nullptr;   // meta as above
     bool q8_ready = false, q8_usable = false;
-    // 6-bit shadow (per-row scale and residual-norm bound) for single-query searches (qb_prefilter.cu): 0.19 of the f32 bytes per scan
+    // 6-bit shadow for single-query searches (qb_prefilter.cu): main records of 5-bit codes, the row's scale and residual-norm bounds (0.16 of the
+    // f32 bytes, streamed by every scan) and a side plane of the codes' low bits (read for the rows the 5-bit codes let through)
     uint8_t* d_q6 = nullptr;  uint32_t q6_row_b = 0;  unsigned int* d_q6_meta = nullptr;   // meta as above
+    uint8_t* d_q6_lo = nullptr;
     bool q6_ready = false, q6_usable = false;
     uint32_t row_stride = 0;         // bytes
     uint32_t elem_size = 4;

@@ -35,6 +35,7 @@ constexpr int PF_PRODUCERS = 2;             // producer warps (one lane each): a
 constexpr int PF_THREADS = 32 * (PF_CONSUMER_WARPS + PF_MAX_PRODUCERS);     // launch bound; the launch uses 32 * (consumers + producers)
 constexpr uint32_t PF_SLOT_BYTES = 12288;  // target bytes per ring slot (a consumer warp holds one slot while the others are in flight)
 constexpr uint32_t PF_CAP = 131072;        // candidate rows per query at most (a few thousand to a few tens of thousands expected on 10M rows)
+constexpr uint32_t PF_LIST_CAP = 1u << 21; // first-stage rows of the 6-bit plane per query at most (dense_q5_filter_kernel)
 
 static int pf_producers() { const int o = qb_opt().prefilter_producers; return (o >= 1 && o <= PF_MAX_PRODUCERS) ? o : PF_PRODUCERS; }
 
@@ -360,32 +361,50 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q8_filter_kernel(const Pf
     }
 }
 
-// ------------------------------------------------------------------------------------------------ 6-bit shadow plane (0.19 of the f32 bytes)
-// x_i = s_r c_i + r_i, c_i = rint(x_i / s_r) in [-31, 31], s_r = max_i |x_i| / 31; stored per row: u_i = c_i + 31 = 4 a_i + b_i as a 4-bit plane of
-// a (d_pad / 2 bytes) and a 2-bit plane of b (d_pad / 4 bytes), d_pad = dim rounded up to 32, then s_r and rho_r >= ||r||_2 (f32, rounded up).
-//   a-plane byte 8v + 4w + j: a of dim 16v + 8w + j (low nibble) and of dim 16v + 8w + 4 + j (high nibble)
-//   b-plane byte 4v + j:      b of dim 16v + 4k + j in bits [2k, 2k + 2)
-// so `word & 0x0F0F0F0F`, `(word >> 4) & 0x0F0F0F0F` and `(word >> 2k) & 0x03030303` are dp4a operands (bytes < 16) against the packed query
-// bytes of four consecutive dimensions.  The query is split into two int8 levels as for the int8 plane, q_i ~ s_q (h_i + l_i / 254), and
-//   H = sum_i h_i c_i = 4 sum h a + sum h b - 31 sum h,  L likewise   (exact: |H|, |L| <= 127 * 31 * dim < 2^24 and the partial sums < 2^24)
+// ------------------------------------------------------------------------------------------------ 6-bit shadow plane, scanned as a 5-bit cascade
+// x_i = s_r c_i + r_i, c_i = rint(x_i / s_r) in [-31, 31], s_r = max_i |x_i| / 31.  The code u_i = c_i + 31 = 4 a_i + 2 b_i + e_i is split into
+// a 5-bit code w_i = u_i >> 1 = 2 a_i + b_i, streamed for every row, and its low bit e_i, read only for the rows the 5-bit code lets through.
+// Main record per row (stride = 5 d_pad / 8 + 12 rounded up to 8 bytes; two records are a multiple of 16), d_pad = dim rounded up to 32:
+//   a plane (d_pad / 2 bytes)   byte 8v + 4k + j: a of dim 16v + 8k + j (low nibble) and of dim 16v + 8k + 4 + j (high nibble)
+//   b plane (d_pad / 8 bytes)   u16 v: bit 4 P(j) + m = b of dim 16v + 4m + j, P = (0, 2, 1, 3)
+//   s_r, rho5 >= ||x - s_r (2w + 1/2 - 31)||_2, rho6 >= ||r||_2   (f32, the norms computed in f64 and rounded up)
+// Side plane: the low bits e in the b plane's layout, d_pad / 8 bytes per row (rounded up to 16).
+// With t = u16 v, y = (t | t << 12) & 0x0F0F0F0F puts nibble P(j) in byte j, so `(y >> m) & 0x01010101` holds the bits of dims 16v + 4m + j in
+// bytes j: OR-ed into the doubled a nibbles it is the dp4a operand 2a + b = w; alone it is the e operand.  The query is split into two int8
+// levels as for the int8 plane, q_i ~ s_q (h_i + l_i / 254) =: q^_i.
+// Stage 1 (dense_q5_filter_kernel) uses the 5-bit reconstruction x_i ~ s_r c5_i, c5_i = 2 w_i + 1/2 - 31 in [-30.5, 31.5]:
+//   H5 = sum_i h_i 2 c5_i = 4 sum h w - 61 sum h, L5 likewise    (integers, |H5| <= 127 * 63 * dim < 2^24: exact in f32)
+//   exact - s_r s_q (H5 + L5 / 254) / 2 = sum_i (q_i - q^_i) s_r c5_i + sum_i q_i r5_i, r5_i = r_i + s_r (e_i - 1/2), bounded by the smaller of
+//     t1 = s_r E1_5,  E1_5 = (1 + 2^-13) ||q||_1 + 0.066 s_q dim      (|r5_i| <= s_r (1 + 2^-13); |c5_i| <= 31.5, 31.5 (1/508 + 2.3e-5) < 0.066)
+//     t2 = ||q||_2 rho5 + e2 (max||x|| + rho5)                        (Cauchy-Schwarz as below; s_r ||c5||_2 <= ||x|| + rho5)
+// Rows that pass are appended with their partial sums sum h (2w - 31), sum l (2w - 31), s_r and rho6 to a first-stage list.
+// Stage 2 (dense_q6_rescreen_kernel) adds sum h e and sum l e from the side plane: that gives back the 6-bit sums H = sum_i h_i c_i, L likewise,
 //   exact - s_r s_q (H + L / 254) = sum_i (q_i - q^_i) s_r c_i + sum_i q_i r_i, bounded by the smaller of
 //     t1 = s_r E1,  E1 = (1/2 + 2^-13) ||q||_1 + s_q dim (31/508)(1 + 0.08)     (|r_i| <= s_r (1/2 + 2^-13), |c_i| <= 31, |q_i - q^_i| <= s_q (1/508 + 2.3e-5))
-//     t2 = ||q||_2 rho_r + e2 (max||x|| + rho_r),  e2 = s_q sqrt(dim)(1/508 + 2.3e-5)(1 + 0.01) >= ||q - q^||_2   (Cauchy-Schwarz; s_r ||c||_2 <= ||x|| + rho_r)
-//   + slack_q = 2 (dim 2^-22 + 2^-17) ||q|| max||x||: the exact f32 sum (<= dim 2^-24 ||q|| ||x||) and the kernel's f32 evaluation of
-//     s_r s_q (H + L / 254) (<= 2^-22 ||q|| (||x|| + rho_r), rho_r <= max(||x||, sqrt(dim) / 62 ||x||) <= max||x|| for dim <= 1024)
-// A row passes iff  s_r s_q (H + L / 254) + min(t1, t2) >= thr_q - slack_q, every bound term rounded towards "pass".
-// Zero and denormal-only rows (max < 1e-30) keep all-zero codes, s_r = 2 max and rho_r = ||x||: their bound is their norm.
+//     t2 = ||q||_2 rho6 + e2 (max||x|| + rho6),  e2 = s_q sqrt(dim)(1/508 + 2.3e-5)(1 + 0.01) >= ||q - q^||_2   (Cauchy-Schwarz; s_r ||c||_2 <= ||x|| + rho6)
+//   and appends the rows that pass to the candidate list.
+// Both stages: + slack_q = 2 (dim 2^-22 + 2^-17) ||q|| max||x||: the exact f32 sum (<= dim 2^-24 ||q|| ||x||) and the kernel's f32 evaluation of
+//   the approximation (<= 2^-22 ||q|| (||x|| + rho); rho <= sqrt(dim) (1 + 2^-13) / 31 ||x|| <= 1.04 ||x|| for dim <= 1024, and <= 2 sqrt(dim) ||x||
+//   for rows below 1e-30, which the 2^-16 of the slack still covers).
+// A row passes a stage iff  approx + min(t1, t2) >= thr_q - slack_q, every bound term rounded towards "pass".  Both bounds hold, so every row
+// whose exact score reaches thr_q passes both stages: the candidate list is a subset of what the 6-bit test alone would pass, and results are unchanged.
+// Zero and denormal-only rows (max < 1e-30) keep all-zero codes c (u = 31, c5 = -1/2), s_r = 2 max, rho6 = ||x||: their bounds hold.
+// bytes per row of the side plane: d_pad / 8, rounded up to 16 so that stage 2 reads it in 16-byte words
+__host__ __device__ constexpr uint32_t q6_lo_stride(uint32_t d_pad) { return (d_pad / 8 + 15) & ~15u; }
+
 __global__ void __launch_bounds__(256) f32_to_q6_rows_kernel(const float* __restrict__ rows, uint64_t stride_f, uint32_t dim, uint32_t d_pad, uint64_t n,
-                                                              uint8_t* __restrict__ out, uint32_t out_stride_b, unsigned int* __restrict__ max_norm_bits,
-                                                              unsigned int* __restrict__ nonfinite) {
+                                                              uint8_t* __restrict__ out, uint32_t out_stride_b, uint8_t* __restrict__ lo_out,
+                                                              unsigned int* __restrict__ max_norm_bits, unsigned int* __restrict__ nonfinite) {
     const int t = threadIdx.x & 7;
     const uint64_t groups = (uint64_t)gridDim.x * (blockDim.x >> 3), g0 = (uint64_t)blockIdx.x * (blockDim.x >> 3) + (threadIdx.x >> 3);
     const uint64_t n_iter = (n + groups - 1) / groups;
+    const uint32_t lo_b = q6_lo_stride(d_pad);
     for (uint64_t it = 0; it < n_iter; ++it) {
         const uint64_t r = g0 + it * groups;
         const bool valid = r < n;
         const float* src = rows + (valid ? r : 0) * stride_f;
         uint8_t* dst = out + (valid ? r : 0) * out_stride_b;
+        uint8_t* lo = lo_out + (valid ? r : 0) * lo_b;
         double ss = 0.0;
         float mx = 0.f;
         bool bad = false;
@@ -404,29 +423,44 @@ __global__ void __launch_bounds__(256) f32_to_q6_rows_kernel(const float* __rest
         const float sr = tiny ? __fmul_ru(mx, 2.0f) : __fdiv_rn(mx, 31.f);
         const float inv = tiny ? 0.f : __fdiv_rn(31.f, mx);
         auto code = [&](uint32_t d) -> int { return (d < dim) ? (int)fminf(fmaxf(rintf(__fmul_rn(src[d], inv)), -31.f), 31.f) : 0; };
-        // r_i = x_i - s_r c_i is exact in f64 up to one rounding of the difference (s_r c_i has <= 29 significant bits)
-        double rr = 0.0;
+        // r_i = x_i - s_r c_i is exact in f64 up to one rounding of the difference (s_r c_i has <= 30 significant bits); likewise for c5_i
+        double rr6 = 0.0, rr5 = 0.0;
         for (uint32_t i = t; i < dim; i += 8) {
-            const double e = (double)src[i] - (double)sr * (double)code(i);
-            rr += e * e;
+            const int c = code(i);
+            const double e6 = (double)src[i] - (double)sr * (double)c;
+            const double e5 = (double)src[i] - (double)sr * ((double)(((c + 31) >> 1) * 2) + 0.5 - 31.0);
+            rr6 += e6 * e6; rr5 += e5 * e5;
         }
 #pragma unroll
-        for (int o = 1; o < 8; o <<= 1) rr += __shfl_xor_sync(0xFFFFFFFFu, rr, o);
+        for (int o = 1; o < 8; o <<= 1) { rr6 += __shfl_xor_sync(0xFFFFFFFFu, rr6, o); rr5 += __shfl_xor_sync(0xFFFFFFFFu, rr5, o); }
         for (uint32_t ab = t; ab < d_pad / 2; ab += 8) {
             const uint32_t d = (ab >> 3) * 16 + ((ab >> 2) & 1) * 8 + (ab & 3);
             if (valid) dst[ab] = (uint8_t)(((code(d) + 31) >> 2) | (((code(d + 4) + 31) >> 2) << 4));
         }
-        for (uint32_t bb = t; bb < d_pad / 4; bb += 8) {
-            const uint32_t d = (bb >> 2) * 16 + (bb & 3);
-            uint32_t v = 0;
+        for (uint32_t v = t; v < d_pad / 16; v += 8) {
+            uint32_t hi = 0, lw = 0;
 #pragma unroll
-            for (int k = 0; k < 4; ++k) v |= (uint32_t)((code(d + 4 * k) + 31) & 3) << (2 * k);
-            if (valid) dst[d_pad / 2 + bb] = (uint8_t)v;
+            for (int j = 0; j < 4; ++j) {
+#pragma unroll
+                for (int m = 0; m < 4; ++m) {
+                    const uint32_t u = (uint32_t)(code(v * 16 + 4 * m + j) + 31), bit = 4 * (((j & 1) << 1) | (j >> 1)) + m;
+                    hi |= ((u >> 1) & 1u) << bit;
+                    lw |= (u & 1u) << bit;
+                }
+            }
+            if (valid) {
+                *reinterpret_cast<uint16_t*>(dst + d_pad / 2 + 2 * v) = (uint16_t)hi;
+                *reinterpret_cast<uint16_t*>(lo + 2 * v) = (uint16_t)lw;
+            }
         }
         if (valid && t == 0) {
             // f64 sums of <= 1024 squares and a square root: relative error < 2^-42, covered by the factor 1 + 2^-40 (then rounded up to f32)
-            const float rho = __double2float_ru(__dmul_ru(sqrt(rr), 1.0 + 0x1p-40));
-            *reinterpret_cast<float2*>(dst + out_stride_b - 8) = make_float2(sr, rho);
+            float* meta = reinterpret_cast<float*>(dst + d_pad / 2 + d_pad / 8);
+            meta[0] = sr;
+            meta[1] = __double2float_ru(__dmul_ru(sqrt(rr5), 1.0 + 0x1p-40));
+            meta[2] = __double2float_ru(__dmul_ru(sqrt(rr6), 1.0 + 0x1p-40));
+            for (uint32_t b = d_pad / 2 + d_pad / 8 + 12; b < out_stride_b; ++b) dst[b] = 0;
+            for (uint32_t b = d_pad / 8; b < lo_b; ++b) lo[b] = 0;
             if (bad || !(ss <= 3.0e38)) atomicOr(nonfinite, 1u);
             else atomicMax(max_norm_bits, __float_as_uint(__double2float_ru(__dmul_ru(sqrt(ss), 1.0 + 0x1p-40))));
         }
@@ -434,8 +468,9 @@ __global__ void __launch_bounds__(256) f32_to_q6_rows_kernel(const float* __rest
 }
 
 struct Pf6Params {
-    const uint8_t* rows;        // 6-bit plane: per row d_pad / 2 bytes of a, d_pad / 4 bytes of b, then the row's f32 scale and residual bound
-    uint32_t stride;            // bytes per row = 3 d_pad / 4 + 8 (a multiple of 8; two rows are a multiple of 16)
+    const uint8_t* rows;        // main records: a plane, b plane, then the row's s_r, rho5, rho6
+    const uint8_t* lo;          // side plane: low bits, q6_lo_stride(d_pad) bytes per row
+    uint32_t stride;            // bytes per main record (a multiple of 8; two rows are a multiple of 16)
     uint32_t d_pad;             // dim rounded up to 32
     uint32_t dim;
     uint64_t n_rows;
@@ -443,35 +478,24 @@ struct Pf6Params {
     uint32_t rows_per_slot, n_slots, slot_bytes;
     const qb_scored_point* samp_out; const uint32_t* samp_cnt; uint32_t top;
     const unsigned int* max_norm_bits;
+    uint4* list; float* list_rho; unsigned int* list_cnt; unsigned int* list_ticket; uint32_t list_cap;   // first-stage list: (row, sum h (2w - 31), sum l (2w - 31), s_r), rho6
     uint32_t* cand; unsigned int* cnt; uint32_t cap;
     const uint32_t* deleted; const uint32_t* deleted2;
     int l2_keep;
 };
 
-// Half a warp per row, two rows per step.  NCH = 16-dimension chunks of a row per lane (d_pad <= NCH * 256)
+// The query as both stages see it: lane hl of a half-warp holds the 16-dimension chunks v = c * 16 + hl (zero past dim) as two packed int8
+// levels per 4 dimensions; the per-query constants of both bounds, rounded towards "pass".  A non-finite query makes every row pass (-> fallback).
 template <int NCH>
-__global__ void __launch_bounds__(PF_THREADS, 1) dense_q6_filter_kernel(const Pf6Params p) {
-    extern __shared__ __align__(128) uint8_t smem[];
-    uint8_t* slots = smem;                                       // [n_slots][slot_bytes]
-    uint64_t* full = reinterpret_cast<uint64_t*>(slots + (size_t)p.n_slots * p.slot_bytes);
-    uint64_t* empty = full + p.n_slots;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint64_t n_tiles = (p.n_rows + p.rows_per_slot - 1) / p.rows_per_slot;
-    const uint64_t n_local = (blockIdx.x < n_tiles) ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-    if (threadIdx.x == 0) {
-        for (uint32_t s = 0; s < p.n_slots; ++s) { qb_mbar_init(&full[s], 1); qb_mbar_init(&empty[s], 1); }
-        qb_fence_barrier_init();
-    }
-    __syncthreads();
-    const int n_prod = (int)(blockDim.x >> 5) - PF_CONSUMER_WARPS;
-    if (warp < n_prod) {
-        if (lane == 0) pf_produce(p, slots, full, empty, warp, n_prod, n_local);
-        return;
-    }
-    const int cw = warp - n_prod;
-    const int half = lane >> 4, hl = lane & 15;
+struct Q6Query {
+    uint32_t hq[NCH][4], lq[NCH][4];
+    int sum_h, sum_l;                       // over the whole query
+    float sq, e1, e1_5, t2a, t2b, thr_adj;
+};
+
+template <int NCH>
+__device__ __forceinline__ void q6_query(const Pf6Params& p, int hl, Q6Query<NCH>& Q) {
     const uint32_t n16 = p.d_pad / 16;
-    // query statistics over the whole vector (each half-warp holds all of it), then this lane's chunks quantised to two int8 levels
     float qmax = 0.f, q1 = 0.f, q2 = 0.f;
     bool qbad = false;
 #pragma unroll
@@ -492,13 +516,10 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q6_filter_kernel(const Pf
     qbad |= (qmax > 0.f && qmax < 1.0e-30f);                     // 127 / qmax would overflow: leave such a query to the exact scan
     const float sq = (qmax > 0.f) ? __fdiv_rn(qmax, 127.f) : 0.f;
     const float inv_sq = (qmax > 0.f && !qbad) ? __fdiv_rn(127.f, qmax) : 0.f;
-    uint32_t hq[NCH][4], lq[NCH][4], aoff[NCH], boff[NCH];
     int sum_h = 0, sum_l = 0;
 #pragma unroll
     for (int c = 0; c < NCH; ++c) {
         const uint32_t v = (uint32_t)(c * 16 + hl);
-        aoff[c] = (v < n16) ? v * 8 : 0;                          // past the row: any valid address, the query chunk is zero
-        boff[c] = p.d_pad / 2 + ((v < n16) ? v * 4 : 0);
 #pragma unroll
         for (int m = 0; m < 4; ++m) {
             int h[4], l[4];
@@ -511,23 +532,59 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q6_filter_kernel(const Pf
                 l[j] = (int)fminf(fmaxf(rintf(__fmul_rn(__fsub_rn(y, hf), 254.f)), -127.f), 127.f);
                 sum_h += h[j]; sum_l += l[j];
             }
-            hq[c][m] = pack_s8x4(h[0], h[1], h[2], h[3]);
-            lq[c][m] = pack_s8x4(l[0], l[1], l[2], l[3]);
+            Q.hq[c][m] = pack_s8x4(h[0], h[1], h[2], h[3]);
+            Q.lq[c][m] = pack_s8x4(l[0], l[1], l[2], l[3]);
         }
     }
 #pragma unroll
     for (int o = 8; o; o >>= 1) { sum_h += __shfl_xor_sync(0xFFFFFFFFu, sum_h, o); sum_l += __shfl_xor_sync(0xFFFFFFFFu, sum_l, o); }
-    // per-query constants of the bound, rounded towards "pass"; a non-finite query makes every row pass (-> fallback to the exact scan)
+    Q.sum_h = sum_h; Q.sum_l = sum_l; Q.sq = sq;
     const float qn = __fmul_ru(__fsqrt_ru(q2), 1.0001f);
     const float mxn = __uint_as_float(*p.max_norm_bits);
-    const float e1 = __fadd_ru(__fmul_ru(q1, 0x1.001p-1f), __fmul_ru(__fmul_ru(sq, (float)p.dim), 0.066f));
+    const float eq = __fmul_ru(__fmul_ru(sq, (float)p.dim), 0.066f);
+    Q.e1 = __fadd_ru(__fmul_ru(q1, 0x1.001p-1f), eq);
+    Q.e1_5 = __fadd_ru(__fmul_ru(q1, 0x1.0008p+0f), eq);
     const float e2 = __fmul_ru(__fmul_ru(sq, __fsqrt_ru((float)p.dim)), 0.00202f);
-    const float t2a = __fadd_ru(qn, e2), t2b = __fmul_ru(e2, mxn);
+    Q.t2a = __fadd_ru(qn, e2); Q.t2b = __fmul_ru(e2, mxn);
     const float slack = __fadd_ru(__fmul_ru(__fmul_ru(__fadd_ru(__fmul_ru((float)p.dim, 0x1p-21f), 0x1p-16f), qn), mxn), 1.0e-37f);
     const float thr = (*p.samp_cnt >= p.top) ? p.samp_out[p.top - 1].score : __int_as_float(0xff800000);
-    const float thr_adj = qbad ? __int_as_float(0x7fc00000) : __fsub_rd(thr, slack);
+    Q.thr_adj = qbad ? __int_as_float(0x7fc00000) : __fsub_rd(thr, slack);
+}
+
+// nibble P(j) of a u16 of the b plane or the side plane to byte j
+__device__ __forceinline__ uint32_t q6_spread(uint32_t t) { return (t | (t << 12)) & 0x0F0F0F0Fu; }
+
+// Stage 1: the 5-bit code of every row through the TMA ring.  Half a warp per row.  NCH = 16-dimension chunks of a row per lane (d_pad <= NCH * 256)
+template <int NCH>
+__global__ void __launch_bounds__(PF_THREADS, 1) dense_q5_filter_kernel(const Pf6Params p) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    uint8_t* slots = smem;                                       // [n_slots][slot_bytes]
+    uint64_t* full = reinterpret_cast<uint64_t*>(slots + (size_t)p.n_slots * p.slot_bytes);
+    uint64_t* empty = full + p.n_slots;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint64_t n_tiles = (p.n_rows + p.rows_per_slot - 1) / p.rows_per_slot;
+    const uint64_t n_local = (blockIdx.x < n_tiles) ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+    if (threadIdx.x == 0) {
+        for (uint32_t s = 0; s < p.n_slots; ++s) { qb_mbar_init(&full[s], 1); qb_mbar_init(&empty[s], 1); }
+        qb_fence_barrier_init();
+    }
+    __syncthreads();
+    const int n_prod = (int)(blockDim.x >> 5) - PF_CONSUMER_WARPS;
+    if (warp < n_prod) {
+        if (lane == 0) pf_produce(p, slots, full, empty, warp, n_prod, n_local);
+        return;
+    }
+    const int cw = warp - n_prod;
+    const int half = lane >> 4, hl = lane & 15;
+    Q6Query<NCH> Q;
+    q6_query<NCH>(p, hl, Q);
+    // lane hl reads chunk c of a row at a_off + 128 c (a plane) and b_off + 32 c (b plane).  Chunks past d_pad meet a zero query; their reads
+    // stay inside the shared memory of the ring: at most 96 bytes past the end of a row, and the ring's barriers (>= 128 bytes) follow its last slot.
+    const uint32_t a_off = (uint32_t)hl * 8, b_off = p.d_pad / 2 + (uint32_t)hl * 2;
+    const uint32_t meta_off = p.d_pad / 2 + p.d_pad / 8;
+    const float sq_half = 0.5f * Q.sq;                             // exact: s_q is 0 or at least 1e-30 / 127
     const float k254 = 1.0f / 254.0f;
-    const float corr_h = (float)(31 * sum_h), corr_l = (float)(31 * sum_l);
+    const int corr_h5 = 61 * Q.sum_h, corr_l5 = 61 * Q.sum_l, corr_h = 31 * Q.sum_h, corr_l = 31 * Q.sum_l;
     uint32_t s = (uint32_t)cw, ph = 0;                            // as in the producers: no 64-bit division per slot
     uint64_t r0 = ((uint64_t)blockIdx.x + (uint64_t)cw * gridDim.x) * p.rows_per_slot;
     const uint64_t r_step = (uint64_t)PF_CONSUMER_WARPS * gridDim.x * p.rows_per_slot;
@@ -536,43 +593,66 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q6_filter_kernel(const Pf
         const uint32_t nr = (uint32_t)(left < p.rows_per_slot ? left : p.rows_per_slot);
         qb_mbar_wait(&full[s], ph);
         const uint8_t* slot = slots + (size_t)s * p.slot_bytes;
-        for (uint32_t r = 0; r < nr; r += 2) {
-            const uint32_t rr = r + (uint32_t)half;
-            const bool valid = rr < nr;
-            const uint8_t* row = slot + (size_t)(valid ? rr : r) * p.stride;
-            int ha = 0, hb = 0, la = 0, lb = 0;
+        // four rows per step, two per half-warp (rows r + half and r + 2 + half): two independent sum chains per lane, and one reduction and
+        // one epilogue for four rows
+        for (uint32_t r = 0; r < nr; r += 4) {
+            const uint32_t ra = r + (uint32_t)half, rb = ra + 2;
+            const bool va = ra < nr, vb = rb < nr;
+            const uint8_t* rowa = slot + (size_t)(va ? ra : r) * p.stride;
+            const uint8_t* rowb = slot + (size_t)(vb ? rb : r) * p.stride;
+            int ha = 0, la = 0, hb = 0, lb = 0;
 #pragma unroll
             for (int c = 0; c < NCH; ++c) {
-                const uint2 wa = *reinterpret_cast<const uint2*>(row + aoff[c]);
-                const uint32_t wb = *reinterpret_cast<const uint32_t*>(row + boff[c]);
-                const uint32_t a[4] = {wa.x & 0x0F0F0F0Fu, (wa.x >> 4) & 0x0F0F0F0Fu, wa.y & 0x0F0F0F0Fu, (wa.y >> 4) & 0x0F0F0F0Fu};
+                const uint2 xa = *reinterpret_cast<const uint2*>(rowa + a_off + 128 * c);
+                const uint2 xb = *reinterpret_cast<const uint2*>(rowb + a_off + 128 * c);
+                const uint32_t ya = q6_spread(*reinterpret_cast<const uint16_t*>(rowa + b_off + 32 * c));
+                const uint32_t yb = q6_spread(*reinterpret_cast<const uint16_t*>(rowb + b_off + 32 * c));
+                const uint32_t wa[4] = {((xa.x << 1) & 0x1E1E1E1Eu) | (ya & 0x01010101u),        ((xa.x >> 3) & 0x1E1E1E1Eu) | ((ya >> 1) & 0x01010101u),
+                                        ((xa.y << 1) & 0x1E1E1E1Eu) | ((ya >> 2) & 0x01010101u), ((xa.y >> 3) & 0x1E1E1E1Eu) | ((ya >> 3) & 0x01010101u)};
+                const uint32_t wb[4] = {((xb.x << 1) & 0x1E1E1E1Eu) | (yb & 0x01010101u),        ((xb.x >> 3) & 0x1E1E1E1Eu) | ((yb >> 1) & 0x01010101u),
+                                        ((xb.y << 1) & 0x1E1E1E1Eu) | ((yb >> 2) & 0x01010101u), ((xb.y >> 3) & 0x1E1E1E1Eu) | ((yb >> 3) & 0x01010101u)};
 #pragma unroll
                 for (int m = 0; m < 4; ++m) {
-                    const uint32_t b = (wb >> (2 * m)) & 0x03030303u;
-                    ha = __dp4a((int)a[m], (int)hq[c][m], ha); la = __dp4a((int)a[m], (int)lq[c][m], la);
-                    hb = __dp4a((int)b, (int)hq[c][m], hb);    lb = __dp4a((int)b, (int)lq[c][m], lb);
+                    ha = __dp4a((int)wa[m], (int)Q.hq[c][m], ha); la = __dp4a((int)wa[m], (int)Q.lq[c][m], la);
+                    hb = __dp4a((int)wb[m], (int)Q.hq[c][m], hb); lb = __dp4a((int)wb[m], (int)Q.lq[c][m], lb);
                 }
             }
-            const int hs = 4 * ha + hb, ls = 4 * la + lb;
-            // both half-warp sums in one butterfly: lanes 0-7 of a half end up with sum h u, lanes 8-15 with sum l u
-            int v = ((hl & 8) ? ls : hs) + __shfl_xor_sync(0xFFFFFFFFu, (hl & 8) ? hs : ls, 8);
-#pragma unroll
-            for (int o = 4; o; o >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);
+            // the four half-warp sums in one butterfly: lanes 0-3 of a half end up with sum h w of row a, 4-7 of row b, 8-11 sum l w of row a, 12-15 of row b
+            int x0 = ((hl & 8) ? la : ha) + __shfl_xor_sync(0xFFFFFFFFu, (hl & 8) ? ha : la, 8);
+            int x1 = ((hl & 8) ? lb : hb) + __shfl_xor_sync(0xFFFFFFFFu, (hl & 8) ? hb : lb, 8);
+            int v = ((hl & 4) ? x1 : x0) + __shfl_xor_sync(0xFFFFFFFFu, (hl & 4) ? x0 : x1, 4);
+            v += __shfl_xor_sync(0xFFFFFFFFu, v, 2);
+            v += __shfl_xor_sync(0xFFFFFFFFu, v, 1);
             const int lsum = __shfl_xor_sync(0xFFFFFFFFu, v, 8);
-            if (hl == 0 && valid) {
-                const float H = __fsub_rn((float)v, corr_h), L = __fsub_rn((float)lsum, corr_l);   // exact: integers below 2^24
-                const float2 sp = *reinterpret_cast<const float2*>(row + p.stride - 8);
-                const float app = __fmul_rn(sp.x, __fmul_rn(sq, __fmaf_rn(L, k254, H)));
-                const float up = __fadd_ru(app, fminf(__fmul_ru(sp.x, e1), __fmaf_ru(sp.y, t2a, t2b)));   // an upper bound of the exact score (up to slack_q)
-                if (!(up < thr_adj)) {
-                    const uint32_t id = (uint32_t)(r0 + rr);
+            bool pass = false;
+            uint4 ent;
+            float rho6;
+            if ((hl == 0 && va) || (hl == 4 && vb)) {
+                const uint8_t* row = hl ? rowb : rowa;
+                const float* meta = reinterpret_cast<const float*>(row + meta_off);
+                const float sr = meta[0], rho5 = meta[1];
+                const float H5 = (float)(4 * v - corr_h5), L5 = (float)(4 * lsum - corr_l5);     // exact: integers below 2^24
+                const float app = __fmul_rn(sr, __fmul_rn(sq_half, __fmaf_rn(L5, k254, H5)));
+                const float up = __fadd_ru(app, fminf(__fmul_ru(sr, Q.e1_5), __fmaf_ru(rho5, Q.t2a, Q.t2b)));   // an upper bound of the exact score (up to slack_q)
+                if (!(up < Q.thr_adj)) {
+                    const uint32_t id = (uint32_t)(r0 + (hl ? rb : ra));
                     bool dead = false;
                     if (p.deleted) dead = (p.deleted[id >> 5] >> (id & 31)) & 1u;
                     if (p.deleted2) dead = dead || ((p.deleted2[id >> 5] >> (id & 31)) & 1u);
-                    if (!dead) {
-                        const unsigned int pos = atomicAdd(p.cnt, 1u);
-                        if (pos < p.cap) p.cand[pos] = id;
-                    }
+                    pass = !dead;
+                    ent = make_uint4(id, (uint32_t)(2 * v - corr_h), (uint32_t)(2 * lsum - corr_l), __float_as_uint(sr));
+                    rho6 = meta[2];
+                }
+            }
+            // one atomic per warp step that lets a row through (lanes 0, 4, 16 and 20 decide)
+            const unsigned int passed = __ballot_sync(0xFFFFFFFFu, pass);
+            if (passed) {
+                unsigned int base = 0;
+                if (lane == 0) base = atomicAdd(p.list_cnt, (unsigned int)__popc(passed));
+                base = __shfl_sync(0xFFFFFFFFu, base, 0);
+                if (pass) {
+                    const unsigned int pos = base + (unsigned int)__popc(passed & ((1u << lane) - 1u));
+                    if (pos < p.list_cap) { p.list[pos] = ent; p.list_rho[pos] = rho6; }
                 }
             }
         }
@@ -580,6 +660,76 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q6_filter_kernel(const Pf
         if (lane == 0) qb_mbar_arrive(&empty[s]);
         s += PF_CONSUMER_WARPS;
         if (s >= p.n_slots) { s -= p.n_slots; ph ^= 1u; }
+    }
+}
+
+// Stage 2: the 6-bit test of the first-stage list, completed from the side plane.  One thread per entry, a grid-stride loop over the count
+// stage 1 left on the device; the query's packed int8 levels in shared memory, read by every thread of a warp at once.  The last CTA to read the
+// count resets it for the next query.  An overflowing list leaves the candidate count above cap, so that the finish kernel raises the fallback flag.
+constexpr int PF_RESCREEN_THREADS = 256;
+template <int NCH>
+__global__ void __launch_bounds__(PF_RESCREEN_THREADS) dense_q6_rescreen_kernel(const Pf6Params p) {
+    __shared__ uint4 s_hq[NCH * 16], s_lq[NCH * 16];             // chunk v: the query bytes of dims 16v + 4m + j in word m
+    __shared__ float s_k[5];
+    __shared__ unsigned int s_n;
+    if (threadIdx.x == 0) {
+        s_n = *reinterpret_cast<volatile unsigned int*>(p.list_cnt);
+        __threadfence();
+        if (atomicAdd(p.list_ticket, 1u) == gridDim.x - 1) { *p.list_cnt = 0u; *p.list_ticket = 0u; }
+    }
+    if (threadIdx.x < 32) {
+        const int hl = threadIdx.x & 15;
+        Q6Query<NCH> Q;
+        q6_query<NCH>(p, hl, Q);
+        if (threadIdx.x < 16) {
+#pragma unroll
+            for (int c = 0; c < NCH; ++c) {
+                s_hq[c * 16 + hl] = make_uint4(Q.hq[c][0], Q.hq[c][1], Q.hq[c][2], Q.hq[c][3]);
+                s_lq[c * 16 + hl] = make_uint4(Q.lq[c][0], Q.lq[c][1], Q.lq[c][2], Q.lq[c][3]);
+            }
+        }
+        if (threadIdx.x == 0) { s_k[0] = Q.sq; s_k[1] = Q.e1; s_k[2] = Q.t2a; s_k[3] = Q.t2b; s_k[4] = Q.thr_adj; }
+    }
+    __syncthreads();
+    const unsigned int n1 = s_n;
+    if (n1 > p.list_cap) {
+        if (blockIdx.x == 0 && threadIdx.x == 0) *p.cnt = p.cap + 1u;
+        return;
+    }
+    const float sq = s_k[0], e1 = s_k[1], t2a = s_k[2], t2b = s_k[3], thr_adj = s_k[4];
+    const float k254 = 1.0f / 254.0f;
+    const uint32_t lo_b = q6_lo_stride(p.d_pad);
+    for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e < n1; e += gridDim.x * blockDim.x) {
+        const uint4 ent = __ldcg(p.list + e);
+        const uint4* lo = reinterpret_cast<const uint4*>(p.lo + (size_t)ent.x * lo_b);
+        uint4 t[NCH * 2];                                          // 128 dimensions each
+#pragma unroll
+        for (int k = 0; k < NCH * 2; ++k) t[k] = (k * 128 < (int)p.d_pad) ? __ldg(lo + k) : make_uint4(0, 0, 0, 0);
+        int hs = 0, ls = 0;
+#pragma unroll
+        for (int k = 0; k < NCH * 2; ++k) {
+            if (k * 128 >= (int)p.d_pad) break;
+            const uint32_t tw[4] = {t[k].x, t[k].y, t[k].z, t[k].w};
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const uint32_t y = q6_spread((tw[i >> 1] >> (16 * (i & 1))) & 0xFFFFu);
+                const uint4 hq = s_hq[k * 8 + i], lq = s_lq[k * 8 + i];
+                const uint32_t hw[4] = {hq.x, hq.y, hq.z, hq.w}, lw[4] = {lq.x, lq.y, lq.z, lq.w};
+#pragma unroll
+                for (int m = 0; m < 4; ++m) {
+                    const uint32_t b = (y >> m) & 0x01010101u;
+                    hs = __dp4a((int)b, (int)hw[m], hs); ls = __dp4a((int)b, (int)lw[m], ls);
+                }
+            }
+        }
+        const float H = (float)((int)ent.y + hs), L = (float)((int)ent.z + ls);                  // exact: integers below 2^24
+        const float sr = __uint_as_float(ent.w), rho6 = __ldcg(p.list_rho + e);
+        const float app = __fmul_rn(sr, __fmul_rn(sq, __fmaf_rn(L, k254, H)));
+        const float up = __fadd_ru(app, fminf(__fmul_ru(sr, e1), __fmaf_ru(rho6, t2a, t2b)));     // an upper bound of the exact score (up to slack_q)
+        if (!(up < thr_adj)) {
+            const unsigned int pos = atomicAdd(p.cnt, 1u);
+            if (pos < p.cap) p.cand[pos] = ent.x;
+        }
     }
 }
 
@@ -701,23 +851,25 @@ static qb_status q8_shadow_ensure(qb_storage* s, cudaStream_t stream) {
     return QB_OK;
 }
 
-// 6-bit shadow plane (codes + the row's scale and residual bound), built like the int8 plane: +19 % HBM
+// 6-bit shadow plane (main records + the side plane of low bits), built like the int8 plane: +19 % HBM
 static qb_status q6_shadow_ensure(qb_storage* s, cudaStream_t stream) {
     std::lock_guard<std::mutex> lk(s->mu);
     if (s->q6_ready) return QB_OK;
     const uint32_t d_pad = (uint32_t)round_up_u64(s->dim, 32);
-    const uint32_t row_b = d_pad / 4 * 3 + 8;
+    const uint32_t row_b = (uint32_t)round_up_u64(d_pad / 2 + d_pad / 8 + 12, 8);
     const size_t bytes = (size_t)s->count * row_b + 16;                  // + 16: a tile's bulk copy is rounded up to 16 bytes (pf_produce)
+    const size_t lo_bytes = (size_t)s->count * q6_lo_stride(d_pad);
     if (!s->d_q6) {
-        QB_CUDA(cudaMalloc(&s->d_q6, std::max<size_t>(bytes, 256)));
+        QB_CUDA(cudaMalloc(&s->d_q6_lo, std::max<size_t>(lo_bytes, 256)));
+        if (cudaMalloc(&s->d_q6, std::max<size_t>(bytes, 256)) != cudaSuccess) { cudaFree(s->d_q6_lo); s->d_q6_lo = nullptr; s->d_q6 = nullptr; return QB_ERR_CUDA; }
         QB_CUDA(cudaMalloc(&s->d_q6_meta, 256));
-        s->hbm_bytes += bytes;
+        s->hbm_bytes += bytes + lo_bytes;
     }
     s->q6_row_b = row_b;
     QB_CUDA(cudaMemsetAsync(s->d_q6_meta, 0, 256, stream));
     const uint64_t blocks = std::min<uint64_t>(ceil_div_u64(std::max<uint64_t>(s->count, 1), 32), (uint64_t)s->sm_count * 16);
     f32_to_q6_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(reinterpret_cast<const float*>(s->d_rows), s->row_stride / 4, s->dim, d_pad, s->count, s->d_q6, row_b,
-                                                                s->d_q6_meta, s->d_q6_meta + 1);
+                                                                s->d_q6_lo, s->d_q6_meta, s->d_q6_meta + 1);
     QB_LAUNCHED();
     QB_CUDA(cudaGetLastError());
     unsigned int meta[2] = {0, 0};
@@ -750,19 +902,25 @@ bool qb_f32_prefilter_usable(qb_storage* s, uint64_t n_rows, uint32_t top, cudaS
 
 // d_q = preprocessed query; the exact top-`top` of the storage lands in d_out / d_out_cnt.  `a` = the scan arguments of the exact
 // in-kernel-top-k path (emit.cand / final_out / done_counter set up by the caller); scratch = c->d_pf (see qb_f32_prefilter_scratch_bytes).
-size_t qb_f32_prefilter_scratch_bytes() { return (size_t)PF_CAP * 12 + 16 * sizeof(qb_scored_point) + 256; }
+size_t qb_f32_prefilter_scratch_bytes() { return 256 + (size_t)PF_CAP * 12 + (size_t)PF_LIST_CAP * 20; }
 
 qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t top, void* d_scratch, unsigned int* d_n_fallbacks, qb_scored_point* d_out, uint32_t* d_out_cnt,
                                   cudaEvent_t prof0, cudaEvent_t prof1, cudaStream_t stream) {
     uint8_t* sc = reinterpret_cast<uint8_t*>(d_scratch);
-    // scratch: [0,16) cnt | [16,32) fallback flag | [32,48) finish ticket | [48,64) sample count | [64, 64+16*8) sample top-k | per-CTA top-k keys | candidate rows
+    // scratch: [0,16) cnt | [16,32) fallback flag | [32,48) finish ticket | [48,64) sample count | [64, 64+16*8) sample top-k |
+    // [192,208) first-stage count | [208,224) its ticket | from 256: per-CTA top-k keys | candidate rows | first-stage list | its rho6 column
+    // (the first 256 bytes are zeroed once, the kernels reset their counters)
     unsigned int* d_cnt = reinterpret_cast<unsigned int*>(sc);
     unsigned int* d_fallback = reinterpret_cast<unsigned int*>(sc + 16);
     uint32_t* d_samp_cnt = reinterpret_cast<uint32_t*>(sc + 48);
     qb_scored_point* d_samp = reinterpret_cast<qb_scored_point*>(sc + 64);
     unsigned int* d_ticket = reinterpret_cast<unsigned int*>(sc + 32);
-    unsigned long long* d_keys = reinterpret_cast<unsigned long long*>(sc + 64 + 16 * sizeof(qb_scored_point));
+    unsigned int* d_list_cnt = reinterpret_cast<unsigned int*>(sc + 192);
+    unsigned int* d_list_ticket = reinterpret_cast<unsigned int*>(sc + 208);
+    unsigned long long* d_keys = reinterpret_cast<unsigned long long*>(sc + 256);
     uint32_t* d_cand = reinterpret_cast<uint32_t*>(d_keys + PF_CAP);
+    uint4* d_list = reinterpret_cast<uint4*>(d_cand + PF_CAP);
+    float* d_list_rho = reinterpret_cast<float*>(d_list + PF_LIST_CAP);
     const uint64_t n = s->count;
     // the candidate list holds n / 32 rows (at most PF_CAP): re-scoring reads a whole f32 row per candidate, and past 1/32 of the rows the
     // exact scan that a longer list would save is no longer far off
@@ -782,18 +940,30 @@ qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t t
     const int plane = pf_plane();
     if (plane == 0 && s->q6_ready && s->q6_usable) {
         Pf6Params p6{};
-        p6.rows = s->d_q6; p6.stride = s->q6_row_b; p6.d_pad = (uint32_t)round_up_u64(s->dim, 32); p6.dim = s->dim; p6.n_rows = n;
+        p6.rows = s->d_q6; p6.lo = s->d_q6_lo; p6.stride = s->q6_row_b; p6.d_pad = (uint32_t)round_up_u64(s->dim, 32); p6.dim = s->dim; p6.n_rows = n;
         p6.q = d_q; p6.samp_out = d_samp; p6.samp_cnt = d_samp_cnt; p6.top = top; p6.max_norm_bits = s->d_q6_meta;
+        // every row up to PF_LIST_CAP rows: the 5-bit stage lets 1-3 % of the rows through on unit-Gaussian data at dim 768 with a 131 072-row
+        // sample, but far more on wider rows or with the 16 384-row sample of a smaller storage
+        p6.list = d_list; p6.list_rho = d_list_rho; p6.list_cnt = d_list_cnt; p6.list_ticket = d_list_ticket; p6.list_cap = (uint32_t)std::min<uint64_t>(PF_LIST_CAP, n);
         p6.cand = d_cand; p6.cnt = d_cnt; p6.cap = cap; p6.deleted = a.emit.deleted; p6.deleted2 = a.emit.deleted2;
         p6.l2_keep = ((uint64_t)n * p6.stride <= (64ull << 20)) ? 1 : 0;
+        const unsigned rs_grid = (unsigned)s->sm_count * 4;
         if (prof0) cudaEventRecord(prof0, stream);
         switch ((p6.d_pad + 255) / 256) {
-            case 1: QB_TRY(launch_ring(dense_q6_filter_kernel<1>, p6, s->sm_count, stream)); break;
-            case 2: QB_TRY(launch_ring(dense_q6_filter_kernel<2>, p6, s->sm_count, stream)); break;
-            case 3: QB_TRY(launch_ring(dense_q6_filter_kernel<3>, p6, s->sm_count, stream)); break;
-            default: QB_TRY(launch_ring(dense_q6_filter_kernel<4>, p6, s->sm_count, stream)); break;
+            case 1: QB_TRY(launch_ring(dense_q5_filter_kernel<1>, p6, s->sm_count, stream)); break;
+            case 2: QB_TRY(launch_ring(dense_q5_filter_kernel<2>, p6, s->sm_count, stream)); break;
+            case 3: QB_TRY(launch_ring(dense_q5_filter_kernel<3>, p6, s->sm_count, stream)); break;
+            default: QB_TRY(launch_ring(dense_q5_filter_kernel<4>, p6, s->sm_count, stream)); break;
         }
         if (prof1) cudaEventRecord(prof1, stream);
+        switch ((p6.d_pad + 255) / 256) {
+            case 1: dense_q6_rescreen_kernel<1><<<rs_grid, PF_RESCREEN_THREADS, 0, stream>>>(p6); break;
+            case 2: dense_q6_rescreen_kernel<2><<<rs_grid, PF_RESCREEN_THREADS, 0, stream>>>(p6); break;
+            case 3: dense_q6_rescreen_kernel<3><<<rs_grid, PF_RESCREEN_THREADS, 0, stream>>>(p6); break;
+            default: dense_q6_rescreen_kernel<4><<<rs_grid, PF_RESCREEN_THREADS, 0, stream>>>(p6); break;
+        }
+        QB_LAUNCHED();
+        QB_CUDA(cudaGetLastError());
     } else if (plane == 2 && s->q8_ready && s->q8_usable) {
         Pf8Params p8{};
         p8.rows = reinterpret_cast<const uint8_t*>(s->d_q8); p8.stride = s->q8_row_b; p8.dim = s->dim; p8.n_rows = n;

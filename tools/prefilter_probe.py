@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """prefilter_probe.py [rows] [dim] — single-query searches over one synthetic cosine storage (generated on the device), device-timed, for several
 ring-slot sizes / producer-warp counts of the shadow-plane filter kernels and the three planes; prints one JSON line.  Results of every variant are compared with the exact scan.
-"candidates" counts, per query, the rows each integer plane's bound lets through (the kernels' bounds restated in torch on the same rows, f64 where they round up)."""
+"candidates" counts, per query, the rows each integer plane's bound lets through (the kernels' bounds restated in torch on the same rows, f64 where they round up):
+on the 6-bit plane, the rows of the 5-bit first stage (q6_stage1) and those of them the 6-bit second stage keeps (q6_stage2)."""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -66,7 +67,7 @@ out["fallbacks"] = int(st.search_stats()[1])
 
 
 def candidate_counts(nq=16, top=10):
-    """Rows with upper bound >= thr_q - slack_q on the 6-bit and int8 planes, thr_q = the exact top-`top` score of the sample prefix."""
+    """Rows with upper bound >= thr_q - slack_q on the 6-bit plane's two stages and the int8 plane, thr_q = the exact top-`top` score of the sample prefix."""
     qd = torch.from_numpy(queries[:nq]).to(dev).double()
     qd = (qd / qd.norm(dim=1, keepdim=True)).float().double()          # cosine queries are normalised
     qmax = qd.abs().amax(1, keepdim=True)
@@ -77,6 +78,7 @@ def candidate_counts(nq=16, top=10):
     q1, qn = qd.abs().sum(1), qd.norm(dim=1)
     sample = min(131072, max(16384, rows // 64))
     e1 = q1 * (0.5 + 2.0 ** -13) + sq[:, 0] * dim * 0.066
+    e1_5 = q1 * (1 + 2.0 ** -13) + sq[:, 0] * dim * 0.066
     e2 = sq[:, 0] * dim ** 0.5 * 0.00202
     e8 = q1 * (0.5 + 2.0 ** -13) + sq[:, 0] * dim * 0.27
     g = torch.Generator(device=dev); g.manual_seed(42)
@@ -90,7 +92,7 @@ def candidate_counts(nq=16, top=10):
     slack6 = 2 * (dim * 2.0 ** -22 + 2.0 ** -17) * qn * mxn
     slack8 = (dim * 2.0 ** -22 + 2.0 ** -17) * (1 + dim ** 0.5 / 127) * qn * mxn
     g.manual_seed(42)
-    thr, c6, c8 = None, torch.zeros(nq, dtype=torch.int64, device=dev), torch.zeros(nq, dtype=torch.int64, device=dev)
+    thr, c5, c6, c8 = None, *(torch.zeros(nq, dtype=torch.int64, device=dev) for _ in range(3))
     for r0, n in chunks:
         x = torch.randn((n, dim), generator=g, device=dev, dtype=torch.float32)
         check(lib().qb_metric_preprocess_device(0, int(qb.Distance.Cosine), dim, n, vp(x.data_ptr()), dim * 4))
@@ -101,13 +103,18 @@ def candidate_counts(nq=16, top=10):
         c = (x * (31 / mx)).round().clamp(-31, 31).double()
         rho = (x.double() - sr * c).norm(dim=1, keepdim=True)
         up6 = sr * sq.T * (c @ h.T + (c @ l.T) / 254) + torch.minimum(sr * e1, rho * (qn + e2) + e2 * mxn)
-        c6 += (up6 >= thr - slack6).sum(0)
+        c5c = 2 * torch.div(c + 31, 2, rounding_mode="floor") + 0.5 - 31      # the 5-bit code's reconstruction
+        rho5 = (x.double() - sr * c5c).norm(dim=1, keepdim=True)
+        up5 = sr * sq.T * (c5c @ h.T + (c5c @ l.T) / 254) + torch.minimum(sr * e1_5, rho5 * (qn + e2) + e2 * mxn)
+        p5 = up5 >= thr - slack6
+        c5 += p5.sum(0)
+        c6 += (p5 & (up6 >= thr - slack6)).sum(0)
         s8 = (mx / 127).double()
         c = (x * (127 / mx)).round().clamp(-127, 127).double()
         up8 = s8 * (sq.T * (c @ h.T + (c @ l.T) / 254) + e8)
         c8 += (up8 >= thr - slack8).sum(0)
-        del x, c, rho, up6, up8
-    return {"q6": c6.tolist(), "int8": c8.tolist(), "sample_rows": sample}
+        del x, c, rho, up6, up8, c5c, rho5, up5, p5
+    return {"q6_stage1": c5.tolist(), "q6_stage2": c6.tolist(), "int8": c8.tolist(), "sample_rows": sample}
 
 
 st.close()
