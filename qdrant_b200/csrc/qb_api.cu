@@ -209,7 +209,7 @@ static void ctx_destroy(QbSearchCtx* c) {
     if (!c) return;
     if (c->stream) cudaStreamSynchronize(c->stream);
     cudaFree(c->d_queries_raw); cudaFree(c->d_queries_enc); cudaFree(c->d_q_off); cudaFree(c->d_thr); cudaFree(c->d_cnt); cudaFree(c->d_done);
-    cudaFree(c->d_cand); cudaFree(c->d_out); cudaFree(c->d_out_counts); cudaFree(c->d_deleted2); cudaFree(c->d_ids); cudaFree(c->d_mma); cudaFree(c->d_pf);
+    cudaFree(c->d_cand); cudaFree(c->d_out); cudaFree(c->d_out_counts); cudaFree(c->d_deleted2); cudaFree(c->d_ids); cudaFree(c->d_mma); cudaFree(c->d_pf); cudaFree(c->d_pf_up5);
     if (c->h_stage) cudaFreeHost(c->h_stage);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
@@ -666,12 +666,13 @@ static qb_status run_search(qb_storage* s, QbSearchCtx* c, uint32_t nq, uint32_t
         // device-side flag falls back to the exact scan below when the prefilter's candidate list overflowed (qb_prefilter.cu)
         if (qb_f32_prefilter_usable(s, n_cand, top, stream)) {
             if (!c->d_pf) { QB_CUDA(cudaMalloc(&c->d_pf, qb_f32_prefilter_scratch_bytes())); QB_CUDA(cudaMemsetAsync(c->d_pf, 0, 256, stream)); }
+            QB_TRY(ensure_dev_elems(&c->d_pf_up5, &c->pf_up5_elems, (size_t)round_up_u64(n_cand, 4)));
             {
                 std::lock_guard<std::mutex> lk(s->mu);
                 if (!s->d_pf_fallbacks) { QB_CUDA(cudaMalloc(&s->d_pf_fallbacks, 256)); QB_CUDA(cudaMemsetAsync(s->d_pf_fallbacks, 0, 256, stream)); }
             }
             profile_acquire(s, &e0, &e1);
-            QB_TRY(qb_f32_prefilter_search(s, a, top, c->d_pf, s->d_pf_fallbacks, d_out, d_counts, e0, e1, stream));
+            QB_TRY(qb_f32_prefilter_search(s, a, top, c->d_pf, c->d_pf_up5, s->d_pf_fallbacks, d_out, d_counts, e0, e1, stream));
             profile_commit(s, e0, e1);
             if (can_flag) *can_flag = false;
             return QB_OK;

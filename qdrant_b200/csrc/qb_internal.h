@@ -26,6 +26,7 @@ struct QbSearchCtx {
     uint32_t* d_deleted2 = nullptr;  size_t deleted2_words = 0;
     uint32_t* d_ids = nullptr;       size_t ids_elems = 0;
     void* d_pf = nullptr;            // single-query bf16 prefilter: counters, sample top-k, candidate rows (qb_prefilter.cu)
+    float* d_pf_up5 = nullptr;       size_t pf_up5_elems = 0;        // single-query prefilter on the 6-bit plane: every row's first-stage bound
     void* d_mma = nullptr;           size_t mma_bytes = 0;           // batched SQ8: sorted query codes / permutation / chunk thresholds
     // pinned host staging
     void* h_stage = nullptr;         size_t h_stage_bytes = 0;
@@ -205,8 +206,8 @@ size_t qb_pq_scratch_bytes(const qb_storage* s, uint32_t nq);
 qb_status qb_f32_shadow_ensure(qb_storage* s, cudaStream_t stream);
 bool qb_f32_prefilter_usable(qb_storage* s, uint64_t n_rows, uint32_t top, cudaStream_t stream);
 size_t qb_f32_prefilter_scratch_bytes();
-qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t top, void* d_scratch, unsigned int* d_n_fallbacks, qb_scored_point* d_out, uint32_t* d_out_cnt,
-                                  cudaEvent_t prof0, cudaEvent_t prof1, cudaStream_t stream);
+qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t top, void* d_scratch, float* d_up5, unsigned int* d_n_fallbacks, qb_scored_point* d_out,
+                                  uint32_t* d_out_cnt, cudaEvent_t prof0, cudaEvent_t prof1, cudaStream_t stream);
 qb_status qb_launch_scan(const qb_storage* s, const QbScanArgs& a, cudaStream_t stream);
 
 // score listed ids for ONE encoded query into d_scores (RawScorer::score_points)

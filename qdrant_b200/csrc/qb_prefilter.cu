@@ -8,7 +8,7 @@
 //     | sum_i q_i bf16(x_i) - sum_i q_i x_i |  <=  2^-9 ||q|| ||x||            (Cauchy-Schwarz on the element-wise rounding errors)
 //   + f32 evaluation of either sum, any order:  <=  dim 2^-24 ||q|| ||x|| each
 //   =>  |approx - exact|  <=  eps_q := (2^-9 + dim 2^-22) ||q|| max_rows ||x||  (1 + 2^-10)
-// Four launches per query, no host synchronisation:
+// Four launches per query, no host synchronisation (the 6-bit plane below takes its sample in its own first stage instead of step 1):
 //   1. the EXACT in-kernel-top-k scan (dense_f32_stream_kernel<., LOCALK>) over a prefix of the rows (1/64 of them, 2^14..2^17) -> thr_q = the k-th best exact score
 //      of the sample (a lower bound of the final k-th score);
 //   2. dense_bf16_filter_kernel: the whole bf16 plane streams through the same TMA-bulk ring (dim * 2 bytes per row); the query sits in
@@ -22,6 +22,7 @@
 #include <algorithm>
 
 #include "qb_internal.h"
+#include "qb_localk.cuh"
 #include "qb_score.cuh"
 
 qb_status qb_dense_f32_scan_localk(const qb_storage* s, const QbScanArgs& a, uint32_t top, uint64_t* n_slots, cudaStream_t stream, uint64_t min_rows = 65536);   // qb_dense.cu
@@ -35,7 +36,7 @@ constexpr int PF_PRODUCERS = 2;             // producer warps (one lane each): a
 constexpr int PF_THREADS = 32 * (PF_CONSUMER_WARPS + PF_MAX_PRODUCERS);     // launch bound; the launch uses 32 * (consumers + producers)
 constexpr uint32_t PF_SLOT_BYTES = 12288;  // target bytes per ring slot (a consumer warp holds one slot while the others are in flight)
 constexpr uint32_t PF_CAP = 131072;        // candidate rows per query at most (a few thousand to a few tens of thousands expected on 10M rows)
-constexpr uint32_t PF_LIST_CAP = 1u << 21; // first-stage rows of the 6-bit plane per query at most (dense_q5_filter_kernel)
+constexpr uint32_t PF_LIST_CAP = 1u << 21; // first-stage rows of the 6-bit plane per query at most (dense_q5_compact_kernel)
 
 static int pf_producers() { const int o = qb_opt().prefilter_producers; return (o >= 1 && o <= PF_MAX_PRODUCERS) ? o : PF_PRODUCERS; }
 
@@ -377,19 +378,20 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q8_filter_kernel(const Pf
 //   exact - s_r s_q (H5 + L5 / 254) / 2 = sum_i (q_i - q^_i) s_r c5_i + sum_i q_i r5_i, r5_i = r_i + s_r (e_i - 1/2), bounded by the smaller of
 //     t1 = s_r E1_5,  E1_5 = (1 + 2^-13) ||q||_1 + 0.066 s_q dim      (|r5_i| <= s_r (1 + 2^-13); |c5_i| <= 31.5, 31.5 (1/508 + 2.3e-5) < 0.066)
 //     t2 = ||q||_2 rho5 + e2 (max||x|| + rho5)                        (Cauchy-Schwarz as below; s_r ||c5||_2 <= ||x|| + rho5)
-// Rows that pass are appended with their partial sums sum h (2w - 31), sum l (2w - 31), s_r and rho6 to a first-stage list.
-// Stage 2 (dense_q6_rescreen_kernel) adds sum h e and sum l e from the side plane: that gives back the 6-bit sums H = sum_i h_i c_i, L likewise,
+// Stage 1 writes this bound for every row and takes the threshold sample (the exact top-k of the prefix's best rows by approximate score);
+// stage 2 (dense_q5_compact_kernel) lists the rows whose bound reaches it.
+// Stage 3 (dense_q6_rescreen_kernel) recomputes the 6-bit sums H = sum_i h_i c_i, L likewise, from the main record and the side plane,
 //   exact - s_r s_q (H + L / 254) = sum_i (q_i - q^_i) s_r c_i + sum_i q_i r_i, bounded by the smaller of
 //     t1 = s_r E1,  E1 = (1/2 + 2^-13) ||q||_1 + s_q dim (31/508)(1 + 0.08)     (|r_i| <= s_r (1/2 + 2^-13), |c_i| <= 31, |q_i - q^_i| <= s_q (1/508 + 2.3e-5))
 //     t2 = ||q||_2 rho6 + e2 (max||x|| + rho6),  e2 = s_q sqrt(dim)(1/508 + 2.3e-5)(1 + 0.01) >= ||q - q^||_2   (Cauchy-Schwarz; s_r ||c||_2 <= ||x|| + rho6)
 //   and appends the rows that pass to the candidate list.
-// Both stages: + slack_q = 2 (dim 2^-22 + 2^-17) ||q|| max||x||: the exact f32 sum (<= dim 2^-24 ||q|| ||x||) and the kernel's f32 evaluation of
+// Both bounds: + slack_q = 2 (dim 2^-22 + 2^-17) ||q|| max||x||: the exact f32 sum (<= dim 2^-24 ||q|| ||x||) and the kernel's f32 evaluation of
 //   the approximation (<= 2^-22 ||q|| (||x|| + rho); rho <= sqrt(dim) (1 + 2^-13) / 31 ||x|| <= 1.04 ||x|| for dim <= 1024, and <= 2 sqrt(dim) ||x||
 //   for rows below 1e-30, which the 2^-16 of the slack still covers).
-// A row passes a stage iff  approx + min(t1, t2) >= thr_q - slack_q, every bound term rounded towards "pass".  Both bounds hold, so every row
-// whose exact score reaches thr_q passes both stages: the candidate list is a subset of what the 6-bit test alone would pass, and results are unchanged.
+// A row passes a bound iff  approx + min(t1, t2) >= thr_q - slack_q, every bound term rounded towards "pass".  Both bounds hold, so every row
+// whose exact score reaches thr_q passes both: the candidate list is a subset of what the 6-bit test alone would pass, and results are unchanged.
 // Zero and denormal-only rows (max < 1e-30) keep all-zero codes c (u = 31, c5 = -1/2), s_r = 2 max, rho6 = ||x||: their bounds hold.
-// bytes per row of the side plane: d_pad / 8, rounded up to 16 so that stage 2 reads it in 16-byte words
+// bytes per row of the side plane: d_pad / 8, rounded up to 16
 __host__ __device__ constexpr uint32_t q6_lo_stride(uint32_t d_pad) { return (d_pad / 8 + 15) & ~15u; }
 
 __global__ void __launch_bounds__(256) f32_to_q6_rows_kernel(const float* __restrict__ rows, uint64_t stride_f, uint32_t dim, uint32_t d_pad, uint64_t n,
@@ -476,9 +478,13 @@ struct Pf6Params {
     uint64_t n_rows;
     const float* q;
     uint32_t rows_per_slot, n_slots, slot_bytes;
-    const qb_scored_point* samp_out; const uint32_t* samp_cnt; uint32_t top;
+    qb_scored_point* samp_out; uint32_t* samp_cnt; uint32_t top;              // threshold sample: written by stage 1, read through q6_query
     const unsigned int* max_norm_bits;
-    uint4* list; float* list_rho; unsigned int* list_cnt; unsigned int* list_ticket; uint32_t list_cap;   // first-stage list: (row, sum h (2w - 31), sum l (2w - 31), s_r), rho6
+    float* up5;                 // stage 1's upper bound of every row
+    uint64_t sample_rows;       // the threshold sample: rows of the tiles that start below this
+    const uint8_t* f32_rows; uint32_t f32_stride; uint32_t id_base;            // exact rescoring of the sample
+    unsigned long long* cta_keys; unsigned int* samp_ticket;                   // per-CTA sample keys, arrival counter of their merge
+    uint32_t* list; unsigned int* list_cnt; unsigned int* list_ticket; uint32_t list_cap;   // first-stage list: row ids
     uint32_t* cand; unsigned int* cnt; uint32_t cap;
     const uint32_t* deleted; const uint32_t* deleted2;
     int l2_keep;
@@ -554,13 +560,87 @@ __device__ __forceinline__ void q6_query(const Pf6Params& p, int hl, Q6Query<NCH
 // nibble P(j) of a u16 of the b plane or the side plane to byte j
 __device__ __forceinline__ uint32_t q6_spread(uint32_t t) { return (t | (t << 12)) & 0x0F0F0F0Fu; }
 
-// Stage 1: the 5-bit code of every row through the TMA ring.  Half a warp per row.  NCH = 16-dimension chunks of a row per lane (d_pad <= NCH * 256)
+// Stage 1: the 5-bit code of every row through the TMA ring.  Half a warp per row.  NCH = 16-dimension chunks of a row per lane (d_pad <= NCH * 256).
+// There is no threshold yet: every row's bound goes to p.up5, and stage 2 compares it.  The rows of the tiles that start below p.sample_rows also
+// compete, by their approximate score, for each warp's list of the `top` best live rows (qb_localk.cuh).  At the end each CTA re-scores the best
+// `top` of its lists exactly, in the finish kernel's order, and the last CTA to finish writes the top `top` of those exact scores to the sample
+// slots.  Any `top` live rows give a lower bound of the k-th best exact score, so the threshold holds however well the approximation ranks rows.
+constexpr size_t PF_SAMPLE_SMEM = (size_t)QB_LOCALK_WARPS * (QB_LOCALK_SLOTS * 8 + 4 * 8 + 4) + QB_LOCALK_SLOTS * 8;   // lists, queues, counts, exact keys
+static_assert(PF_CONSUMER_WARPS == QB_LOCALK_WARPS, "the CTA merge sorts one list per consumer warp");
+
+template <int NCH, bool SAMPLE>
+__device__ __forceinline__ void q5_tile(const Pf6Params& p, const Q6Query<NCH>& Q, const uint8_t* slot, uint32_t nr, uint64_t r0, int lane, LkState& lk,
+                                        unsigned long long* lk_queue, unsigned int* lk_count) {
+    const int half = lane >> 4, hl = lane & 15;
+    // lane hl reads chunk c of a row at a_off + 128 c (a plane) and b_off + 32 c (b plane).  Chunks past d_pad meet a zero query; their reads
+    // stay inside the shared memory of the ring: at most 96 bytes past the end of a row, and the ring's barriers (>= 128 bytes) follow its last slot.
+    const uint32_t a_off = (uint32_t)hl * 8, b_off = p.d_pad / 2 + (uint32_t)hl * 2;
+    const uint32_t meta_off = p.d_pad / 2 + p.d_pad / 8;
+    const float sq_half = 0.5f * Q.sq;                             // exact: s_q is 0 or at least 1e-30 / 127
+    const float k254 = 1.0f / 254.0f;
+    const int corr_h5 = 61 * Q.sum_h, corr_l5 = 61 * Q.sum_l;
+    // four rows per step, two per half-warp (rows r + half and r + 2 + half): two independent sum chains per lane, and one reduction and
+    // one epilogue for four rows
+    for (uint32_t r = 0; r < nr; r += 4) {
+        const uint32_t ra = r + (uint32_t)half, rb = ra + 2;
+        const bool va = ra < nr, vb = rb < nr;
+        const uint8_t* rowa = slot + (size_t)(va ? ra : r) * p.stride;
+        const uint8_t* rowb = slot + (size_t)(vb ? rb : r) * p.stride;
+        int ha = 0, la = 0, hb = 0, lb = 0;
+#pragma unroll
+        for (int c = 0; c < NCH; ++c) {
+            const uint2 xa = *reinterpret_cast<const uint2*>(rowa + a_off + 128 * c);
+            const uint2 xb = *reinterpret_cast<const uint2*>(rowb + a_off + 128 * c);
+            const uint32_t ya = q6_spread(*reinterpret_cast<const uint16_t*>(rowa + b_off + 32 * c));
+            const uint32_t yb = q6_spread(*reinterpret_cast<const uint16_t*>(rowb + b_off + 32 * c));
+            const uint32_t wa[4] = {((xa.x << 1) & 0x1E1E1E1Eu) | (ya & 0x01010101u),        ((xa.x >> 3) & 0x1E1E1E1Eu) | ((ya >> 1) & 0x01010101u),
+                                    ((xa.y << 1) & 0x1E1E1E1Eu) | ((ya >> 2) & 0x01010101u), ((xa.y >> 3) & 0x1E1E1E1Eu) | ((ya >> 3) & 0x01010101u)};
+            const uint32_t wb[4] = {((xb.x << 1) & 0x1E1E1E1Eu) | (yb & 0x01010101u),        ((xb.x >> 3) & 0x1E1E1E1Eu) | ((yb >> 1) & 0x01010101u),
+                                    ((xb.y << 1) & 0x1E1E1E1Eu) | ((yb >> 2) & 0x01010101u), ((xb.y >> 3) & 0x1E1E1E1Eu) | ((yb >> 3) & 0x01010101u)};
+#pragma unroll
+            for (int m = 0; m < 4; ++m) {
+                ha = __dp4a((int)wa[m], (int)Q.hq[c][m], ha); la = __dp4a((int)wa[m], (int)Q.lq[c][m], la);
+                hb = __dp4a((int)wb[m], (int)Q.hq[c][m], hb); lb = __dp4a((int)wb[m], (int)Q.lq[c][m], lb);
+            }
+        }
+        // the four half-warp sums in one butterfly: lanes 0-3 of a half end up with sum h w of row a, 4-7 of row b, 8-11 sum l w of row a, 12-15 of row b
+        int x0 = ((hl & 8) ? la : ha) + __shfl_xor_sync(0xFFFFFFFFu, (hl & 8) ? ha : la, 8);
+        int x1 = ((hl & 8) ? lb : hb) + __shfl_xor_sync(0xFFFFFFFFu, (hl & 8) ? hb : lb, 8);
+        int v = ((hl & 4) ? x1 : x0) + __shfl_xor_sync(0xFFFFFFFFu, (hl & 4) ? x0 : x1, 4);
+        v += __shfl_xor_sync(0xFFFFFFFFu, v, 2);
+        v += __shfl_xor_sync(0xFFFFFFFFu, v, 1);
+        const int lsum = __shfl_xor_sync(0xFFFFFFFFu, v, 8);
+        const bool mine = (hl == 0 && va) || (hl == 4 && vb);      // lanes 0, 16, 4 and 20 hold rows r, r + 1, r + 2 and r + 3
+        float app = 0.f, up = 0.f;
+        if (mine) {
+            const float* meta = reinterpret_cast<const float*>((hl ? rowb : rowa) + meta_off);
+            const float sr = meta[0], rho5 = meta[1];
+            const float H5 = (float)(4 * v - corr_h5), L5 = (float)(4 * lsum - corr_l5);     // exact: integers below 2^24
+            app = __fmul_rn(sr, __fmul_rn(sq_half, __fmaf_rn(L5, k254, H5)));
+            up = __fadd_ru(app, fminf(__fmul_ru(sr, Q.e1_5), __fmaf_ru(rho5, Q.t2a, Q.t2b)));   // an upper bound of the exact score (up to slack_q)
+        }
+        // lanes 0-3 store the bounds of rows r .. r + 3: one contiguous store per step
+        const float u = __shfl_sync(0xFFFFFFFFu, up, ((lane & 1) << 4) | ((lane & 2) << 1));
+        if (lane < 4 && r + (uint32_t)lane < nr) p.up5[r0 + r + (uint32_t)lane] = u;
+        if (SAMPLE) {
+            if (mine && !(app < lk.wthr)) lk_push(p.deleted, p.deleted2, 0u, app, (uint32_t)(r0 + (hl ? rb : ra)), lk_queue, lk_count);
+            __syncwarp();
+            const unsigned int n_queued = *reinterpret_cast<volatile unsigned int*>(lk_count);
+            if (n_queued) lk = lk_drain(lk, lk_queue, lk_count, lane, n_queued);
+        }
+    }
+}
+
 template <int NCH>
 __global__ void __launch_bounds__(PF_THREADS, 1) dense_q5_filter_kernel(const Pf6Params p) {
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* slots = smem;                                       // [n_slots][slot_bytes]
     uint64_t* full = reinterpret_cast<uint64_t*>(slots + (size_t)p.n_slots * p.slot_bytes);
     uint64_t* empty = full + p.n_slots;
+    unsigned long long* lists = reinterpret_cast<unsigned long long*>(empty + p.n_slots);       // [warps][QB_LOCALK_SLOTS]
+    unsigned long long* lk_queue = lists + QB_LOCALK_WARPS * QB_LOCALK_SLOTS;                   // [warps][4]
+    unsigned int* lk_count = reinterpret_cast<unsigned int*>(lk_queue + QB_LOCALK_WARPS * 4);   // [warps]
+    unsigned long long* ex = reinterpret_cast<unsigned long long*>(lk_count + QB_LOCALK_WARPS); // [QB_LOCALK_SLOTS] exact keys of the CTA's sample
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint64_t n_tiles = (p.n_rows + p.rows_per_slot - 1) / p.rows_per_slot;
     const uint64_t n_local = (blockIdx.x < n_tiles) ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
@@ -568,6 +648,7 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q5_filter_kernel(const Pf
         for (uint32_t s = 0; s < p.n_slots; ++s) { qb_mbar_init(&full[s], 1); qb_mbar_init(&empty[s], 1); }
         qb_fence_barrier_init();
     }
+    if (threadIdx.x < QB_LOCALK_WARPS) lk_count[threadIdx.x] = 0u;
     __syncthreads();
     const int n_prod = (int)(blockDim.x >> 5) - PF_CONSUMER_WARPS;
     if (warp < n_prod) {
@@ -575,16 +656,10 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q5_filter_kernel(const Pf
         return;
     }
     const int cw = warp - n_prod;
-    const int half = lane >> 4, hl = lane & 15;
     Q6Query<NCH> Q;
-    q6_query<NCH>(p, hl, Q);
-    // lane hl reads chunk c of a row at a_off + 128 c (a plane) and b_off + 32 c (b plane).  Chunks past d_pad meet a zero query; their reads
-    // stay inside the shared memory of the ring: at most 96 bytes past the end of a row, and the ring's barriers (>= 128 bytes) follow its last slot.
-    const uint32_t a_off = (uint32_t)hl * 8, b_off = p.d_pad / 2 + (uint32_t)hl * 2;
-    const uint32_t meta_off = p.d_pad / 2 + p.d_pad / 8;
-    const float sq_half = 0.5f * Q.sq;                             // exact: s_q is 0 or at least 1e-30 / 127
-    const float k254 = 1.0f / 254.0f;
-    const int corr_h5 = 61 * Q.sum_h, corr_l5 = 61 * Q.sum_l, corr_h = 31 * Q.sum_h, corr_l = 31 * Q.sum_l;
+    q6_query<NCH>(p, lane & 15, Q);
+    // this warp's `top` best sample rows by approximate score (lanes >= top hold the maximum so that they are never the minimum)
+    LkState lk{(lane < (int)p.top) ? 0ull : ~0ull, 0ull, __int_as_float(0xff800000)};
     uint32_t s = (uint32_t)cw, ph = 0;                            // as in the producers: no 64-bit division per slot
     uint64_t r0 = ((uint64_t)blockIdx.x + (uint64_t)cw * gridDim.x) * p.rows_per_slot;
     const uint64_t r_step = (uint64_t)PF_CONSUMER_WARPS * gridDim.x * p.rows_per_slot;
@@ -593,84 +668,118 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q5_filter_kernel(const Pf
         const uint32_t nr = (uint32_t)(left < p.rows_per_slot ? left : p.rows_per_slot);
         qb_mbar_wait(&full[s], ph);
         const uint8_t* slot = slots + (size_t)s * p.slot_bytes;
-        // four rows per step, two per half-warp (rows r + half and r + 2 + half): two independent sum chains per lane, and one reduction and
-        // one epilogue for four rows
-        for (uint32_t r = 0; r < nr; r += 4) {
-            const uint32_t ra = r + (uint32_t)half, rb = ra + 2;
-            const bool va = ra < nr, vb = rb < nr;
-            const uint8_t* rowa = slot + (size_t)(va ? ra : r) * p.stride;
-            const uint8_t* rowb = slot + (size_t)(vb ? rb : r) * p.stride;
-            int ha = 0, la = 0, hb = 0, lb = 0;
-#pragma unroll
-            for (int c = 0; c < NCH; ++c) {
-                const uint2 xa = *reinterpret_cast<const uint2*>(rowa + a_off + 128 * c);
-                const uint2 xb = *reinterpret_cast<const uint2*>(rowb + a_off + 128 * c);
-                const uint32_t ya = q6_spread(*reinterpret_cast<const uint16_t*>(rowa + b_off + 32 * c));
-                const uint32_t yb = q6_spread(*reinterpret_cast<const uint16_t*>(rowb + b_off + 32 * c));
-                const uint32_t wa[4] = {((xa.x << 1) & 0x1E1E1E1Eu) | (ya & 0x01010101u),        ((xa.x >> 3) & 0x1E1E1E1Eu) | ((ya >> 1) & 0x01010101u),
-                                        ((xa.y << 1) & 0x1E1E1E1Eu) | ((ya >> 2) & 0x01010101u), ((xa.y >> 3) & 0x1E1E1E1Eu) | ((ya >> 3) & 0x01010101u)};
-                const uint32_t wb[4] = {((xb.x << 1) & 0x1E1E1E1Eu) | (yb & 0x01010101u),        ((xb.x >> 3) & 0x1E1E1E1Eu) | ((yb >> 1) & 0x01010101u),
-                                        ((xb.y << 1) & 0x1E1E1E1Eu) | ((yb >> 2) & 0x01010101u), ((xb.y >> 3) & 0x1E1E1E1Eu) | ((yb >> 3) & 0x01010101u)};
-#pragma unroll
-                for (int m = 0; m < 4; ++m) {
-                    ha = __dp4a((int)wa[m], (int)Q.hq[c][m], ha); la = __dp4a((int)wa[m], (int)Q.lq[c][m], la);
-                    hb = __dp4a((int)wb[m], (int)Q.hq[c][m], hb); lb = __dp4a((int)wb[m], (int)Q.lq[c][m], lb);
-                }
-            }
-            // the four half-warp sums in one butterfly: lanes 0-3 of a half end up with sum h w of row a, 4-7 of row b, 8-11 sum l w of row a, 12-15 of row b
-            int x0 = ((hl & 8) ? la : ha) + __shfl_xor_sync(0xFFFFFFFFu, (hl & 8) ? ha : la, 8);
-            int x1 = ((hl & 8) ? lb : hb) + __shfl_xor_sync(0xFFFFFFFFu, (hl & 8) ? hb : lb, 8);
-            int v = ((hl & 4) ? x1 : x0) + __shfl_xor_sync(0xFFFFFFFFu, (hl & 4) ? x0 : x1, 4);
-            v += __shfl_xor_sync(0xFFFFFFFFu, v, 2);
-            v += __shfl_xor_sync(0xFFFFFFFFu, v, 1);
-            const int lsum = __shfl_xor_sync(0xFFFFFFFFu, v, 8);
-            bool pass = false;
-            uint4 ent;
-            float rho6;
-            if ((hl == 0 && va) || (hl == 4 && vb)) {
-                const uint8_t* row = hl ? rowb : rowa;
-                const float* meta = reinterpret_cast<const float*>(row + meta_off);
-                const float sr = meta[0], rho5 = meta[1];
-                const float H5 = (float)(4 * v - corr_h5), L5 = (float)(4 * lsum - corr_l5);     // exact: integers below 2^24
-                const float app = __fmul_rn(sr, __fmul_rn(sq_half, __fmaf_rn(L5, k254, H5)));
-                const float up = __fadd_ru(app, fminf(__fmul_ru(sr, Q.e1_5), __fmaf_ru(rho5, Q.t2a, Q.t2b)));   // an upper bound of the exact score (up to slack_q)
-                if (!(up < Q.thr_adj)) {
-                    const uint32_t id = (uint32_t)(r0 + (hl ? rb : ra));
-                    bool dead = false;
-                    if (p.deleted) dead = (p.deleted[id >> 5] >> (id & 31)) & 1u;
-                    if (p.deleted2) dead = dead || ((p.deleted2[id >> 5] >> (id & 31)) & 1u);
-                    pass = !dead;
-                    ent = make_uint4(id, (uint32_t)(2 * v - corr_h), (uint32_t)(2 * lsum - corr_l), __float_as_uint(sr));
-                    rho6 = meta[2];
-                }
-            }
-            // one atomic per warp step that lets a row through (lanes 0, 4, 16 and 20 decide)
-            const unsigned int passed = __ballot_sync(0xFFFFFFFFu, pass);
-            if (passed) {
-                unsigned int base = 0;
-                if (lane == 0) base = atomicAdd(p.list_cnt, (unsigned int)__popc(passed));
-                base = __shfl_sync(0xFFFFFFFFu, base, 0);
-                if (pass) {
-                    const unsigned int pos = base + (unsigned int)__popc(passed & ((1u << lane) - 1u));
-                    if (pos < p.list_cap) { p.list[pos] = ent; p.list_rho[pos] = rho6; }
-                }
-            }
-        }
+        // a warp's tiles ascend: the sample tiles come first, and the loop after them does no top-k work
+        if (r0 < p.sample_rows) q5_tile<NCH, true>(p, Q, slot, nr, r0, lane, lk, lk_queue + cw * 4, &lk_count[cw]);
+        else q5_tile<NCH, false>(p, Q, slot, nr, r0, lane, lk, lk_queue + cw * 4, &lk_count[cw]);
         __syncwarp();
         if (lane == 0) qb_mbar_arrive(&empty[s]);
         s += PF_CONSUMER_WARPS;
         if (s >= p.n_slots) { s -= p.n_slots; ph ^= 1u; }
     }
+    // CTA merge of the eight lists (consumer warps only, named barrier), exact scores of its best `top` by four warps (one 8-lane group per
+    // row), those keys ranked into the CTA's list, and the merge of all lists in the last CTA
+    if (lane < QB_LOCALK_SLOTS) lists[cw * QB_LOCALK_SLOTS + lane] = (lk.my_key == ~0ull) ? 0ull : lk.my_key;
+    asm volatile("bar.sync 1, %0;" ::"n"(PF_CONSUMER_WARPS * 32) : "memory");
+    if (cw == 0) lk_cta_sort(lists, lane);
+    asm volatile("bar.sync 1, %0;" ::"n"(PF_CONSUMER_WARPS * 32) : "memory");
+    if (cw < QB_LOCALK_SLOTS / 4) {
+        const int i = cw * 4 + (lane >> 3);
+        const unsigned long long k = (i < (int)p.top) ? lists[i] : 0ull;
+        const uint32_t row = k ? qb_key_id(k) : 0u;
+        const float sc = qbs::score_avx_group8<qbs::M_DOT>(reinterpret_cast<const float*>(p.f32_rows + (size_t)row * p.f32_stride), p.q, p.dim, lane & 7);
+        if ((lane & 7) == 0) ex[i] = k ? qb_pack_key(sc, row + p.id_base) : 0ull;
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(PF_CONSUMER_WARPS * 32) : "memory");
+    if (cw == 0) {
+        if (lane < QB_LOCALK_SLOTS) {
+            const unsigned long long k = ex[lane];
+            int rank = 0;                                          // descending; equal (empty) keys keep their order
+#pragma unroll
+            for (int j = 0; j < QB_LOCALK_SLOTS; ++j) rank += (ex[j] > k || (ex[j] == k && j < lane)) ? 1 : 0;
+            p.cta_keys[(unsigned long long)blockIdx.x * QB_LOCALK_SLOTS + rank] = k;
+        }
+        lk_last_cta_merge(p.cta_keys, p.top, p.samp_out, p.samp_cnt, p.samp_ticket, lane);
+    }
 }
 
-// Stage 2: the 6-bit test of the first-stage list, completed from the side plane.  One thread per entry, a grid-stride loop over the count
-// stage 1 left on the device; the query's packed int8 levels in shared memory, read by every thread of a warp at once.  The last CTA to read the
-// count resets it for the next query.  An overflowing list leaves the candidate count above cap, so that the finish kernel raises the fallback flag.
+// Stage 2: rows whose bound reaches the sample threshold, not deleted, to the first-stage list (row ids).  A CTA compacts 16 rows per thread
+// per step with ONE atomic: 1-3 % of the rows pass, spread evenly, so an atomic per warp step would meet a pass almost every time, and tens of
+// thousands of atomics on one counter serialise.  More rows than list_cap leave the count above it: stage 3 then raises the fallback.
+constexpr int PF_COMPACT_THREADS = 256;
+template <int NCH>
+__global__ void __launch_bounds__(PF_COMPACT_THREADS) dense_q5_compact_kernel(const Pf6Params p) {
+    constexpr int UNROLL = 4;                                     // float4 loads in flight per thread
+    constexpr int WARPS = PF_COMPACT_THREADS / 32;
+    __shared__ float s_thr;
+    __shared__ unsigned int s_warp[WARPS], s_base;
+    if (threadIdx.x < 32) {
+        Q6Query<NCH> Q;
+        q6_query<NCH>(p, threadIdx.x & 15, Q);
+        if (threadIdx.x == 0) s_thr = Q.thr_adj;
+    }
+    __syncthreads();
+    const float thr_adj = s_thr;                                  // NaN (a non-finite query): every row passes
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint64_t n4 = (p.n_rows + 3) / 4, step = (uint64_t)gridDim.x * PF_COMPACT_THREADS * UNROLL;
+    for (uint64_t b = (uint64_t)blockIdx.x * PF_COMPACT_THREADS * UNROLL; b < n4; b += step) {     // uniform per CTA
+        float4 u4[UNROLL];
+#pragma unroll
+        for (int j = 0; j < UNROLL; ++j) {
+            const uint64_t i = b + (uint64_t)j * PF_COMPACT_THREADS + threadIdx.x;
+            u4[j] = (i < n4) ? __ldcs(reinterpret_cast<const float4*>(p.up5) + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+        uint32_t mask = 0;                                        // bit 4 j + k: row 4 (b + j * threads + tid) + k
+#pragma unroll
+        for (int j = 0; j < UNROLL; ++j) {
+            const uint64_t i = b + (uint64_t)j * PF_COMPACT_THREADS + threadIdx.x;
+            const float u[4] = {u4[j].x, u4[j].y, u4[j].z, u4[j].w};
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const uint64_t row = 4 * i + k;
+                if (row < p.n_rows && !(u[k] < thr_adj)) {
+                    const uint32_t id = (uint32_t)row;
+                    bool dead = false;
+                    if (p.deleted) dead = (p.deleted[id >> 5] >> (id & 31)) & 1u;
+                    if (p.deleted2) dead = dead || ((p.deleted2[id >> 5] >> (id & 31)) & 1u);
+                    mask |= dead ? 0u : 1u << (4 * j + k);
+                }
+            }
+        }
+        const int c = __popc(mask);
+        int incl = c;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xFFFFFFFFu, incl, o); if (lane >= o) incl += t; }
+        if (lane == 31) s_warp[warp] = (unsigned int)incl;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            unsigned int total = 0;
+#pragma unroll
+            for (int w = 0; w < WARPS; ++w) { const unsigned int t = s_warp[w]; s_warp[w] = total; total += t; }
+            s_base = total ? atomicAdd(p.list_cnt, total) : 0u;
+        }
+        __syncthreads();
+        if (mask) {
+            unsigned int pos = s_base + s_warp[warp] + (unsigned int)(incl - c);
+            for (uint32_t m = mask; m; m &= m - 1) {
+                const int bit = __ffs((int)m) - 1;
+                if (pos < p.list_cap) p.list[pos] = (uint32_t)(4 * (b + (uint64_t)(bit >> 2) * PF_COMPACT_THREADS + threadIdx.x) + (bit & 3));
+                ++pos;
+            }
+        }
+        __syncthreads();                                          // s_warp / s_base are rewritten by the next step
+    }
+}
+
+// Stage 3: the 6-bit test of the first-stage list.  Half a warp per entry recomputes the exact 6-bit sums H = sum_i h_i c_i, L likewise, from
+// the main record and the side plane: u = c + 31 = 2w + e is a dp4a operand, and H = sum h u - 31 sum h.  The test is the one of the 6-bit
+// plane above.  The query's packed int8 levels are staged once per CTA in shared memory.  The last CTA to read the list's count resets it for
+// the next query.  An overflowing list leaves the candidate count above cap, so that the finish kernel raises the fallback flag.
 constexpr int PF_RESCREEN_THREADS = 256;
 template <int NCH>
 __global__ void __launch_bounds__(PF_RESCREEN_THREADS) dense_q6_rescreen_kernel(const Pf6Params p) {
     __shared__ uint4 s_hq[NCH * 16], s_lq[NCH * 16];             // chunk v: the query bytes of dims 16v + 4m + j in word m
     __shared__ float s_k[5];
+    __shared__ int s_corr[2];
     __shared__ unsigned int s_n;
     if (threadIdx.x == 0) {
         s_n = *reinterpret_cast<volatile unsigned int*>(p.list_cnt);
@@ -688,7 +797,10 @@ __global__ void __launch_bounds__(PF_RESCREEN_THREADS) dense_q6_rescreen_kernel(
                 s_lq[c * 16 + hl] = make_uint4(Q.lq[c][0], Q.lq[c][1], Q.lq[c][2], Q.lq[c][3]);
             }
         }
-        if (threadIdx.x == 0) { s_k[0] = Q.sq; s_k[1] = Q.e1; s_k[2] = Q.t2a; s_k[3] = Q.t2b; s_k[4] = Q.thr_adj; }
+        if (threadIdx.x == 0) {
+            s_k[0] = Q.sq; s_k[1] = Q.e1; s_k[2] = Q.t2a; s_k[3] = Q.t2b; s_k[4] = Q.thr_adj;
+            s_corr[0] = 31 * Q.sum_h; s_corr[1] = 31 * Q.sum_l;
+        }
     }
     __syncthreads();
     const unsigned int n1 = s_n;
@@ -697,57 +809,77 @@ __global__ void __launch_bounds__(PF_RESCREEN_THREADS) dense_q6_rescreen_kernel(
         return;
     }
     const float sq = s_k[0], e1 = s_k[1], t2a = s_k[2], t2b = s_k[3], thr_adj = s_k[4];
+    const int corr_h = s_corr[0], corr_l = s_corr[1];
     const float k254 = 1.0f / 254.0f;
-    const uint32_t lo_b = q6_lo_stride(p.d_pad);
-    for (uint32_t e = blockIdx.x * blockDim.x + threadIdx.x; e < n1; e += gridDim.x * blockDim.x) {
-        const uint4 ent = __ldcg(p.list + e);
-        const uint4* lo = reinterpret_cast<const uint4*>(p.lo + (size_t)ent.x * lo_b);
-        uint4 t[NCH * 2];                                          // 128 dimensions each
+    const int lane = threadIdx.x & 31, half = lane >> 4, hl = lane & 15;
+    uint32_t hq[NCH][4], lq[NCH][4];
 #pragma unroll
-        for (int k = 0; k < NCH * 2; ++k) t[k] = (k * 128 < (int)p.d_pad) ? __ldg(lo + k) : make_uint4(0, 0, 0, 0);
+    for (int c = 0; c < NCH; ++c) {
+        const uint4 h = s_hq[c * 16 + hl], l = s_lq[c * 16 + hl];
+        hq[c][0] = h.x; hq[c][1] = h.y; hq[c][2] = h.z; hq[c][3] = h.w;
+        lq[c][0] = l.x; lq[c][1] = l.y; lq[c][2] = l.z; lq[c][3] = l.w;
+    }
+    const uint32_t n16 = p.d_pad / 16, lo_b = q6_lo_stride(p.d_pad);
+    const uint32_t a_off = (uint32_t)hl * 8, b_off = p.d_pad / 2 + (uint32_t)hl * 2, meta_off = p.d_pad / 2 + p.d_pad / 8;
+    const uint32_t warps = gridDim.x * (blockDim.x >> 5), gw = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    for (uint32_t e0 = 2 * gw; e0 < n1; e0 += 2 * warps) {       // uniform per warp: two entries per step
+        const uint32_t e = e0 + (uint32_t)half;
+        const bool valid = e < n1;
+        const uint32_t row = __ldcg(p.list + (valid ? e : e0));
+        const uint8_t* rec = p.rows + (size_t)row * p.stride;
+        const uint8_t* lo = p.lo + (size_t)row * lo_b;
         int hs = 0, ls = 0;
 #pragma unroll
-        for (int k = 0; k < NCH * 2; ++k) {
-            if (k * 128 >= (int)p.d_pad) break;
-            const uint32_t tw[4] = {t[k].x, t[k].y, t[k].z, t[k].w};
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const uint32_t y = q6_spread((tw[i >> 1] >> (16 * (i & 1))) & 0xFFFFu);
-                const uint4 hq = s_hq[k * 8 + i], lq = s_lq[k * 8 + i];
-                const uint32_t hw[4] = {hq.x, hq.y, hq.z, hq.w}, lw[4] = {lq.x, lq.y, lq.z, lq.w};
+        for (int c = 0; c < NCH; ++c) {
+            if ((uint32_t)(c * 16 + hl) < n16) {
+                const uint2 x = __ldg(reinterpret_cast<const uint2*>(rec + a_off + 128 * c));
+                const uint32_t y = q6_spread(__ldg(reinterpret_cast<const unsigned short*>(rec + b_off + 32 * c)));
+                const uint32_t z = q6_spread(__ldg(reinterpret_cast<const unsigned short*>(lo + 2 * hl + 32 * c)));
+                const uint32_t w[4] = {((x.x << 1) & 0x1E1E1E1Eu) | (y & 0x01010101u),        ((x.x >> 3) & 0x1E1E1E1Eu) | ((y >> 1) & 0x01010101u),
+                                       ((x.y << 1) & 0x1E1E1E1Eu) | ((y >> 2) & 0x01010101u), ((x.y >> 3) & 0x1E1E1E1Eu) | ((y >> 3) & 0x01010101u)};
 #pragma unroll
                 for (int m = 0; m < 4; ++m) {
-                    const uint32_t b = (y >> m) & 0x01010101u;
-                    hs = __dp4a((int)b, (int)hw[m], hs); ls = __dp4a((int)b, (int)lw[m], ls);
+                    const uint32_t u = (w[m] << 1) | ((z >> m) & 0x01010101u);
+                    hs = __dp4a((int)u, (int)hq[c][m], hs); ls = __dp4a((int)u, (int)lq[c][m], ls);
                 }
             }
         }
-        const float H = (float)((int)ent.y + hs), L = (float)((int)ent.z + ls);                  // exact: integers below 2^24
-        const float sr = __uint_as_float(ent.w), rho6 = __ldcg(p.list_rho + e);
-        const float app = __fmul_rn(sr, __fmul_rn(sq, __fmaf_rn(L, k254, H)));
-        const float up = __fadd_ru(app, fminf(__fmul_ru(sr, e1), __fmaf_ru(rho6, t2a, t2b)));     // an upper bound of the exact score (up to slack_q)
-        if (!(up < thr_adj)) {
-            const unsigned int pos = atomicAdd(p.cnt, 1u);
-            if (pos < p.cap) p.cand[pos] = ent.x;
+        // lanes 0-7 of a half end up with sum h u, 8-15 with sum l u
+        int v = ((hl & 8) ? ls : hs) + __shfl_xor_sync(0xFFFFFFFFu, (hl & 8) ? hs : ls, 8);
+        v += __shfl_xor_sync(0xFFFFFFFFu, v, 4);
+        v += __shfl_xor_sync(0xFFFFFFFFu, v, 2);
+        v += __shfl_xor_sync(0xFFFFFFFFu, v, 1);
+        const int lsum = __shfl_xor_sync(0xFFFFFFFFu, v, 8);
+        if (hl == 0 && valid) {
+            const float* meta = reinterpret_cast<const float*>(rec + meta_off);
+            const float H = (float)(v - corr_h), L = (float)(lsum - corr_l);                    // exact: integers below 2^24
+            const float sr = __ldg(meta), rho6 = __ldg(meta + 2);
+            const float app = __fmul_rn(sr, __fmul_rn(sq, __fmaf_rn(L, k254, H)));
+            const float up = __fadd_ru(app, fminf(__fmul_ru(sr, e1), __fmaf_ru(rho6, t2a, t2b)));     // an upper bound of the exact score (up to slack_q)
+            if (!(up < thr_adj)) {
+                const unsigned int pos = atomicAdd(p.cnt, 1u);
+                if (pos < p.cap) p.cand[pos] = row;
+            }
         }
     }
 }
 
-// the ring of any filter kernel above: slots of ~PF_SLOT_BYTES (an even number of rows), as many as fit, one CTA per SM
+// the ring of any filter kernel above: slots of ~PF_SLOT_BYTES (an even number of rows), as many as fit, one CTA per SM; `extra_smem` bytes
+// follow the ring's barriers
 template <typename P>
-qb_status launch_ring(void (*kernel)(P), P& p, int sm_count, cudaStream_t stream) {
+qb_status launch_ring(void (*kernel)(P), P& p, int sm_count, cudaStream_t stream, size_t extra_smem = 0) {
     const uint32_t kMaxSmem = 227 * 1024;
     const uint32_t target = qb_opt().prefilter_slot_bytes ? qb_opt().prefilter_slot_bytes : PF_SLOT_BYTES;
     uint32_t rps = (target / p.stride) & ~1u;
     if (rps < 2) rps = 2;
     p.rows_per_slot = rps;
     p.slot_bytes = rps * p.stride;
-    uint32_t n_slots = (kMaxSmem - 2048) / p.slot_bytes;
+    uint32_t n_slots = (kMaxSmem - 2048 - (uint32_t)extra_smem) / p.slot_bytes;
     if (n_slots > 64) n_slots = 64;
     n_slots = (n_slots / PF_CONSUMER_WARPS) * PF_CONSUMER_WARPS;
     QB_CHECK(n_slots >= (uint32_t)PF_CONSUMER_WARPS, QB_ERR_INVALID, "prefilter: rows too wide for the ring");
     p.n_slots = n_slots;
-    const size_t smem = (size_t)n_slots * p.slot_bytes + (size_t)n_slots * 16;
+    const size_t smem = (size_t)n_slots * p.slot_bytes + (size_t)n_slots * 16 + extra_smem;
     QB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem));
     const uint64_t n_tiles = ceil_div_u64(p.n_rows, p.rows_per_slot);
     const unsigned grid = (unsigned)std::min<uint64_t>(n_tiles, (uint64_t)sm_count);
@@ -901,15 +1033,16 @@ bool qb_f32_prefilter_usable(qb_storage* s, uint64_t n_rows, uint32_t top, cudaS
 }
 
 // d_q = preprocessed query; the exact top-`top` of the storage lands in d_out / d_out_cnt.  `a` = the scan arguments of the exact
-// in-kernel-top-k path (emit.cand / final_out / done_counter set up by the caller); scratch = c->d_pf (see qb_f32_prefilter_scratch_bytes).
-size_t qb_f32_prefilter_scratch_bytes() { return 256 + (size_t)PF_CAP * 12 + (size_t)PF_LIST_CAP * 20; }
+// in-kernel-top-k path (emit.cand / final_out / done_counter set up by the caller); scratch = c->d_pf (see qb_f32_prefilter_scratch_bytes),
+// d_up5 = s->count floats (rounded up to 4) for the 6-bit plane's per-row bounds.
+size_t qb_f32_prefilter_scratch_bytes() { return 256 + (size_t)PF_CAP * 12 + (size_t)PF_LIST_CAP * 4; }
 
-qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t top, void* d_scratch, unsigned int* d_n_fallbacks, qb_scored_point* d_out, uint32_t* d_out_cnt,
-                                  cudaEvent_t prof0, cudaEvent_t prof1, cudaStream_t stream) {
+qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t top, void* d_scratch, float* d_up5, unsigned int* d_n_fallbacks, qb_scored_point* d_out,
+                                  uint32_t* d_out_cnt, cudaEvent_t prof0, cudaEvent_t prof1, cudaStream_t stream) {
     uint8_t* sc = reinterpret_cast<uint8_t*>(d_scratch);
     // scratch: [0,16) cnt | [16,32) fallback flag | [32,48) finish ticket | [48,64) sample count | [64, 64+16*8) sample top-k |
-    // [192,208) first-stage count | [208,224) its ticket | from 256: per-CTA top-k keys | candidate rows | first-stage list | its rho6 column
-    // (the first 256 bytes are zeroed once, the kernels reset their counters)
+    // [192,208) first-stage count | [208,224) its ticket | [224,240) ticket of the sample merge | from 256: per-CTA top-k keys |
+    // candidate rows | first-stage list  (the first 256 bytes are zeroed once, the kernels reset their counters)
     unsigned int* d_cnt = reinterpret_cast<unsigned int*>(sc);
     unsigned int* d_fallback = reinterpret_cast<unsigned int*>(sc + 16);
     uint32_t* d_samp_cnt = reinterpret_cast<uint32_t*>(sc + 48);
@@ -917,14 +1050,55 @@ qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t t
     unsigned int* d_ticket = reinterpret_cast<unsigned int*>(sc + 32);
     unsigned int* d_list_cnt = reinterpret_cast<unsigned int*>(sc + 192);
     unsigned int* d_list_ticket = reinterpret_cast<unsigned int*>(sc + 208);
+    unsigned int* d_samp_ticket = reinterpret_cast<unsigned int*>(sc + 224);
     unsigned long long* d_keys = reinterpret_cast<unsigned long long*>(sc + 256);
     uint32_t* d_cand = reinterpret_cast<uint32_t*>(d_keys + PF_CAP);
-    uint4* d_list = reinterpret_cast<uint4*>(d_cand + PF_CAP);
-    float* d_list_rho = reinterpret_cast<float*>(d_list + PF_LIST_CAP);
+    uint32_t* d_list = d_cand + PF_CAP;
     const uint64_t n = s->count;
     // the candidate list holds n / 32 rows (at most PF_CAP): re-scoring reads a whole f32 row per candidate, and past 1/32 of the rows the
     // exact scan that a longer list would save is no longer far off
     const uint32_t cap = (uint32_t)std::min<uint64_t>(PF_CAP, n / 32);
+    const float* d_q = reinterpret_cast<const float*>(a.d_q_enc);
+    const int plane = pf_plane();
+    uint64_t n_slots = 0;
+    if (plane == 0 && s->q6_ready && s->q6_usable) {
+        // 1. stage 1 over the whole 6-bit plane: every row's 5-bit bound, and the exact top-k of the best rows of a prefix by approximate
+        //    score as the threshold sample.  The prefix is n / 8 rows: the threshold is then the top-k of 1.25 M rows at 10 M rows, and the
+        //    tests that delete all but a few rows of the first third of a storage still find fewer than k live rows in it.
+        uint64_t sample = n / 8;
+        if (qb_opt().sample_rows) sample = std::min<uint64_t>(n, std::max<uint64_t>(16384, qb_opt().sample_rows & ~(uint64_t)3));   // experiments
+        Pf6Params p6{};
+        p6.rows = s->d_q6; p6.lo = s->d_q6_lo; p6.stride = s->q6_row_b; p6.d_pad = (uint32_t)round_up_u64(s->dim, 32); p6.dim = s->dim; p6.n_rows = n;
+        p6.q = d_q; p6.samp_out = d_samp; p6.samp_cnt = d_samp_cnt; p6.top = top; p6.max_norm_bits = s->d_q6_meta;
+        p6.up5 = d_up5; p6.sample_rows = sample;
+        p6.f32_rows = reinterpret_cast<const uint8_t*>(s->d_rows); p6.f32_stride = s->row_stride; p6.id_base = a.emit.id_base;
+        p6.cta_keys = d_keys; p6.samp_ticket = d_samp_ticket;
+        // 2. the rows whose bound reaches the threshold, up to PF_LIST_CAP of them: 1-3 % of the rows on unit-Gaussian data at dim 768, but
+        //    far more on wider rows or on a storage whose prefix ranks badly
+        p6.list = d_list; p6.list_cnt = d_list_cnt; p6.list_ticket = d_list_ticket; p6.list_cap = (uint32_t)std::min<uint64_t>(PF_LIST_CAP, n);
+        p6.cand = d_cand; p6.cnt = d_cnt; p6.cap = cap; p6.deleted = a.emit.deleted; p6.deleted2 = a.emit.deleted2;
+        p6.l2_keep = ((uint64_t)n * p6.stride <= (64ull << 20)) ? 1 : 0;
+        const unsigned cp_grid = (unsigned)s->sm_count * 8, rs_grid = (unsigned)s->sm_count * 4;
+        QB_CHECK((uint64_t)s->sm_count * QB_LOCALK_SLOTS <= PF_CAP, QB_ERR_INVALID, "prefilter: %d CTAs exceed the key buffer", s->sm_count);
+        if (prof0) cudaEventRecord(prof0, stream);
+        switch ((p6.d_pad + 255) / 256) {
+            case 1: QB_TRY(launch_ring(dense_q5_filter_kernel<1>, p6, s->sm_count, stream, PF_SAMPLE_SMEM)); break;
+            case 2: QB_TRY(launch_ring(dense_q5_filter_kernel<2>, p6, s->sm_count, stream, PF_SAMPLE_SMEM)); break;
+            case 3: QB_TRY(launch_ring(dense_q5_filter_kernel<3>, p6, s->sm_count, stream, PF_SAMPLE_SMEM)); break;
+            default: QB_TRY(launch_ring(dense_q5_filter_kernel<4>, p6, s->sm_count, stream, PF_SAMPLE_SMEM)); break;
+        }
+        if (prof1) cudaEventRecord(prof1, stream);
+        // 2b. the 6-bit test of the listed rows
+        switch ((p6.d_pad + 255) / 256) {
+            case 1: dense_q5_compact_kernel<1><<<cp_grid, PF_COMPACT_THREADS, 0, stream>>>(p6); dense_q6_rescreen_kernel<1><<<rs_grid, PF_RESCREEN_THREADS, 0, stream>>>(p6); break;
+            case 2: dense_q5_compact_kernel<2><<<cp_grid, PF_COMPACT_THREADS, 0, stream>>>(p6); dense_q6_rescreen_kernel<2><<<rs_grid, PF_RESCREEN_THREADS, 0, stream>>>(p6); break;
+            case 3: dense_q5_compact_kernel<3><<<cp_grid, PF_COMPACT_THREADS, 0, stream>>>(p6); dense_q6_rescreen_kernel<3><<<rs_grid, PF_RESCREEN_THREADS, 0, stream>>>(p6); break;
+            default: dense_q5_compact_kernel<4><<<cp_grid, PF_COMPACT_THREADS, 0, stream>>>(p6); dense_q6_rescreen_kernel<4><<<rs_grid, PF_RESCREEN_THREADS, 0, stream>>>(p6); break;
+        }
+        QB_LAUNCHED();
+        QB_LAUNCHED();
+        QB_CUDA(cudaGetLastError());
+    } else {
     // 1. exact top-k of a prefix
     // 1/64 of the rows, 2^14..2^17: a shard of a sharded search (1.25M rows at N = 8) should not spend a fifth of its step on the sample
     uint64_t sample = std::min<uint64_t>(131072, std::max<uint64_t>(16384, (n / 64) & ~(uint64_t)3));
@@ -932,39 +1106,10 @@ qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t t
     QbScanArgs as = a;
     as.row_begin = 0; as.row_end = sample;
     as.emit.final_out = d_samp; as.emit.final_count = d_samp_cnt; as.emit.run_if = nullptr;
-    uint64_t n_slots = 0;
     QB_TRY(qb_dense_f32_scan_localk(s, as, top, &n_slots, stream, 4096));
     QB_CHECK(n_slots != 0 && n_slots <= 4096, QB_ERR_CUDA, "prefilter: the sample scan did not launch (%llu slots)", (unsigned long long)n_slots);
     // 2. filter pass over the whole shadow plane
-    const float* d_q = reinterpret_cast<const float*>(a.d_q_enc);
-    const int plane = pf_plane();
-    if (plane == 0 && s->q6_ready && s->q6_usable) {
-        Pf6Params p6{};
-        p6.rows = s->d_q6; p6.lo = s->d_q6_lo; p6.stride = s->q6_row_b; p6.d_pad = (uint32_t)round_up_u64(s->dim, 32); p6.dim = s->dim; p6.n_rows = n;
-        p6.q = d_q; p6.samp_out = d_samp; p6.samp_cnt = d_samp_cnt; p6.top = top; p6.max_norm_bits = s->d_q6_meta;
-        // every row up to PF_LIST_CAP rows: the 5-bit stage lets 1-3 % of the rows through on unit-Gaussian data at dim 768 with a 131 072-row
-        // sample, but far more on wider rows or with the 16 384-row sample of a smaller storage
-        p6.list = d_list; p6.list_rho = d_list_rho; p6.list_cnt = d_list_cnt; p6.list_ticket = d_list_ticket; p6.list_cap = (uint32_t)std::min<uint64_t>(PF_LIST_CAP, n);
-        p6.cand = d_cand; p6.cnt = d_cnt; p6.cap = cap; p6.deleted = a.emit.deleted; p6.deleted2 = a.emit.deleted2;
-        p6.l2_keep = ((uint64_t)n * p6.stride <= (64ull << 20)) ? 1 : 0;
-        const unsigned rs_grid = (unsigned)s->sm_count * 4;
-        if (prof0) cudaEventRecord(prof0, stream);
-        switch ((p6.d_pad + 255) / 256) {
-            case 1: QB_TRY(launch_ring(dense_q5_filter_kernel<1>, p6, s->sm_count, stream)); break;
-            case 2: QB_TRY(launch_ring(dense_q5_filter_kernel<2>, p6, s->sm_count, stream)); break;
-            case 3: QB_TRY(launch_ring(dense_q5_filter_kernel<3>, p6, s->sm_count, stream)); break;
-            default: QB_TRY(launch_ring(dense_q5_filter_kernel<4>, p6, s->sm_count, stream)); break;
-        }
-        if (prof1) cudaEventRecord(prof1, stream);
-        switch ((p6.d_pad + 255) / 256) {
-            case 1: dense_q6_rescreen_kernel<1><<<rs_grid, PF_RESCREEN_THREADS, 0, stream>>>(p6); break;
-            case 2: dense_q6_rescreen_kernel<2><<<rs_grid, PF_RESCREEN_THREADS, 0, stream>>>(p6); break;
-            case 3: dense_q6_rescreen_kernel<3><<<rs_grid, PF_RESCREEN_THREADS, 0, stream>>>(p6); break;
-            default: dense_q6_rescreen_kernel<4><<<rs_grid, PF_RESCREEN_THREADS, 0, stream>>>(p6); break;
-        }
-        QB_LAUNCHED();
-        QB_CUDA(cudaGetLastError());
-    } else if (plane == 2 && s->q8_ready && s->q8_usable) {
+    if (plane == 2 && s->q8_ready && s->q8_usable) {
         Pf8Params p8{};
         p8.rows = reinterpret_cast<const uint8_t*>(s->d_q8); p8.stride = s->q8_row_b; p8.dim = s->dim; p8.n_rows = n;
         p8.q = d_q; p8.samp_out = d_samp; p8.samp_cnt = d_samp_cnt; p8.top = top; p8.max_norm_bits = s->d_q8_meta;
@@ -994,6 +1139,7 @@ qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t t
         default: QB_TRY(launch_ring(dense_bf16_filter_kernel<4>, p, s->sm_count, stream)); break;
     }
     if (prof1) cudaEventRecord(prof1, stream);
+    }
     }
     // 3. exact scores + top-k of the survivors (or the fallback flag): one CTA per SM, enough of them that a CTA's share fits in 32 KB
     const unsigned fin_grid = (unsigned)std::max<uint32_t>((uint32_t)s->sm_count, ceil_div_u64(PF_CAP, 4096));

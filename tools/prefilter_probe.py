@@ -2,7 +2,9 @@
 """prefilter_probe.py [rows] [dim] — single-query searches over one synthetic cosine storage (generated on the device), device-timed, for several
 ring-slot sizes / producer-warp counts of the shadow-plane filter kernels and the three planes; prints one JSON line.  Results of every variant are compared with the exact scan.
 "candidates" counts, per query, the rows each integer plane's bound lets through (the kernels' bounds restated in torch on the same rows, f64 where they round up):
-on the 6-bit plane, the rows of the 5-bit first stage (q6_stage1) and those of them the 6-bit second stage keeps (q6_stage2)."""
+on the 6-bit plane, for each candidate size of its threshold sample (n / 16, n / 8, n / 4 rows), the rows of the 5-bit first stage (q6_stage1) and those of
+them the 6-bit test keeps (q6_stage2), with the threshold restated as the exact top-k of the prefix (the kernel ranks the prefix by its approximate score
+first, so its threshold can only be lower, by the ranking error); on the int8 plane, with the f32 sample of 1/64 of the rows it keeps."""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -67,7 +69,8 @@ out["fallbacks"] = int(st.search_stats()[1])
 
 
 def candidate_counts(nq=16, top=10):
-    """Rows with upper bound >= thr_q - slack_q on the 6-bit plane's two stages and the int8 plane, thr_q = the exact top-`top` score of the sample prefix."""
+    """Rows with upper bound >= thr_q - slack_q on the 6-bit plane's two stages (per prefix size) and the int8 plane, thr_q = the exact top-`top`
+    score of the sample prefix."""
     qd = torch.from_numpy(queries[:nq]).to(dev).double()
     qd = (qd / qd.norm(dim=1, keepdim=True)).float().double()          # cosine queries are normalised
     qmax = qd.abs().amax(1, keepdim=True)
@@ -76,28 +79,41 @@ def candidate_counts(nq=16, top=10):
     h = y.round().clamp(-127, 127)
     l = ((y - h) * 254).round().clamp(-127, 127)
     q1, qn = qd.abs().sum(1), qd.norm(dim=1)
-    sample = min(131072, max(16384, rows // 64))
+    prefixes = {"n/16": rows // 16, "n/8": rows // 8, "n/4": rows // 4}
+    sample8 = min(131072, max(16384, rows // 64))
     e1 = q1 * (0.5 + 2.0 ** -13) + sq[:, 0] * dim * 0.066
     e1_5 = q1 * (1 + 2.0 ** -13) + sq[:, 0] * dim * 0.066
     e2 = sq[:, 0] * dim ** 0.5 * 0.00202
     e8 = q1 * (0.5 + 2.0 ** -13) + sq[:, 0] * dim * 0.27
-    g = torch.Generator(device=dev); g.manual_seed(42)
-    chunks, mxn = [], 0.0
-    for r0 in range(0, rows, 500_000):
-        n = min(500_000, rows - r0)
-        x = torch.randn((n, dim), generator=g, device=dev, dtype=torch.float32)
-        check(lib().qb_metric_preprocess_device(0, int(qb.Distance.Cosine), dim, n, vp(x.data_ptr()), dim * 4))
+    g = torch.Generator(device=dev)
+
+    def chunks():
+        g.manual_seed(42)
+        for r0 in range(0, rows, 500_000):
+            n = min(500_000, rows - r0)
+            x = torch.randn((n, dim), generator=g, device=dev, dtype=torch.float32)
+            check(lib().qb_metric_preprocess_device(0, int(qb.Distance.Cosine), dim, n, vp(x.data_ptr()), dim * 4))
+            yield r0, n, x
+
+    # pass 1: max row norm, and the exact top-`top` of every prefix
+    mxn, best = 0.0, {k: None for k in prefixes}
+    for r0, n, x in chunks():
         mxn = max(mxn, float(x.double().norm(dim=1).max()))
-        chunks.append((r0, n))
+        for k, p in prefixes.items():
+            if r0 < p:
+                s = x[: p - r0].double() @ qd.T
+                best[k] = s if best[k] is None else torch.cat([best[k], s])
+                best[k] = best[k].topk(top, dim=0).values
+        if r0 == 0:
+            thr8 = (x[:sample8].double() @ qd.T).topk(top, dim=0).values[-1]
+    thr = {k: v[-1] for k, v in best.items()}
     slack6 = 2 * (dim * 2.0 ** -22 + 2.0 ** -17) * qn * mxn
     slack8 = (dim * 2.0 ** -22 + 2.0 ** -17) * (1 + dim ** 0.5 / 127) * qn * mxn
-    g.manual_seed(42)
-    thr, c5, c6, c8 = None, *(torch.zeros(nq, dtype=torch.int64, device=dev) for _ in range(3))
-    for r0, n in chunks:
-        x = torch.randn((n, dim), generator=g, device=dev, dtype=torch.float32)
-        check(lib().qb_metric_preprocess_device(0, int(qb.Distance.Cosine), dim, n, vp(x.data_ptr()), dim * 4))
-        if thr is None:
-            thr = (x[:sample].double() @ qd.T).topk(top, dim=0).values[-1]
+    c5 = {k: torch.zeros(nq, dtype=torch.int64, device=dev) for k in prefixes}
+    c6 = {k: torch.zeros(nq, dtype=torch.int64, device=dev) for k in prefixes}
+    c8 = torch.zeros(nq, dtype=torch.int64, device=dev)
+    # pass 2: the bounds of every row against each threshold
+    for r0, n, x in chunks():
         mx = x.abs().amax(1, keepdim=True)
         sr = (mx / 31).double()
         c = (x * (31 / mx)).round().clamp(-31, 31).double()
@@ -106,15 +122,17 @@ def candidate_counts(nq=16, top=10):
         c5c = 2 * torch.div(c + 31, 2, rounding_mode="floor") + 0.5 - 31      # the 5-bit code's reconstruction
         rho5 = (x.double() - sr * c5c).norm(dim=1, keepdim=True)
         up5 = sr * sq.T * (c5c @ h.T + (c5c @ l.T) / 254) + torch.minimum(sr * e1_5, rho5 * (qn + e2) + e2 * mxn)
-        p5 = up5 >= thr - slack6
-        c5 += p5.sum(0)
-        c6 += (p5 & (up6 >= thr - slack6)).sum(0)
+        for k in prefixes:
+            p5 = up5 >= thr[k] - slack6
+            c5[k] += p5.sum(0)
+            c6[k] += (p5 & (up6 >= thr[k] - slack6)).sum(0)
         s8 = (mx / 127).double()
         c = (x * (127 / mx)).round().clamp(-127, 127).double()
         up8 = s8 * (sq.T * (c @ h.T + (c @ l.T) / 254) + e8)
-        c8 += (up8 >= thr - slack8).sum(0)
-        del x, c, rho, up6, up8, c5c, rho5, up5, p5
-    return {"q6_stage1": c5.tolist(), "q6_stage2": c6.tolist(), "int8": c8.tolist(), "sample_rows": sample}
+        c8 += (up8 >= thr8 - slack8).sum(0)
+        del x, c, rho, up6, up8, c5c, rho5, up5
+    return {"q6": {k: {"sample_rows": prefixes[k], "q6_stage1": c5[k].tolist(), "q6_stage2": c6[k].tolist()} for k in prefixes},
+            "int8": c8.tolist(), "int8_sample_rows": sample8}
 
 
 st.close()
