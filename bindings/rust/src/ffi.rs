@@ -99,6 +99,8 @@ extern "C" {
     pub fn qb_comm_stream(c: *mut qb_comm) -> *mut c_void;
     pub fn qb_comm_check(c: *mut qb_comm) -> qb_status;
     pub fn qb_hnsw_create_plain(s: *mut qb_storage, links_bin: *const u8, n_bytes: u64, m: u32, m0: u32, out: *mut *mut qb_hnsw) -> qb_status;
+    pub fn qb_hnsw_create_compressed(s: *mut qb_storage, bytes: *const u8, n_bytes: u64, out: *mut *mut qb_hnsw) -> qb_status;
+    pub fn qb_hnsw_links(g: *const qb_hnsw, level: u32, ids: *const u32, n_ids: u32, cap: u32, out: *mut u32, counts: *mut u32) -> qb_status;
     pub fn qb_hnsw_destroy(g: *mut qb_hnsw);
     pub fn qb_hnsw_info(g: *const qb_hnsw, n_points: *mut u32, levels: *mut u32, hbm_bytes: *mut u64) -> qb_status;
     pub fn qb_hnsw_search_batch(g: *mut qb_hnsw, queries: *const f32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, deleted_bitmap: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters) -> qb_status;

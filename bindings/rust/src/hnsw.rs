@@ -1,6 +1,6 @@
 //! `GraphLayers::search` (lib/segment/src/index/hnsw_index/graph_layers.rs:530-561) for a batch of queries with the traversal on the GPU.
-//! SOURCE ONLY (see ffi.rs).  The graph is handed over as the bytes of `links.bin` in GraphLinksFormat::Plain (graph_links/view.rs:121-135);
-//! compressed graphs are converted once with `GraphLinks::to_edges` + `serialize_graph_links(.., GraphLinksFormatParam::Plain, ..)`.
+//! SOURCE ONLY (see ffi.rs).  The graph is handed over as the bytes of `links.bin`, either in GraphLinksFormat::Compressed (what
+//! the reference writes for every index it builds, view.rs:137-163; decoded on the device) or in GraphLinksFormat::Plain (view.rs:121-135).
 use common::types::{PointOffsetType, ScoredPointOffset};
 
 use super::ffi::*;
@@ -16,6 +16,14 @@ impl<'a> B200Hnsw<'a> {
     pub fn from_plain_links(storage: &'a B200Storage, links_bin: &[u8], m: usize, m0: usize) -> OperationResult<Self> {
         let mut raw = std::ptr::null_mut();
         let st = unsafe { qb_hnsw_create_plain(storage.raw, links_bin.as_ptr(), links_bin.len() as u64, m as u32, m0 as u32, &mut raw) };
+        if st != QB_OK { return Err(OperationError::service_error(last_error())); }
+        Ok(Self { raw, _storage: std::marker::PhantomData })
+    }
+
+    /// `links.bin` in GraphLinksFormat::Compressed; m and m0 come from its header.  CompressedWithVectors is refused.
+    pub fn from_compressed_links(storage: &'a B200Storage, links_bin: &[u8]) -> OperationResult<Self> {
+        let mut raw = std::ptr::null_mut();
+        let st = unsafe { qb_hnsw_create_compressed(storage.raw, links_bin.as_ptr(), links_bin.len() as u64, &mut raw) };
         if st != QB_OK { return Err(OperationError::service_error(last_error())); }
         Ok(Self { raw, _storage: std::marker::PhantomData })
     }

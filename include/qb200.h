@@ -350,12 +350,22 @@ QB_API qb_status qb_comm_check(qb_comm* c);
  * boundary stays available (qb_scorer_*), this entry removes it.
  *
  * links_bin = the bytes of the segment's `links.bin` in GraphLinksFormat::Plain (graph_links/header.rs:9-20,
- * graph_links/view.rs:121-135): HeaderPlain, level offsets, reindex, neighbors, padding, offsets.  (The compressed
- * formats are decoded by the caller, as GraphLinks::to_edges does.)  m / m0 = HnswM (hnsw_index/mod.rs:34-40), both <= 64.
- * The graph is bound to `s` (dense f32 or SQ8; the quantized storage when the segment searches quantized) and must
- * outlive neither it nor its searches. */
+ * graph_links/view.rs:121-135): HeaderPlain, level offsets, reindex, neighbors, padding, offsets.  m / m0 = HnswM
+ * (hnsw_index/mod.rs:34-40), both <= 64.  The graph is bound to `s` (dense f32 or SQ8; the quantized storage when the
+ * segment searches quantized) and must outlive neither it nor its searches. */
 typedef struct qb_hnsw qb_hnsw;
 QB_API qb_status qb_hnsw_create_plain(qb_storage* s, const uint8_t* links_bin, uint64_t n_bytes, uint32_t m, uint32_t m0, qb_hnsw** out);
+/* The same graph from `links.bin` in GraphLinksFormat::Compressed, the format the reference writes for every HNSW index it
+ * builds (graph_links/header.rs:22-34, view.rs:137-163; hnsw/build.rs:548-562).  m / m0 come from the header.  The file is
+ * copied to the device once and decoded there into the arrays qb_hnsw_create_plain uploads; the search is the same.
+ * Every value taken from the file is checked before it is followed: a malformed file returns QB_ERR_INVALID and leaves the
+ * device usable.  CompressedWithVectors (version word ...FF02, inline storage) and m0 > 64 return QB_ERR_UNSUPPORTED. */
+QB_API qb_status qb_hnsw_create_compressed(qb_storage* s, const uint8_t* bytes, uint64_t n_bytes, qb_hnsw** out);
+/* GraphLinks::links (view.rs:238-263) for n_ids points on one level, from the device-resident graph of either loader:
+ * out[i * cap .. i * cap + min(counts[i], cap)) = point ids[i]'s links in the graph's stored order, counts[i] = their full
+ * number.  QB_ERR_INVALID when a point is out of range or its top level is below `level` (view.rs:354-369).  Synchronous. */
+QB_API qb_status qb_hnsw_links(const qb_hnsw* g, uint32_t level, const uint32_t* ids, uint32_t n_ids, uint32_t cap, uint32_t* out /* n_ids x cap */,
+                               uint32_t* counts);
 QB_API void qb_hnsw_destroy(qb_hnsw* g);
 QB_API qb_status qb_hnsw_info(const qb_hnsw* g, uint32_t* n_points, uint32_t* levels, uint64_t* hbm_bytes);
 /*   queries         n_queries x dim raw f32 (Metric::preprocess + encode_query on the device)

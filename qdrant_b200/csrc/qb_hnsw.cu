@@ -26,6 +26,10 @@
 // Graph layout: the reference's plain `links.bin` (graph_links/header.rs:9-20, view.rs:121-135, serializer.rs:53-200) is
 // taken as is for the upper levels (level_offsets, reindex, neighbors, offsets); level 0 — every hop of the beam search —
 // is re-laid at upload as a fixed-stride [n][m0] table so a hop needs ONE coalesced 128-B read instead of offsets -> range.
+// The compressed `links.bin` every current index is written in (GraphLinksFormatParam::Compressed, hnsw/build.rs:548-562) is
+// decoded on the device into exactly those arrays (qb_hnsw_create_compressed, below), so one traversal serves both formats.
+#include <cub/device/device_scan.cuh>
+
 #include <algorithm>
 
 #include "qb_internal.h"
@@ -402,15 +406,17 @@ extern "C" qb_status qb_hnsw_create_plain(qb_storage* s, const uint8_t* links_bi
     const uint8_t* p_re = p_lo + 8 * levels;
     const uint8_t* p_nb = p_re + 4 * n;
     const uint8_t* p_of = p_nb + 4 * n_nb + pad;
+    std::vector<uint64_t> lo(levels + 1);
     {   // level offsets index the offsets table: validate before the device ever follows them
-        std::vector<uint64_t> lo(levels);
         memcpy(lo.data(), p_lo, 8 * levels);
         for (uint64_t l = 0; l < levels; ++l) QB_CHECK(lo[l] < n_off, QB_ERR_INVALID, "hnsw_create_plain: level offset %llu out of range", (unsigned long long)l);
+        lo[levels] = n_off - 1;
     }
     cudaError_t ce = cudaSetDevice(s->device);
     if (ce != cudaSuccess) { qb_set_error("hnsw_create_plain: %s", cudaGetErrorString(ce)); return QB_ERR_CUDA; }
     qb_hnsw* g = new qb_hnsw();
     g->st = s; g->n_points = (uint32_t)n; g->m = m; g->m0 = m0; g->levels = (uint32_t)levels;
+    g->level_offsets_ext = std::move(lo); g->n_offsets = n_off; g->n_neighbors = n_nb;
     bool ok = cudaMalloc(&g->d_links0, std::max<size_t>((size_t)n * m0 * 4, 256)) == cudaSuccess &&
               cudaMalloc(&g->d_level_offsets, std::max<size_t>(8 * levels, 256)) == cudaSuccess &&
               cudaMalloc(&g->d_reindex, std::max<size_t>(4 * n, 256)) == cudaSuccess &&
@@ -431,6 +437,319 @@ extern "C" qb_status qb_hnsw_create_plain(qb_storage* s, const uint8_t* links_bi
     }
     if (ce != cudaSuccess) { qb_set_error("hnsw_create_plain: upload: %s", cudaGetErrorString(ce)); qb_hnsw_destroy(g); return QB_ERR_CUDA; }
     *out = g;
+    return QB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ compressed links.bin
+// GraphLinksFormat::Compressed (graph_links/header.rs:22-34, view.rs:137-163, serializer.rs:62-194):
+//   HeaderCompressed, 64 B little-endian, nothing after byte 32 aligned:
+//     0 point_count | 8 version 0xFFFF_FFFF_FFFF_FF01 | 16 levels_count | 24 total_neighbors_bytes | 32 offsets length (u64) |
+//     40 base_bits, 41 delta_bits, 42 chunk_len_log2 (u8 each) | 43 m (u64) | 51 m0 (u64) | 59 five zero bytes
+//   then levels_count u64 level offsets, point_count u32 reindex, total_neighbors_bytes of packed links, the compressed offsets.
+// Offsets (common/src/bitpacking_ordered.rs:12-39, 165-197, 292-315): chunks of 2^chunk_len_log2 values — a base_bits base,
+// then delta_bits deltas from that base, byte-padded — and a 7-byte 0xFF tail.  The values are BYTE offsets into the packed
+// links, in the plain format's index space (view.rs:209-218).
+// Links of one (node, level) (bitpacking_links.rs:23-133; bit I/O bitpacking.rs:14-186, LSB first): the first
+// min(count, level_m) are sorted and delta-coded (wrapping u32 sums) after a 5-bit header `bits_per_sorted - 8`; the rest are
+// raw, bits_per_unsorted = max(8, packed_bits(point_count - 1)) bits each (view.rs:155-159).  The count is implicit in the byte
+// length L: ns = min(level_m, (8L - 5) / bps), nu = (8L - 5 - ns * bps) / bits_per_unsorted; L == 0: no links.
+// Ids may repeat and may be >= point_count (graph_links/tests.rs:59-80); the traversal skips the latter, as for plain graphs.
+namespace {
+
+constexpr uint64_t HNSW_VERSION_COMPRESSED = 0xFFFFFFFFFFFFFF01ull;
+constexpr uint64_t HNSW_VERSION_COMPRESSED_WITH_VECTORS = 0xFFFFFFFFFFFFFF02ull;
+constexpr uint64_t HC_PAD = 16;   // the device copy of the file is padded so the funnel-shift load below never leaves the allocation
+enum : uint32_t { HC_OFFSET_PAST_END = 1u, HC_OFFSETS_DECREASE = 2u, HC_REINDEX = 4u };
+
+__device__ __forceinline__ uint64_t hc_min(uint64_t a, uint64_t b) { return a < b ? a : b; }
+__device__ __forceinline__ uint64_t hc_mask(uint32_t bits) { return bits >= 64 ? ~0ull : ((1ull << bits) - 1ull); }
+
+// little-endian u64 at any byte address: two aligned 8-byte loads and a funnel shift
+__device__ __forceinline__ uint64_t hc_load_le64(const uint8_t* p) {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+    const uint64_t* w = reinterpret_cast<const uint64_t*>(a & ~uintptr_t(7));
+    const uint32_t sh = (uint32_t)(a & 7) * 8;
+    const uint64_t lo = __ldg(w);
+    return sh ? (lo >> sh) | (__ldg(w + 1) << (64 - sh)) : lo;
+}
+
+// BitReader::read::<u32> of a `bits`-wide value at bit `bitpos` (bits <= 39, so bitpos % 8 + bits fits one 8-byte word)
+__device__ __forceinline__ uint32_t hc_bits(const uint8_t* base, uint64_t bitpos, uint32_t bits) {
+    return (uint32_t)((hc_load_le64(base + (bitpos >> 3)) >> (bitpos & 7)) & hc_mask(bits));
+}
+
+struct HcOffsets {
+    const uint8_t* data;          // compressed offsets
+    uint64_t length, chunk_bytes, limit;   // limit = total_neighbors_bytes
+    uint32_t base_bits, delta_bits, log2;
+};
+
+// Reader::decode_chunk (bitpacking_ordered.rs:292-315), one thread per value; the 7-byte tail keeps every 8-byte read in the data
+__global__ void hnsw_c_offsets_kernel(const HcOffsets p, uint64_t* __restrict__ out, uint32_t* __restrict__ flag) {
+    const uint64_t base_mask = hc_mask(p.base_bits), delta_mask = hc_mask(p.delta_bits), in_chunk = (1ull << p.log2) - 1ull;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.length; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint8_t* c = p.data + (i >> p.log2) * p.chunk_bytes;
+        uint64_t v = hc_load_le64(c) & base_mask;
+        const uint64_t j = i & in_chunk;
+        if (j) {
+            const uint64_t bit = p.base_bits + (j - 1) * p.delta_bits;
+            v += (hc_load_le64(c + (bit >> 3)) >> (bit & 7)) & delta_mask;
+        }
+        if (v > p.limit) atomicOr(flag, HC_OFFSET_PAST_END);
+        out[i] = v;
+    }
+}
+
+struct HcLinks {
+    const uint8_t* links;         // packed links
+    const uint64_t* byte_off;     // decoded offsets [n_entries + 1]
+    uint64_t n_entries, limit;
+    uint32_t n_points, m, m0, bits_unsorted;
+};
+
+// the implicit shape of entry e (iterate_packed_links, bitpacking_links.rs:75-107); entries [0, n_points) are level 0 (view.rs:205-206)
+__device__ __forceinline__ void hc_shape(const HcLinks& p, uint64_t e, uint64_t s, uint64_t t, uint32_t& bps, uint64_t& ns, uint64_t& nu) {
+    ns = nu = 0; bps = 8;
+    if (t == s) return;
+    bps = (p.links[s] & 31u) + 8u;
+    const uint64_t bits = 8 * (t - s) - 5;
+    ns = hc_min(e < p.n_points ? p.m0 : p.m, bits / bps);
+    nu = (bits - ns * bps) / p.bits_unsorted;
+}
+
+// links per entry (counts[n_entries] = 0, so the exclusive scan ends on the total), and the file's checks that need the device
+__global__ void hnsw_c_counts_kernel(const HcLinks p, const uint32_t* __restrict__ reindex, uint64_t* __restrict__ counts, uint32_t* __restrict__ flag) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e <= p.n_entries; e += stride) {
+        uint64_t c = 0;
+        if (e < p.n_entries) {
+            const uint64_t s = p.byte_off[e], t = p.byte_off[e + 1];
+            if (t < s) atomicOr(flag, HC_OFFSETS_DECREASE);
+            else if (t <= p.limit) { uint32_t bps; uint64_t ns, nu; hc_shape(p, e, s, t, bps, ns, nu); c = ns + nu; }
+        }
+        counts[e] = c;
+    }
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n_points; i += stride)
+        if (reindex[i] >= p.n_points) atomicOr(flag, HC_REINDEX);
+}
+
+// one warp per entry: lane j decodes value j (j + 32, ...) at its own bit position; the sorted part is a warp inclusive scan of
+// the deltas (wrapping u32 adds, PackedLinksIterator::next_sorted) with a carry across passes of 32
+__global__ void hnsw_c_links_kernel(const HcLinks p, const uint64_t* __restrict__ offsets, uint32_t* __restrict__ neighbors) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint64_t n_warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+    for (uint64_t e = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; e < p.n_entries; e += n_warps) {
+        const uint64_t s = p.byte_off[e], t = p.byte_off[e + 1];
+        uint32_t bps; uint64_t ns, nu;
+        hc_shape(p, e, s, t, bps, ns, nu);
+        uint32_t* out = neighbors + offsets[e];
+        const uint64_t bit0 = 8 * s + 5;
+        uint32_t carry = 0;
+        for (uint64_t k0 = 0; k0 < ns; k0 += 32) {
+            const uint64_t k = k0 + lane;
+            uint32_t v = k < ns ? hc_bits(p.links, bit0 + k * bps, bps) : 0u;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const uint32_t o = __shfl_up_sync(0xFFFFFFFFu, v, d);
+                if (lane >= (uint32_t)d) v += o;
+            }
+            v += carry;
+            if (k < ns) out[k] = v;
+            carry = __shfl_sync(0xFFFFFFFFu, v, 31);
+        }
+        const uint64_t bit1 = bit0 + ns * bps;
+        for (uint64_t k = lane; k < nu; k += 32) out[ns + k] = hc_bits(p.links, bit1 + k * p.bits_unsorted, p.bits_unsorted);
+    }
+}
+
+// offsets[length .. length + n) = total: an upper-level lookup level_offsets[l] + reindex[p] stays inside the table (and reads an
+// empty list) even when a link leads to a point that is not on that level
+__global__ void hnsw_c_pad_kernel(uint64_t* offsets, uint64_t length, uint64_t n) {
+    const uint64_t total = offsets[length - 1];
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) offsets[length + i] = total;
+}
+
+// qb_hnsw_links: GraphLinks::links (view.rs:238-263) for a batch of points on one level, from the traversal's own arrays
+__global__ void hnsw_links_gather_kernel(const uint32_t* __restrict__ ids, uint32_t n_ids, uint32_t level, uint64_t level_base, uint64_t on_level,
+                                         const uint32_t* __restrict__ reindex, const uint64_t* __restrict__ offsets, uint64_t n_offsets,
+                                         const uint32_t* __restrict__ neighbors, uint64_t n_neighbors, uint32_t cap, uint32_t* __restrict__ out,
+                                         uint32_t* __restrict__ counts, uint32_t* __restrict__ flag) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_ids; i += gridDim.x * blockDim.x) {
+        const uint32_t id = ids[i];
+        counts[i] = 0;
+        uint64_t idx = id;
+        if (level) {
+            const uint32_t r = reindex[id];
+            if (r >= on_level) { atomicOr(flag, 1u); continue; }   // point_level(id) < level (view.rs:354-369)
+            idx = level_base + r;
+        }
+        if (idx + 1 >= n_offsets) { atomicOr(flag, 2u); continue; }
+        const uint64_t b = offsets[idx], e = offsets[idx + 1];
+        if (b > e || e > n_neighbors) { atomicOr(flag, 2u); continue; }
+        counts[i] = (uint32_t)hc_min(e - b, 0xFFFFFFFFull);
+        const uint64_t n = hc_min(e - b, cap);
+        for (uint64_t k = 0; k < n; ++k) out[(size_t)i * cap + k] = neighbors[b + k];
+    }
+}
+
+// device temporaries of one call, freed on every exit path
+struct HcScratch {
+    std::vector<void*> bufs;
+    cudaError_t alloc(void** p, size_t bytes) {
+        *p = nullptr;
+        const cudaError_t e = cudaMalloc(p, std::max<size_t>(bytes, 256));
+        if (e == cudaSuccess) bufs.push_back(*p);
+        return e;
+    }
+    ~HcScratch() { for (void* b : bufs) cudaFree(b); }
+};
+
+inline unsigned hc_grid(uint64_t items, uint64_t per_block, uint64_t max_blocks) {
+    return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(ceil_div_u64(items, per_block), max_blocks));
+}
+
+}  // namespace
+
+extern "C" qb_status qb_hnsw_create_compressed(qb_storage* s, const uint8_t* bytes, uint64_t n_bytes, qb_hnsw** out) {
+    QB_CHECK(s && bytes && out, QB_ERR_INVALID, "hnsw_create_compressed: null argument");
+    *out = nullptr;
+    QB_CHECK(n_bytes >= 64, QB_ERR_INVALID, "hnsw_create_compressed: %llu bytes is smaller than HeaderCompressed", (unsigned long long)n_bytes);
+    auto u64_at = [&](uint64_t o) { uint64_t v; memcpy(&v, bytes + o, 8); return v; };   // the file is little-endian, like every host this builds for
+    const uint64_t n = u64_at(0), version = u64_at(8), levels = u64_at(16), nb_bytes = u64_at(24), length = u64_at(32), m = u64_at(43), m0 = u64_at(51);
+    const uint32_t base_bits = bytes[40], delta_bits = bytes[41], log2 = bytes[42];
+    QB_CHECK(version != HNSW_VERSION_COMPRESSED_WITH_VECTORS, QB_ERR_UNSUPPORTED,
+             "hnsw_create_compressed: CompressedWithVectors (inline storage) graphs are searched from the quantized vectors stored with the links "
+             "(graph_layers.rs:336-388), a different algorithm; this loader takes GraphLinksFormat::Compressed");
+    QB_CHECK(version == HNSW_VERSION_COMPRESSED, QB_ERR_INVALID, "hnsw_create_compressed: version word %016llx is not HEADER_VERSION_COMPRESSED (a plain links.bin?)",
+             (unsigned long long)version);
+    QB_CHECK(n == s->count, QB_ERR_INVALID, "hnsw_create_compressed: graph has %llu points, storage %llu", (unsigned long long)n, (unsigned long long)s->count);
+    QB_CHECK(n <= 0xFFFFFFFFull, QB_ERR_INVALID, "hnsw_create_compressed: %llu points", (unsigned long long)n);
+    QB_CHECK(m >= 1 && m0 >= 1, QB_ERR_INVALID, "hnsw_create_compressed: m %llu / m0 %llu", (unsigned long long)m, (unsigned long long)m0);
+    QB_CHECK(m <= HNSW_MAX_LINKS && m0 <= HNSW_MAX_LINKS, QB_ERR_UNSUPPORTED, "hnsw_create_compressed: m %llu / m0 %llu outside [1,%u]", (unsigned long long)m,
+             (unsigned long long)m0, HNSW_MAX_LINKS);
+    QB_CHECK(levels <= 64 && (levels >= 1 || n == 0), QB_ERR_INVALID, "hnsw_create_compressed: %llu levels", (unsigned long long)levels);
+    // Parameters::validate (bitpacking_ordered.rs:165-180)
+    QB_CHECK(base_bits >= 1 && base_bits <= 64 && delta_bits >= 1 && delta_bits <= 56 && log2 <= 7, QB_ERR_INVALID,
+             "hnsw_create_compressed: offsets parameters base_bits %u delta_bits %u chunk_len_log2 %u", base_bits, delta_bits, log2);
+    const uint64_t body = 64 + 8 * levels + 4 * n;
+    QB_CHECK(body <= n_bytes && nb_bytes <= n_bytes - body, QB_ERR_INVALID, "hnsw_create_compressed: %llu bytes, header describes %llu before the offsets",
+             (unsigned long long)n_bytes, (unsigned long long)(body + nb_bytes));
+    const uint64_t rest = n_bytes - body - nb_bytes;
+    const uint64_t chunk_bytes = ceil_div_u64(base_bits + (uint64_t)delta_bits * ((1ull << log2) - 1), 8);
+    const uint64_t chunks = length / (1ull << log2) + ((length & ((1ull << log2) - 1)) ? 1 : 0);
+    QB_CHECK(length >= 1 && chunks <= rest / chunk_bytes && chunks * chunk_bytes + 7 <= rest, QB_ERR_INVALID,
+             "hnsw_create_compressed: %llu offsets do not fit the %llu bytes after the links", (unsigned long long)length, (unsigned long long)rest);
+    const uint64_t used = body + nb_bytes + chunks * chunk_bytes + 7;
+    // level offsets with the extra last element (read_level_offsets, view.rs:381-393): level 0 is the first n entries, every level's
+    // range inside the table
+    std::vector<uint64_t> lo(levels + 1);
+    memcpy(lo.data(), bytes + 64, 8 * levels);
+    lo[levels] = length - 1;
+    for (uint64_t l = 0; l < levels; ++l)
+        QB_CHECK(lo[l] <= lo[l + 1] && (l != 0 || (lo[0] == 0 && lo[1] == n)), QB_ERR_INVALID, "hnsw_create_compressed: level offset %llu (%llu) out of range",
+                 (unsigned long long)l, (unsigned long long)lo[l]);
+    const uint32_t bits_unsorted = std::max<uint32_t>(8, n > 1 ? 64 - __builtin_clzll(n - 1) : 0);
+
+    cudaError_t ce = cudaSetDevice(s->device);
+    if (ce != cudaSuccess) { qb_set_error("hnsw_create_compressed: %s", cudaGetErrorString(ce)); return QB_ERR_CUDA; }
+    qb_hnsw* g = new qb_hnsw();
+    g->st = s; g->n_points = (uint32_t)n; g->m = (uint32_t)m; g->m0 = (uint32_t)m0; g->levels = (uint32_t)levels;
+    g->level_offsets_ext = lo; g->n_offsets = length;
+    auto fail = [&](qb_status st, const char* what, cudaError_t e) {
+        qb_set_error("hnsw_create_compressed: %s: %s", what, cudaGetErrorString(e));
+        qb_hnsw_destroy(g);
+        return st;
+    };
+    HcScratch tmp;
+    uint8_t* d_file = nullptr; uint64_t* d_byte_off = nullptr; uint64_t* d_counts = nullptr; uint32_t* d_flag = nullptr;
+    bool ok = cudaMalloc(&g->d_links0, std::max<size_t>((size_t)n * m0 * 4, 256)) == cudaSuccess &&
+              cudaMalloc(&g->d_level_offsets, std::max<size_t>(8 * levels, 256)) == cudaSuccess &&
+              cudaMalloc(&g->d_reindex, std::max<size_t>(4 * n, 256)) == cudaSuccess &&
+              cudaMalloc(&g->d_offsets, 8 * (length + n) + 256) == cudaSuccess && cudaMalloc(&g->d_work, 256) == cudaSuccess &&
+              cudaMalloc(&g->d_stats, 256) == cudaSuccess &&
+              tmp.alloc((void**)&d_file, used + HC_PAD) == cudaSuccess && tmp.alloc((void**)&d_byte_off, 8 * length) == cudaSuccess &&
+              tmp.alloc((void**)&d_counts, 8 * length) == cudaSuccess && tmp.alloc((void**)&d_flag, 4) == cudaSuccess;
+    if (!ok) return fail(QB_ERR_OOM, "cudaMalloc failed", cudaGetLastError());
+    // the file goes to HBM once; everything below reads it there
+    ce = cudaMemcpy(d_file, bytes, used, cudaMemcpyHostToDevice);
+    if (ce == cudaSuccess) ce = cudaMemset(d_file + used, 0, HC_PAD);
+    if (ce == cudaSuccess) ce = cudaMemcpy(g->d_level_offsets, d_file + 64, 8 * levels, cudaMemcpyDeviceToDevice);
+    if (ce == cudaSuccess) ce = cudaMemcpy(g->d_reindex, d_file + 64 + 8 * levels, 4 * n, cudaMemcpyDeviceToDevice);
+    if (ce == cudaSuccess) ce = cudaMemset(g->d_stats, 0, 256);
+    if (ce == cudaSuccess) ce = cudaMemset(d_flag, 0, 4);
+    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "upload", ce);
+
+    HcOffsets po{d_file + body + nb_bytes, length, chunk_bytes, nb_bytes, base_bits, delta_bits, log2};
+    hnsw_c_offsets_kernel<<<hc_grid(length, 256, 132 * 16), 256>>>(po, d_byte_off, d_flag);
+    QB_LAUNCHED();
+    HcLinks pl{d_file + body, d_byte_off, length - 1, nb_bytes, (uint32_t)n, (uint32_t)m, (uint32_t)m0, bits_unsorted};
+    hnsw_c_counts_kernel<<<hc_grid(std::max<uint64_t>(length, n), 256, 132 * 16), 256>>>(pl, g->d_reindex, d_counts, d_flag);
+    QB_LAUNCHED();
+    // plain element offsets = exclusive scan of the counts
+    size_t scan_bytes = 0;
+    ce = cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_counts, g->d_offsets, (int64_t)length);
+    void* d_scan = nullptr;
+    if (ce == cudaSuccess) ce = tmp.alloc(&d_scan, scan_bytes);
+    if (ce == cudaSuccess) ce = cub::DeviceScan::ExclusiveSum(d_scan, scan_bytes, d_counts, g->d_offsets, (int64_t)length);
+    QB_LAUNCHED();
+    uint32_t flag = 0;
+    uint64_t total = 0;
+    if (ce == cudaSuccess) ce = cudaMemcpy(&flag, d_flag, 4, cudaMemcpyDeviceToHost);
+    if (ce == cudaSuccess) ce = cudaMemcpy(&total, g->d_offsets + (length - 1), 8, cudaMemcpyDeviceToHost);
+    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "decode", ce);
+    if (flag) {
+        qb_set_error("hnsw_create_compressed: %s", (flag & HC_OFFSET_PAST_END) ? "a links offset lies past total_neighbors_bytes"
+                                                   : (flag & HC_OFFSETS_DECREASE) ? "links offsets decrease"
+                                                                                  : "a reindex entry is >= point_count");
+        qb_hnsw_destroy(g);
+        return QB_ERR_INVALID;
+    }
+    g->n_neighbors = total;
+    g->hbm_bytes = (uint64_t)n * m0 * 4 + 8 * levels + 4 * n + 4 * total + 8 * (length + n);
+    if (cudaMalloc(&g->d_neighbors, std::max<size_t>(4 * total, 256)) != cudaSuccess) return fail(QB_ERR_OOM, "cudaMalloc failed", cudaGetLastError());
+    hnsw_c_links_kernel<<<hc_grid(length - 1, 8, 132 * 32), 256>>>(pl, g->d_offsets, g->d_neighbors);
+    QB_LAUNCHED();
+    hnsw_c_pad_kernel<<<hc_grid(n, 256, 132 * 4), 256>>>(g->d_offsets, length, n);
+    QB_LAUNCHED();
+    if (n) {
+        hnsw_links0_kernel<<<hc_grid(n * m0, 256, 132 * 16), 256>>>(g->d_neighbors, g->d_offsets, (uint32_t)n, (uint32_t)m0, g->d_links0);
+        QB_LAUNCHED();
+    }
+    ce = cudaDeviceSynchronize();
+    if (ce == cudaSuccess) ce = cudaGetLastError();
+    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "decode", ce);
+    *out = g;
+    return QB_OK;
+}
+
+extern "C" qb_status qb_hnsw_links(const qb_hnsw* g, uint32_t level, const uint32_t* ids, uint32_t n_ids, uint32_t cap, uint32_t* out, uint32_t* counts) {
+    QB_CHECK(g && (ids || n_ids == 0) && (counts || n_ids == 0) && (out || cap == 0 || n_ids == 0), QB_ERR_INVALID, "hnsw_links: null argument");
+    QB_CHECK(level < g->levels, QB_ERR_INVALID, "hnsw_links: level %u but the graph has %u levels", level, g->levels);
+    for (uint32_t i = 0; i < n_ids; ++i) QB_CHECK(ids[i] < g->n_points, QB_ERR_INVALID, "hnsw_links: point %u out of range", ids[i]);
+    if (n_ids == 0) return QB_OK;
+    // a point is on `level` iff its reindex is below every level's point count up to there (point_level, view.rs:354-369)
+    const std::vector<uint64_t>& lo = g->level_offsets_ext;
+    uint64_t on_level = ~0ull;
+    for (uint32_t l = 1; l <= level; ++l) on_level = std::min<uint64_t>(on_level, lo[l + 1] >= lo[l] ? lo[l + 1] - lo[l] : 0);
+    QB_CUDA(cudaSetDevice(g->st->device));
+    HcScratch tmp;
+    uint32_t *d_ids = nullptr, *d_out = nullptr, *d_counts = nullptr, *d_flag = nullptr;
+    QB_CUDA(tmp.alloc((void**)&d_ids, 4ull * n_ids));
+    QB_CUDA(tmp.alloc((void**)&d_out, 4ull * n_ids * cap));
+    QB_CUDA(tmp.alloc((void**)&d_counts, 4ull * n_ids));
+    QB_CUDA(tmp.alloc((void**)&d_flag, 4));
+    QB_CUDA(cudaMemcpy(d_ids, ids, 4ull * n_ids, cudaMemcpyHostToDevice));
+    QB_CUDA(cudaMemset(d_flag, 0, 4));
+    hnsw_links_gather_kernel<<<hc_grid(n_ids, 128, 132 * 8), 128>>>(d_ids, n_ids, level, level ? lo[level] : 0, on_level, g->d_reindex, g->d_offsets, g->n_offsets,
+                                                                    g->d_neighbors, g->n_neighbors, cap, d_out, d_counts, d_flag);
+    QB_LAUNCHED();
+    QB_CUDA(cudaGetLastError());
+    uint32_t flag = 0;
+    QB_CUDA(cudaMemcpy(&flag, d_flag, 4, cudaMemcpyDeviceToHost));
+    QB_CHECK(!(flag & 1u), QB_ERR_INVALID, "hnsw_links: a point's top level is below %u", level);
+    QB_CHECK(!(flag & 2u), QB_ERR_INVALID, "hnsw_links: the graph's offsets point outside its tables");
+    QB_CUDA(cudaMemcpy(counts, d_counts, 4ull * n_ids, cudaMemcpyDeviceToHost));
+    if (cap) QB_CUDA(cudaMemcpy(out, d_out, 4ull * n_ids * cap, cudaMemcpyDeviceToHost));
     return QB_OK;
 }
 

@@ -137,6 +137,10 @@ struct qb_hnsw {
     uint32_t* d_neighbors = nullptr;
     uint64_t* d_offsets = nullptr;
     uint64_t hbm_bytes = 0;
+    // host copy of the level offsets with the extra last element (offset count - 1, view.rs:381-393); offsets / neighbours
+    // counts as the file describes them (qb_hnsw_links bounds its reads by these)
+    std::vector<uint64_t> level_offsets_ext;
+    uint64_t n_offsets = 0, n_neighbors = 0;
     // search scratch (one batch at a time per graph handle; mu serialises)
     std::mutex mu;
     uint32_t* d_visited = nullptr; uint64_t visited_words = 0; unsigned visited_slots = 0;

@@ -196,14 +196,29 @@ private:
 };
 
 // GraphLayers::search (index/hnsw_index/graph_layers.rs:530-561) for a batch of queries, traversal and scoring on the device.
-// The graph is the segment's links.bin in GraphLinksFormat::Plain (graph_links/view.rs:121-135).
+// The graph is the segment's links.bin in GraphLinksFormat::Plain (graph_links/view.rs:121-135) or, through compressed(),
+// in GraphLinksFormat::Compressed (view.rs:137-163), the format the reference writes for every index it builds.
 class HnswGraph {
 public:
     HnswGraph(const VectorStorage& storage, const uint8_t* links_bin, uint64_t n_bytes, uint32_t m, uint32_t m0) {
         check(qb_hnsw_create_plain(storage.raw(), links_bin, n_bytes, m, m0, &h_));
     }
+    // m and m0 are read from the compressed file's header
+    static std::unique_ptr<HnswGraph> compressed(const VectorStorage& storage, const uint8_t* links_bin, uint64_t n_bytes) {
+        qb_hnsw* h = nullptr;
+        check(qb_hnsw_create_compressed(storage.raw(), links_bin, n_bytes, &h));
+        return std::unique_ptr<HnswGraph>(new HnswGraph(h));
+    }
     ~HnswGraph() { qb_hnsw_destroy(h_); }
     HnswGraph(const HnswGraph&) = delete;
+    // GraphLinks::links (view.rs:238-263): the point's links on `level`, in stored order
+    std::vector<PointOffsetType> links(PointOffsetType point, uint32_t level) const {
+        uint32_t count = 0;
+        check(qb_hnsw_links(h_, level, &point, 1, 0, nullptr, &count));
+        std::vector<PointOffsetType> out(count);
+        if (count) check(qb_hnsw_links(h_, level, &point, 1, count, out.data(), &count));
+        return out;
+    }
     // entry_point / entry_level = GraphLayers::get_entry_point(filters, custom_entry_points); deleted = the filter as a bitmap (bit = 1: skip)
     std::vector<std::vector<ScoredPointOffset>> search(const float* queries, uint32_t n_queries, uint32_t top, uint32_t ef, PointOffsetType entry_point,
                                                        uint32_t entry_level, const uint64_t* deleted = nullptr) const {
@@ -216,6 +231,7 @@ public:
     }
 
 private:
+    explicit HnswGraph(qb_hnsw* h) : h_(h) {}
     qb_hnsw* h_ = nullptr;
 };
 

@@ -709,7 +709,8 @@ def set_option(name: str, value: int) -> None:
 
 class HnswGraph:
     """GraphLayers::search with the traversal on the device (qb_hnsw_*): a graph in the reference's plain links.bin layout
-    bound to a storage (dense f32 or SQ8); search() answers a batch of queries in one call."""
+    bound to a storage (dense f32 or SQ8); search() answers a batch of queries in one call.  from_compressed() takes the
+    compressed links.bin the reference writes for every index it builds."""
 
     def __init__(self, storage: _Storage, links_bin, m: int, m0: int):
         self._storage = storage
@@ -718,6 +719,38 @@ class HnswGraph:
         h = vp()
         check(lib().qb_hnsw_create_plain(storage._h, blob.ctypes.data_as(u8p), blob.size, int(m), int(m0), C.byref(h)))
         self._h = h
+
+    @classmethod
+    def from_compressed(cls, storage: _Storage, links_bin) -> "HnswGraph":
+        """A graph from `links.bin` in GraphLinksFormat::Compressed (m and m0 are in its header), decoded on the device."""
+        self = cls.__new__(cls)
+        self._storage = storage
+        self._h = vp()
+        blob = np.ascontiguousarray(np.frombuffer(links_bin, dtype=np.uint8) if isinstance(links_bin, (bytes, bytearray)) else links_bin,
+                                    dtype=np.uint8).reshape(-1)
+        h = vp()
+        check(lib().qb_hnsw_create_compressed(storage._h, blob.ctypes.data_as(u8p), blob.size, C.byref(h)))
+        self._h = h
+        return self
+
+    def links(self, level: int, ids, cap: int = 0):
+        """GraphLinks::links for each of `ids` on `level`, in the graph's stored order: a list of uint32 arrays.  cap = 0 returns every
+        link (two calls: counts first); cap > 0 truncates each list to cap links."""
+        ids = np.ascontiguousarray(np.atleast_1d(ids), dtype=np.uint32)
+        n = ids.size
+        counts = np.zeros(n, dtype=np.uint32)
+        if cap <= 0:
+            check(lib().qb_hnsw_links(self._h, int(level), ids.ctypes.data_as(u32p), n, 0, None, counts.ctypes.data_as(u32p)))
+            cap = int(counts.max()) if n else 0
+        out = np.zeros((n, max(cap, 1)), dtype=np.uint32)
+        check(lib().qb_hnsw_links(self._h, int(level), ids.ctypes.data_as(u32p), n, int(cap), out.ctypes.data_as(u32p), counts.ctypes.data_as(u32p)))
+        return [out[i, : min(int(counts[i]), cap)].copy() for i in range(n)]
+
+    def info(self) -> tuple[int, int, int]:
+        """(points, levels, bytes of HBM the graph holds)"""
+        a, b, c = C.c_uint32(), C.c_uint32(), C.c_uint64()
+        check(lib().qb_hnsw_info(self._h, C.byref(a), C.byref(b), C.byref(c)))
+        return int(a.value), int(b.value), int(c.value)
 
     def search(self, queries, top: int, ef: int, entry_point: int, entry_level: int, point_deleted=None, counters: Optional[HwCounters] = None):
         q = np.atleast_2d(_f32(queries))
