@@ -18,6 +18,8 @@ pub const QB_ERR_NO_DEVICE: qb_status = -6;
 pub const QB_DIST_COSINE: i32 = 0; pub const QB_DIST_EUCLID: i32 = 1; pub const QB_DIST_DOT: i32 = 2; pub const QB_DIST_MANHATTAN: i32 = 3;
 pub const QB_DT_F32: i32 = 0; pub const QB_DT_F16: i32 = 1; pub const QB_DT_U8: i32 = 2;
 pub const QB_QD_COSINE: i32 = 0; pub const QB_QD_DOT: i32 = 1; pub const QB_QD_L1: i32 = 2; pub const QB_QD_L2: i32 = 3;
+// qb_hnsw_algorithm (SearchAlgorithm, graph_layers.rs:80-84)
+pub const QB_HNSW_ALGO_HNSW: i32 = 0; pub const QB_HNSW_ALGO_ACORN: i32 = 1;
 
 #[repr(C)]
 pub struct qb_storage { _private: [u8; 0] }
@@ -105,6 +107,8 @@ extern "C" {
     pub fn qb_hnsw_info(g: *const qb_hnsw, n_points: *mut u32, levels: *mut u32, hbm_bytes: *mut u64) -> qb_status;
     pub fn qb_hnsw_search_batch(g: *mut qb_hnsw, queries: *const f32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, deleted_bitmap: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters) -> qb_status;
     pub fn qb_hnsw_search_batch_device(g: *mut qb_hnsw, dev_queries: *const f32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, dev_out: *mut qb_scored_point, dev_counts: *mut u32) -> qb_status;
+    pub fn qb_hnsw_search_batch_algo(g: *mut qb_hnsw, queries: *const f32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, deleted_bitmap: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters, algorithm: i32) -> qb_status;
+    pub fn qb_hnsw_search_batch_device_algo(g: *mut qb_hnsw, dev_queries: *const f32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, dev_out: *mut qb_scored_point, dev_counts: *mut u32, algorithm: i32) -> qb_status;
     pub fn qb_hnsw_stats(g: *mut qb_hnsw, hops: *mut u64, scored_points: *mut u64, reset: i32) -> qb_status;
     pub fn qb_search_stats(s: *mut qb_storage, searches: *mut u64, reruns: *mut u64, reset: i32) -> qb_status;
     pub fn qb_profile_enable(s: *mut qb_storage, on: i32) -> qb_status;

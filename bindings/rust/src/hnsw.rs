@@ -4,6 +4,7 @@
 use common::types::{PointOffsetType, ScoredPointOffset};
 
 use super::ffi::*;
+use crate::index::hnsw_index::graph_layers::SearchAlgorithm;
 use super::raw_scorer::{last_error, B200Storage};
 use crate::common::operation_error::{OperationError, OperationResult};
 
@@ -29,14 +30,17 @@ impl<'a> B200Hnsw<'a> {
     }
 
     /// `entry` = GraphLayers::get_entry_point(filters, custom_entry_points) (it depends on the filter, so it stays host logic);
-    /// `deleted` = the filter as a bitmap (bit = 1: check_vector fails), or None.
-    pub fn search_batch(&self, queries: &[f32], n_queries: usize, top: usize, ef: usize, entry: (PointOffsetType, usize), deleted: Option<&[u64]>)
-        -> Vec<Vec<ScoredPointOffset>> {
+    /// `deleted` = the filter as a bitmap (bit = 1: check_vector fails), or None;
+    /// `algorithm` = the level-0 algorithm GraphLayers::search dispatches on, as hnsw/read_view/search.rs:59-86 chooses it.
+    pub fn search_batch(&self, queries: &[f32], n_queries: usize, top: usize, ef: usize, entry: (PointOffsetType, usize), deleted: Option<&[u64]>,
+                        algorithm: SearchAlgorithm) -> Vec<Vec<ScoredPointOffset>> {
         let mut out = vec![qb_scored_point::default(); n_queries * top];
         let mut counts = vec![0u32; n_queries];
+        let algo = match algorithm { SearchAlgorithm::Hnsw => QB_HNSW_ALGO_HNSW, SearchAlgorithm::Acorn => QB_HNSW_ALGO_ACORN };
         let st = unsafe {
-            qb_hnsw_search_batch(self.raw, queries.as_ptr(), n_queries as u32, top as u32, ef as u32, entry.0, entry.1 as u32,
-                                 deleted.map_or(std::ptr::null(), |d| d.as_ptr()), std::ptr::null(), out.as_mut_ptr(), counts.as_mut_ptr(), std::ptr::null_mut())
+            qb_hnsw_search_batch_algo(self.raw, queries.as_ptr(), n_queries as u32, top as u32, ef as u32, entry.0, entry.1 as u32,
+                                      deleted.map_or(std::ptr::null(), |d| d.as_ptr()), std::ptr::null(), out.as_mut_ptr(), counts.as_mut_ptr(),
+                                      std::ptr::null_mut(), algo)
         };
         assert!(st == QB_OK, "{}", last_error());
         (0..n_queries).map(|q| out[q * top..q * top + counts[q] as usize].iter().map(|p| ScoredPointOffset { idx: p.idx, score: p.score }).collect()).collect()

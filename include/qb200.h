@@ -382,6 +382,27 @@ QB_API qb_status qb_hnsw_search_batch(qb_hnsw* g, const float* queries, uint32_t
 /* same with queries / outputs resident in HBM, enqueued on qb_storage_stream(s); no host synchronisation */
 QB_API qb_status qb_hnsw_search_batch_device(qb_hnsw* g, const float* dev_queries, uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point,
                                              uint32_t entry_level, qb_scored_point* dev_out, uint32_t* dev_counts);
+/* The level-0 algorithm of GraphLayers::search (SearchAlgorithm, graph_layers.rs:80-84); search_entry through the upper
+ * levels is the same for both.
+ *   QB_HNSW_ALGO_HNSW   search_on_level (:108-148): links that fail the filter are neither scored nor traversed.
+ *   QB_HNSW_ALGO_ACORN  search_on_level_acorn (:154-243), ACORN-1: a filtered-out link is explored instead, and those of its own
+ *                       links that pass the filter are scored (up to m0 per explored list).  Hops and scored points are counted
+ *                       per scorer call, as for HNSW.  Unfiltered, it visits and scores exactly what HNSW does.
+ * The choice stays with the caller, as in hnsw/read_view/search.rs:59-86: ACORN when the request sets
+ * SearchParams.acorn.enable, the graph has m0 != 0, there is a filter, and the filter's estimated cardinality over the
+ * segment's available points is at most acorn.max_selectivity (default 0.4, types.rs:622); HNSW otherwise.  Searches over a
+ * CompressedWithVectors graph never use ACORN (search.rs:91-92); this library does not load those graphs.  ACORN uses the
+ * same visited state as HNSW; its per-hop buffers take up to 16 * m0 * m0 bytes of shared memory per query in flight. */
+typedef enum { QB_HNSW_ALGO_HNSW = 0, QB_HNSW_ALGO_ACORN = 1 } qb_hnsw_algorithm;
+/* qb_hnsw_search_batch / qb_hnsw_search_batch_device with the level-0 algorithm chosen; the two calls above are these with
+ * QB_HNSW_ALGO_HNSW */
+QB_API qb_status qb_hnsw_search_batch_algo(qb_hnsw* g, const float* queries, uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point,
+                                           uint32_t entry_level, const uint64_t* deleted_bitmap, const volatile int32_t* is_stopped,
+                                           qb_scored_point* out, uint32_t* out_counts, qb_hw_counters* counters /* optional */,
+                                           qb_hnsw_algorithm algorithm);
+QB_API qb_status qb_hnsw_search_batch_device_algo(qb_hnsw* g, const float* dev_queries, uint32_t n_queries, uint32_t top, uint32_t ef,
+                                                  uint32_t entry_point, uint32_t entry_level, qb_scored_point* dev_out, uint32_t* dev_counts,
+                                                  qb_hnsw_algorithm algorithm);
 /* scorer calls (hops) and scored points since the last reset, summed over all searches on this graph (waits for them) */
 QB_API qb_status qb_hnsw_stats(qb_hnsw* g, uint64_t* hops, uint64_t* scored_points, int32_t reset);
 

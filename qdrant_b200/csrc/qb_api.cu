@@ -1623,9 +1623,9 @@ extern "C" qb_status qb_storage_set_on_disk(qb_storage* s, int32_t on_disk) {
 }
 
 // ------------------------------------------------------------------------------------------------ HNSW on the device
-extern "C" qb_status qb_hnsw_search_batch(qb_hnsw* g, const float* queries, uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point,
-                                          uint32_t entry_level, const uint64_t* deleted_bitmap, const volatile int32_t* is_stopped, qb_scored_point* out,
-                                          uint32_t* out_counts, qb_hw_counters* counters) {
+extern "C" qb_status qb_hnsw_search_batch_algo(qb_hnsw* g, const float* queries, uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point,
+                                               uint32_t entry_level, const uint64_t* deleted_bitmap, const volatile int32_t* is_stopped, qb_scored_point* out,
+                                               uint32_t* out_counts, qb_hw_counters* counters, qb_hnsw_algorithm algorithm) {
     QB_CHECK(g && out && out_counts, QB_ERR_INVALID, "hnsw_search_batch: null argument");
     QB_CHECK(n_queries == 0 || queries, QB_ERR_INVALID, "hnsw_search_batch: null queries");
     QB_CHECK(top >= 1 && top <= 4096, QB_ERR_INVALID, "hnsw_search_batch: top %u outside [1,4096]", top);
@@ -1657,7 +1657,8 @@ extern "C" qb_status qb_hnsw_search_batch(qb_hnsw* g, const float* queries, uint
         QB_CUDA(cudaMemcpyAsync(c->d_deleted2, deleted_bitmap, words64 * 8, cudaMemcpyHostToDevice, stream));
         d_del2 = c->d_deleted2;
     }
-    QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, d_del2, c->d_out, c->d_out_counts, stream));
+    QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, d_del2, c->d_out, c->d_out_counts, stream,
+                          (int)algorithm));
     QB_CUDA(cudaMemcpyAsync(hs + raw_bytes, c->d_out, res_bytes, cudaMemcpyDeviceToHost, stream));
     QB_CUDA(cudaMemcpyAsync(hs + raw_bytes + res_bytes, c->d_out_counts, cnt_bytes, cudaMemcpyDeviceToHost, stream));
     QB_CUDA(cudaStreamSynchronize(stream));
@@ -1673,8 +1674,15 @@ extern "C" qb_status qb_hnsw_search_batch(qb_hnsw* g, const float* queries, uint
     return QB_OK;
 }
 
-extern "C" qb_status qb_hnsw_search_batch_device(qb_hnsw* g, const float* dev_queries, uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point,
-                                                 uint32_t entry_level, qb_scored_point* dev_out, uint32_t* dev_counts) {
+extern "C" qb_status qb_hnsw_search_batch(qb_hnsw* g, const float* queries, uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point,
+                                          uint32_t entry_level, const uint64_t* deleted_bitmap, const volatile int32_t* is_stopped, qb_scored_point* out,
+                                          uint32_t* out_counts, qb_hw_counters* counters) {
+    return qb_hnsw_search_batch_algo(g, queries, n_queries, top, ef, entry_point, entry_level, deleted_bitmap, is_stopped, out, out_counts, counters,
+                                     QB_HNSW_ALGO_HNSW);
+}
+
+extern "C" qb_status qb_hnsw_search_batch_device_algo(qb_hnsw* g, const float* dev_queries, uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point,
+                                                      uint32_t entry_level, qb_scored_point* dev_out, uint32_t* dev_counts, qb_hnsw_algorithm algorithm) {
     QB_CHECK(g && dev_queries && dev_out && dev_counts, QB_ERR_INVALID, "hnsw_search_batch_device: null argument");
     QB_CHECK(top >= 1 && top <= 4096, QB_ERR_INVALID, "hnsw_search_batch_device: top %u outside [1,4096]", top);
     if (n_queries == 0) return QB_OK;
@@ -1689,9 +1697,15 @@ extern "C" qb_status qb_hnsw_search_batch_device(qb_hnsw* g, const float* dev_qu
     QB_TRY(prepare_queries(s, dev_queries, n_queries, reinterpret_cast<float*>(c->d_queries_raw), c->d_queries_enc, c->d_q_off, c->stream));
     cudaEvent_t e0, e1;
     profile_begin(s, c, c->stream, &e0, &e1);
-    QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, nullptr, dev_out, dev_counts, c->stream));
+    QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, nullptr, dev_out, dev_counts, c->stream,
+                          (int)algorithm));
     profile_end(s, c->stream, e0, e1);
     return QB_OK;
+}
+
+extern "C" qb_status qb_hnsw_search_batch_device(qb_hnsw* g, const float* dev_queries, uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point,
+                                                 uint32_t entry_level, qb_scored_point* dev_out, uint32_t* dev_counts) {
+    return qb_hnsw_search_batch_device_algo(g, dev_queries, n_queries, top, ef, entry_point, entry_level, dev_out, dev_counts, QB_HNSW_ALGO_HNSW);
 }
 
 extern "C" qb_status qb_hnsw_stats(qb_hnsw* g, uint64_t* hops, uint64_t* scored_points, int32_t reset) {

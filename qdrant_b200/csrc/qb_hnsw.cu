@@ -72,16 +72,20 @@ struct HnswParams {
     qb_scored_point* out; uint32_t* out_counts; uint32_t id_base;
     unsigned long long* stats;                   // [0] hops (scorer calls), [1] scored points
     int prefetch;                                // 1: bulk-prefetch the surviving neighbours' vectors into L2 before scoring
+    // ACORN only (appended so the HNSW kernels' parameter offsets stay as they were)
+    uint32_t hop_cap;                            // per-hop buffers: a power of two >= m0 * m0
 };
 
 struct HnswSmem {
     unsigned long long* keys[2];
     uint8_t* flags[2];
-    unsigned long long* newk;   // [HNSW_MAX_LINKS]
-    uint32_t* ids;              // [HNSW_MAX_LINKS]
-    float* sc;                  // [HNSW_MAX_LINKS]
+    unsigned long long* newk;   // [HNSW_MAX_LINKS] (ACORN: [hop_cap])
+    uint32_t* ids;              // [HNSW_MAX_LINKS] (ACORN: [hop_cap])
+    float* sc;                  // [HNSW_MAX_LINKS] (ACORN: [hop_cap])
     const uint8_t* q;           // query
 };
+
+enum { ALGO_HNSW = 0, ALGO_ACORN = 1 };   // qb_hnsw_algorithm
 
 template <int KIND, int METRIC>
 __device__ __forceinline__ float score_one(const HnswParams& p, const uint8_t* q_smem, float q_off, uint32_t id, int t) {
@@ -131,25 +135,119 @@ __device__ __forceinline__ bool hnsw_filtered_out(const HnswParams& p, uint32_t 
     return d;
 }
 
-template <int KIND, int METRIC, int NT>
+// ---- ACORN-1 level-0 step (search_on_level_acorn, graph_layers.rs:154-243) for the candidate `cand` = keys[best].
+// The reference's order-dependent loops reduce to set operations here because a links0 row holds at most m0 ids:
+//  * 1-hop: the loop breaks once to_score.len() >= m0, which only the m0-th link of a row of m0 fresh passing links can reach, so
+//    the break never skips a link.  Every fresh link is marked in hop1 (test-and-set); passing ones go to to_score, the rest to
+//    to_explore.
+//  * 2-hop: a list breaks once it has added m0 points to to_score, again only at its last link, so every list is read to the end.
+//    A passing link is scored the first time the pass meets it if it was not in hop1 before: test-and-set on hop1 finds that
+//    first meeting, so all lists are processed at once by the whole CTA.
+//  * hop2_visited_list cannot change what is scored, so it is not kept.  A passing link enters hop2 only on the step that also marks
+//    it in hop1 (hop1 marks are never undone), so for a passing link `hop1.check || hop2.check_and_update` is the hop1 check; a
+//    filtered-out 2-hop link is neither scored nor marked in hop1 whatever that test returns.  The reference's hop2 only saves
+//    filter lookups; here it would cost a second bitmap per CTA and an atomic per filtered-out 2-hop link.
+//  * to_score's order only decides the merge order of distinct keys, which the sorted merge does not depend on.
+// Leaves s_n = |to_score| with the ids in sm.ids, and the marks logged.
+template <int KIND, int NT>
+__device__ __forceinline__ void acorn_collect(const HnswParams& p, const HnswSmem& sm, uint32_t* xids, uint32_t cand, uint32_t* visited, uint32_t* vlog,
+                                              unsigned int& s_n, unsigned int& s_nx, unsigned int& s_nlog, unsigned int* s_warp_cnt) {
+    const int tid = threadIdx.x;
+    if (tid < 64) {
+        const uint32_t l = (uint32_t)tid < p.m0 ? p.links0[(size_t)cand * p.m0 + tid] : HNSW_EMPTY;
+        const bool fresh = l < p.n_points && ((atomicOr(&visited[l >> 5], 1u << (l & 31)) >> (l & 31)) & 1u) == 0u;
+        const bool pass = fresh && !hnsw_filtered_out(p, l);
+        const unsigned int bs = __ballot_sync(0xFFFFFFFFu, pass), bx = __ballot_sync(0xFFFFFFFFu, fresh && !pass);
+        if ((tid & 31) == 0) { s_warp_cnt[tid >> 5] = __popc(bs); s_warp_cnt[2 + (tid >> 5)] = __popc(bx); }
+        __syncwarp();
+        asm volatile("bar.sync 1, 64;" ::: "memory");
+        const unsigned int lt = (1u << (tid & 31)) - 1u;
+        const uint32_t ps = ((tid >> 5) ? s_warp_cnt[0] : 0u) + __popc(bs & lt);
+        const uint32_t px = ((tid >> 5) ? s_warp_cnt[2] : 0u) + __popc(bx & lt);
+        if (pass) {
+            if (p.prefetch) prefetch_point<KIND>(p, l);
+            sm.ids[ps] = l;
+        } else if (fresh) {
+            xids[px] = l;
+        }
+        if (fresh) {
+            const uint32_t lp = s_nlog + ps + px;
+            if (lp < p.vlog_cap) vlog[lp] = l;
+        }
+        asm volatile("bar.sync 1, 64;" ::: "memory");
+        if (tid == 0) {
+            s_n = s_warp_cnt[0] + s_warp_cnt[1]; s_nx = s_warp_cnt[2] + s_warp_cnt[3];
+            s_nlog += s_n + s_nx;
+        }
+    }
+    __syncthreads();
+    const uint32_t nx = s_nx, m0 = p.m0;
+    for (uint32_t e = tid; e < nx * m0; e += NT) {
+        const uint32_t h1 = xids[e / m0];
+        const uint32_t l = p.links0[(size_t)h1 * m0 + (e % m0)];
+        if (l >= p.n_points) continue;
+        if (hnsw_filtered_out(p, l)) continue;
+        const uint32_t bit = 1u << (l & 31);
+        if (atomicOr(&visited[l >> 5], bit) & bit) continue;                // hop1_visited_list.check, then marked on acceptance
+        if (p.prefetch) prefetch_point<KIND>(p, l);
+        sm.ids[atomicAdd(&s_n, 1u)] = l;
+        const uint32_t lp = atomicAdd(&s_nlog, 1u);
+        if (lp < p.vlog_cap) vlog[lp] = l;
+    }
+    __syncthreads();
+}
+
+// descending bitonic sort of newk[0 .. n) (n <= hop_cap), padded with empty keys (0) to a power of two
+template <int NT>
+__device__ __forceinline__ void acorn_sort_desc(unsigned long long* newk, uint32_t n) {
+    uint32_t P = 1;
+    while (P < n) P <<= 1;
+    for (uint32_t i = n + threadIdx.x; i < P; i += NT) newk[i] = 0ull;
+    __syncthreads();
+    for (uint32_t k = 2; k <= P; k <<= 1) {
+        for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+            for (uint32_t i = threadIdx.x; i < P; i += NT) {
+                const uint32_t o = i ^ j;
+                if (o > i) {
+                    const unsigned long long a = newk[i], b = newk[o];
+                    if (((i & k) == 0) ? (a < b) : (a > b)) { newk[i] = b; newk[o] = a; }
+                }
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// number of keys in keys[0 .. len) (distinct, descending) greater than k
+__device__ __forceinline__ uint32_t count_greater(const unsigned long long* keys, uint32_t len, unsigned long long k) {
+    uint32_t lo = 0, hi = len;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (keys[mid] > k) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+
+template <int KIND, int METRIC, int NT, int ALGO>
 __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
     constexpr int HNSW_THREADS = NT;
     extern __shared__ __align__(16) uint8_t smem_raw[];
-    __shared__ unsigned int s_q, s_best, s_n, s_nvalid, s_len, s_nlog, s_cur, s_changed, s_warp_cnt[2];
+    __shared__ unsigned int s_q, s_best, s_n, s_nvalid, s_len, s_nlog, s_cur, s_changed, s_warp_cnt[ALGO == ALGO_ACORN ? 4 : 2];
     __shared__ float s_cur_score;
+    __shared__ unsigned int s_nx;   // ACORN: |to_explore|
     const int tid = threadIdx.x;
     const uint32_t ef = p.ef;
     HnswSmem sm;
+    uint32_t* xids = nullptr;   // ACORN: to_explore [HNSW_MAX_LINKS]
     {
+        const uint32_t hop = ALGO == ALGO_ACORN ? p.hop_cap : HNSW_MAX_LINKS;
         uint8_t* b = smem_raw;
         sm.q = b; b += (p.q_bytes + 15u) & ~15u;
         sm.keys[0] = reinterpret_cast<unsigned long long*>(b); b += (size_t)ef * 8;
         sm.keys[1] = reinterpret_cast<unsigned long long*>(b); b += (size_t)ef * 8;
-        sm.newk = reinterpret_cast<unsigned long long*>(b); b += HNSW_MAX_LINKS * 8;
-        sm.ids = reinterpret_cast<uint32_t*>(b); b += HNSW_MAX_LINKS * 4;
-        sm.sc = reinterpret_cast<float*>(b); b += HNSW_MAX_LINKS * 4;
+        sm.newk = reinterpret_cast<unsigned long long*>(b); b += (size_t)hop * 8;
+        sm.ids = reinterpret_cast<uint32_t*>(b); b += (size_t)hop * 4;
+        sm.sc = reinterpret_cast<float*>(b); b += (size_t)hop * 4;
         sm.flags[0] = b; b += (ef + 15u) & ~15u;
         sm.flags[1] = b;
+        if (ALGO == ALGO_ACORN) { b += (ef + 15u) & ~15u; xids = reinterpret_cast<uint32_t*>(b); }
     }
     uint32_t* visited = p.visited + (size_t)blockIdx.x * p.visited_words;
     uint32_t* vlog = p.vlog + (size_t)blockIdx.x * p.vlog_cap;
@@ -237,6 +335,52 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
             const uint32_t best = s_best;
             if (best == 0xFFFFFFFFu) break;
             const uint32_t cand = qb_key_id(keys[best]);
+            if constexpr (ALGO == ALGO_ACORN) {
+                if (tid == 0) flags[best] = 1;
+                acorn_collect<KIND, NT>(p, sm, xids, cand, visited, vlog, s_n, s_nx, s_nlog, s_warp_cnt);
+                const uint32_t n = s_n;
+                if (tid == 0) { if (n) { ++hops; evals += n; } s_nvalid = 0; }
+                if (n == 0) { __syncthreads(); continue; }
+                // score_points_unfiltered(to_score)
+                if (KIND == HK_DENSE_SMALL) {
+                    for (uint32_t i = tid; i < n; i += HNSW_THREADS) sm.sc[i] = score_one<KIND, METRIC>(p, sm.q, q_off, sm.ids[i], 0);
+                } else {
+                    score_list<KIND, METRIC, NT>(p, sm, q_off, n);
+                }
+                __syncthreads();
+                // keys that can enter `nearest`, compacted, sorted, at most ef of them
+                const unsigned long long lower = (len == ef) ? keys[ef - 1] : 0ull;
+                for (uint32_t i = tid; i < n; i += HNSW_THREADS) {
+                    const unsigned long long k = qb_pack_key(sm.sc[i], sm.ids[i]);
+                    if (k > lower) sm.newk[atomicAdd(&s_nvalid, 1u)] = k;
+                }
+                __syncthreads();
+                const uint32_t nv = s_nvalid;
+                if (nv == 0) continue;
+                acorn_sort_desc<NT>(sm.newk, nv);
+                const uint32_t nk_len = min(nv, ef);
+                // merge: rank = own index + number of greater keys in the other list (both sorted: binary search)
+                unsigned long long* nk = sm.keys[cb ^ 1];
+                uint8_t* nf = sm.flags[cb ^ 1];
+                for (uint32_t i = tid; i < len; i += HNSW_THREADS) {
+                    const unsigned long long k = keys[i];
+                    const uint32_t r = i + count_greater(sm.newk, nk_len, k);
+                    if (r < ef) { nk[r] = k; nf[r] = flags[i]; }
+                }
+                for (uint32_t j = tid; j < nk_len; j += HNSW_THREADS) {
+                    const unsigned long long k = sm.newk[j];
+                    const uint32_t r = j + count_greater(keys, len, k);
+                    if (r < ef) {
+                        nk[r] = k; nf[r] = 0;
+                        if (QB_HNSW_LINK_PREFETCH && p.prefetch) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.links0 + (size_t)qb_key_id(k) * p.m0));
+                    }
+                }
+                __syncthreads();
+                if (tid == 0) s_len = min(len + nk_len, ef);
+                cb ^= 1;
+                __syncthreads();
+                continue;
+            }
             // 2. its level-0 links that pass the filter and were not visited (test-and-set), in link order
             if (tid < 64) {
                 const uint32_t l = (uint32_t)tid < p.m0 ? p.links0[(size_t)cand * p.m0 + tid] : HNSW_EMPTY;
@@ -330,12 +474,12 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
     if (tid == 0 && p.stats) { atomicAdd(&p.stats[0], hops); atomicAdd(&p.stats[1], evals); }
 }
 
-template <int KIND, int NT>
+template <int KIND, int NT, int ALGO>
 qb_status launch_kind(int metric, const HnswParams& p, unsigned grid, size_t smem, cudaStream_t stream) {
 #define QB_HNSW_LAUNCH(M)                                                                                              \
     do {                                                                                                               \
-        QB_CUDA(cudaFuncSetAttribute(hnsw_search_kernel<KIND, M, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        hnsw_search_kernel<KIND, M, NT><<<grid, NT, smem, stream>>>(p);                                                \
+        QB_CUDA(cudaFuncSetAttribute(hnsw_search_kernel<KIND, M, NT, ALGO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        hnsw_search_kernel<KIND, M, NT, ALGO><<<grid, NT, smem, stream>>>(p);                                          \
     } while (0)
     if (KIND == HK_SQ8 || KIND == HK_SQ8_LANEX) QB_HNSW_LAUNCH(M_DOT);
     else if (metric == M_EUCLID) QB_HNSW_LAUNCH(M_EUCLID);
@@ -347,30 +491,39 @@ qb_status launch_kind(int metric, const HnswParams& p, unsigned grid, size_t sme
     return QB_OK;
 }
 
-template <int KIND, int METRIC, int NT>
+template <int KIND, int METRIC, int NT, int ALGO>
 int occupancy_of(size_t smem) {
     int nb = 0;
-    cudaFuncSetAttribute(hnsw_search_kernel<KIND, METRIC, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, hnsw_search_kernel<KIND, METRIC, NT>, NT, smem) != cudaSuccess) nb = 1;
+    cudaFuncSetAttribute(hnsw_search_kernel<KIND, METRIC, NT, ALGO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, hnsw_search_kernel<KIND, METRIC, NT, ALGO>, NT, smem) != cudaSuccess) nb = 1;
     return nb < 1 ? 1 : nb;
 }
-template <int NT>
+template <int NT, int ALGO>
 int occupancy_dispatch(int kind, int metric, size_t smem) {
     switch (kind) {
-        case HK_DENSE_AVX: return metric == M_EUCLID ? occupancy_of<HK_DENSE_AVX, M_EUCLID, NT>(smem) : metric == M_MANHATTAN ? occupancy_of<HK_DENSE_AVX, M_MANHATTAN, NT>(smem) : occupancy_of<HK_DENSE_AVX, M_DOT, NT>(smem);
-        case HK_DENSE_SMALL: return metric == M_EUCLID ? occupancy_of<HK_DENSE_SMALL, M_EUCLID, NT>(smem) : metric == M_MANHATTAN ? occupancy_of<HK_DENSE_SMALL, M_MANHATTAN, NT>(smem) : occupancy_of<HK_DENSE_SMALL, M_DOT, NT>(smem);
-        case HK_SQ8: return occupancy_of<HK_SQ8, M_DOT, NT>(smem);
-        default: return occupancy_of<HK_SQ8_LANEX, M_DOT, NT>(smem);
+        case HK_DENSE_AVX: return metric == M_EUCLID ? occupancy_of<HK_DENSE_AVX, M_EUCLID, NT, ALGO>(smem) : metric == M_MANHATTAN ? occupancy_of<HK_DENSE_AVX, M_MANHATTAN, NT, ALGO>(smem) : occupancy_of<HK_DENSE_AVX, M_DOT, NT, ALGO>(smem);
+        case HK_DENSE_SMALL: return metric == M_EUCLID ? occupancy_of<HK_DENSE_SMALL, M_EUCLID, NT, ALGO>(smem) : metric == M_MANHATTAN ? occupancy_of<HK_DENSE_SMALL, M_MANHATTAN, NT, ALGO>(smem) : occupancy_of<HK_DENSE_SMALL, M_DOT, NT, ALGO>(smem);
+        case HK_SQ8: return occupancy_of<HK_SQ8, M_DOT, NT, ALGO>(smem);
+        default: return occupancy_of<HK_SQ8_LANEX, M_DOT, NT, ALGO>(smem);
     }
 }
-template <int NT>
+template <int NT, int ALGO>
 qb_status launch_dispatch(int kind, int metric, const HnswParams& p, unsigned grid, size_t smem, cudaStream_t stream) {
     switch (kind) {
-        case HK_DENSE_AVX: return launch_kind<HK_DENSE_AVX, NT>(metric, p, grid, smem, stream);
-        case HK_DENSE_SMALL: return launch_kind<HK_DENSE_SMALL, NT>(metric, p, grid, smem, stream);
-        case HK_SQ8: return launch_kind<HK_SQ8, NT>(metric, p, grid, smem, stream);
-        default: return launch_kind<HK_SQ8_LANEX, NT>(metric, p, grid, smem, stream);
+        case HK_DENSE_AVX: return launch_kind<HK_DENSE_AVX, NT, ALGO>(metric, p, grid, smem, stream);
+        case HK_DENSE_SMALL: return launch_kind<HK_DENSE_SMALL, NT, ALGO>(metric, p, grid, smem, stream);
+        case HK_SQ8: return launch_kind<HK_SQ8, NT, ALGO>(metric, p, grid, smem, stream);
+        default: return launch_kind<HK_SQ8_LANEX, NT, ALGO>(metric, p, grid, smem, stream);
     }
+}
+template <int ALGO>
+int occupancy_nt(int nt, int kind, int metric, size_t smem) {
+    return nt == 128 ? occupancy_dispatch<128, ALGO>(kind, metric, smem) : (nt == 64 ? occupancy_dispatch<64, ALGO>(kind, metric, smem) : occupancy_dispatch<256, ALGO>(kind, metric, smem));
+}
+template <int ALGO>
+qb_status launch_nt(int nt, int kind, int metric, const HnswParams& p, unsigned grid, size_t smem, cudaStream_t stream) {
+    return nt == 128 ? launch_dispatch<128, ALGO>(kind, metric, p, grid, smem, stream)
+                     : (nt == 64 ? launch_dispatch<64, ALGO>(kind, metric, p, grid, smem, stream) : launch_dispatch<256, ALGO>(kind, metric, p, grid, smem, stream));
 }
 
 }  // namespace
@@ -378,6 +531,16 @@ qb_status launch_dispatch(int kind, int metric, const HnswParams& p, unsigned gr
 // ------------------------------------------------------------------------------------------------ host side
 static size_t hnsw_smem_bytes(uint32_t q_bytes, uint32_t ef) {
     return (size_t)((q_bytes + 15u) & ~15u) + (size_t)ef * 16 + HNSW_MAX_LINKS * 16 + 2 * (size_t)((ef + 15u) & ~15u);
+}
+// ACORN: to_score holds up to m0 * m0 ids (a passing 1-hop links and at most m0 - a explored lists of m0), its keys sorted in a
+// power-of-two buffer; plus to_explore
+static uint32_t acorn_hop_cap(uint32_t m0) {
+    uint32_t c = HNSW_MAX_LINKS;
+    while (c < m0 * m0) c <<= 1;
+    return c;
+}
+static size_t acorn_smem_bytes(uint32_t q_bytes, uint32_t ef, uint32_t hop_cap) {
+    return (size_t)((q_bytes + 15u) & ~15u) + (size_t)ef * 16 + (size_t)hop_cap * 16 + 2 * (size_t)((ef + 15u) & ~15u) + HNSW_MAX_LINKS * 4;
 }
 
 __global__ void hnsw_links0_kernel(const uint32_t* __restrict__ neighbors, const uint64_t* __restrict__ offsets, uint32_t n, uint32_t m0, uint32_t* __restrict__ links0) {
@@ -773,8 +936,9 @@ extern "C" qb_status qb_hnsw_info(const qb_hnsw* g, uint32_t* n_points, uint32_t
 
 // queries already encoded (d_q_enc / d_q_off); results to device buffers; enqueued on `stream`, no synchronisation
 qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, uint32_t nq, uint32_t top, uint32_t ef, uint32_t entry, uint32_t entry_level,
-                         const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts, cudaStream_t stream) {
+                         const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts, cudaStream_t stream, int algo) {
     qb_storage* s = g->st;
+    QB_CHECK(algo == ALGO_HNSW || algo == ALGO_ACORN, QB_ERR_INVALID, "hnsw_search: algorithm %d is neither QB_HNSW_ALGO_HNSW nor QB_HNSW_ALGO_ACORN", algo);
     QB_CHECK(entry < g->n_points, QB_ERR_INVALID, "hnsw_search: entry point %u out of range", entry);
     QB_CHECK(entry_level < std::max<uint32_t>(g->levels, 1), QB_ERR_INVALID, "hnsw_search: entry level %u but the graph has %u levels", entry_level, g->levels);
     ef = std::max(ef, top);   // graph_layers.rs:551
@@ -793,12 +957,14 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
     p.nq = nq; p.top = top; p.ef = ef; p.entry = entry; p.entry_level = entry_level;
     p.deleted = s->d_deleted; p.deleted2 = d_deleted2;
     p.out = d_out; p.out_counts = d_counts; p.id_base = s->id_base; p.stats = g->d_stats;
-    const size_t smem = hnsw_smem_bytes(p.q_bytes, ef);
+    const bool acorn = algo == ALGO_ACORN;
+    p.hop_cap = acorn ? acorn_hop_cap(g->m0) : HNSW_MAX_LINKS;
+    const size_t smem = acorn ? acorn_smem_bytes(p.q_bytes, ef, p.hop_cap) : hnsw_smem_bytes(p.q_bytes, ef);
     QB_CHECK(smem <= 200 * 1024, QB_ERR_UNSUPPORTED, "hnsw_search: query (%u B) + ef %u need %zu B of shared memory", p.q_bytes, ef, smem);
     // threads per CTA: 256 = one 8-lane group per level-0 link (m0 = 32), fewer queries in flight per SM; 128 (default) = two scoring rounds
     // per hop, twice the resident queries.  The traversal is a chain of dependent memory round trips, so queries in flight is what hides them.
     const int nt = qb_opt().hnsw_threads == 256 ? 256 : (qb_opt().hnsw_threads == 64 ? 64 : 128);
-    const int per_sm = nt == 128 ? occupancy_dispatch<128>(kind, metric, smem) : (nt == 64 ? occupancy_dispatch<64>(kind, metric, smem) : occupancy_dispatch<256>(kind, metric, smem));
+    const int per_sm = acorn ? occupancy_nt<ALGO_ACORN>(nt, kind, metric, smem) : occupancy_nt<ALGO_HNSW>(nt, kind, metric, smem);
     p.prefetch = qb_opt().hnsw_no_prefetch ? 0 : 1;
     const unsigned max_grid = (unsigned)s->sm_count * (unsigned)per_sm;
     const unsigned grid = std::min<unsigned>(max_grid, nq);
@@ -814,8 +980,7 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
     }
     p.visited = g->d_visited; p.visited_words = words; p.vlog = g->d_vlog; p.vlog_cap = g->vlog_cap; p.work = g->d_work;
     QB_CUDA(cudaMemsetAsync(g->d_work, 0, 4, stream));
-    return nt == 128 ? launch_dispatch<128>(kind, metric, p, grid, smem, stream)
-                     : (nt == 64 ? launch_dispatch<64>(kind, metric, p, grid, smem, stream) : launch_dispatch<256>(kind, metric, p, grid, smem, stream));
+    return acorn ? launch_nt<ALGO_ACORN>(nt, kind, metric, p, grid, smem, stream) : launch_nt<ALGO_HNSW>(nt, kind, metric, p, grid, smem, stream);
 }
 
 qb_status qb_hnsw_read_stats(qb_hnsw* g, cudaStream_t stream) {

@@ -151,7 +151,7 @@ struct qb_hnsw {
 };
 
 qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, uint32_t nq, uint32_t top, uint32_t ef, uint32_t entry, uint32_t entry_level,
-                         const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts, cudaStream_t stream);
+                         const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts, cudaStream_t stream, int algo /* qb_hnsw_algorithm */);
 qb_status qb_hnsw_read_stats(qb_hnsw* g, cudaStream_t stream);
 
 // One rank of a sharded search (qb_comm.cu): an exchange buffer every peer maps + the peers' buffers

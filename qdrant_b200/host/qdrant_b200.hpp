@@ -219,12 +219,16 @@ public:
         if (count) check(qb_hnsw_links(h_, level, &point, 1, count, out.data(), &count));
         return out;
     }
+    // SearchAlgorithm (graph_layers.rs:80-84): the level-0 algorithm; the caller decides as hnsw/read_view/search.rs:59-86 does
+    enum class SearchAlgorithm : int32_t { Hnsw = QB_HNSW_ALGO_HNSW, Acorn = QB_HNSW_ALGO_ACORN };
     // entry_point / entry_level = GraphLayers::get_entry_point(filters, custom_entry_points); deleted = the filter as a bitmap (bit = 1: skip)
     std::vector<std::vector<ScoredPointOffset>> search(const float* queries, uint32_t n_queries, uint32_t top, uint32_t ef, PointOffsetType entry_point,
-                                                       uint32_t entry_level, const uint64_t* deleted = nullptr) const {
+                                                       uint32_t entry_level, const uint64_t* deleted = nullptr,
+                                                       SearchAlgorithm algorithm = SearchAlgorithm::Hnsw) const {
         std::vector<ScoredPointOffset> flat((size_t)n_queries * top);
         std::vector<uint32_t> counts(n_queries);
-        check(qb_hnsw_search_batch(h_, queries, n_queries, top, ef, entry_point, entry_level, deleted, nullptr, flat.data(), counts.data(), nullptr));
+        check(qb_hnsw_search_batch_algo(h_, queries, n_queries, top, ef, entry_point, entry_level, deleted, nullptr, flat.data(), counts.data(), nullptr,
+                                        static_cast<qb_hnsw_algorithm>(algorithm)));
         std::vector<std::vector<ScoredPointOffset>> out(n_queries);
         for (uint32_t q = 0; q < n_queries; ++q) out[q].assign(flat.begin() + (size_t)q * top, flat.begin() + (size_t)q * top + counts[q]);
         return out;

@@ -752,7 +752,14 @@ class HnswGraph:
         check(lib().qb_hnsw_info(self._h, C.byref(a), C.byref(b), C.byref(c)))
         return int(a.value), int(b.value), int(c.value)
 
-    def search(self, queries, top: int, ef: int, entry_point: int, entry_level: int, point_deleted=None, counters: Optional[HwCounters] = None):
+    ALGORITHMS = {"hnsw": 0, "acorn": 1}   # qb_hnsw_algorithm (SearchAlgorithm, graph_layers.rs:80-84)
+
+    def search(self, queries, top: int, ef: int, entry_point: int, entry_level: int, point_deleted=None, counters: Optional[HwCounters] = None,
+               algorithm: str = "hnsw"):
+        """algorithm: "hnsw" (search_on_level) or "acorn" (ACORN-1, search_on_level_acorn) on level 0; which one a filtered request
+        takes is the caller's decision (include/qb200.h, qb_hnsw_algorithm)."""
+        if algorithm not in self.ALGORITHMS:
+            raise ValueError(f"algorithm {algorithm!r} is not one of {sorted(self.ALGORITHMS)}")
         q = np.atleast_2d(_f32(queries))
         if q.shape[1] != self._storage.dim:
             raise ValueError(f"queries have dim {q.shape[1]}, storage has {self._storage.dim}")
@@ -760,9 +767,9 @@ class HnswGraph:
         out = np.zeros((nq, max(top, 1)), dtype=SCORED_POINT_OFFSET)
         counts = np.zeros(nq, dtype=np.uint32)
         bm = _bitmap(point_deleted, self._storage.count)
-        check(lib().qb_hnsw_search_batch(self._h, q.ctypes.data_as(f32p), nq, int(top), int(ef), int(entry_point), int(entry_level),
-                                         None if bm is None else bm.ctypes.data_as(u64p), None, out.ctypes.data_as(C.POINTER(ScoredPoint)),
-                                         counts.ctypes.data_as(u32p), None if counters is None else C.byref(counters)))
+        check(lib().qb_hnsw_search_batch_algo(self._h, q.ctypes.data_as(f32p), nq, int(top), int(ef), int(entry_point), int(entry_level),
+                                              None if bm is None else bm.ctypes.data_as(u64p), None, out.ctypes.data_as(C.POINTER(ScoredPoint)),
+                                              counts.ctypes.data_as(u32p), None if counters is None else C.byref(counters), self.ALGORITHMS[algorithm]))
         return [out[i, : counts[i]].copy() for i in range(nq)]
 
     def stats(self, reset: bool = True) -> tuple[int, int]:
