@@ -1,12 +1,21 @@
 //! `GraphLayers::search` (lib/segment/src/index/hnsw_index/graph_layers.rs:530-561) for a batch of queries with the traversal on the GPU.
 //! SOURCE ONLY (see ffi.rs).  The graph is handed over as the bytes of `links.bin`, either in GraphLinksFormat::Compressed (what
 //! the reference writes for every index it builds, view.rs:137-163; decoded on the device) or in GraphLinksFormat::Plain (view.rs:121-135).
+use common::counter::hardware_counter::HardwareCounterCell;
 use common::types::{PointOffsetType, ScoredPointOffset};
 
 use super::ffi::*;
+use crate::data_types::vectors::{QueryVector, VectorInternal};
 use crate::index::hnsw_index::graph_layers::SearchAlgorithm;
 use super::raw_scorer::{last_error, B200Storage};
 use crate::common::operation_error::{OperationError, OperationResult};
+
+// qb_query_kind (include/qb200.h), passed as i32
+const QB_QUERY_RECO_BEST_SCORE: i32 = 1;
+const QB_QUERY_RECO_SUM_SCORES: i32 = 2;
+const QB_QUERY_DISCOVER: i32 = 3;
+const QB_QUERY_CONTEXT: i32 = 4;
+const QB_QUERY_FEEDBACK_NAIVE: i32 = 5;
 
 pub struct B200Hnsw<'a> { raw: *mut qb_hnsw, _storage: std::marker::PhantomData<&'a B200Storage> }
 unsafe impl Send for B200Hnsw<'_> {}
@@ -44,5 +53,81 @@ impl<'a> B200Hnsw<'a> {
         };
         assert!(st == QB_OK, "{}", last_error());
         (0..n_queries).map(|q| out[q * top..q * top + counts[q] as usize].iter().map(|p| ScoredPointOffset { idx: p.idx, score: p.score }).collect()).collect()
+    }
+
+    /// `GraphLayers::search` with a custom `FilteredScorer` for ONE query vector of `search_vectors_with_graph`
+    /// (hnsw/read_view/search.rs:181-208): RecommendBestScore / RecommendSumScores / Context through qb_hnsw_search_custom_batch,
+    /// Discover through qb_hnsw_search_discover_batch (both stages of discover_search_with_graph, :314-349, in one call).
+    /// Nearest goes through `search_batch`; a feedback query goes through `search_feedback` (its pairs and coefficients are computed
+    /// by the caller's FeedbackQuery).  `custom_entry_points` is GraphLayers::search's argument (not used for discover).
+    pub fn search_custom(&self, query: &QueryVector, top: usize, ef: usize, entry: (PointOffsetType, usize), deleted: Option<&[u64]>,
+                         custom_entry_points: Option<&[PointOffsetType]>, algorithm: SearchAlgorithm, hc: &HardwareCounterCell)
+                         -> OperationResult<Vec<ScoredPointOffset>> {
+        let dense = |v: &VectorInternal| -> OperationResult<Vec<f32>> {
+            match v { VectorInternal::Dense(d) => Ok(d.clone()), _ => Err(OperationError::service_error("device traversal: dense examples only")) }
+        };
+        let (kind, mut flat, n_a, n_b) = match query {
+            QueryVector::RecommendBestScore(r) | QueryVector::RecommendSumScores(r) => {
+                let kind = if matches!(query, QueryVector::RecommendBestScore(_)) { QB_QUERY_RECO_BEST_SCORE } else { QB_QUERY_RECO_SUM_SCORES };
+                (kind, Vec::new(), r.positives.len(), r.negatives.len())
+            }
+            QueryVector::Context(c) => (QB_QUERY_CONTEXT, Vec::new(), c.pairs.len(), 0),
+            QueryVector::Discover(d) => (QB_QUERY_DISCOVER, Vec::new(), d.pairs.len(), 0),
+            _ => return Err(OperationError::service_error("search_custom: nearest / feedback queries have their own calls")),
+        };
+        match query {
+            QueryVector::RecommendBestScore(r) | QueryVector::RecommendSumScores(r) => {
+                for v in r.positives.iter().chain(r.negatives.iter()) { flat.extend(dense(v)?); }
+            }
+            QueryVector::Context(c) => { for p in &c.pairs { flat.extend(dense(&p.positive)?); flat.extend(dense(&p.negative)?); } }
+            QueryVector::Discover(d) => {
+                flat.extend(dense(&d.target)?);
+                for p in &d.pairs { flat.extend(dense(&p.positive)?); flat.extend(dense(&p.negative)?); }
+            }
+            _ => unreachable!(),
+        }
+        let mut out = vec![qb_scored_point::default(); top];
+        let mut count = 0u32;
+        let mut counters = qb_hw_counters::default();
+        let algo = match algorithm { SearchAlgorithm::Hnsw => QB_HNSW_ALGO_HNSW, SearchAlgorithm::Acorn => QB_HNSW_ALGO_ACORN };
+        let del = deleted.map_or(std::ptr::null(), |d| d.as_ptr());
+        let st = unsafe {
+            if kind == QB_QUERY_DISCOVER {
+                qb_hnsw_search_discover_batch(self.raw, flat.as_ptr(), n_a as u32, 1, top as u32, ef as u32, entry.0, entry.1 as u32, del, std::ptr::null(),
+                                              out.as_mut_ptr(), &mut count, &mut counters, algo)
+            } else {
+                let n_custom = custom_entry_points.map_or(0, |c| c.len() as u32);
+                qb_hnsw_search_custom_batch(self.raw, kind, flat.as_ptr(), n_a as u32, n_b as u32, std::ptr::null(), 1, top as u32, ef as u32, entry.0,
+                                            entry.1 as u32, custom_entry_points.map_or(std::ptr::null(), |c| c.as_ptr()), &n_custom, n_custom.max(1),
+                                            del, std::ptr::null(), out.as_mut_ptr(), &mut count, &mut counters, algo)
+            }
+        };
+        if st != QB_OK { return Err(OperationError::service_error(last_error())); }
+        hc.cpu_counter().incr_delta(counters.cpu as usize);
+        hc.vector_io_read().incr_delta(counters.vector_io_read as usize);
+        Ok(out[..count as usize].iter().map(|p| ScoredPointOffset { idx: p.idx, score: p.score }).collect())
+    }
+
+    /// A naive-feedback query (FeedbackQuery, feedback_query.rs:150-226) through the device traversal: `target`, then its context pairs
+    /// as (positive, negative) rows in `pairs`, `a` and each pair's partial_computation.
+    pub fn search_feedback(&self, target: &[f32], pairs: &[f32], a: f32, partial: &[f32], top: usize, ef: usize, entry: (PointOffsetType, usize),
+                           deleted: Option<&[u64]>, algorithm: SearchAlgorithm, hc: &HardwareCounterCell) -> OperationResult<Vec<ScoredPointOffset>> {
+        let mut flat = target.to_vec();
+        flat.extend_from_slice(pairs);
+        let mut coef = vec![a];
+        coef.extend_from_slice(partial);
+        let mut out = vec![qb_scored_point::default(); top];
+        let mut count = 0u32;
+        let mut counters = qb_hw_counters::default();
+        let algo = match algorithm { SearchAlgorithm::Hnsw => QB_HNSW_ALGO_HNSW, SearchAlgorithm::Acorn => QB_HNSW_ALGO_ACORN };
+        let st = unsafe {
+            qb_hnsw_search_custom_batch(self.raw, QB_QUERY_FEEDBACK_NAIVE, flat.as_ptr(), partial.len() as u32, 0, coef.as_ptr(), 1, top as u32, ef as u32,
+                                        entry.0, entry.1 as u32, std::ptr::null(), std::ptr::null(), 0, deleted.map_or(std::ptr::null(), |d| d.as_ptr()),
+                                        std::ptr::null(), out.as_mut_ptr(), &mut count, &mut counters, algo)
+        };
+        if st != QB_OK { return Err(OperationError::service_error(last_error())); }
+        hc.cpu_counter().incr_delta(counters.cpu as usize);
+        hc.vector_io_read().incr_delta(counters.vector_io_read as usize);
+        Ok(out[..count as usize].iter().map(|p| ScoredPointOffset { idx: p.idx, score: p.score }).collect())
     }
 }

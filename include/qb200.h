@@ -406,6 +406,49 @@ QB_API qb_status qb_hnsw_search_batch_device_algo(qb_hnsw* g, const float* dev_q
 /* scorer calls (hops) and scored points since the last reset, summed over all searches on this graph (waits for them) */
 QB_API qb_status qb_hnsw_stats(qb_hnsw* g, uint64_t* hops, uint64_t* scored_points, int32_t reset);
 
+/* Custom queries (recommend, context, feedback) through the device traversal: GraphLayers::search with a custom FilteredScorer
+ * (hnsw/read_view/search.rs:181-208).  A point's score is qb_score_points on a qb_scorer_create_custom / qb_scorer_create_feedback
+ * scorer of the same examples, bit for bit.
+ *   kind, n_a, n_b  one kind and one shape per call (qb_scorer_create_custom's table); queries of other shapes go in other calls.
+ *                   QB_QUERY_DISCOVER here is ONE discover search (the reference's second stage); qb_hnsw_search_discover_batch
+ *                   below runs both stages
+ *   vectors         n_queries x E x dim raw f32, each query's E examples in the qb_scorer_create_custom layout
+ *   coef            QB_QUERY_FEEDBACK_NAIVE: n_queries x (1 + n_a) values [a, partial_computation of pair 0, ...]; NULL otherwise
+ *   custom_entry_points  optional, n_queries x n_custom point offsets in entry_point's id space (GraphLayers::search's
+ *                   custom_entry_points), custom_counts[q] of
+ *                   them valid.  Per query the device restates get_entry_point (graph_layers.rs:506-528): of the candidates that pass
+ *                   the filter, the one with the highest point level, the LAST of several equal maxima (Iterator::max_by_key); if
+ *                   none passes, entry_point / entry_level
+ *   counters        cpu += scored points x E x cpu units, vector_io_read += scored points x io units (custom_query_scorer.rs:78-111)
+ * The rest is as for qb_hnsw_search_batch_algo.  Dense f32 and SQ8 storages only (QB_ERR_UNSUPPORTED otherwise).
+ *
+ * Ties.  Context scores are sums of fast_sigmoid(min(d, 0)): every point that satisfies all pairs scores exactly 0.0, so custom
+ * scores tie often.  The device orders equal scores by id (score desc, id asc) in every comparison of the level-0 search:
+ * `nearest` insertion and eviction, the candidate order and the stop test; the greedy descent through the upper levels moves
+ * only to a strictly greater score, as the reference does.  The reference leaves ties to heap order, so on a plateau the two
+ * traversals may visit different points.  The contract: lists equal the reference traversal whenever scores are distinct, and
+ * on ties they equal the reference traversal with every level-0 comparison made on (score desc, id asc) keys. */
+QB_API qb_status qb_hnsw_search_custom_batch(qb_hnsw* g, qb_query_kind kind, const float* vectors, uint32_t n_a, uint32_t n_b, const float* coef,
+                                             uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point, uint32_t entry_level,
+                                             const uint32_t* custom_entry_points, const uint32_t* custom_counts, uint32_t n_custom,
+                                             const uint64_t* deleted_bitmap, const volatile int32_t* is_stopped, qb_scored_point* out,
+                                             uint32_t* out_counts, qb_hw_counters* counters /* optional */, qb_hnsw_algorithm algorithm);
+/* Discover (discover_search_with_graph, search.rs:314-349) as one call with no host round trip between its stages:
+ *   1. a context search over the query's pairs: top 10 (DISCOVERY_ENTRY_POINT_COUNT), the same ef, filter, algorithm and entry
+ *      point; it scores the encoded pair examples of the discover query (the target is skipped, nothing is encoded twice);
+ *   2. the discover search, with the stage-1 list as the query's custom entry points (get_entry_point, as above).
+ *   vectors   n_queries x (1 + 2 n_pairs) x dim raw f32: the target, then n_pairs (positive, negative) pairs; n_pairs >= 1
+ * Hops, scored points and counters sum both stages (one HardwareCounterCell in the reference); the tie contract is the one above.
+ * This is the reference's path when the search is not rescored: dense storages, or quantized searches without oversampling or
+ * rescoring.  A rescored quantized discover oversamples and rescores stage 1 against the original vectors
+ * (search_with_graph -> postprocess_search_result); compose it from the parts: qb_hnsw_search_custom_batch(QB_QUERY_CONTEXT) with
+ * the oversampled top, qb_scorer_create_custom(original storage, QB_QUERY_CONTEXT, ...) + qb_rescore down to 10, then
+ * qb_hnsw_search_custom_batch(QB_QUERY_DISCOVER) with those ids as custom_entry_points. */
+QB_API qb_status qb_hnsw_search_discover_batch(qb_hnsw* g, const float* vectors, uint32_t n_pairs, uint32_t n_queries, uint32_t top, uint32_t ef,
+                                               uint32_t entry_point, uint32_t entry_level, const uint64_t* deleted_bitmap,
+                                               const volatile int32_t* is_stopped, qb_scored_point* out, uint32_t* out_counts,
+                                               qb_hw_counters* counters /* optional */, qb_hnsw_algorithm algorithm);
+
 /* ---------------------------------------------------------------- profiling hooks ------------------- */
 /* Fused searches run a fast path first and rerun without it when the device reports that one of its assumptions did not
  * hold (candidate buffer overflow, a dot product outside the f32-exact window, a survivor segment full).  searches =

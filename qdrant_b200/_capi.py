@@ -102,6 +102,10 @@ SIGNATURES = {
                                               u32p, C.POINTER(HwCounters), C.c_int32]),
     "qb_hnsw_search_batch_device_algo": (C.c_int32, [vp, vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, vp, vp, C.c_int32]),
     "qb_hnsw_stats": (C.c_int32, [vp, u64p, u64p, C.c_int32]),
+    "qb_hnsw_search_custom_batch": (C.c_int32, [vp, C.c_int, f32p, C.c_uint32, C.c_uint32, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                u32p, u32p, C.c_uint32, u64p, i32p, C.POINTER(ScoredPoint), u32p, C.POINTER(HwCounters), C.c_int32]),
+    "qb_hnsw_search_discover_batch": (C.c_int32, [vp, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, u64p, i32p,
+                                                  C.POINTER(ScoredPoint), u32p, C.POINTER(HwCounters), C.c_int32]),
     "qb_profile_enable": (C.c_int32, [vp, C.c_int32]),
     "qb_profile_read": (C.c_int32, [vp, u64p, C.POINTER(C.c_double), C.c_int32]),
 }

@@ -1708,6 +1708,126 @@ extern "C" qb_status qb_hnsw_search_batch_device(qb_hnsw* g, const float* dev_qu
     return qb_hnsw_search_batch_device_algo(g, dev_queries, n_queries, top, ef, entry_point, entry_level, dev_out, dev_counts, QB_HNSW_ALGO_HNSW);
 }
 
+// custom queries through the device traversal; discover_pairs > 0: the two-stage discover of that many pairs (kind = DISCOVER)
+static qb_status hnsw_custom_run(qb_hnsw* g, qb_query_kind kind, const float* vectors, uint32_t n_a, uint32_t n_b, const float* coef, uint32_t n_queries,
+                                 uint32_t top, uint32_t ef, uint32_t entry_point, uint32_t entry_level, const uint32_t* cep, const uint32_t* cep_counts,
+                                 uint32_t n_custom, const uint64_t* deleted_bitmap, const volatile int32_t* is_stopped, qb_scored_point* out,
+                                 uint32_t* out_counts, qb_hw_counters* counters, qb_hnsw_algorithm algorithm, bool discover, const char* what) {
+    QB_CHECK(g && out && out_counts, QB_ERR_INVALID, "%s: null argument", what);
+    QB_CHECK(n_queries == 0 || vectors, QB_ERR_INVALID, "%s: null vectors", what);
+    QB_CHECK(top >= 1 && top <= 4096, QB_ERR_INVALID, "%s: top %u outside [1,4096]", what, top);
+    uint32_t ne = 0;
+    QB_TRY(check_custom(kind, n_a, n_b, &ne));
+    QB_CHECK(!discover || n_a >= 1, QB_ERR_INVALID, "%s: discover needs at least one (positive, negative) pair for its context stage", what);
+    const bool fb = kind == QB_QUERY_FEEDBACK_NAIVE;
+    QB_CHECK(fb == (coef != nullptr), QB_ERR_INVALID, "%s: coef is required for feedback queries and must be NULL otherwise", what);
+    QB_CHECK(!cep || (cep_counts && n_custom >= 1), QB_ERR_INVALID, "%s: custom_entry_points need custom_counts and n_custom >= 1", what);
+    qb_storage* s = g->st;
+    QB_CHECK((s->kind == QB_KIND_DENSE && s->dtype == QB_DT_F32) || s->kind == QB_KIND_SQ8, QB_ERR_UNSUPPORTED,
+             "%s: device traversal supports dense f32 and SQ8 storages (others go through qb_score_points per hop)", what);
+    if (cep) {
+        for (uint32_t q = 0; q < n_queries; ++q) {
+            QB_CHECK(cep_counts[q] <= n_custom, QB_ERR_INVALID, "%s: custom_counts[%u] = %u > n_custom %u", what, q, cep_counts[q], n_custom);
+            for (uint32_t i = 0; i < cep_counts[q]; ++i)
+                QB_CHECK(cep[(size_t)q * n_custom + i] < g->n_points, QB_ERR_INVALID, "%s: custom entry point %u out of range", what, cep[(size_t)q * n_custom + i]);
+        }
+    }
+    if (n_queries == 0) return QB_OK;
+    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    QB_TRY(use_device(s->device));
+    std::lock_guard<std::mutex> glk(g->mu);
+    QbSearchCtx* c = nullptr;
+    QB_TRY(qb_ctx_acquire(s, &c));
+    struct Rel { qb_storage* s; QbSearchCtx* c; ~Rel() { qb_ctx_release(s, c); } } rel{s, c};
+    cudaStream_t stream = c->stream;
+    const size_t nv = (size_t)n_queries * ne;   // example vectors, encoded back to back: query q's are [q * ne, (q + 1) * ne)
+    const size_t raw_bytes = nv * s->dim * 4, res_bytes = (size_t)n_queries * top * sizeof(qb_scored_point), cnt_bytes = (size_t)n_queries * 4;
+    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, raw_bytes + res_bytes + cnt_bytes + 16));
+    uint8_t* hs = reinterpret_cast<uint8_t*>(c->h_stage);
+    memcpy(hs, vectors, raw_bytes);
+    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, raw_bytes + nv * pre_stride_f(s) * 4));
+    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, (nv + 256) * qb_encoded_query_bytes(s)));
+    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, nv));
+    QB_TRY(ensure_dev_elems(&c->d_out, &c->out_elems, (size_t)n_queries * top));
+    QB_TRY(ensure_dev_elems(&c->d_out_counts, &c->out_counts_elems, (size_t)n_queries + 4));
+    QB_CUDA(cudaMemcpyAsync(c->d_queries_raw, hs, raw_bytes, cudaMemcpyHostToDevice, stream));
+    float* d_pre = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c->d_queries_raw) + raw_bytes);
+    QB_TRY(prepare_queries(s, reinterpret_cast<const float*>(c->d_queries_raw), (uint32_t)nv, d_pre, c->d_queries_enc, c->d_q_off, stream));
+    const uint32_t* d_del2 = nullptr;
+    if (deleted_bitmap) {
+        const uint64_t words64 = ceil_div_u64(s->count, 64);
+        QB_TRY(ensure_dev_elems(&c->d_deleted2, &c->deleted2_words, (size_t)words64 * 2));
+        QB_CUDA(cudaMemcpyAsync(c->d_deleted2, deleted_bitmap, words64 * 8, cudaMemcpyHostToDevice, stream));
+        d_del2 = c->d_deleted2;
+    }
+    // per-call buffers: coefficients, custom entry points (as scored points: the stage-1 lists of discover have that layout), counts
+    constexpr uint32_t DISCOVERY_ENTRY_POINT_COUNT = 10;   // search.rs:325
+    const uint32_t n_coef = fb ? 1 + n_a : 0;
+    const uint32_t n_cep = discover ? DISCOVERY_ENTRY_POINT_COUNT : (cep ? n_custom : 0);
+    const size_t coef_bytes = round_up_u64((size_t)n_queries * n_coef * 4, 256), cep_bytes = round_up_u64((size_t)n_queries * n_cep * sizeof(qb_scored_point), 256);
+    std::vector<uint8_t> h_extra(coef_bytes + cep_bytes + (size_t)n_queries * 4, 0);
+    if (fb) memcpy(h_extra.data(), coef, (size_t)n_queries * n_coef * 4);
+    if (cep && !discover) {
+        qb_scored_point* hp = reinterpret_cast<qb_scored_point*>(h_extra.data() + coef_bytes);
+        for (size_t i = 0; i < (size_t)n_queries * n_cep; ++i) hp[i].idx = cep[i];
+        memcpy(h_extra.data() + coef_bytes + cep_bytes, cep_counts, (size_t)n_queries * 4);
+    }
+    struct Scratch { void* p = nullptr; ~Scratch() { cudaFree(p); } } extra;
+    QB_CUDA(cudaMalloc(&extra.p, h_extra.size() + 256));
+    uint8_t* d_extra = reinterpret_cast<uint8_t*>(extra.p);
+    if (fb || (cep && !discover)) QB_CUDA(cudaMemcpyAsync(d_extra, h_extra.data(), h_extra.size(), cudaMemcpyHostToDevice, stream));
+    QbHnswCustom cq{};
+    cq.kind = (int)kind; cq.n_a = n_a; cq.n_b = n_b; cq.n_ex = ne; cq.ex_first = 0; cq.ex_stride = ne;
+    cq.d_coef = fb ? reinterpret_cast<const float*>(d_extra) : nullptr; cq.n_coef = n_coef;
+    qb_scored_point* d_cep = reinterpret_cast<qb_scored_point*>(d_extra + coef_bytes);
+    uint32_t* d_cep_counts = reinterpret_cast<uint32_t*>(d_extra + coef_bytes + cep_bytes);
+    if (n_cep) { cq.d_cep = d_cep; cq.d_cep_counts = d_cep_counts; cq.n_cep = n_cep; }
+    cudaEvent_t e0, e1;
+    profile_begin(s, c, stream, &e0, &e1);   // qb_profile_*: the traversal kernels (both stages of discover)
+    if (discover) {
+        // stage 1: the context search over the pairs (encoded examples 1 .. 2 n_pairs of each query), top 10, its lists left on the device
+        QbHnswCustom ctx{};
+        ctx.kind = QB_QUERY_CONTEXT; ctx.n_a = n_a; ctx.n_b = 0; ctx.n_ex = 2 * n_a; ctx.ex_first = 1; ctx.ex_stride = ne;
+        ctx.stats_slot = 1; ctx.internal_out = true;
+        QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, DISCOVERY_ENTRY_POINT_COUNT, ef, entry_point, entry_level, d_del2, d_cep,
+                              d_cep_counts, stream, (int)algorithm, &ctx));
+    }
+    QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, d_del2, c->d_out, c->d_out_counts, stream,
+                          (int)algorithm, &cq));
+    profile_end(s, stream, e0, e1);
+    QB_CUDA(cudaMemcpyAsync(hs + raw_bytes, c->d_out, res_bytes, cudaMemcpyDeviceToHost, stream));
+    QB_CUDA(cudaMemcpyAsync(hs + raw_bytes + res_bytes, c->d_out_counts, cnt_bytes, cudaMemcpyDeviceToHost, stream));
+    QB_CUDA(cudaStreamSynchronize(stream));
+    memcpy(out, hs + raw_bytes, res_bytes);
+    memcpy(out_counts, hs + raw_bytes + res_bytes, cnt_bytes);
+    if (counters) {
+        // per scored point: E similarities of cpu units, one read of the vector (custom_query_scorer.rs:78-111, qb_score_points)
+        uint64_t ev[2] = {0, 0};
+        QB_TRY(qb_hnsw_read_stats(g, stream, ev));
+        counters->cpu += (ev[0] * ne + ev[1] * (2ull * n_a)) * cpu_units_per_point(s);
+        counters->vector_io_read += (ev[0] + ev[1]) * io_units_per_point(s);
+    }
+    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    return QB_OK;
+}
+
+extern "C" qb_status qb_hnsw_search_custom_batch(qb_hnsw* g, qb_query_kind kind, const float* vectors, uint32_t n_a, uint32_t n_b, const float* coef,
+                                                 uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point, uint32_t entry_level,
+                                                 const uint32_t* custom_entry_points, const uint32_t* custom_counts, uint32_t n_custom,
+                                                 const uint64_t* deleted_bitmap, const volatile int32_t* is_stopped, qb_scored_point* out,
+                                                 uint32_t* out_counts, qb_hw_counters* counters, qb_hnsw_algorithm algorithm) {
+    return hnsw_custom_run(g, kind, vectors, n_a, n_b, coef, n_queries, top, ef, entry_point, entry_level, custom_entry_points, custom_counts, n_custom,
+                           deleted_bitmap, is_stopped, out, out_counts, counters, algorithm, false, "hnsw_search_custom_batch");
+}
+
+extern "C" qb_status qb_hnsw_search_discover_batch(qb_hnsw* g, const float* vectors, uint32_t n_pairs, uint32_t n_queries, uint32_t top, uint32_t ef,
+                                                   uint32_t entry_point, uint32_t entry_level, const uint64_t* deleted_bitmap,
+                                                   const volatile int32_t* is_stopped, qb_scored_point* out, uint32_t* out_counts,
+                                                   qb_hw_counters* counters, qb_hnsw_algorithm algorithm) {
+    return hnsw_custom_run(g, QB_QUERY_DISCOVER, vectors, n_pairs, 0, nullptr, n_queries, top, ef, entry_point, entry_level, nullptr, nullptr, 0,
+                           deleted_bitmap, is_stopped, out, out_counts, counters, algorithm, true, "hnsw_search_discover_batch");
+}
+
 extern "C" qb_status qb_hnsw_stats(qb_hnsw* g, uint64_t* hops, uint64_t* scored_points, int32_t reset) {
     QB_CHECK(g, QB_ERR_INVALID, "hnsw_stats: null graph");
     QB_TRY(use_device(g->st->device));

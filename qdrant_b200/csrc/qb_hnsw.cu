@@ -32,6 +32,7 @@
 
 #include <algorithm>
 
+#include "qb_fold.cuh"
 #include "qb_internal.h"
 #include "qb_score.cuh"
 
@@ -45,6 +46,7 @@ namespace {
 constexpr uint32_t HNSW_MAX_LINKS = 64;      // links scored per hop (m0 <= 64)
 constexpr uint32_t HNSW_EMPTY = 0xFFFFFFFFu;
 constexpr uint32_t HNSW_MAX_EF = 4096;
+constexpr uint32_t HNSW_CUSTOM_SMEM = 48 * 1024;   // custom queries: examples up to this size are staged in shared memory
 
 enum { HK_DENSE_AVX = 0, HK_DENSE_SMALL = 1, HK_SQ8 = 2, HK_SQ8_LANEX = 3 };
 
@@ -74,6 +76,15 @@ struct HnswParams {
     int prefetch;                                // 1: bulk-prefetch the surviving neighbours' vectors into L2 before scoring
     // ACORN only (appended so the HNSW kernels' parameter offsets stay as they were)
     uint32_t hop_cap;                            // per-hop buffers: a power of two >= m0 * m0
+    // custom queries only (appended likewise).  Query q's examples are encoded queries ex_first .. ex_first + n_ex of the
+    // ex_stride that q_enc / q_off hold per query (discover's context stage skips the target: ex_first = 1)
+    int ckind; uint32_t n_a, n_b;                // qb_query_kind and its shape (qbf::fold)
+    uint32_t n_ex, ex_first, ex_stride;
+    uint32_t ex_smem;                            // 1: the examples are staged in shared memory, 0: read from q_enc (too large)
+    uint32_t q_smem;                             // bytes of shared memory the query / examples take
+    const float* coef; uint32_t n_coef;          // feedback: [a, partial...] per query
+    const qb_scored_point* cep; const uint32_t* cep_counts; uint32_t n_cep;   // custom_entry_points: [nq][n_cep], .idx used
+    uint64_t lo_end;                             // level_offsets[levels] (point_level, view.rs:354-369)
 };
 
 struct HnswSmem {
@@ -82,7 +93,7 @@ struct HnswSmem {
     unsigned long long* newk;   // [HNSW_MAX_LINKS] (ACORN: [hop_cap])
     uint32_t* ids;              // [HNSW_MAX_LINKS] (ACORN: [hop_cap])
     float* sc;                  // [HNSW_MAX_LINKS] (ACORN: [hop_cap])
-    const uint8_t* q;           // query
+    const uint8_t* q;           // query (custom: the first example, in shared or global memory; example e at q + e * q_bytes)
 };
 
 enum { ALGO_HNSW = 0, ALGO_ACORN = 1 };   // qb_hnsw_algorithm
@@ -100,18 +111,35 @@ __device__ __forceinline__ float score_one(const HnswParams& p, const uint8_t* q
     }
 }
 
+// a nearest query: the similarity; a custom query: Query::score_by over the E examples (qb_fold.cuh), each similarity by the same
+// chain as a nearest query's, so a score equals qb_score_points on a qb_scorer_create_custom / _feedback scorer.  The fold asks for
+// every example exactly once, at points every lane of a group reaches together (its branches on similarities are group-uniform),
+// so the shuffles of score_one stay converged.
+// q = the query's index: its q_off / coefficients are found from it
+template <int KIND, int METRIC, int CUSTOM>
+__device__ __forceinline__ float score_q(const HnswParams& p, const HnswSmem& sm, float q_off, uint32_t id, int t, uint32_t q) {
+    if constexpr (CUSTOM) {
+        const float* off = p.q_off ? p.q_off + (size_t)q * p.ex_stride + p.ex_first : nullptr;
+        return qbf::fold(p.ckind, p.n_a, p.n_b, p.coef ? p.coef + (size_t)q * p.n_coef : nullptr, [&](uint32_t e) {
+            return score_one<KIND, METRIC>(p, sm.q + (size_t)e * p.q_bytes, off ? off[e] : 0.0f, id, t);
+        });
+    } else {
+        return score_one<KIND, METRIC>(p, sm.q, q_off, id, t);
+    }
+}
+
 // scores ids[0..n) into sc[0..n): one 8-lane group per id (dense small dims: one thread per id)
-template <int KIND, int METRIC, int NT>
-__device__ __forceinline__ void score_list(const HnswParams& p, const HnswSmem& sm, float q_off, uint32_t n) {
+template <int KIND, int METRIC, int NT, int CUSTOM>
+__device__ __forceinline__ void score_list(const HnswParams& p, const HnswSmem& sm, float q_off, uint32_t n, uint32_t q) {
     constexpr int HNSW_GROUPS = NT / 8;
     const int tid = threadIdx.x;
     if (KIND == HK_DENSE_SMALL) {
-        if ((uint32_t)tid < n) sm.sc[tid] = score_one<KIND, METRIC>(p, sm.q, q_off, sm.ids[tid], 0);
+        if ((uint32_t)tid < n) sm.sc[tid] = score_q<KIND, METRIC, CUSTOM>(p, sm, q_off, sm.ids[tid], 0, q);
     } else {
         const int g = tid >> 3, t = tid & 7;
         for (uint32_t i = g; i < ((n + HNSW_GROUPS - 1) / HNSW_GROUPS) * HNSW_GROUPS; i += HNSW_GROUPS) {   // whole warps stay converged for the shuffles
             const uint32_t id = sm.ids[i < n ? i : 0];
-            const float s = score_one<KIND, METRIC>(p, sm.q, q_off, id, t);
+            const float s = score_q<KIND, METRIC, CUSTOM>(p, sm, q_off, id, t, q);
             if (i < n && t == 0) sm.sc[i] = s;
         }
     }
@@ -133,6 +161,31 @@ __device__ __forceinline__ bool hnsw_filtered_out(const HnswParams& p, uint32_t 
     if (p.deleted) d = (p.deleted[id >> 5] >> (id & 31)) & 1u;
     if (p.deleted2) d = d || ((p.deleted2[id >> 5] >> (id & 31)) & 1u);
     return d;
+}
+
+// GraphLinksView::point_level (view.rs:354-369): the first level whose point count the point's reindex reaches, minus one
+__device__ __forceinline__ uint32_t hnsw_point_level(const HnswParams& p, uint32_t id) {
+    const uint64_t r = p.reindex[id];
+    for (uint32_t l = 1; l < p.levels; ++l) {
+        const uint64_t a = p.level_offsets[l], b = l + 1 < p.levels ? p.level_offsets[l + 1] : p.lo_end;
+        if (r >= b - a) return l - 1;
+    }
+    return p.levels ? p.levels - 1 : 0;
+}
+
+// GraphLayers::get_entry_point (graph_layers.rs:506-528) for query q: of its custom entry points that pass the filter, the one with the
+// highest level, the LAST of equal maxima (Iterator::max_by_key); none -> the caller's entry point
+__device__ __forceinline__ void hnsw_custom_entry(const HnswParams& p, uint32_t q, uint32_t& entry, uint32_t& level) {
+    entry = p.entry; level = p.entry_level;
+    if (!p.cep) return;
+    const uint32_t nc = min(p.cep_counts[q], p.n_cep);
+    bool found = false;
+    for (uint32_t i = 0; i < nc; ++i) {
+        const uint32_t id = p.cep[(size_t)q * p.n_cep + i].idx;
+        if (id >= p.n_points || hnsw_filtered_out(p, id)) continue;
+        const uint32_t l = hnsw_point_level(p, id);
+        if (!found || l >= level) { found = true; entry = id; level = l; }
+    }
 }
 
 // ---- ACORN-1 level-0 step (search_on_level_acorn, graph_layers.rs:154-243) for the candidate `cand` = keys[best].
@@ -225,13 +278,15 @@ __device__ __forceinline__ uint32_t count_greater(const unsigned long long* keys
     return lo;
 }
 
-template <int KIND, int METRIC, int NT, int ALGO>
+// CUSTOM = 1: a custom query (recommend / discover / context / feedback) scored through qbf::fold, with per-query custom entry points
+template <int KIND, int METRIC, int NT, int ALGO, int CUSTOM>
 __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
     constexpr int HNSW_THREADS = NT;
     extern __shared__ __align__(16) uint8_t smem_raw[];
     __shared__ unsigned int s_q, s_best, s_n, s_nvalid, s_len, s_nlog, s_cur, s_changed, s_warp_cnt[ALGO == ALGO_ACORN ? 4 : 2];
     __shared__ float s_cur_score;
     __shared__ unsigned int s_nx;   // ACORN: |to_explore|
+    __shared__ unsigned int s_entry, s_entry_level;   // CUSTOM: get_entry_point of this query
     const int tid = threadIdx.x;
     const uint32_t ef = p.ef;
     HnswSmem sm;
@@ -239,7 +294,7 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
     {
         const uint32_t hop = ALGO == ALGO_ACORN ? p.hop_cap : HNSW_MAX_LINKS;
         uint8_t* b = smem_raw;
-        sm.q = b; b += (p.q_bytes + 15u) & ~15u;
+        sm.q = b; b += ((CUSTOM ? p.q_smem : p.q_bytes) + 15u) & ~15u;
         sm.keys[0] = reinterpret_cast<unsigned long long*>(b); b += (size_t)ef * 8;
         sm.keys[1] = reinterpret_cast<unsigned long long*>(b); b += (size_t)ef * 8;
         sm.newk = reinterpret_cast<unsigned long long*>(b); b += (size_t)hop * 8;
@@ -259,24 +314,46 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
         const uint32_t q = s_q;
         if (q >= p.nq) break;
         // ---- query into shared memory
-        {
+        if constexpr (!CUSTOM) {
             const uint4* src = reinterpret_cast<const uint4*>(p.q_enc + (size_t)q * p.q_bytes);
             uint4* dst = reinterpret_cast<uint4*>(const_cast<uint8_t*>(sm.q));
             for (uint32_t i = tid; i < (p.q_bytes + 15u) / 16u; i += HNSW_THREADS) dst[i] = src[i];
+        } else {
+            // the examples: into shared memory when they fit, else read where they are (the same arithmetic either way)
+            const size_t first = (size_t)q * p.ex_stride + p.ex_first;
+            const uint8_t* src = p.q_enc + first * p.q_bytes;
+            if (p.ex_smem) {
+                const uint4* s4 = reinterpret_cast<const uint4*>(src);
+                uint4* dst = reinterpret_cast<uint4*>(smem_raw);   // the query region of the layout above
+                for (uint32_t i = tid; i < (p.n_ex * p.q_bytes) / 16u; i += HNSW_THREADS) dst[i] = s4[i];
+                sm.q = smem_raw;
+            } else {
+                sm.q = src;
+            }
         }
-        const float q_off = p.q_off ? p.q_off[q] : 0.0f;
-        if (tid == 0) { s_nlog = 0; sm.ids[0] = p.entry; }
+        const float q_off = (!CUSTOM && p.q_off) ? p.q_off[q] : 0.0f;
+        if (tid == 0) {
+            s_nlog = 0;
+            if constexpr (CUSTOM) {
+                uint32_t e, l;
+                hnsw_custom_entry(p, q, e, l);
+                s_entry = e; s_entry_level = l; sm.ids[0] = e;
+            } else {
+                sm.ids[0] = p.entry;
+            }
+        }
         __syncthreads();
+        // `CUSTOM ? s_entry : p.entry` is written out at each use, not bound to a local, so the nearest-query kernels compile as before
 
         // ---- search_entry: greedy descent from the entry point's level to level 1 (graph_layers.rs:247-316)
-        score_list<KIND, METRIC, NT>(p, sm, q_off, 1);      // score_point(entry)
+        score_list<KIND, METRIC, NT, CUSTOM>(p, sm, q_off, 1, q);      // score_point(entry)
         __syncthreads();
-        if (tid == 0) { s_cur = p.entry; s_cur_score = sm.sc[0]; ++hops; ++evals; }
+        if (tid == 0) { s_cur = CUSTOM ? s_entry : p.entry; s_cur_score = sm.sc[0]; ++hops; ++evals; }
         __syncthreads();
-        for (uint32_t lvl = p.entry_level; lvl >= 1; --lvl) {
+        for (uint32_t lvl = CUSTOM ? s_entry_level : p.entry_level; lvl >= 1; --lvl) {
             // search_entry_on_level re-scores its entry point on every level (graph_layers.rs:298-301): same value, but the scorer call
             // and the scored point are metered, so they are counted here too
-            if (tid == 0 && lvl != p.entry_level) { ++hops; ++evals; }
+            if (tid == 0 && lvl != (CUSTOM ? s_entry_level : p.entry_level)) { ++hops; ++evals; }
             for (;;) {
                 const uint32_t cur = s_cur;
                 // links of `cur` on this level: neighbors[offsets[idx] .. offsets[idx + 1]), idx = level_offsets[lvl] + reindex[cur] (view.rs:203-215)
@@ -298,7 +375,7 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
                 }
                 __syncthreads();
                 const uint32_t n = s_n;
-                score_list<KIND, METRIC, NT>(p, sm, q_off, n);
+                score_list<KIND, METRIC, NT, CUSTOM>(p, sm, q_off, n, q);
                 __syncthreads();
                 if (tid == 0) {
                     bool changed = false;
@@ -343,9 +420,9 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
                 if (n == 0) { __syncthreads(); continue; }
                 // score_points_unfiltered(to_score)
                 if (KIND == HK_DENSE_SMALL) {
-                    for (uint32_t i = tid; i < n; i += HNSW_THREADS) sm.sc[i] = score_one<KIND, METRIC>(p, sm.q, q_off, sm.ids[i], 0);
+                    for (uint32_t i = tid; i < n; i += HNSW_THREADS) sm.sc[i] = score_q<KIND, METRIC, CUSTOM>(p, sm, q_off, sm.ids[i], 0, q);
                 } else {
-                    score_list<KIND, METRIC, NT>(p, sm, q_off, n);
+                    score_list<KIND, METRIC, NT, CUSTOM>(p, sm, q_off, n, q);
                 }
                 __syncthreads();
                 // keys that can enter `nearest`, compacted, sorted, at most ef of them
@@ -405,7 +482,7 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
             if (tid == 0) { s_nlog += n; if (n) { ++hops; evals += n; } s_nvalid = 0; }
             if (n == 0) { __syncthreads(); continue; }
             // 3. score
-            score_list<KIND, METRIC, NT>(p, sm, q_off, n);
+            score_list<KIND, METRIC, NT, CUSTOM>(p, sm, q_off, n, q);
             __syncthreads();
             // 4. keys of the new points; the ones that cannot enter a full list are dropped here (key 0 = empty)
             const unsigned long long lower = (len == ef) ? keys[ef - 1] : 0ull;
@@ -474,12 +551,12 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
     if (tid == 0 && p.stats) { atomicAdd(&p.stats[0], hops); atomicAdd(&p.stats[1], evals); }
 }
 
-template <int KIND, int NT, int ALGO>
+template <int KIND, int NT, int ALGO, int CUSTOM>
 qb_status launch_kind(int metric, const HnswParams& p, unsigned grid, size_t smem, cudaStream_t stream) {
 #define QB_HNSW_LAUNCH(M)                                                                                              \
     do {                                                                                                               \
-        QB_CUDA(cudaFuncSetAttribute(hnsw_search_kernel<KIND, M, NT, ALGO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        hnsw_search_kernel<KIND, M, NT, ALGO><<<grid, NT, smem, stream>>>(p);                                          \
+        QB_CUDA(cudaFuncSetAttribute(hnsw_search_kernel<KIND, M, NT, ALGO, CUSTOM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        hnsw_search_kernel<KIND, M, NT, ALGO, CUSTOM><<<grid, NT, smem, stream>>>(p);                                          \
     } while (0)
     if (KIND == HK_SQ8 || KIND == HK_SQ8_LANEX) QB_HNSW_LAUNCH(M_DOT);
     else if (metric == M_EUCLID) QB_HNSW_LAUNCH(M_EUCLID);
@@ -491,39 +568,39 @@ qb_status launch_kind(int metric, const HnswParams& p, unsigned grid, size_t sme
     return QB_OK;
 }
 
-template <int KIND, int METRIC, int NT, int ALGO>
+template <int KIND, int METRIC, int NT, int ALGO, int CUSTOM>
 int occupancy_of(size_t smem) {
     int nb = 0;
-    cudaFuncSetAttribute(hnsw_search_kernel<KIND, METRIC, NT, ALGO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, hnsw_search_kernel<KIND, METRIC, NT, ALGO>, NT, smem) != cudaSuccess) nb = 1;
+    cudaFuncSetAttribute(hnsw_search_kernel<KIND, METRIC, NT, ALGO, CUSTOM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, hnsw_search_kernel<KIND, METRIC, NT, ALGO, CUSTOM>, NT, smem) != cudaSuccess) nb = 1;
     return nb < 1 ? 1 : nb;
 }
-template <int NT, int ALGO>
+template <int NT, int ALGO, int CUSTOM>
 int occupancy_dispatch(int kind, int metric, size_t smem) {
     switch (kind) {
-        case HK_DENSE_AVX: return metric == M_EUCLID ? occupancy_of<HK_DENSE_AVX, M_EUCLID, NT, ALGO>(smem) : metric == M_MANHATTAN ? occupancy_of<HK_DENSE_AVX, M_MANHATTAN, NT, ALGO>(smem) : occupancy_of<HK_DENSE_AVX, M_DOT, NT, ALGO>(smem);
-        case HK_DENSE_SMALL: return metric == M_EUCLID ? occupancy_of<HK_DENSE_SMALL, M_EUCLID, NT, ALGO>(smem) : metric == M_MANHATTAN ? occupancy_of<HK_DENSE_SMALL, M_MANHATTAN, NT, ALGO>(smem) : occupancy_of<HK_DENSE_SMALL, M_DOT, NT, ALGO>(smem);
-        case HK_SQ8: return occupancy_of<HK_SQ8, M_DOT, NT, ALGO>(smem);
-        default: return occupancy_of<HK_SQ8_LANEX, M_DOT, NT, ALGO>(smem);
+        case HK_DENSE_AVX: return metric == M_EUCLID ? occupancy_of<HK_DENSE_AVX, M_EUCLID, NT, ALGO, CUSTOM>(smem) : metric == M_MANHATTAN ? occupancy_of<HK_DENSE_AVX, M_MANHATTAN, NT, ALGO, CUSTOM>(smem) : occupancy_of<HK_DENSE_AVX, M_DOT, NT, ALGO, CUSTOM>(smem);
+        case HK_DENSE_SMALL: return metric == M_EUCLID ? occupancy_of<HK_DENSE_SMALL, M_EUCLID, NT, ALGO, CUSTOM>(smem) : metric == M_MANHATTAN ? occupancy_of<HK_DENSE_SMALL, M_MANHATTAN, NT, ALGO, CUSTOM>(smem) : occupancy_of<HK_DENSE_SMALL, M_DOT, NT, ALGO, CUSTOM>(smem);
+        case HK_SQ8: return occupancy_of<HK_SQ8, M_DOT, NT, ALGO, CUSTOM>(smem);
+        default: return occupancy_of<HK_SQ8_LANEX, M_DOT, NT, ALGO, CUSTOM>(smem);
     }
 }
-template <int NT, int ALGO>
+template <int NT, int ALGO, int CUSTOM>
 qb_status launch_dispatch(int kind, int metric, const HnswParams& p, unsigned grid, size_t smem, cudaStream_t stream) {
     switch (kind) {
-        case HK_DENSE_AVX: return launch_kind<HK_DENSE_AVX, NT, ALGO>(metric, p, grid, smem, stream);
-        case HK_DENSE_SMALL: return launch_kind<HK_DENSE_SMALL, NT, ALGO>(metric, p, grid, smem, stream);
-        case HK_SQ8: return launch_kind<HK_SQ8, NT, ALGO>(metric, p, grid, smem, stream);
-        default: return launch_kind<HK_SQ8_LANEX, NT, ALGO>(metric, p, grid, smem, stream);
+        case HK_DENSE_AVX: return launch_kind<HK_DENSE_AVX, NT, ALGO, CUSTOM>(metric, p, grid, smem, stream);
+        case HK_DENSE_SMALL: return launch_kind<HK_DENSE_SMALL, NT, ALGO, CUSTOM>(metric, p, grid, smem, stream);
+        case HK_SQ8: return launch_kind<HK_SQ8, NT, ALGO, CUSTOM>(metric, p, grid, smem, stream);
+        default: return launch_kind<HK_SQ8_LANEX, NT, ALGO, CUSTOM>(metric, p, grid, smem, stream);
     }
 }
 template <int ALGO>
 int occupancy_nt(int nt, int kind, int metric, size_t smem) {
-    return nt == 128 ? occupancy_dispatch<128, ALGO>(kind, metric, smem) : (nt == 64 ? occupancy_dispatch<64, ALGO>(kind, metric, smem) : occupancy_dispatch<256, ALGO>(kind, metric, smem));
+    return nt == 128 ? occupancy_dispatch<128, ALGO, 0>(kind, metric, smem) : (nt == 64 ? occupancy_dispatch<64, ALGO, 0>(kind, metric, smem) : occupancy_dispatch<256, ALGO, 0>(kind, metric, smem));
 }
 template <int ALGO>
 qb_status launch_nt(int nt, int kind, int metric, const HnswParams& p, unsigned grid, size_t smem, cudaStream_t stream) {
-    return nt == 128 ? launch_dispatch<128, ALGO>(kind, metric, p, grid, smem, stream)
-                     : (nt == 64 ? launch_dispatch<64, ALGO>(kind, metric, p, grid, smem, stream) : launch_dispatch<256, ALGO>(kind, metric, p, grid, smem, stream));
+    return nt == 128 ? launch_dispatch<128, ALGO, 0>(kind, metric, p, grid, smem, stream)
+                     : (nt == 64 ? launch_dispatch<64, ALGO, 0>(kind, metric, p, grid, smem, stream) : launch_dispatch<256, ALGO, 0>(kind, metric, p, grid, smem, stream));
 }
 
 }  // namespace
@@ -936,7 +1013,7 @@ extern "C" qb_status qb_hnsw_info(const qb_hnsw* g, uint32_t* n_points, uint32_t
 
 // queries already encoded (d_q_enc / d_q_off); results to device buffers; enqueued on `stream`, no synchronisation
 qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, uint32_t nq, uint32_t top, uint32_t ef, uint32_t entry, uint32_t entry_level,
-                         const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts, cudaStream_t stream, int algo) {
+                         const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts, cudaStream_t stream, int algo, const QbHnswCustom* custom) {
     qb_storage* s = g->st;
     QB_CHECK(algo == ALGO_HNSW || algo == ALGO_ACORN, QB_ERR_INVALID, "hnsw_search: algorithm %d is neither QB_HNSW_ALGO_HNSW nor QB_HNSW_ALGO_ACORN", algo);
     QB_CHECK(entry < g->n_points, QB_ERR_INVALID, "hnsw_search: entry point %u out of range", entry);
@@ -959,12 +1036,30 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
     p.out = d_out; p.out_counts = d_counts; p.id_base = s->id_base; p.stats = g->d_stats;
     const bool acorn = algo == ALGO_ACORN;
     p.hop_cap = acorn ? acorn_hop_cap(g->m0) : HNSW_MAX_LINKS;
-    const size_t smem = acorn ? acorn_smem_bytes(p.q_bytes, ef, p.hop_cap) : hnsw_smem_bytes(p.q_bytes, ef);
-    QB_CHECK(smem <= 200 * 1024, QB_ERR_UNSUPPORTED, "hnsw_search: query (%u B) + ef %u need %zu B of shared memory", p.q_bytes, ef, smem);
+    uint32_t q_smem = p.q_bytes;
+    if (custom) {
+        p.ckind = custom->kind; p.n_a = custom->n_a; p.n_b = custom->n_b;
+        p.n_ex = custom->n_ex; p.ex_first = custom->ex_first; p.ex_stride = custom->ex_stride;
+        p.coef = custom->d_coef; p.n_coef = custom->n_coef;
+        p.cep = custom->d_cep; p.cep_counts = custom->d_cep_counts; p.n_cep = custom->n_cep;
+        p.lo_end = g->level_offsets_ext.empty() ? 0 : g->level_offsets_ext.back();
+        p.stats = g->d_stats + 2 * custom->stats_slot;
+        if (custom->internal_out) p.id_base = 0;
+        // the examples are staged in shared memory when they fit in HNSW_CUSTOM_SMEM, which keeps several queries in flight per SM;
+        // larger sets are read from global memory (L1 / L2) by the same chains
+        const uint64_t ex_bytes = (uint64_t)p.n_ex * p.q_bytes;
+        p.ex_smem = ex_bytes <= HNSW_CUSTOM_SMEM ? 1u : 0u;
+        q_smem = p.ex_smem ? (uint32_t)ex_bytes : 0u;
+        p.q_smem = q_smem;
+    }
+    const size_t smem = acorn ? acorn_smem_bytes(q_smem, ef, p.hop_cap) : hnsw_smem_bytes(q_smem, ef);
+    QB_CHECK(smem <= 200 * 1024, QB_ERR_UNSUPPORTED, "hnsw_search: query (%u B) + ef %u need %zu B of shared memory", q_smem, ef, smem);
     // threads per CTA: 256 = one 8-lane group per level-0 link (m0 = 32), fewer queries in flight per SM; 128 (default) = two scoring rounds
     // per hop, twice the resident queries.  The traversal is a chain of dependent memory round trips, so queries in flight is what hides them.
-    const int nt = qb_opt().hnsw_threads == 256 ? 256 : (qb_opt().hnsw_threads == 64 ? 64 : 128);
-    const int per_sm = acorn ? occupancy_nt<ALGO_ACORN>(nt, kind, metric, smem) : occupancy_nt<ALGO_HNSW>(nt, kind, metric, smem);
+    // Custom queries are instantiated for 128 threads only.
+    const int nt = custom ? 128 : (qb_opt().hnsw_threads == 256 ? 256 : (qb_opt().hnsw_threads == 64 ? 64 : 128));
+    const int per_sm = custom ? (acorn ? occupancy_dispatch<128, ALGO_ACORN, 1>(kind, metric, smem) : occupancy_dispatch<128, ALGO_HNSW, 1>(kind, metric, smem))
+                              : (acorn ? occupancy_nt<ALGO_ACORN>(nt, kind, metric, smem) : occupancy_nt<ALGO_HNSW>(nt, kind, metric, smem));
     p.prefetch = qb_opt().hnsw_no_prefetch ? 0 : 1;
     const unsigned max_grid = (unsigned)s->sm_count * (unsigned)per_sm;
     const unsigned grid = std::min<unsigned>(max_grid, nq);
@@ -980,14 +1075,17 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
     }
     p.visited = g->d_visited; p.visited_words = words; p.vlog = g->d_vlog; p.vlog_cap = g->vlog_cap; p.work = g->d_work;
     QB_CUDA(cudaMemsetAsync(g->d_work, 0, 4, stream));
+    if (custom)
+        return acorn ? launch_dispatch<128, ALGO_ACORN, 1>(kind, metric, p, grid, smem, stream) : launch_dispatch<128, ALGO_HNSW, 1>(kind, metric, p, grid, smem, stream);
     return acorn ? launch_nt<ALGO_ACORN>(nt, kind, metric, p, grid, smem, stream) : launch_nt<ALGO_HNSW>(nt, kind, metric, p, grid, smem, stream);
 }
 
-qb_status qb_hnsw_read_stats(qb_hnsw* g, cudaStream_t stream) {
-    unsigned long long h[2] = {0, 0};
-    QB_CUDA(cudaMemcpyAsync(h, g->d_stats, 16, cudaMemcpyDeviceToHost, stream));
+qb_status qb_hnsw_read_stats(qb_hnsw* g, cudaStream_t stream, uint64_t* evals_by_slot) {
+    unsigned long long h[4] = {0, 0, 0, 0};
+    QB_CUDA(cudaMemcpyAsync(h, g->d_stats, 32, cudaMemcpyDeviceToHost, stream));
     QB_CUDA(cudaStreamSynchronize(stream));
-    QB_CUDA(cudaMemsetAsync(g->d_stats, 0, 16, stream));
-    g->hops += h[0]; g->evals += h[1];
+    QB_CUDA(cudaMemsetAsync(g->d_stats, 0, 32, stream));
+    g->hops += h[0] + h[2]; g->evals += h[1] + h[3];
+    if (evals_by_slot) { evals_by_slot[0] = h[1]; evals_by_slot[1] = h[3]; }
     return QB_OK;
 }

@@ -150,9 +150,22 @@ struct qb_hnsw {
     uint64_t hops = 0, evals = 0;
 };
 
+// A batch of custom queries for qb_hnsw_launch: query q's examples are the encoded queries ex_first .. ex_first + n_ex of the
+// ex_stride that d_q_enc / d_q_off hold per query.  d_cep: custom entry points [nq][n_cep] (.idx read), d_cep_counts[q] of them valid.
+struct QbHnswCustom {
+    int kind; uint32_t n_a, n_b;                 // qb_query_kind and its shape
+    uint32_t n_ex, ex_first, ex_stride;
+    const float* d_coef; uint32_t n_coef;        // feedback: [a, partial...] per query, else null / 0
+    const qb_scored_point* d_cep; const uint32_t* d_cep_counts; uint32_t n_cep;
+    uint32_t stats_slot;                         // hops / scored points go to stats slot 0 or 1 (qb_hnsw_read_stats)
+    bool internal_out;                           // results as point offsets, without the storage's id_base (discover's context stage)
+};
+
 qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, uint32_t nq, uint32_t top, uint32_t ef, uint32_t entry, uint32_t entry_level,
-                         const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts, cudaStream_t stream, int algo /* qb_hnsw_algorithm */);
-qb_status qb_hnsw_read_stats(qb_hnsw* g, cudaStream_t stream);
+                         const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts, cudaStream_t stream, int algo /* qb_hnsw_algorithm */,
+                         const QbHnswCustom* custom = nullptr);
+// adds the device counters to g->hops / g->evals and clears them; evals_by_slot (optional, [2]) receives each slot's scored points
+qb_status qb_hnsw_read_stats(qb_hnsw* g, cudaStream_t stream, uint64_t* evals_by_slot = nullptr);
 
 // One rank of a sharded search (qb_comm.cu): an exchange buffer every peer maps + the peers' buffers
 constexpr uint32_t QB_MAX_WORLD = 16;

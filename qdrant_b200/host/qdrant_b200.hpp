@@ -233,8 +233,37 @@ public:
         for (uint32_t q = 0; q < n_queries; ++q) out[q].assign(flat.begin() + (size_t)q * top, flat.begin() + (size_t)q * top + counts[q]);
         return out;
     }
+    // custom queries (search.rs:181-208): vectors = n_queries x E x dim in the build_custom_scorer layout; coef = n_queries x (1 + n_a) for
+    // feedback, else null; custom_entry_points = n_queries x n_custom ids, custom_counts[q] valid (or null)
+    std::vector<std::vector<ScoredPointOffset>> search_custom(qb_query_kind kind, const float* vectors, uint32_t n_a, uint32_t n_b, const float* coef,
+                                                              uint32_t n_queries, uint32_t top, uint32_t ef, PointOffsetType entry_point, uint32_t entry_level,
+                                                              const uint32_t* custom_entry_points = nullptr, const uint32_t* custom_counts = nullptr,
+                                                              uint32_t n_custom = 0, const uint64_t* deleted = nullptr,
+                                                              SearchAlgorithm algorithm = SearchAlgorithm::Hnsw) const {
+        std::vector<ScoredPointOffset> flat((size_t)n_queries * top);
+        std::vector<uint32_t> counts(n_queries);
+        check(qb_hnsw_search_custom_batch(h_, kind, vectors, n_a, n_b, coef, n_queries, top, ef, entry_point, entry_level, custom_entry_points, custom_counts,
+                                          n_custom, deleted, nullptr, flat.data(), counts.data(), nullptr, static_cast<qb_hnsw_algorithm>(algorithm)));
+        return split(flat, counts, top);
+    }
+    // discover_search_with_graph (search.rs:314-349): context stage for 10 entry points, then the discover search, in one call;
+    // vectors = n_queries x (1 + 2 n_pairs) x dim (target, then the pairs)
+    std::vector<std::vector<ScoredPointOffset>> search_discover(const float* vectors, uint32_t n_pairs, uint32_t n_queries, uint32_t top, uint32_t ef,
+                                                                PointOffsetType entry_point, uint32_t entry_level, const uint64_t* deleted = nullptr,
+                                                                SearchAlgorithm algorithm = SearchAlgorithm::Hnsw) const {
+        std::vector<ScoredPointOffset> flat((size_t)n_queries * top);
+        std::vector<uint32_t> counts(n_queries);
+        check(qb_hnsw_search_discover_batch(h_, vectors, n_pairs, n_queries, top, ef, entry_point, entry_level, deleted, nullptr, flat.data(), counts.data(),
+                                            nullptr, static_cast<qb_hnsw_algorithm>(algorithm)));
+        return split(flat, counts, top);
+    }
 
 private:
+    static std::vector<std::vector<ScoredPointOffset>> split(const std::vector<ScoredPointOffset>& flat, const std::vector<uint32_t>& counts, uint32_t top) {
+        std::vector<std::vector<ScoredPointOffset>> out(counts.size());
+        for (size_t q = 0; q < counts.size(); ++q) out[q].assign(flat.begin() + q * top, flat.begin() + q * top + counts[q]);
+        return out;
+    }
     explicit HnswGraph(qb_hnsw* h) : h_(h) {}
     qb_hnsw* h_ = nullptr;
 };

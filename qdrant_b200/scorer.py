@@ -772,6 +772,64 @@ class HnswGraph:
                                               counts.ctypes.data_as(u32p), None if counters is None else C.byref(counters), self.ALGORITHMS[algorithm]))
         return [out[i, : counts[i]].copy() for i in range(nq)]
 
+    def _examples(self, examples, n_ex: int):
+        ex = _f32(examples)
+        if ex.ndim == 2:
+            ex = ex[None]
+        if ex.ndim != 3 or ex.shape[1] != n_ex or ex.shape[2] != self._storage.dim:
+            raise ValueError(f"examples must be [queries, {n_ex}, {self._storage.dim}], got {ex.shape}")
+        return np.ascontiguousarray(ex)
+
+    def search_custom(self, kind: QueryKind, examples, n_a: int, n_b: int = 0, coef=None, top: int = 10, ef: int = 64, entry_point: int = 0,
+                      entry_level: int = 0, point_deleted=None, counters: Optional[HwCounters] = None, custom_entry_points=None,
+                      algorithm: str = "hnsw"):
+        """Custom queries through the device traversal (qb_hnsw_search_custom_batch).  examples: [queries, E, dim] raw f32 in the
+        qb_scorer_create_custom layout (one kind and shape per call); coef: [queries, 1 + n_a] [a, partial...] for feedback queries;
+        custom_entry_points: one sequence of point offsets per query (GraphLayers::search's custom_entry_points), or None."""
+        if algorithm not in self.ALGORITHMS:
+            raise ValueError(f"algorithm {algorithm!r} is not one of {sorted(self.ALGORITHMS)}")
+        kind = int(kind)
+        n_ex = {1: n_a + n_b, 2: n_a + n_b, 3: 1 + 2 * n_a, 4: 2 * n_a, 5: 1 + 2 * n_a}.get(kind, 0)
+        ex = self._examples(examples, n_ex) if n_ex else _f32(examples)
+        nq = ex.shape[0] if n_ex else 0
+        cf = None if coef is None else np.ascontiguousarray(_f32(coef).reshape(nq, -1))
+        cep_arr = cep_cnt = None
+        width = 0
+        if custom_entry_points is not None:
+            if len(custom_entry_points) != nq:
+                raise ValueError(f"custom_entry_points has {len(custom_entry_points)} lists for {nq} queries")
+            width = max(1, max((len(c) for c in custom_entry_points), default=1))
+            cep_arr = np.zeros((nq, width), np.uint32)
+            cep_cnt = np.zeros(nq, np.uint32)
+            for i, c in enumerate(custom_entry_points):
+                cep_arr[i, : len(c)] = np.asarray(c, dtype=np.uint32)
+                cep_cnt[i] = len(c)
+        out = np.zeros((max(nq, 1), max(top, 1)), dtype=SCORED_POINT_OFFSET)
+        counts = np.zeros(max(nq, 1), dtype=np.uint32)
+        bm = _bitmap(point_deleted, self._storage.count)
+        check(lib().qb_hnsw_search_custom_batch(self._h, kind, ex.ctypes.data_as(f32p), int(n_a), int(n_b), None if cf is None else cf.ctypes.data_as(f32p),
+                                                nq, int(top), int(ef), int(entry_point), int(entry_level),
+                                                None if cep_arr is None else cep_arr.ctypes.data_as(u32p), None if cep_cnt is None else cep_cnt.ctypes.data_as(u32p),
+                                                width, None if bm is None else bm.ctypes.data_as(u64p), None, out.ctypes.data_as(C.POINTER(ScoredPoint)),
+                                                counts.ctypes.data_as(u32p), None if counters is None else C.byref(counters), self.ALGORITHMS[algorithm]))
+        return [out[i, : counts[i]].copy() for i in range(nq)]
+
+    def search_discover(self, examples, n_pairs: int, top: int = 10, ef: int = 64, entry_point: int = 0, entry_level: int = 0, point_deleted=None,
+                        counters: Optional[HwCounters] = None, algorithm: str = "hnsw"):
+        """Discover as the reference runs it on an indexed segment (qb_hnsw_search_discover_batch): a context search over the pairs for
+        10 entry points, then the discover search from them, in one call.  examples: [queries, 1 + 2 n_pairs, dim] (target, then pairs)."""
+        if algorithm not in self.ALGORITHMS:
+            raise ValueError(f"algorithm {algorithm!r} is not one of {sorted(self.ALGORITHMS)}")
+        ex = self._examples(examples, 1 + 2 * int(n_pairs))
+        nq = ex.shape[0]
+        out = np.zeros((nq, max(top, 1)), dtype=SCORED_POINT_OFFSET)
+        counts = np.zeros(nq, dtype=np.uint32)
+        bm = _bitmap(point_deleted, self._storage.count)
+        check(lib().qb_hnsw_search_discover_batch(self._h, ex.ctypes.data_as(f32p), int(n_pairs), nq, int(top), int(ef), int(entry_point), int(entry_level),
+                                                  None if bm is None else bm.ctypes.data_as(u64p), None, out.ctypes.data_as(C.POINTER(ScoredPoint)),
+                                                  counts.ctypes.data_as(u32p), None if counters is None else C.byref(counters), self.ALGORITHMS[algorithm]))
+        return [out[i, : counts[i]].copy() for i in range(nq)]
+
     def stats(self, reset: bool = True) -> tuple[int, int]:
         a, b = C.c_uint64(), C.c_uint64()
         check(lib().qb_hnsw_stats(self._h, C.byref(a), C.byref(b), 1 if reset else 0))
