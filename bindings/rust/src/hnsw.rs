@@ -38,6 +38,32 @@ impl<'a> B200Hnsw<'a> {
         Ok(Self { raw, _storage: std::marker::PhantomData })
     }
 
+    /// Builds the graph on the device, in place of `build_hnsw_on_gpu` (gpu/gpu_graph_builder.rs) and of the CPU
+    /// `GraphLayersBuilder::link_new_point` pool (hnsw/build.rs:285-355) for a dense f32 storage.  The adapter keeps on the host:
+    /// the level draw (`GraphLayersBuilder::get_random_layer`, one u8 per point), the mapping between point offsets and the
+    /// storage's rows, the deleted flags (set on the storage beforehand), and writing `links.bin` in the compressed format from
+    /// `export_plain` (GraphLinksSerializer).  Returns the graph and its entry point (id, level).
+    pub fn build(storage: &'a B200Storage, m: usize, m0: usize, ef_construct: usize, levels: &[u8], batch: usize, serial_points: usize)
+        -> OperationResult<(Self, (PointOffsetType, usize))> {
+        let mut raw = std::ptr::null_mut();
+        let (mut entry, mut level) = (0u32, 0u32);
+        let st = unsafe {
+            qb_hnsw_build(storage.raw, m as u32, m0 as u32, ef_construct as u32, levels.as_ptr(), batch as u32, serial_points as u32, &mut raw, &mut entry,
+                          &mut level)
+        };
+        if st != QB_OK { return Err(OperationError::service_error(last_error())); }
+        Ok((Self { raw, _storage: std::marker::PhantomData }, (entry, level as usize)))
+    }
+
+    /// The graph as a plain `links.bin` (GraphLinksFormat::Plain), whichever way it was made.
+    pub fn export_plain(&self) -> OperationResult<Vec<u8>> {
+        let mut n = 0u64;
+        if unsafe { qb_hnsw_export_plain(self.raw, std::ptr::null_mut(), 0, &mut n) } != QB_OK { return Err(OperationError::service_error(last_error())); }
+        let mut out = vec![0u8; n as usize];
+        if unsafe { qb_hnsw_export_plain(self.raw, out.as_mut_ptr(), n, &mut n) } != QB_OK { return Err(OperationError::service_error(last_error())); }
+        Ok(out)
+    }
+
     /// `entry` = GraphLayers::get_entry_point(filters, custom_entry_points) (it depends on the filter, so it stays host logic);
     /// `deleted` = the filter as a bitmap (bit = 1: check_vector fails), or None;
     /// `algorithm` = the level-0 algorithm GraphLayers::search dispatches on, as hnsw/read_view/search.rs:59-86 chooses it.

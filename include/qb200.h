@@ -368,6 +368,25 @@ QB_API qb_status qb_hnsw_links(const qb_hnsw* g, uint32_t level, const uint32_t*
                                uint32_t* counts);
 QB_API void qb_hnsw_destroy(qb_hnsw* g);
 QB_API qb_status qb_hnsw_info(const qb_hnsw* g, uint32_t* n_points, uint32_t* levels, uint64_t* hbm_bytes);
+/* Builds the HNSW graph of a dense f32 storage on the device, with the schedule of the reference's GPU builder
+ * (gpu/gpu_graph_builder.rs:19-101, gpu_level_builder.rs:12-96, batched_points.rs:36-163) and the CPU builder's per-point
+ * arithmetic (search_on_level with ef = max(ef_construct, m0), fill_from_sorted_with_heuristic, connect_with_heuristic):
+ *   - points sorted by level descending, then id; the first is the entry point (returned in entry_point / entry_level);
+ *   - the first serial_points points of that order are inserted one at a time (0 = 256, SINGLE_THREADED_HNSW_BUILD_THRESHOLD);
+ *   - the rest in batches of at most `batch` points on one level (0 = 512, GPU_GROUPS_COUNT_DEFAULT), level by level from the top.
+ * A batch's points search the level as it was before the batch; their backlinks are then applied target by target in batch order
+ * (the reference races them under per-point locks).  So the graph is a pure function of (rows, levels, m, m0, ef_construct, batch,
+ * serial_points): two builds give the same graph, and batch = 1 gives the serial CPU build in the sorted order.
+ *   levels    one per point, <= 30: the reference draws them from an unseeded RNG (get_random_layer), the caller draws them here
+ * Points with the storage's resident deleted flag (qb_storage_set_deleted) are not inserted (iter_internal_excluding(deleted)): they keep
+ * their level and have no links.  m, m0 <= 64 and ef <= 4096 (else QB_ERR_UNSUPPORTED); a level > 30, an empty storage or no point left
+ * to insert: QB_ERR_INVALID.  Other storages: QB_ERR_UNSUPPORTED (build over the original vectors, then bind the exported graph to the
+ * quantized storage).  The result is the handle qb_hnsw_create_plain would make from the graph's plain links.bin.  Synchronous. */
+QB_API qb_status qb_hnsw_build(qb_storage* s, uint32_t m, uint32_t m0, uint32_t ef_construct, const uint8_t* levels /* n */, uint32_t batch,
+                               uint32_t serial_points, qb_hnsw** out, uint32_t* entry_point, uint32_t* entry_level);
+/* The graph of any handle as a plain links.bin (graph_links/header.rs:9-20, serializer.rs:53-200).  *n_bytes = its size; out = NULL
+ * asks for the size only, else cap must hold it (QB_ERR_INVALID).  Synchronous. */
+QB_API qb_status qb_hnsw_export_plain(const qb_hnsw* g, uint8_t* out, uint64_t cap, uint64_t* n_bytes);
 /*   queries         n_queries x dim raw f32 (Metric::preprocess + encode_query on the device)
  *   ef              beam width; max(ef, top) is used (graph_layers.rs:551)
  *   entry_point / entry_level   GraphLayers::get_entry_point's answer (entry_points.rs; it depends on the filter, so the

@@ -1,0 +1,680 @@
+// qb_hnsw_traverse.cuh — the device HNSW traversal (hnsw_search_kernel) and the pieces it is made of: the kernel parameters, the
+// per-hop scoring, the ACORN-1 step, the beam search.  qb_hnsw.cu instantiates it for searches, qb_hnsw_build.cu for the inserts of a
+// graph build (ALGO_BUILD), so both run the same beam search.  The design notes are in qb_hnsw.cu's header.
+#pragma once
+#include <algorithm>
+
+#include "qb_fold.cuh"
+#include "qb_internal.h"
+#include "qb_score.cuh"
+
+using namespace qbs;
+
+namespace {
+
+#ifndef QB_HNSW_LINK_PREFETCH
+#define QB_HNSW_LINK_PREFETCH 1      // build-time experiment knob
+#endif
+constexpr uint32_t HNSW_MAX_LINKS = 64;      // links scored per hop (m0 <= 64)
+constexpr uint32_t HNSW_EMPTY = 0xFFFFFFFFu;
+constexpr uint32_t HNSW_MAX_EF = 4096;
+constexpr uint32_t HNSW_CUSTOM_SMEM = 48 * 1024;   // custom queries: examples up to this size are staged in shared memory
+
+enum { HK_DENSE_AVX = 0, HK_DENSE_SMALL = 1, HK_SQ8 = 2, HK_SQ8_LANEX = 3 };
+
+struct HnswParams {
+    // graph
+    const uint32_t* links0;        // [n][m0], HNSW_EMPTY padded
+    const uint64_t* level_offsets; // [levels]
+    const uint32_t* reindex;       // [n]
+    const uint32_t* neighbors;     // plain neighbours (all levels; only levels >= 1 are read here)
+    const uint64_t* offsets;       // [total_offsets]
+    uint32_t n_points, m, m0, levels;
+    // storage
+    const uint8_t* rows; uint32_t stride; uint32_t dim;             // dense f32
+    const uint8_t* codes; const float* voff; uint32_t ad; float multiplier; int l1;   // SQ8
+    // queries
+    const uint8_t* q_enc; uint32_t q_bytes; const float* q_off;
+    uint32_t nq, top, ef;
+    uint32_t entry, entry_level;
+    const uint32_t* deleted; const uint32_t* deleted2;
+    // per-CTA scratch
+    uint32_t* visited; uint64_t visited_words;   // [grid][visited_words]
+    uint32_t* vlog; uint32_t vlog_cap;           // [grid][vlog_cap]
+    unsigned int* work;                          // next query index
+    // results
+    qb_scored_point* out; uint32_t* out_counts; uint32_t id_base;
+    unsigned long long* stats;                   // [0] hops (scorer calls), [1] scored points
+    int prefetch;                                // 1: bulk-prefetch the surviving neighbours' vectors into L2 before scoring
+    // ACORN only (appended so the HNSW kernels' parameter offsets stay as they were)
+    uint32_t hop_cap;                            // per-hop buffers: a power of two >= m0 * m0
+    // custom queries only (appended likewise).  Query q's examples are encoded queries ex_first .. ex_first + n_ex of the
+    // ex_stride that q_enc / q_off hold per query (discover's context stage skips the target: ex_first = 1)
+    int ckind; uint32_t n_a, n_b;                // qb_query_kind and its shape (qbf::fold)
+    uint32_t n_ex, ex_first, ex_stride;
+    uint32_t ex_smem;                            // 1: the examples are staged in shared memory, 0: read from q_enc (too large)
+    uint32_t q_smem;                             // bytes of shared memory the query / examples take
+    const float* coef; uint32_t n_coef;          // feedback: [a, partial...] per query
+    const qb_scored_point* cep; const uint32_t* cep_counts; uint32_t n_cep;   // custom_entry_points: [nq][n_cep], .idx used
+    uint64_t lo_end;                             // level_offsets[levels] (point_level, view.rs:354-369)
+    // ALGO_BUILD only (appended likewise): one launch inserts (b_insert = 1) or greedily descends (0) the points b_pts[0 .. nq) on one
+    // level whose rows are links0 [rows][m0] (m0 = that level's m), row of a point = b_remap[id] (null: the id).  b_entry[i] is point
+    // i's entry, replaced by the best point found.  An insert writes its point's row and its backlinks (target << 32 | i, source) to
+    // b_tkey / b_tval [nq][m0] (~0 = none).
+    const uint32_t* b_pts; uint32_t* b_entry; const uint32_t* b_remap; uint32_t b_insert;
+    unsigned long long* b_tkey; uint32_t* b_tval;
+};
+
+struct HnswSmem {
+    unsigned long long* keys[2];
+    uint8_t* flags[2];
+    unsigned long long* newk;   // [HNSW_MAX_LINKS] (ACORN: [hop_cap])
+    uint32_t* ids;              // [HNSW_MAX_LINKS] (ACORN: [hop_cap])
+    float* sc;                  // [HNSW_MAX_LINKS] (ACORN: [hop_cap])
+    const uint8_t* q;           // query (custom: the first example, in shared or global memory; example e at q + e * q_bytes)
+};
+
+enum { ALGO_HNSW = 0, ALGO_ACORN = 1 };   // qb_hnsw_algorithm
+enum { ALGO_BUILD = 2 };                  // an insert of qb_hnsw_build: HNSW level search of a stored point, then its links (qb_hnsw_build.cu)
+
+// ALGO_BUILD: a point's row in its level's table
+__device__ __forceinline__ uint32_t hnsw_build_row(const HnswParams& p, uint32_t id) { return p.b_remap ? p.b_remap[id] : id; }
+
+template <int KIND, int METRIC>
+__device__ __forceinline__ float score_one(const HnswParams& p, const uint8_t* q_smem, float q_off, uint32_t id, int t) {
+    if (KIND == HK_DENSE_AVX) {
+        return score_avx_group8<METRIC>(reinterpret_cast<const float*>(p.rows + (size_t)id * p.stride), reinterpret_cast<const float*>(q_smem), p.dim, t);
+    } else if (KIND == HK_DENSE_SMALL) {
+        return score_small<METRIC>(reinterpret_cast<const float*>(p.rows + (size_t)id * p.stride), reinterpret_cast<const float*>(q_smem), p.dim);
+    } else {
+        const float raw = sq8_raw_group8<KIND == HK_SQ8_LANEX>(reinterpret_cast<const uint4*>(p.codes + (size_t)id * p.ad), reinterpret_cast<const uint4*>(q_smem),
+                                                               p.ad >> 4, t, p.l1);
+        return __fadd_rn(__fadd_rn(__fmul_rn(p.multiplier, raw), q_off), p.voff[id]);   // postprocess_score, encoded_vectors_u8.rs:101-103
+    }
+}
+
+// a nearest query: the similarity; a custom query: Query::score_by over the E examples (qb_fold.cuh), each similarity by the same
+// chain as a nearest query's, so a score equals qb_score_points on a qb_scorer_create_custom / _feedback scorer.  The fold asks for
+// every example exactly once, at points every lane of a group reaches together (its branches on similarities are group-uniform),
+// so the shuffles of score_one stay converged.
+// q = the query's index: its q_off / coefficients are found from it
+template <int KIND, int METRIC, int CUSTOM>
+__device__ __forceinline__ float score_q(const HnswParams& p, const HnswSmem& sm, float q_off, uint32_t id, int t, uint32_t q) {
+    if constexpr (CUSTOM) {
+        const float* off = p.q_off ? p.q_off + (size_t)q * p.ex_stride + p.ex_first : nullptr;
+        return qbf::fold(p.ckind, p.n_a, p.n_b, p.coef ? p.coef + (size_t)q * p.n_coef : nullptr, [&](uint32_t e) {
+            return score_one<KIND, METRIC>(p, sm.q + (size_t)e * p.q_bytes, off ? off[e] : 0.0f, id, t);
+        });
+    } else {
+        return score_one<KIND, METRIC>(p, sm.q, q_off, id, t);
+    }
+}
+
+// scores ids[0..n) into sc[0..n): one 8-lane group per id (dense small dims: one thread per id)
+template <int KIND, int METRIC, int NT, int CUSTOM>
+__device__ __forceinline__ void score_list(const HnswParams& p, const HnswSmem& sm, float q_off, uint32_t n, uint32_t q) {
+    constexpr int HNSW_GROUPS = NT / 8;
+    const int tid = threadIdx.x;
+    if (KIND == HK_DENSE_SMALL) {
+        if ((uint32_t)tid < n) sm.sc[tid] = score_q<KIND, METRIC, CUSTOM>(p, sm, q_off, sm.ids[tid], 0, q);
+    } else {
+        const int g = tid >> 3, t = tid & 7;
+        for (uint32_t i = g; i < ((n + HNSW_GROUPS - 1) / HNSW_GROUPS) * HNSW_GROUPS; i += HNSW_GROUPS) {   // whole warps stay converged for the shuffles
+            const uint32_t id = sm.ids[i < n ? i : 0];
+            const float s = score_q<KIND, METRIC, CUSTOM>(p, sm, q_off, id, t, q);
+            if (i < n && t == 0) sm.sc[i] = s;
+        }
+    }
+}
+
+// scores the stored rows ids[0 .. n) against the stored row `qrow` (global memory) with GROUPS 8-lane groups of the calling lanes
+// lid = 0 .. GROUPS * 8 - 1 (dense small dims: one lane per id), so every score is the chain score_list uses; f(j, score) runs on one
+// lane per id.  All GROUPS * 8 lanes must call it (the groups' shuffles span whole warps).
+template <int KIND, int METRIC, int GROUPS, class F>
+__device__ __forceinline__ void hnsw_score_rows(const HnswParams& p, const uint8_t* qrow, const uint32_t* ids, uint32_t n, int lid, F f) {
+    if (KIND == HK_DENSE_SMALL) {
+        for (uint32_t j = lid; j < n; j += GROUPS * 8) f(j, score_one<KIND, METRIC>(p, qrow, 0.0f, ids[j], 0));
+    } else {
+        const int g = lid >> 3, t = lid & 7;
+        for (uint32_t j = g; j < ((n + GROUPS - 1) / GROUPS) * GROUPS; j += GROUPS) {
+            const float s = score_one<KIND, METRIC>(p, qrow, 0.0f, ids[j < n ? j : 0], t);
+            if (j < n && t == 0) f(j, s);
+        }
+    }
+}
+
+// one TMA-engine instruction pulls a whole vector (dim * 4 bytes) from HBM into L2, so that the group's demand loads — which the
+// compiler keeps only 3-4 deep — are L2 hits instead of HBM round trips
+__device__ __forceinline__ void prefetch_row_l2(const void* p, uint32_t bytes) {
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
+}
+template <int KIND>
+__device__ __forceinline__ void prefetch_point(const HnswParams& p, uint32_t id) {
+    if (KIND == HK_DENSE_AVX || KIND == HK_DENSE_SMALL) prefetch_row_l2(p.rows + (size_t)id * p.stride, p.stride);
+    else prefetch_row_l2(p.codes + (size_t)id * p.ad, p.ad);
+}
+
+__device__ __forceinline__ bool hnsw_filtered_out(const HnswParams& p, uint32_t id) {
+    bool d = false;
+    if (p.deleted) d = (p.deleted[id >> 5] >> (id & 31)) & 1u;
+    if (p.deleted2) d = d || ((p.deleted2[id >> 5] >> (id & 31)) & 1u);
+    return d;
+}
+
+// GraphLinksView::point_level (view.rs:354-369): the first level whose point count the point's reindex reaches, minus one
+__device__ __forceinline__ uint32_t hnsw_point_level(const HnswParams& p, uint32_t id) {
+    const uint64_t r = p.reindex[id];
+    for (uint32_t l = 1; l < p.levels; ++l) {
+        const uint64_t a = p.level_offsets[l], b = l + 1 < p.levels ? p.level_offsets[l + 1] : p.lo_end;
+        if (r >= b - a) return l - 1;
+    }
+    return p.levels ? p.levels - 1 : 0;
+}
+
+// GraphLayers::get_entry_point (graph_layers.rs:506-528) for query q: of its custom entry points that pass the filter, the one with the
+// highest level, the LAST of equal maxima (Iterator::max_by_key); none -> the caller's entry point
+__device__ __forceinline__ void hnsw_custom_entry(const HnswParams& p, uint32_t q, uint32_t& entry, uint32_t& level) {
+    entry = p.entry; level = p.entry_level;
+    if (!p.cep) return;
+    const uint32_t nc = min(p.cep_counts[q], p.n_cep);
+    bool found = false;
+    for (uint32_t i = 0; i < nc; ++i) {
+        const uint32_t id = p.cep[(size_t)q * p.n_cep + i].idx;
+        if (id >= p.n_points || hnsw_filtered_out(p, id)) continue;
+        const uint32_t l = hnsw_point_level(p, id);
+        if (!found || l >= level) { found = true; entry = id; level = l; }
+    }
+}
+
+// ---- ACORN-1 level-0 step (search_on_level_acorn, graph_layers.rs:154-243) for the candidate `cand` = keys[best].
+// The reference's order-dependent loops reduce to set operations here because a links0 row holds at most m0 ids:
+//  * 1-hop: the loop breaks once to_score.len() >= m0, which only the m0-th link of a row of m0 fresh passing links can reach, so
+//    the break never skips a link.  Every fresh link is marked in hop1 (test-and-set); passing ones go to to_score, the rest to
+//    to_explore.
+//  * 2-hop: a list breaks once it has added m0 points to to_score, again only at its last link, so every list is read to the end.
+//    A passing link is scored the first time the pass meets it if it was not in hop1 before: test-and-set on hop1 finds that
+//    first meeting, so all lists are processed at once by the whole CTA.
+//  * hop2_visited_list cannot change what is scored, so it is not kept.  A passing link enters hop2 only on the step that also marks
+//    it in hop1 (hop1 marks are never undone), so for a passing link `hop1.check || hop2.check_and_update` is the hop1 check; a
+//    filtered-out 2-hop link is neither scored nor marked in hop1 whatever that test returns.  The reference's hop2 only saves
+//    filter lookups; here it would cost a second bitmap per CTA and an atomic per filtered-out 2-hop link.
+//  * to_score's order only decides the merge order of distinct keys, which the sorted merge does not depend on.
+// Leaves s_n = |to_score| with the ids in sm.ids, and the marks logged.
+template <int KIND, int NT>
+__device__ __forceinline__ void acorn_collect(const HnswParams& p, const HnswSmem& sm, uint32_t* xids, uint32_t cand, uint32_t* visited, uint32_t* vlog,
+                                              unsigned int& s_n, unsigned int& s_nx, unsigned int& s_nlog, unsigned int* s_warp_cnt) {
+    const int tid = threadIdx.x;
+    if (tid < 64) {
+        const uint32_t l = (uint32_t)tid < p.m0 ? p.links0[(size_t)cand * p.m0 + tid] : HNSW_EMPTY;
+        const bool fresh = l < p.n_points && ((atomicOr(&visited[l >> 5], 1u << (l & 31)) >> (l & 31)) & 1u) == 0u;
+        const bool pass = fresh && !hnsw_filtered_out(p, l);
+        const unsigned int bs = __ballot_sync(0xFFFFFFFFu, pass), bx = __ballot_sync(0xFFFFFFFFu, fresh && !pass);
+        if ((tid & 31) == 0) { s_warp_cnt[tid >> 5] = __popc(bs); s_warp_cnt[2 + (tid >> 5)] = __popc(bx); }
+        __syncwarp();
+        asm volatile("bar.sync 1, 64;" ::: "memory");
+        const unsigned int lt = (1u << (tid & 31)) - 1u;
+        const uint32_t ps = ((tid >> 5) ? s_warp_cnt[0] : 0u) + __popc(bs & lt);
+        const uint32_t px = ((tid >> 5) ? s_warp_cnt[2] : 0u) + __popc(bx & lt);
+        if (pass) {
+            if (p.prefetch) prefetch_point<KIND>(p, l);
+            sm.ids[ps] = l;
+        } else if (fresh) {
+            xids[px] = l;
+        }
+        if (fresh) {
+            const uint32_t lp = s_nlog + ps + px;
+            if (lp < p.vlog_cap) vlog[lp] = l;
+        }
+        asm volatile("bar.sync 1, 64;" ::: "memory");
+        if (tid == 0) {
+            s_n = s_warp_cnt[0] + s_warp_cnt[1]; s_nx = s_warp_cnt[2] + s_warp_cnt[3];
+            s_nlog += s_n + s_nx;
+        }
+    }
+    __syncthreads();
+    const uint32_t nx = s_nx, m0 = p.m0;
+    for (uint32_t e = tid; e < nx * m0; e += NT) {
+        const uint32_t h1 = xids[e / m0];
+        const uint32_t l = p.links0[(size_t)h1 * m0 + (e % m0)];
+        if (l >= p.n_points) continue;
+        if (hnsw_filtered_out(p, l)) continue;
+        const uint32_t bit = 1u << (l & 31);
+        if (atomicOr(&visited[l >> 5], bit) & bit) continue;                // hop1_visited_list.check, then marked on acceptance
+        if (p.prefetch) prefetch_point<KIND>(p, l);
+        sm.ids[atomicAdd(&s_n, 1u)] = l;
+        const uint32_t lp = atomicAdd(&s_nlog, 1u);
+        if (lp < p.vlog_cap) vlog[lp] = l;
+    }
+    __syncthreads();
+}
+
+// descending bitonic sort of newk[0 .. n) (n <= hop_cap), padded with empty keys (0) to a power of two
+template <int NT>
+__device__ __forceinline__ void acorn_sort_desc(unsigned long long* newk, uint32_t n) {
+    uint32_t P = 1;
+    while (P < n) P <<= 1;
+    for (uint32_t i = n + threadIdx.x; i < P; i += NT) newk[i] = 0ull;
+    __syncthreads();
+    for (uint32_t k = 2; k <= P; k <<= 1) {
+        for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+            for (uint32_t i = threadIdx.x; i < P; i += NT) {
+                const uint32_t o = i ^ j;
+                if (o > i) {
+                    const unsigned long long a = newk[i], b = newk[o];
+                    if (((i & k) == 0) ? (a < b) : (a > b)) { newk[i] = b; newk[o] = a; }
+                }
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// number of keys in keys[0 .. len) (distinct, descending) greater than k
+__device__ __forceinline__ uint32_t count_greater(const unsigned long long* keys, uint32_t len, unsigned long long k) {
+    uint32_t lo = 0, hi = len;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (keys[mid] > k) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+
+// CUSTOM = 1: a custom query (recommend / discover / context / feedback) scored through qbf::fold, with per-query custom entry points
+template <int KIND, int METRIC, int NT, int ALGO, int CUSTOM>
+__global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
+    constexpr int HNSW_THREADS = NT;
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    __shared__ unsigned int s_q, s_best, s_n, s_nvalid, s_len, s_nlog, s_cur, s_changed, s_warp_cnt[ALGO == ALGO_ACORN ? 4 : 2];
+    __shared__ float s_cur_score;
+    __shared__ unsigned int s_nx;   // ACORN: |to_explore|
+    __shared__ unsigned int s_entry, s_entry_level;   // CUSTOM: get_entry_point of this query
+    const int tid = threadIdx.x;
+    const uint32_t ef = p.ef;
+    HnswSmem sm;
+    uint32_t* xids = nullptr;   // ACORN: to_explore [HNSW_MAX_LINKS]
+    {
+        const uint32_t hop = ALGO == ALGO_ACORN ? p.hop_cap : HNSW_MAX_LINKS;
+        uint8_t* b = smem_raw;
+        sm.q = b; b += ((CUSTOM ? p.q_smem : p.q_bytes) + 15u) & ~15u;
+        sm.keys[0] = reinterpret_cast<unsigned long long*>(b); b += (size_t)ef * 8;
+        sm.keys[1] = reinterpret_cast<unsigned long long*>(b); b += (size_t)ef * 8;
+        sm.newk = reinterpret_cast<unsigned long long*>(b); b += (size_t)hop * 8;
+        sm.ids = reinterpret_cast<uint32_t*>(b); b += (size_t)hop * 4;
+        sm.sc = reinterpret_cast<float*>(b); b += (size_t)hop * 4;
+        sm.flags[0] = b; b += (ef + 15u) & ~15u;
+        sm.flags[1] = b;
+        if (ALGO == ALGO_ACORN) { b += (ef + 15u) & ~15u; xids = reinterpret_cast<uint32_t*>(b); }
+    }
+    uint32_t* visited = p.visited + (size_t)blockIdx.x * p.visited_words;
+    uint32_t* vlog = p.vlog + (size_t)blockIdx.x * p.vlog_cap;
+    unsigned long long hops = 0, evals = 0;   // thread 0 only
+
+    for (;;) {
+        if (tid == 0) s_q = atomicAdd(p.work, 1u);
+        __syncthreads();
+        const uint32_t q = s_q;
+        if (q >= p.nq) break;
+        // ---- query into shared memory
+        if constexpr (ALGO == ALGO_BUILD) {
+            // the point being inserted: its stored row is the query (FilteredScorer::new_internal)
+            const uint4* src = reinterpret_cast<const uint4*>(p.rows + (size_t)p.b_pts[q] * p.stride);
+            uint4* dst = reinterpret_cast<uint4*>(const_cast<uint8_t*>(sm.q));
+            for (uint32_t i = tid; i < p.q_bytes / 16u; i += HNSW_THREADS) dst[i] = src[i];
+        } else if constexpr (!CUSTOM) {
+            const uint4* src = reinterpret_cast<const uint4*>(p.q_enc + (size_t)q * p.q_bytes);
+            uint4* dst = reinterpret_cast<uint4*>(const_cast<uint8_t*>(sm.q));
+            for (uint32_t i = tid; i < (p.q_bytes + 15u) / 16u; i += HNSW_THREADS) dst[i] = src[i];
+        } else {
+            // the examples: into shared memory when they fit, else read where they are (the same arithmetic either way)
+            const size_t first = (size_t)q * p.ex_stride + p.ex_first;
+            const uint8_t* src = p.q_enc + first * p.q_bytes;
+            if (p.ex_smem) {
+                const uint4* s4 = reinterpret_cast<const uint4*>(src);
+                uint4* dst = reinterpret_cast<uint4*>(smem_raw);   // the query region of the layout above
+                for (uint32_t i = tid; i < (p.n_ex * p.q_bytes) / 16u; i += HNSW_THREADS) dst[i] = s4[i];
+                sm.q = smem_raw;
+            } else {
+                sm.q = src;
+            }
+        }
+        const float q_off = (!CUSTOM && p.q_off) ? p.q_off[q] : 0.0f;
+        if (tid == 0) {
+            s_nlog = 0;
+            if constexpr (CUSTOM) {
+                uint32_t e, l;
+                hnsw_custom_entry(p, q, e, l);
+                s_entry = e; s_entry_level = l; sm.ids[0] = e;
+            } else if constexpr (ALGO == ALGO_BUILD) {
+                sm.ids[0] = p.b_entry[q];
+            } else {
+                sm.ids[0] = p.entry;
+            }
+        }
+        __syncthreads();
+        // `CUSTOM ? s_entry : p.entry` is written out at each use, not bound to a local, so the nearest-query kernels compile as before
+
+        // ---- search_entry: greedy descent from the entry point's level to level 1 (graph_layers.rs:247-316)
+        score_list<KIND, METRIC, NT, CUSTOM>(p, sm, q_off, 1, q);      // score_point(entry)
+        __syncthreads();
+        if (tid == 0) { s_cur = CUSTOM ? s_entry : (ALGO == ALGO_BUILD ? sm.ids[0] : p.entry); s_cur_score = sm.sc[0]; ++hops; ++evals; }
+        __syncthreads();
+        for (uint32_t lvl = CUSTOM ? s_entry_level : p.entry_level; lvl >= 1; --lvl) {
+            // search_entry_on_level re-scores its entry point on every level (graph_layers.rs:298-301): same value, but the scorer call
+            // and the scored point are metered, so they are counted here too
+            if (tid == 0 && lvl != (CUSTOM ? s_entry_level : p.entry_level)) { ++hops; ++evals; }
+            for (;;) {
+                const uint32_t cur = s_cur;
+                // links of `cur` on this level: neighbors[offsets[idx] .. offsets[idx + 1]), idx = level_offsets[lvl] + reindex[cur] (view.rs:203-215)
+                if (tid < 32) {
+                    const uint64_t idx = p.level_offsets[lvl] + p.reindex[cur];
+                    const uint64_t b = p.offsets[idx], e = p.offsets[idx + 1];
+                    uint32_t cnt = 0;
+                    // filter (check_batched keeps matches in order), then truncate to level_m (point_scorer.rs:270-277)
+                    for (uint64_t base = b; base < e && cnt < p.m; base += 32) {
+                        const uint64_t i = base + tid;
+                        const uint32_t l = i < e ? p.neighbors[i] : HNSW_EMPTY;
+                        const bool keep = l != HNSW_EMPTY && l < p.n_points && !hnsw_filtered_out(p, l);
+                        const unsigned int bal = __ballot_sync(0xFFFFFFFFu, keep);
+                        const uint32_t pos = cnt + __popc(bal & ((1u << tid) - 1u));
+                        if (keep && pos < p.m && pos < HNSW_MAX_LINKS) { sm.ids[pos] = l; if (p.prefetch) prefetch_point<KIND>(p, l); }
+                        cnt += __popc(bal);
+                    }
+                    if (tid == 0) s_n = min(min(cnt, p.m), HNSW_MAX_LINKS);
+                }
+                __syncthreads();
+                const uint32_t n = s_n;
+                score_list<KIND, METRIC, NT, CUSTOM>(p, sm, q_off, n, q);
+                __syncthreads();
+                if (tid == 0) {
+                    bool changed = false;
+                    uint32_t c = cur; float cs = s_cur_score;
+                    for (uint32_t i = 0; i < n; ++i) if (sm.sc[i] > cs) { changed = true; c = sm.ids[i]; cs = sm.sc[i]; }
+                    s_cur = c; s_cur_score = cs; s_changed = changed ? 1u : 0u;
+                    if (n) { ++hops; evals += n; }
+                }
+                __syncthreads();
+                if (!s_changed) break;
+            }
+        }
+
+        if constexpr (ALGO == ALGO_BUILD) {
+            // a point below this level: search_entry_on_level (graph_layers.rs:279-316) on the level's rows, a row's links being the
+            // prefix before its first HNSW_EMPTY; the entry moves to a strictly better link, the first in link order
+            if (!p.b_insert) {
+                for (;;) {
+                    const uint32_t cur = s_cur;
+                    if (tid < 64) {
+                        const uint32_t l = (uint32_t)tid < p.m0 ? p.links0[(size_t)hnsw_build_row(p, cur) * p.m0 + tid] : HNSW_EMPTY;
+                        if (l != HNSW_EMPTY) sm.ids[tid] = l;
+                        const unsigned int bal = __ballot_sync(0xFFFFFFFFu, l != HNSW_EMPTY);
+                        if ((tid & 31) == 0) s_warp_cnt[tid >> 5] = __popc(bal);
+                    }
+                    __syncthreads();
+                    const uint32_t n = s_warp_cnt[0] + s_warp_cnt[1];
+                    score_list<KIND, METRIC, NT, CUSTOM>(p, sm, q_off, n, q);
+                    __syncthreads();
+                    if (tid == 0) {
+                        bool changed = false;
+                        uint32_t c = cur; float cs = s_cur_score;
+                        for (uint32_t i = 0; i < n; ++i) if (sm.sc[i] > cs) { changed = true; c = sm.ids[i]; cs = sm.sc[i]; }
+                        s_cur = c; s_cur_score = cs; s_changed = changed ? 1u : 0u;
+                    }
+                    __syncthreads();
+                    if (!s_changed) break;
+                }
+                if (tid == 0) p.b_entry[q] = s_cur;
+                __syncthreads();
+                continue;
+            }
+        }
+
+        // ---- search_on_level(level 0, ef): nearest = [level entry], entry visited
+        if (tid == 0) {
+            const uint32_t e0 = s_cur;
+            sm.keys[0][0] = qb_pack_key(s_cur_score, e0);
+            sm.flags[0][0] = 0;
+            s_len = 1;
+            atomicOr(&visited[e0 >> 5], 1u << (e0 & 31));
+            vlog[0] = e0; s_nlog = 1;
+        }
+        __syncthreads();
+        int cb = 0;   // current buffer
+        for (;;) {
+            unsigned long long* keys = sm.keys[cb];
+            uint8_t* flags = sm.flags[cb];
+            const uint32_t len = s_len;
+            // 1. best not-yet-expanded entry
+            if (tid == 0) s_best = 0xFFFFFFFFu;
+            __syncthreads();
+            for (uint32_t i = tid; i < len; i += HNSW_THREADS) if (!flags[i]) atomicMin(&s_best, i);
+            __syncthreads();
+            const uint32_t best = s_best;
+            if (best == 0xFFFFFFFFu) break;
+            const uint32_t cand = qb_key_id(keys[best]);
+            if constexpr (ALGO == ALGO_ACORN) {
+                if (tid == 0) flags[best] = 1;
+                acorn_collect<KIND, NT>(p, sm, xids, cand, visited, vlog, s_n, s_nx, s_nlog, s_warp_cnt);
+                const uint32_t n = s_n;
+                if (tid == 0) { if (n) { ++hops; evals += n; } s_nvalid = 0; }
+                if (n == 0) { __syncthreads(); continue; }
+                // score_points_unfiltered(to_score)
+                if (KIND == HK_DENSE_SMALL) {
+                    for (uint32_t i = tid; i < n; i += HNSW_THREADS) sm.sc[i] = score_q<KIND, METRIC, CUSTOM>(p, sm, q_off, sm.ids[i], 0, q);
+                } else {
+                    score_list<KIND, METRIC, NT, CUSTOM>(p, sm, q_off, n, q);
+                }
+                __syncthreads();
+                // keys that can enter `nearest`, compacted, sorted, at most ef of them
+                const unsigned long long lower = (len == ef) ? keys[ef - 1] : 0ull;
+                for (uint32_t i = tid; i < n; i += HNSW_THREADS) {
+                    const unsigned long long k = qb_pack_key(sm.sc[i], sm.ids[i]);
+                    if (k > lower) sm.newk[atomicAdd(&s_nvalid, 1u)] = k;
+                }
+                __syncthreads();
+                const uint32_t nv = s_nvalid;
+                if (nv == 0) continue;
+                acorn_sort_desc<NT>(sm.newk, nv);
+                const uint32_t nk_len = min(nv, ef);
+                // merge: rank = own index + number of greater keys in the other list (both sorted: binary search)
+                unsigned long long* nk = sm.keys[cb ^ 1];
+                uint8_t* nf = sm.flags[cb ^ 1];
+                for (uint32_t i = tid; i < len; i += HNSW_THREADS) {
+                    const unsigned long long k = keys[i];
+                    const uint32_t r = i + count_greater(sm.newk, nk_len, k);
+                    if (r < ef) { nk[r] = k; nf[r] = flags[i]; }
+                }
+                for (uint32_t j = tid; j < nk_len; j += HNSW_THREADS) {
+                    const unsigned long long k = sm.newk[j];
+                    const uint32_t r = j + count_greater(keys, len, k);
+                    if (r < ef) {
+                        nk[r] = k; nf[r] = 0;
+                        if (QB_HNSW_LINK_PREFETCH && p.prefetch) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.links0 + (size_t)(ALGO == ALGO_BUILD ? hnsw_build_row(p, qb_key_id(k)) : qb_key_id(k)) * p.m0));
+                    }
+                }
+                __syncthreads();
+                if (tid == 0) s_len = min(len + nk_len, ef);
+                cb ^= 1;
+                __syncthreads();
+                continue;
+            }
+            // 2. its level-0 links that pass the filter and were not visited (test-and-set), in link order
+            if (tid < 64) {
+                const uint32_t l = (uint32_t)tid < p.m0 ? p.links0[(size_t)(ALGO == ALGO_BUILD ? hnsw_build_row(p, cand) : cand) * p.m0 + tid] : HNSW_EMPTY;
+                bool keep = l < p.n_points && !hnsw_filtered_out(p, l);
+                if (keep) keep = ((atomicOr(&visited[l >> 5], 1u << (l & 31)) >> (l & 31)) & 1u) == 0u;
+                const unsigned int bal = __ballot_sync(0xFFFFFFFFu, keep);
+                if ((tid & 31) == 0) s_warp_cnt[tid >> 5] = __popc(bal);
+                __syncwarp();
+                // two warps: positions of warp 1 follow warp 0's
+                asm volatile("bar.sync 1, 64;" ::: "memory");
+                const uint32_t pos = ((tid >> 5) ? s_warp_cnt[0] : 0u) + __popc(bal & ((1u << (tid & 31)) - 1u));
+                if (keep) {
+                    if (p.prefetch) prefetch_point<KIND>(p, l);          // HBM -> L2 for the whole vector, in flight while the list is published
+                    sm.ids[pos] = l;
+                    const uint32_t lp = s_nlog + pos;
+                    if (lp < p.vlog_cap) vlog[lp] = l;
+                }
+                if (tid == 0) { flags[best] = 1; s_n = s_warp_cnt[0] + s_warp_cnt[1]; }
+            }
+            __syncthreads();
+            const uint32_t n = s_n;
+            if (tid == 0) { s_nlog += n; if (n) { ++hops; evals += n; } s_nvalid = 0; }
+            if (n == 0) { __syncthreads(); continue; }
+            // 3. score
+            score_list<KIND, METRIC, NT, CUSTOM>(p, sm, q_off, n, q);
+            __syncthreads();
+            // 4. keys of the new points; the ones that cannot enter a full list are dropped here (key 0 = empty)
+            const unsigned long long lower = (len == ef) ? keys[ef - 1] : 0ull;
+            if ((uint32_t)tid < n) {
+                unsigned long long k = qb_pack_key(sm.sc[tid], sm.ids[tid]);
+                if (k <= lower) k = 0ull; else atomicAdd(&s_nvalid, 1u);
+                sm.newk[tid] = k;
+            }
+            __syncthreads();
+            const uint32_t nvalid = s_nvalid;
+            if (nvalid == 0) continue;
+            // 5. merge into the other buffer: rank = own index + number of greater keys in the other list
+            unsigned long long* nk = sm.keys[cb ^ 1];
+            uint8_t* nf = sm.flags[cb ^ 1];
+            for (uint32_t i = tid; i < len; i += HNSW_THREADS) {
+                const unsigned long long k = keys[i];
+                uint32_t r = i;
+                for (uint32_t j = 0; j < n; ++j) r += (sm.newk[j] > k) ? 1u : 0u;
+                if (r < ef) { nk[r] = k; nf[r] = flags[i]; }
+            }
+            if ((uint32_t)tid >= HNSW_THREADS - HNSW_MAX_LINKS) {   // the last two warps place the new keys
+                const uint32_t j = (uint32_t)tid - (HNSW_THREADS - HNSW_MAX_LINKS);
+                const unsigned long long k = j < n ? sm.newk[j] : 0ull;
+                if (k) {
+                    uint32_t r = 0;
+                    for (uint32_t j2 = 0; j2 < n; ++j2) r += (sm.newk[j2] > k) ? 1u : 0u;
+                    uint32_t lo = 0, hi = len;   // first index with keys[idx] < k (keys are distinct and descending)
+                    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (keys[mid] > k) lo = mid + 1; else hi = mid; }
+                    r += lo;
+                    if (r < ef) {
+                        nk[r] = k; nf[r] = 0;
+                        // every point that enters `nearest` is a future candidate: pull its level-0 link row (one 128-byte line at m0 = 32) into L2 now
+                        if (QB_HNSW_LINK_PREFETCH && p.prefetch) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.links0 + (size_t)(ALGO == ALGO_BUILD ? hnsw_build_row(p, qb_key_id(k)) : qb_key_id(k)) * p.m0));
+                    }
+                }
+            }
+            __syncthreads();
+            if (tid == 0) s_len = min(len + nvalid, ef);
+            cb ^= 1;
+            __syncthreads();
+        }
+
+        if constexpr (ALGO == ALGO_BUILD) {
+            // the point's next entry is the best it found (link_new_point, graph_layers_builder.rs:417-475); its links are
+            // fill_from_sorted_with_heuristic (links_container.rs:47-71) over `nearest`: candidate c is kept unless a kept link scores
+            // higher against c than the point does.  The kept links go to sm.ids, their number to s_n.
+            const unsigned long long* keys = sm.keys[cb];
+            const uint32_t len = s_len, pt = p.b_pts[q];
+            if (tid == 0) { p.b_entry[q] = qb_key_id(keys[0]); s_n = 0; }
+            __syncthreads();
+            for (uint32_t c = 0; c < len; ++c) {
+                const uint32_t nsel = s_n;
+                if (nsel >= p.m0) break;
+                const uint32_t cid = qb_key_id(keys[c]);
+                const float cs = qb_key_score(keys[c]);
+                if (tid == 0) s_changed = 0;
+                __syncthreads();
+                hnsw_score_rows<KIND, METRIC, NT / 8>(p, p.rows + (size_t)cid * p.stride, sm.ids, nsel, tid, [&](uint32_t, float s) {
+                    if (s > cs) s_changed = 1;
+                });
+                __syncthreads();
+                if (tid == 0 && !s_changed) { sm.ids[nsel] = cid; s_n = nsel + 1; }
+                __syncthreads();
+            }
+            // the point's row, and its backlinks for the backlink pass
+            const uint32_t nsel = s_n;
+            uint32_t* row = const_cast<uint32_t*>(p.links0) + (size_t)hnsw_build_row(p, pt) * p.m0;
+            for (uint32_t j = tid; j < p.m0; j += HNSW_THREADS) {
+                const uint32_t l = j < nsel ? sm.ids[j] : HNSW_EMPTY;
+                row[j] = l;
+                p.b_tkey[(size_t)q * p.m0 + j] = j < nsel ? (((unsigned long long)l << 32) | q) : ~0ull;
+                p.b_tval[(size_t)q * p.m0 + j] = pt;
+            }
+        }
+        // ---- results: into_iter_sorted().take(top) (graph_layers.rs:560)
+        if constexpr (ALGO != ALGO_BUILD) {
+            const unsigned long long* keys = sm.keys[cb];
+            const uint32_t len = s_len, cnt = min(len, p.top);
+            for (uint32_t i = tid; i < cnt; i += HNSW_THREADS) {
+                qb_scored_point sp;
+                sp.idx = qb_key_id(keys[i]) + p.id_base;
+                sp.score = qb_key_score(keys[i]);
+                p.out[(size_t)q * p.top + i] = sp;
+            }
+            if (tid == 0) p.out_counts[q] = cnt;
+        }
+        // ---- un-set the visited bits this query set
+        {
+            const uint32_t nlog = s_nlog;
+            if (nlog <= p.vlog_cap) {
+                for (uint32_t i = tid; i < nlog; i += HNSW_THREADS) visited[vlog[i] >> 5] = 0u;
+            } else {
+                for (uint64_t i = tid; i < p.visited_words; i += HNSW_THREADS) visited[i] = 0u;
+            }
+        }
+        __syncthreads();
+    }
+    if (tid == 0 && p.stats) { atomicAdd(&p.stats[0], hops); atomicAdd(&p.stats[1], evals); }
+}
+
+template <int KIND, int NT, int ALGO, int CUSTOM>
+qb_status launch_kind(int metric, const HnswParams& p, unsigned grid, size_t smem, cudaStream_t stream) {
+#define QB_HNSW_LAUNCH(M)                                                                                              \
+    do {                                                                                                               \
+        QB_CUDA(cudaFuncSetAttribute(hnsw_search_kernel<KIND, M, NT, ALGO, CUSTOM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+        hnsw_search_kernel<KIND, M, NT, ALGO, CUSTOM><<<grid, NT, smem, stream>>>(p);                                          \
+    } while (0)
+    if (KIND == HK_SQ8 || KIND == HK_SQ8_LANEX) QB_HNSW_LAUNCH(M_DOT);
+    else if (metric == M_EUCLID) QB_HNSW_LAUNCH(M_EUCLID);
+    else if (metric == M_MANHATTAN) QB_HNSW_LAUNCH(M_MANHATTAN);
+    else QB_HNSW_LAUNCH(M_DOT);
+#undef QB_HNSW_LAUNCH
+    QB_LAUNCHED();
+    QB_CUDA(cudaGetLastError());
+    return QB_OK;
+}
+
+template <int KIND, int METRIC, int NT, int ALGO, int CUSTOM>
+int occupancy_of(size_t smem) {
+    int nb = 0;
+    cudaFuncSetAttribute(hnsw_search_kernel<KIND, METRIC, NT, ALGO, CUSTOM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, hnsw_search_kernel<KIND, METRIC, NT, ALGO, CUSTOM>, NT, smem) != cudaSuccess) nb = 1;
+    return nb < 1 ? 1 : nb;
+}
+template <int NT, int ALGO, int CUSTOM>
+int occupancy_dispatch(int kind, int metric, size_t smem) {
+    switch (kind) {
+        case HK_DENSE_AVX: return metric == M_EUCLID ? occupancy_of<HK_DENSE_AVX, M_EUCLID, NT, ALGO, CUSTOM>(smem) : metric == M_MANHATTAN ? occupancy_of<HK_DENSE_AVX, M_MANHATTAN, NT, ALGO, CUSTOM>(smem) : occupancy_of<HK_DENSE_AVX, M_DOT, NT, ALGO, CUSTOM>(smem);
+        case HK_DENSE_SMALL: return metric == M_EUCLID ? occupancy_of<HK_DENSE_SMALL, M_EUCLID, NT, ALGO, CUSTOM>(smem) : metric == M_MANHATTAN ? occupancy_of<HK_DENSE_SMALL, M_MANHATTAN, NT, ALGO, CUSTOM>(smem) : occupancy_of<HK_DENSE_SMALL, M_DOT, NT, ALGO, CUSTOM>(smem);
+        case HK_SQ8: return occupancy_of<HK_SQ8, M_DOT, NT, ALGO, CUSTOM>(smem);
+        default: return occupancy_of<HK_SQ8_LANEX, M_DOT, NT, ALGO, CUSTOM>(smem);
+    }
+}
+template <int NT, int ALGO, int CUSTOM>
+qb_status launch_dispatch(int kind, int metric, const HnswParams& p, unsigned grid, size_t smem, cudaStream_t stream) {
+    switch (kind) {
+        case HK_DENSE_AVX: return launch_kind<HK_DENSE_AVX, NT, ALGO, CUSTOM>(metric, p, grid, smem, stream);
+        case HK_DENSE_SMALL: return launch_kind<HK_DENSE_SMALL, NT, ALGO, CUSTOM>(metric, p, grid, smem, stream);
+        case HK_SQ8: return launch_kind<HK_SQ8, NT, ALGO, CUSTOM>(metric, p, grid, smem, stream);
+        default: return launch_kind<HK_SQ8_LANEX, NT, ALGO, CUSTOM>(metric, p, grid, smem, stream);
+    }
+}
+template <int ALGO>
+int occupancy_nt(int nt, int kind, int metric, size_t smem) {
+    return nt == 128 ? occupancy_dispatch<128, ALGO, 0>(kind, metric, smem) : (nt == 64 ? occupancy_dispatch<64, ALGO, 0>(kind, metric, smem) : occupancy_dispatch<256, ALGO, 0>(kind, metric, smem));
+}
+template <int ALGO>
+qb_status launch_nt(int nt, int kind, int metric, const HnswParams& p, unsigned grid, size_t smem, cudaStream_t stream) {
+    return nt == 128 ? launch_dispatch<128, ALGO, 0>(kind, metric, p, grid, smem, stream)
+                     : (nt == 64 ? launch_dispatch<64, ALGO, 0>(kind, metric, p, grid, smem, stream) : launch_dispatch<256, ALGO, 0>(kind, metric, p, grid, smem, stream));
+}
+
+
+// shared memory of one CTA of hnsw_search_kernel with HNSW level 0 (also ALGO_BUILD): query, two key buffers, the hop's lists, two flag buffers
+inline size_t hnsw_smem_bytes(uint32_t q_bytes, uint32_t ef) {
+    return (size_t)((q_bytes + 15u) & ~15u) + (size_t)ef * 16 + HNSW_MAX_LINKS * 16 + 2 * (size_t)((ef + 15u) & ~15u);
+}
+
+}  // namespace

@@ -164,6 +164,9 @@ struct QbHnswCustom {
 qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, uint32_t nq, uint32_t top, uint32_t ef, uint32_t entry, uint32_t entry_level,
                          const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts, cudaStream_t stream, int algo /* qb_hnsw_algorithm */,
                          const QbHnswCustom* custom = nullptr);
+// completes a handle whose plain arrays (d_level_offsets, d_reindex, d_neighbors, d_offsets and the host-side counts) are on the device:
+// the level-0 table and the search scratch (qb_hnsw.cu).  On failure the caller destroys g.  who = the error messages' prefix.
+qb_status qb_hnsw_finish_plain(qb_hnsw* g, const char* who);
 // adds the device counters to g->hops / g->evals and clears them; evals_by_slot (optional, [2]) receives each slot's scored points
 qb_status qb_hnsw_read_stats(qb_hnsw* g, cudaStream_t stream, uint64_t* evals_by_slot = nullptr);
 

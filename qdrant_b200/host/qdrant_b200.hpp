@@ -209,6 +209,22 @@ public:
         check(qb_hnsw_create_compressed(storage.raw(), links_bin, n_bytes, &h));
         return std::unique_ptr<HnswGraph>(new HnswGraph(h));
     }
+    // builds the graph of a dense f32 storage on the device (qb_hnsw_build); levels: one per point, <= 30; batch / serial_points 0 = 512 / 256.
+    // The entry point the search starts from is returned in entry_point / entry_level.
+    static std::unique_ptr<HnswGraph> build(const VectorStorage& storage, uint32_t m, uint32_t m0, uint32_t ef_construct, const std::vector<uint8_t>& levels,
+                                            uint32_t batch, uint32_t serial_points, uint32_t& entry_point, uint32_t& entry_level) {
+        qb_hnsw* h = nullptr;
+        check(qb_hnsw_build(storage.raw(), m, m0, ef_construct, levels.data(), batch, serial_points, &h, &entry_point, &entry_level));
+        return std::unique_ptr<HnswGraph>(new HnswGraph(h));
+    }
+    // the graph as a plain links.bin (qb_hnsw_export_plain)
+    std::vector<uint8_t> export_plain() const {
+        uint64_t n = 0;
+        check(qb_hnsw_export_plain(h_, nullptr, 0, &n));
+        std::vector<uint8_t> out(n);
+        check(qb_hnsw_export_plain(h_, out.data(), n, &n));
+        return out;
+    }
     ~HnswGraph() { qb_hnsw_destroy(h_); }
     HnswGraph(const HnswGraph&) = delete;
     // GraphLinks::links (view.rs:238-263): the point's links on `level`, in stored order

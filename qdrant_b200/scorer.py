@@ -733,6 +733,39 @@ class HnswGraph:
         self._h = h
         return self
 
+    @classmethod
+    def build(cls, storage: _Storage, m: int = 16, ef_construct: int = 100, levels=None, seed: int = 0, batch: int = 0, serial_points: int = 0,
+              m0: Optional[int] = None) -> "HnswGraph":
+        """Builds the graph of a dense f32 storage on the device (qb_hnsw_build; m0 defaults to 2m).  levels: one per point (<= 30);
+        by default round(-ln(U) / ln(m)) with U uniform in (0, 1] from numpy's generator seeded with `seed` (get_random_layer,
+        graph_layers_builder.rs:388-396).  batch / serial_points 0 = 512 / 256.  The entry point is in .entry_point / .entry_level."""
+        m0 = 2 * m if m0 is None else m0
+        n = storage.count
+        if levels is None:
+            u = 1.0 - np.random.default_rng(seed).random(n)
+            levels = np.minimum(np.round(-np.log(u) / np.log(max(m, 2))), 30)
+        lv = np.ascontiguousarray(levels, dtype=np.int64)
+        if lv.shape != (n,):
+            raise ValueError(f"levels has shape {lv.shape}, storage has {n} points")
+        lv = np.ascontiguousarray(np.clip(lv, 0, 255), dtype=np.uint8)   # a level > 30 is rejected by the library
+        self = cls.__new__(cls)
+        self._storage = storage
+        self._h = vp()
+        h, e, el = vp(), C.c_uint32(), C.c_uint32()
+        check(lib().qb_hnsw_build(storage._h, int(m), int(m0), int(ef_construct), lv.ctypes.data_as(u8p), int(batch), int(serial_points), C.byref(h),
+                                  C.byref(e), C.byref(el)))
+        self._h = h
+        self.entry_point, self.entry_level, self.levels = int(e.value), int(el.value), lv
+        return self
+
+    def export_plain(self) -> np.ndarray:
+        """The graph as a plain links.bin (qb_hnsw_export_plain), for any handle."""
+        n = C.c_uint64()
+        check(lib().qb_hnsw_export_plain(self._h, None, 0, C.byref(n)))
+        out = np.zeros(n.value, dtype=np.uint8)
+        check(lib().qb_hnsw_export_plain(self._h, out.ctypes.data_as(u8p), n.value, C.byref(n)))
+        return out
+
     def links(self, level: int, ids, cap: int = 0):
         """GraphLinks::links for each of `ids` on `level`, in the graph's stored order: a list of uint32 arrays.  cap = 0 returns every
         link (two calls: counts first); cap > 0 truncates each list to cap links."""
