@@ -178,8 +178,9 @@ QB_API qb_status qb_scorer_take_counters(qb_scorer* sc, qb_hw_counters* out);
  * Ties: ScoredPointOffset orders by score only, so which of several equal-score points survives at the
  * k-th boundary is unspecified in the reference; this library orders by (score desc, id asc).
  * How the scan is carried out never changes the result: large dense f32 storages keep compact shadow planes of their rows
- * (built on the first search that uses them, rebuilt after qb_storage_write_rows*: + 26 % HBM for the int8 plane of single-query
- * searches on >= 2^19 rows, + 50 % for the bf16 plane of batches of >= 32 queries; dot / cosine only), batched SQ8 / PQ scans run
+ * (built on the first search that uses them, rebuilt after qb_storage_write_rows*: single-query searches on >= 2^19 rows take + 19 % HBM
+ * for the 6-bit plane and + 14 % for its block-scaled 4-bit first stage at dim 768 (5.9 + 4.4 GB at 10M x 768; option prefilter_stage1 = 5
+ * drops the latter), or + 26 % for the int8 plane, + 50 % for the bf16 plane of batches of >= 32 queries; dot / cosine only), batched SQ8 / PQ scans run
  * prefilter kernels — in every case the rows that can reach the top-k are re-scored with the reference's exact arithmetic before
  * selection, and a case the prefilter cannot decide falls back to the exact scan (qb_search_stats counts those).
  * qb_set_option("disable_prefilter" / "disable_mma", 1) keeps a process on the exact kernels and allocates no plane. */

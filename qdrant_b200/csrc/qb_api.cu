@@ -60,6 +60,7 @@ QbOptions& qb_opt() {
         v.disable_localk = getenv("QB_DISABLE_LOCALK") != nullptr;
         v.disable_prefilter = getenv("QB_DISABLE_PREFILTER") != nullptr;
         v.prefilter_plane = (int)num("QB_PREFILTER_PLANE", 0);
+        v.prefilter_stage1 = (int)num("QB_PREFILTER_STAGE1", 0);
         v.prefilter_slot_bytes = (uint32_t)num("QB_PREFILTER_SLOT_BYTES", 0);
         v.disable_mma = getenv("QB_DISABLE_MMA") != nullptr;
         v.mma_no_segments = getenv("QB_MMA_NO_SEGMENTS") != nullptr;
@@ -81,6 +82,7 @@ extern "C" qb_status qb_set_option(const char* name, int64_t value) {
     if (n == "disable_localk") o.disable_localk = value != 0;
     else if (n == "disable_prefilter") o.disable_prefilter = value != 0;
     else if (n == "prefilter_plane") o.prefilter_plane = (int)value;
+    else if (n == "prefilter_stage1") o.prefilter_stage1 = (int)value;
     else if (n == "prefilter_slot_bytes") o.prefilter_slot_bytes = (uint32_t)value;
     else if (n == "prefilter_producers") o.prefilter_producers = (int)value;
     else if (n == "disable_mma") o.disable_mma = value != 0;
@@ -266,6 +268,7 @@ extern "C" qb_status qb_storage_write_rows(qb_storage* s, uint64_t first_row, ui
     s->bf16_ready = false;   // the bf16 shadow (if any) no longer mirrors the rows
     s->q8_ready = false;
     s->q6_ready = false;
+    s->q4b_ready = false;
     return QB_OK;
 }
 
@@ -281,6 +284,7 @@ extern "C" qb_status qb_storage_write_rows_device(qb_storage* s, uint64_t first_
     s->bf16_ready = false;
     s->q8_ready = false;
     s->q6_ready = false;
+    s->q4b_ready = false;
     return QB_OK;
 }
 
@@ -440,7 +444,7 @@ extern "C" void qb_storage_destroy(qb_storage* s) {
     ctx_destroy(s->dev_ctx);
     for (auto& pr : s->prof_pending) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
     for (auto& pr : s->prof_free) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); }
-    cudaFree(s->d_rows); cudaFree(s->d_bf16); cudaFree(s->d_bf16_meta); cudaFree(s->d_q8); cudaFree(s->d_q8_meta); cudaFree(s->d_q6); cudaFree(s->d_q6_lo); cudaFree(s->d_q6_meta); cudaFree(s->d_codes); cudaFree(s->d_voff); cudaFree(s->d_pq_div); cudaFree(s->d_centroids); cudaFree(s->d_pq_codes);
+    cudaFree(s->d_rows); cudaFree(s->d_bf16); cudaFree(s->d_bf16_meta); cudaFree(s->d_q8); cudaFree(s->d_q8_meta); cudaFree(s->d_q6); cudaFree(s->d_q6_lo); cudaFree(s->d_q6_meta); cudaFree(s->d_q4b); cudaFree(s->d_codes); cudaFree(s->d_voff); cudaFree(s->d_pq_div); cudaFree(s->d_centroids); cudaFree(s->d_pq_codes);
     cudaFree(s->d_bq_rows); cudaFree(s->d_mean_std); cudaFree(s->d_deleted); cudaFree(s->d_pf_fallbacks);
     cudaGetLastError();
     delete s;

@@ -50,6 +50,7 @@ struct QbOptions {
     int prefilter_producers = 0;       // single-query prefilter: producer warps per CTA (0 = default)
     uint32_t prefilter_slot_bytes = 0; // single-query prefilter: target bytes per ring slot (0 = default)
     int prefilter_plane = 0;          // single-query prefilter: 0 = 6-bit shadow plane when the storage allows it, 1 = bf16, 2 = int8 shadow plane
+    int prefilter_stage1 = 0;         // first stage of the 6-bit plane's scan: 5 = its own 5-bit codes (no extra plane), otherwise the block-scaled 4-bit plane
     bool disable_prefilter = false;   // single-query dense f32 searches: always the exact f32 scan (no bf16 shadow plane, qb_prefilter.cu)
     uint32_t mma_seg_cap = 0;      // 0 = 256 survivor slots per (query, CTA) segment of the tensor-core scan
     uint64_t sample_rows = 0;

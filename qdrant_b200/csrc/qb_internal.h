@@ -58,6 +58,10 @@ struct qb_storage {
     uint8_t* d_q6 = nullptr;  uint32_t q6_row_b = 0;  unsigned int* d_q6_meta = nullptr;   // meta as above
     uint8_t* d_q6_lo = nullptr;
     bool q6_ready = false, q6_usable = false;
+    // block-scaled 4-bit records (codes, a u8 scale per 16 dims, the row's scale and residual-norm bound: 0.14 of the f32 bytes), streamed
+    // by the first stage of the 6-bit plane's scan in place of its 5-bit codes
+    uint8_t* d_q4b = nullptr;  uint32_t q4b_row_b = 0;
+    bool q4b_ready = false;
     uint32_t row_stride = 0;         // bytes
     uint32_t elem_size = 4;
 

@@ -568,9 +568,12 @@ __device__ __forceinline__ uint32_t q6_spread(uint32_t t) { return (t | (t << 12
 constexpr size_t PF_SAMPLE_SMEM = (size_t)QB_LOCALK_WARPS * (QB_LOCALK_SLOTS * 8 + 4 * 8 + 4) + QB_LOCALK_SLOTS * 8;   // lists, queues, counts, exact keys
 static_assert(PF_CONSUMER_WARPS == QB_LOCALK_WARPS, "the CTA merge sorts one list per consumer warp");
 
+template <int NCH>
+__device__ __forceinline__ void stage1_query(const Pf6Params& p, int hl, Q6Query<NCH>& Q) { q6_query<NCH>(p, hl, Q); }
+
 template <int NCH, bool SAMPLE>
-__device__ __forceinline__ void q5_tile(const Pf6Params& p, const Q6Query<NCH>& Q, const uint8_t* slot, uint32_t nr, uint64_t r0, int lane, LkState& lk,
-                                        unsigned long long* lk_queue, unsigned int* lk_count) {
+__device__ __forceinline__ void stage1_tile(const Pf6Params& p, const Q6Query<NCH>& Q, const uint8_t* slot, uint32_t nr, uint64_t r0, int lane, LkState& lk,
+                                            unsigned long long* lk_queue, unsigned int* lk_count) {
     const int half = lane >> 4, hl = lane & 15;
     // lane hl reads chunk c of a row at a_off + 128 c (a plane) and b_off + 32 c (b plane).  Chunks past d_pad meet a zero query; their reads
     // stay inside the shared memory of the ring: at most 96 bytes past the end of a row, and the ring's barriers (>= 128 bytes) follow its last slot.
@@ -631,8 +634,186 @@ __device__ __forceinline__ void q5_tile(const Pf6Params& p, const Q6Query<NCH>& 
     }
 }
 
+// ------------------------------------------------------------------------------------------------ block-scaled 4-bit plane: the default stage 1
+// With one scale per row, a 4-bit step is set by the row's largest coordinate (~3.2 sigma at dim 768) and leaves a residual of ~0.125 ||x||:
+// that bound lets about a quarter of the rows through.  Here each 16-dimension chunk b of the lane mapping above has its own scale
+//   s_r = max_i |x_i| / 7 (f32),   k_b = ceil(255 max_{i in b} |x_i| / max_i |x_i|) in [1, 255] (0 for an all-zero chunk),   s_b = s_r k_b / 255,
+//   x_i = s_b c_i + r_i,  c_i = rint(x_i / s_b) in [-7, 7]
+// (k_b is rounded up, so s_b >= max_b / 7 up to a few f32 roundings and |x_i / s_b| < 7.5: the codes need no clamping, |r_i| <= s_b (1/2 + 2^-13)).
+// Record per row (stride q4b_stride(d_pad), a multiple of 8; 440 bytes at dim 768 against the 5-bit stage's 496):
+//   codes (d_pad / 2 bytes)      byte 8v + 4k + j: c + 8 of dim 16v + 8k + j (low nibble) and of dim 16v + 8k + 4 + j (high nibble), as the 6-bit
+//                                plane's a plane: `x & 0x0F0F0F0F` and `(x >> 4) & 0x0F0F0F0F` of the two words of a chunk are dp4a operands of
+//                                dims 16v + 4m + j (m = 0..3), the order of the query levels of Q6Query
+//   scales (d_pad / 16 bytes)    byte v: k_b of chunk v
+//   s_r, rho4 >= ||x - x^||_2    (f32 at a 4-byte boundary; rho4 computed in f64 and rounded up, x^_i = s_b c_i)
+// With the query's int8 levels q^_i = s_q (h_i + l_i / 254) and H_b = sum_{i in b} h_i c_i, L_b likewise (dp4a on c + 8, minus 8 sum_b h):
+//   approx = sum_b s_b s_q (H_b + L_b / 254) = s_r s_q / 64770 * sum_b k_b (254 H_b + L_b)
+//   exact - approx = sum_i (q_i - q^_i) x^_i + sum_i q_i r_i, bounded by the smaller of
+//     t1 = sum_b s_b E_b = s_r / 255 sum_b k_b E_b,  E_b = (1/2 + 2^-13) ||q_b||_1 + 0.014 s_q n_b    (|r_i| <= s_b (1/2 + 2^-13); |c_i| <= 7 and
+//          |q_i - q^_i| <= s_q (1/508 + 2.3e-5): 7 (1/508 + 2.3e-5) < 0.014; n_b = dims of chunk b below dim)
+//     t2 = ||q||_2 rho4 + e2 (max||x|| + rho4)                       (Cauchy-Schwarz as for the 6-bit plane; ||x^||_2 <= ||x|| + rho4)
+//   + ev = 2^-19 (||q|| + e2)(max||x|| + rho4): the kernel's f32 evaluation of approx.  254 H_b + L_b is an integer below 2^22 (exact); a lane
+//     sums k_b (254 H_b + L_b) over its <= 4 chunks by FMA, the half-warp adds with 4 further roundings, and three products follow: <= 16 roundings
+//     of at most 2^-23 each, relative to sum_i |q^_i x^_i| <= ||q^|| ||x^|| <= (||q|| + e2)(max||x|| + rho4).
+// A row passes iff  approx + min(t1, t2) + ev >= thr_q - slack_q, every bound term rounded towards "pass", with the 6-bit plane's slack_q
+// (which covers the exact f32 sum).  The bound holds for every row, so the first-stage list stays a superset of the rows whose exact score
+// reaches thr_q, and stages 2 and 3 run unchanged on it.  Zero and denormal-only rows (max < 1e-30) keep codes 0, k_b = 255, s_r = 2 max, rho4 = ||x||.
+__host__ __device__ constexpr uint32_t q4b_meta_off(uint32_t d_pad) { return (d_pad / 2 + d_pad / 16 + 3) & ~3u; }
+__host__ __device__ constexpr uint32_t q4b_stride(uint32_t d_pad) { return (q4b_meta_off(d_pad) + 8 + 7) & ~7u; }
+
+__global__ void __launch_bounds__(256) f32_to_q4b_rows_kernel(const float* __restrict__ rows, uint64_t stride_f, uint32_t dim, uint32_t d_pad, uint64_t n,
+                                                               uint8_t* __restrict__ out, uint32_t out_stride_b) {
+    const int t = threadIdx.x & 7;
+    const uint64_t groups = (uint64_t)gridDim.x * (blockDim.x >> 3), g0 = (uint64_t)blockIdx.x * (blockDim.x >> 3) + (threadIdx.x >> 3);
+    const uint64_t n_iter = (n + groups - 1) / groups;
+    const uint32_t meta_off = q4b_meta_off(d_pad);
+    for (uint64_t it = 0; it < n_iter; ++it) {
+        const uint64_t r = g0 + it * groups;
+        const bool valid = r < n;
+        const float* src = rows + (valid ? r : 0) * stride_f;
+        uint8_t* dst = out + (valid ? r : 0) * out_stride_b;
+        float mx = 0.f;
+        for (uint32_t i = t; i < dim; i += 8) mx = fmaxf(mx, fabsf(src[i]));
+#pragma unroll
+        for (int o = 1; o < 8; o <<= 1) mx = fmaxf(mx, __shfl_xor_sync(0xFFFFFFFFu, mx, o));
+        const bool tiny = !(mx >= 1.0e-30f);
+        const float sr = tiny ? __fmul_ru(mx, 2.0f) : __fdiv_rn(mx, 7.f);
+        const float kr = tiny ? 0.f : __fdiv_rn(255.f, mx);
+        double rr = 0.0;
+        for (uint32_t v = t; v < d_pad / 16; v += 8) {
+            float mb = 0.f;
+#pragma unroll
+            for (int k = 0; k < 16; ++k) mb = (v * 16 + k < dim) ? fmaxf(mb, fabsf(src[v * 16 + k])) : mb;
+            const int kb = tiny ? 255 : (mb > 0.f ? (int)fminf(fmaxf(ceilf(__fmul_rn(mb, kr)), 1.f), 255.f) : 0);
+            const float inv = (tiny || kb == 0) ? 0.f : __fdiv_rn(255.f, __fmul_rn(sr, (float)kb));
+            uint32_t w0 = 0, w1 = 0;
+#pragma unroll
+            for (int k = 0; k < 16; ++k) {
+                const float x = (v * 16 + k < dim) ? src[v * 16 + k] : 0.f;
+                const int c = (int)fminf(fmaxf(rintf(__fmul_rn(x, inv)), -7.f), 7.f);
+                // x - s_b c = (255 x - s_r (k_b c)) / 255: both products exact in f64, then one rounding for the difference and one for the quotient
+                const double e = ((double)x * 255.0 - (double)sr * (double)(kb * c)) / 255.0;
+                rr += e * e;
+                const uint32_t nib = (uint32_t)(c + 8) << (8 * (k & 3) + 4 * ((k >> 2) & 1));    // dim 16v + 4m + j: word m >> 1, byte j, nibble m & 1
+                if (k < 8) w0 |= nib; else w1 |= nib;
+            }
+            if (valid) {
+                *reinterpret_cast<uint2*>(dst + 8 * v) = make_uint2(w0, w1);
+                dst[d_pad / 2 + v] = (uint8_t)kb;
+            }
+        }
+#pragma unroll
+        for (int o = 1; o < 8; o <<= 1) rr += __shfl_xor_sync(0xFFFFFFFFu, rr, o);
+        if (valid && t == 0) {
+            for (uint32_t b = d_pad / 2 + d_pad / 16; b < meta_off; ++b) dst[b] = 0;
+            float* meta = reinterpret_cast<float*>(dst + meta_off);
+            meta[0] = sr;
+            meta[1] = __double2float_ru(__dmul_ru(sqrt(rr), 1.0 + 0x1p-40));       // as rho5 / rho6 of the 6-bit plane
+            for (uint32_t b = meta_off + 8; b < out_stride_b; ++b) dst[b] = 0;
+        }
+    }
+}
+
+// The query for the block-scaled stage: the 6-bit plane's (levels, t2, slack, threshold) and per chunk of this lane the code offset and E_b.
 template <int NCH>
-__global__ void __launch_bounds__(PF_THREADS, 1) dense_q5_filter_kernel(const Pf6Params p) {
+struct Q4bQuery {
+    Q6Query<NCH> q6;
+    int corr[NCH];                // 8 (254 sum h + sum l) over chunk c: the codes are stored as c + 8
+    float e1[NCH];                // E_b of chunk c (zero past d_pad)
+    float sq_k, k255, ev_a, ev_b; // s_q / 64770; 1/255 rounded up; ev = rho4 ev_a + ev_b
+};
+
+template <int NCH>
+__device__ __forceinline__ void stage1_query(const Pf6Params& p, int hl, Q4bQuery<NCH>& Q) {
+    q6_query<NCH>(p, hl, Q.q6);
+    const uint32_t n16 = p.d_pad / 16;
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+        const uint32_t v = (uint32_t)(c * 16 + hl);
+        float q1 = 0.f, nb = 0.f;
+#pragma unroll
+        for (int k = 0; k < 16; ++k) {
+            const bool in = v < n16 && v * 16 + k < p.dim;
+            q1 = __fadd_ru(q1, in ? fabsf(p.q[v * 16 + k]) : 0.f);
+            nb += in ? 1.f : 0.f;
+        }
+        int sh = 0, sl = 0;
+#pragma unroll
+        for (int m = 0; m < 4; ++m) { sh = __dp4a((int)Q.q6.hq[c][m], 0x01010101, sh); sl = __dp4a((int)Q.q6.lq[c][m], 0x01010101, sl); }
+        Q.corr[c] = 8 * (254 * sh + sl);
+        Q.e1[c] = __fadd_ru(__fmul_ru(q1, 0x1.001p-1f), __fmul_ru(Q.q6.sq, __fmul_ru(nb, 0.014f)));
+    }
+    Q.sq_k = __fdiv_rn(Q.q6.sq, 64770.f);
+    Q.k255 = __fdiv_ru(1.f, 255.f);
+    Q.ev_a = __fmul_ru(Q.q6.t2a, 0x1p-19f);
+    Q.ev_b = __fmul_ru(Q.ev_a, __uint_as_float(*p.max_norm_bits));
+}
+
+// As the 5-bit tile above: four rows per step, two per half-warp; each lane sums k_b (254 H_b + L_b) and k_b E_b over its chunks, and one
+// butterfly of these four floats serves the four rows.
+template <int NCH, bool SAMPLE>
+__device__ __forceinline__ void stage1_tile(const Pf6Params& p, const Q4bQuery<NCH>& Q, const uint8_t* slot, uint32_t nr, uint64_t r0, int lane, LkState& lk,
+                                            unsigned long long* lk_queue, unsigned int* lk_count) {
+    const int half = lane >> 4, hl = lane & 15;
+    // lane hl reads chunk c of a row at c_off + 128 c (codes) and k_off + 16 c (its scale); past d_pad the query is zero and the reads stay
+    // inside the ring's shared memory, as in the 5-bit tile
+    const uint32_t c_off = (uint32_t)hl * 8, k_off = p.d_pad / 2 + (uint32_t)hl, meta_off = q4b_meta_off(p.d_pad);
+    for (uint32_t r = 0; r < nr; r += 4) {
+        const uint32_t ra = r + (uint32_t)half, rb = ra + 2;
+        const bool va = ra < nr, vb = rb < nr;
+        const uint8_t* rowa = slot + (size_t)(va ? ra : r) * p.stride;
+        const uint8_t* rowb = slot + (size_t)(vb ? rb : r) * p.stride;
+        float aa = 0.f, ta = 0.f, ab = 0.f, tb = 0.f;
+#pragma unroll
+        for (int c = 0; c < NCH; ++c) {
+            const uint2 xa = *reinterpret_cast<const uint2*>(rowa + c_off + 128 * c);
+            const uint2 xb = *reinterpret_cast<const uint2*>(rowb + c_off + 128 * c);
+            // integer -> float by the exponent trick (exact for |x| < 2^22; I2F is quarter rate and sits on every row's chain)
+            const float ka = __fsub_rn(__int_as_float(0x4B000000 | rowa[k_off + 16 * c]), 8388608.f);
+            const float kb = __fsub_rn(__int_as_float(0x4B000000 | rowb[k_off + 16 * c]), 8388608.f);
+            const uint32_t wa[4] = {xa.x & 0x0F0F0F0Fu, (xa.x >> 4) & 0x0F0F0F0Fu, xa.y & 0x0F0F0F0Fu, (xa.y >> 4) & 0x0F0F0F0Fu};
+            const uint32_t wb[4] = {xb.x & 0x0F0F0F0Fu, (xb.x >> 4) & 0x0F0F0F0Fu, xb.y & 0x0F0F0F0Fu, (xb.y >> 4) & 0x0F0F0F0Fu};
+            int ha = 0, la = 0, hb = 0, lb = 0;
+#pragma unroll
+            for (int m = 0; m < 4; ++m) {
+                ha = __dp4a((int)wa[m], (int)Q.q6.hq[c][m], ha); la = __dp4a((int)wa[m], (int)Q.q6.lq[c][m], la);
+                hb = __dp4a((int)wb[m], (int)Q.q6.hq[c][m], hb); lb = __dp4a((int)wb[m], (int)Q.q6.lq[c][m], lb);
+            }
+            const float fa = __fsub_rn(__int_as_float(0x4B400000 + 254 * ha + la - Q.corr[c]), 12582912.f);    // |254 H_b + L_b| < 2^22
+            const float fb = __fsub_rn(__int_as_float(0x4B400000 + 254 * hb + lb - Q.corr[c]), 12582912.f);
+            aa = __fmaf_rn(ka, fa, aa); ta = __fmaf_ru(ka, Q.e1[c], ta);
+            ab = __fmaf_rn(kb, fb, ab); tb = __fmaf_ru(kb, Q.e1[c], tb);
+        }
+        // as in the 5-bit tile: lanes 0-3 of a half end up with the approx sum of row a, 4-7 of row b, 8-11 the t1 sum of row a, 12-15 of row b
+        float x0 = __fadd_ru((hl & 8) ? ta : aa, __shfl_xor_sync(0xFFFFFFFFu, (hl & 8) ? aa : ta, 8));
+        float x1 = __fadd_ru((hl & 8) ? tb : ab, __shfl_xor_sync(0xFFFFFFFFu, (hl & 8) ? ab : tb, 8));
+        float v = __fadd_ru((hl & 4) ? x1 : x0, __shfl_xor_sync(0xFFFFFFFFu, (hl & 4) ? x0 : x1, 4));
+        v = __fadd_ru(v, __shfl_xor_sync(0xFFFFFFFFu, v, 2));
+        v = __fadd_ru(v, __shfl_xor_sync(0xFFFFFFFFu, v, 1));
+        const float tsum = __shfl_xor_sync(0xFFFFFFFFu, v, 8);
+        const bool mine = (hl == 0 && va) || (hl == 4 && vb);
+        float app = 0.f, up = 0.f;
+        if (mine) {
+            const float* meta = reinterpret_cast<const float*>((hl ? rowb : rowa) + meta_off);
+            const float sr = meta[0], rho4 = meta[1];
+            app = __fmul_rn(sr, __fmul_rn(Q.sq_k, v));
+            const float t1 = __fmul_ru(sr, __fmul_ru(tsum, Q.k255));
+            up = __fadd_ru(__fadd_ru(app, fminf(t1, __fmaf_ru(rho4, Q.q6.t2a, Q.q6.t2b))), __fmaf_ru(rho4, Q.ev_a, Q.ev_b));   // >= exact score - slack_q
+        }
+        const float u = __shfl_sync(0xFFFFFFFFu, up, ((lane & 1) << 4) | ((lane & 2) << 1));
+        if (lane < 4 && r + (uint32_t)lane < nr) p.up5[r0 + r + (uint32_t)lane] = u;
+        if (SAMPLE) {
+            if (mine && !(app < lk.wthr)) lk_push(p.deleted, p.deleted2, 0u, app, (uint32_t)(r0 + (hl ? rb : ra)), lk_queue, lk_count);
+            __syncwarp();
+            const unsigned int n_queued = *reinterpret_cast<volatile unsigned int*>(lk_count);
+            if (n_queued) lk = lk_drain(lk, lk_queue, lk_count, lane, n_queued);
+        }
+    }
+}
+
+// Stage 1 on either plane (Query = Q6Query: the 5-bit code of the 6-bit plane's main records; Q4bQuery: the block-scaled 4-bit plane)
+template <int NCH, class Query>
+__device__ __forceinline__ void stage1_run(const Pf6Params& p) {
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* slots = smem;                                       // [n_slots][slot_bytes]
     uint64_t* full = reinterpret_cast<uint64_t*>(slots + (size_t)p.n_slots * p.slot_bytes);
@@ -656,8 +837,8 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q5_filter_kernel(const Pf
         return;
     }
     const int cw = warp - n_prod;
-    Q6Query<NCH> Q;
-    q6_query<NCH>(p, lane & 15, Q);
+    Query Q;
+    stage1_query<NCH>(p, lane & 15, Q);
     // this warp's `top` best sample rows by approximate score (lanes >= top hold the maximum so that they are never the minimum)
     LkState lk{(lane < (int)p.top) ? 0ull : ~0ull, 0ull, __int_as_float(0xff800000)};
     uint32_t s = (uint32_t)cw, ph = 0;                            // as in the producers: no 64-bit division per slot
@@ -669,8 +850,8 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q5_filter_kernel(const Pf
         qb_mbar_wait(&full[s], ph);
         const uint8_t* slot = slots + (size_t)s * p.slot_bytes;
         // a warp's tiles ascend: the sample tiles come first, and the loop after them does no top-k work
-        if (r0 < p.sample_rows) q5_tile<NCH, true>(p, Q, slot, nr, r0, lane, lk, lk_queue + cw * 4, &lk_count[cw]);
-        else q5_tile<NCH, false>(p, Q, slot, nr, r0, lane, lk, lk_queue + cw * 4, &lk_count[cw]);
+        if (r0 < p.sample_rows) stage1_tile<NCH, true>(p, Q, slot, nr, r0, lane, lk, lk_queue + cw * 4, &lk_count[cw]);
+        else stage1_tile<NCH, false>(p, Q, slot, nr, r0, lane, lk, lk_queue + cw * 4, &lk_count[cw]);
         __syncwarp();
         if (lane == 0) qb_mbar_arrive(&empty[s]);
         s += PF_CONSUMER_WARPS;
@@ -701,6 +882,13 @@ __global__ void __launch_bounds__(PF_THREADS, 1) dense_q5_filter_kernel(const Pf
         lk_last_cta_merge(p.cta_keys, p.top, p.samp_out, p.samp_cnt, p.samp_ticket, lane);
     }
 }
+
+template <int NCH>
+__global__ void __launch_bounds__(PF_THREADS, 1) dense_q5_filter_kernel(const Pf6Params p) { stage1_run<NCH, Q6Query<NCH>>(p); }
+
+// p.rows / p.stride: the block-scaled plane (the ring streams it); stages 2 and 3 take the 6-bit plane's
+template <int NCH>
+__global__ void __launch_bounds__(PF_THREADS, 1) dense_q4b_filter_kernel(const Pf6Params p) { stage1_run<NCH, Q4bQuery<NCH>>(p); }
 
 // Stage 2: rows whose bound reaches the sample threshold, not deleted, to the first-stage list (row ids).  A CTA compacts 16 rows per thread
 // per step with ONE atomic: 1-3 % of the rows pass, spread evenly, so an atomic per warp step would meet a pass almost every time, and tens of
@@ -864,14 +1052,14 @@ __global__ void __launch_bounds__(PF_RESCREEN_THREADS) dense_q6_rescreen_kernel(
     }
 }
 
-// the ring of any filter kernel above: slots of ~PF_SLOT_BYTES (an even number of rows), as many as fit, one CTA per SM; `extra_smem` bytes
-// follow the ring's barriers
+// the ring of any filter kernel above: slots of ~PF_SLOT_BYTES (a multiple of `row_step` rows: the rows a warp takes per step), as many as
+// fit, one CTA per SM; `extra_smem` bytes follow the ring's barriers
 template <typename P>
-qb_status launch_ring(void (*kernel)(P), P& p, int sm_count, cudaStream_t stream, size_t extra_smem = 0) {
+qb_status launch_ring(void (*kernel)(P), P& p, int sm_count, cudaStream_t stream, size_t extra_smem = 0, uint32_t row_step = 2) {
     const uint32_t kMaxSmem = 227 * 1024;
     const uint32_t target = qb_opt().prefilter_slot_bytes ? qb_opt().prefilter_slot_bytes : PF_SLOT_BYTES;
-    uint32_t rps = (target / p.stride) & ~1u;
-    if (rps < 2) rps = 2;
+    uint32_t rps = target / p.stride / row_step * row_step;
+    if (rps < row_step) rps = row_step;
     p.rows_per_slot = rps;
     p.slot_bytes = rps * p.stride;
     uint32_t n_slots = (kMaxSmem - 2048 - (uint32_t)extra_smem) / p.slot_bytes;
@@ -1012,6 +1200,30 @@ static qb_status q6_shadow_ensure(qb_storage* s, cudaStream_t stream) {
     return QB_OK;
 }
 
+// block-scaled 4-bit plane (stage 1 of the 6-bit plane's scan), built like the planes above: +14 % HBM at dim 768, on top of the 6-bit plane
+static qb_status q4b_shadow_ensure(qb_storage* s, cudaStream_t stream) {
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (s->q4b_ready) return QB_OK;
+    const uint32_t d_pad = (uint32_t)round_up_u64(s->dim, 32);
+    const uint32_t row_b = q4b_stride(d_pad);
+    const size_t bytes = (size_t)s->count * row_b + 16;                  // + 16: a tile's bulk copy is rounded up to 16 bytes (pf_produce)
+    if (!s->d_q4b) {
+        if (cudaMalloc(&s->d_q4b, std::max<size_t>(bytes, 256)) != cudaSuccess) { s->d_q4b = nullptr; return QB_ERR_CUDA; }
+        s->hbm_bytes += bytes;
+    }
+    s->q4b_row_b = row_b;
+    const uint64_t blocks = std::min<uint64_t>(ceil_div_u64(std::max<uint64_t>(s->count, 1), 32), (uint64_t)s->sm_count * 16);
+    f32_to_q4b_rows_kernel<<<(unsigned)blocks, 256, 0, stream>>>(reinterpret_cast<const float*>(s->d_rows), s->row_stride / 4, s->dim, d_pad, s->count, s->d_q4b, row_b);
+    QB_LAUNCHED();
+    QB_CUDA(cudaGetLastError());
+    QB_CUDA(cudaStreamSynchronize(stream));
+    s->q4b_ready = true;
+    return QB_OK;
+}
+
+// option prefilter_stage1: 5 = the 5-bit code of the 6-bit plane's main records as stage 1 (no block-scaled plane); anything else = the block-scaled plane
+static bool pf_stage1_q4b() { return qb_opt().prefilter_stage1 != 5; }
+
 // option prefilter_plane: 0 = the 6-bit plane, 1 = bf16, 2 = int8 (the integer planes need dim * 127 * 62 < 2^24 and <= 4 chunks per lane: dim <= 1024,
 // which every prefiltered storage meets).  Only the selected plane is built; when it cannot be allocated, the bf16 plane is tried.
 static int pf_plane() { const int o = qb_opt().prefilter_plane; return (o == 1 || o == 2) ? o : 0; }
@@ -1022,7 +1234,10 @@ bool qb_f32_prefilter_usable(qb_storage* s, uint64_t n_rows, uint32_t top, cudaS
     if (s->distance != QB_DIST_DOT && s->distance != QB_DIST_COSINE) return false;       // the bound is on a dot product
     if (qb_opt().disable_prefilter || n_rows != s->count || n_rows < (1ull << 19) || top > 16 || s->dim < 32 || round_up_u64(s->dim, 8) > 1024) return false;
     if (pf_plane() == 0) {
-        if (q6_shadow_ensure(s, stream) == QB_OK) return s->q6_usable;
+        if (q6_shadow_ensure(s, stream) == QB_OK) {
+            if (s->q6_usable && pf_stage1_q4b() && q4b_shadow_ensure(s, stream) != QB_OK) cudaGetLastError();   // no room: the 5-bit stage 1
+            return s->q6_usable;
+        }
         cudaGetLastError();                                                               // e.g. no room for the plane: try the bf16 one / stay exact
     } else if (pf_plane() == 2) {
         if (q8_shadow_ensure(s, stream) == QB_OK) return s->q8_usable;
@@ -1081,11 +1296,23 @@ qb_status qb_f32_prefilter_search(qb_storage* s, const QbScanArgs& a, uint32_t t
         const unsigned cp_grid = (unsigned)s->sm_count * 8, rs_grid = (unsigned)s->sm_count * 4;
         QB_CHECK((uint64_t)s->sm_count * QB_LOCALK_SLOTS <= PF_CAP, QB_ERR_INVALID, "prefilter: %d CTAs exceed the key buffer", s->sm_count);
         if (prof0) cudaEventRecord(prof0, stream);
-        switch ((p6.d_pad + 255) / 256) {
-            case 1: QB_TRY(launch_ring(dense_q5_filter_kernel<1>, p6, s->sm_count, stream, PF_SAMPLE_SMEM)); break;
-            case 2: QB_TRY(launch_ring(dense_q5_filter_kernel<2>, p6, s->sm_count, stream, PF_SAMPLE_SMEM)); break;
-            case 3: QB_TRY(launch_ring(dense_q5_filter_kernel<3>, p6, s->sm_count, stream, PF_SAMPLE_SMEM)); break;
-            default: QB_TRY(launch_ring(dense_q5_filter_kernel<4>, p6, s->sm_count, stream, PF_SAMPLE_SMEM)); break;
+        if (pf_stage1_q4b() && s->q4b_ready) {
+            // stage 1 on the block-scaled plane: the ring streams its records, every other field stays the 6-bit plane's
+            Pf6Params p4 = p6;
+            p4.rows = s->d_q4b; p4.stride = s->q4b_row_b;
+            switch ((p4.d_pad + 255) / 256) {
+                case 1: QB_TRY(launch_ring(dense_q4b_filter_kernel<1>, p4, s->sm_count, stream, PF_SAMPLE_SMEM, 4)); break;
+                case 2: QB_TRY(launch_ring(dense_q4b_filter_kernel<2>, p4, s->sm_count, stream, PF_SAMPLE_SMEM, 4)); break;
+                case 3: QB_TRY(launch_ring(dense_q4b_filter_kernel<3>, p4, s->sm_count, stream, PF_SAMPLE_SMEM, 4)); break;
+                default: QB_TRY(launch_ring(dense_q4b_filter_kernel<4>, p4, s->sm_count, stream, PF_SAMPLE_SMEM, 4)); break;
+            }
+        } else {
+            switch ((p6.d_pad + 255) / 256) {
+                case 1: QB_TRY(launch_ring(dense_q5_filter_kernel<1>, p6, s->sm_count, stream, PF_SAMPLE_SMEM, 4)); break;
+                case 2: QB_TRY(launch_ring(dense_q5_filter_kernel<2>, p6, s->sm_count, stream, PF_SAMPLE_SMEM, 4)); break;
+                case 3: QB_TRY(launch_ring(dense_q5_filter_kernel<3>, p6, s->sm_count, stream, PF_SAMPLE_SMEM, 4)); break;
+                default: QB_TRY(launch_ring(dense_q5_filter_kernel<4>, p6, s->sm_count, stream, PF_SAMPLE_SMEM, 4)); break;
+            }
         }
         if (prof1) cudaEventRecord(prof1, stream);
         // 2b. the 6-bit test of the listed rows

@@ -2,8 +2,8 @@
 """prefilter_probe.py [rows] [dim] — single-query searches over one synthetic cosine storage (generated on the device), device-timed, for several
 ring-slot sizes / producer-warp counts of the shadow-plane filter kernels and the three planes; prints one JSON line.  Results of every variant are compared with the exact scan.
 "candidates" counts, per query, the rows each integer plane's bound lets through (the kernels' bounds restated in torch on the same rows, f64 where they round up):
-on the 6-bit plane, for each candidate size of its threshold sample (n / 16, n / 8, n / 4 rows), the rows of the 5-bit first stage (q6_stage1) and those of
-them the 6-bit test keeps (q6_stage2), with the threshold restated as the exact top-k of the prefix (the kernel ranks the prefix by its approximate score
+on the 6-bit plane, for each candidate size of its threshold sample (n / 16, n / 8, n / 4 rows), the rows of the 5-bit first stage (q6_stage1), those of
+them the 6-bit test keeps (q6_stage2) and the rows of the block-scaled 4-bit first stage (q4b_stage1, the default), with the threshold restated as the exact top-k of the prefix (the kernel ranks the prefix by its approximate score
 first, so its threshold can only be lower, by the ranking error); on the int8 plane, with the f32 sample of 1/64 of the rows it keeps."""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -112,6 +112,7 @@ def candidate_counts(nq=16, top=10):
     c5 = {k: torch.zeros(nq, dtype=torch.int64, device=dev) for k in prefixes}
     c6 = {k: torch.zeros(nq, dtype=torch.int64, device=dev) for k in prefixes}
     c8 = torch.zeros(nq, dtype=torch.int64, device=dev)
+    c4b = {k: torch.zeros(nq, dtype=torch.int64, device=dev) for k in prefixes}
     # pass 2: the bounds of every row against each threshold
     for r0, n, x in chunks():
         mx = x.abs().amax(1, keepdim=True)
@@ -122,16 +123,30 @@ def candidate_counts(nq=16, top=10):
         c5c = 2 * torch.div(c + 31, 2, rounding_mode="floor") + 0.5 - 31      # the 5-bit code's reconstruction
         rho5 = (x.double() - sr * c5c).norm(dim=1, keepdim=True)
         up5 = sr * sq.T * (c5c @ h.T + (c5c @ l.T) / 254) + torch.minimum(sr * e1_5, rho5 * (qn + e2) + e2 * mxn)
+        # the block-scaled 4-bit stage (dense_q4b_filter_kernel): k_b per 16 dims, codes in [-7, 7], bound approx + min(t1, t2) + ev
+        nb = -(-dim // 16)
+        xp = torch.nn.functional.pad(x, (0, nb * 16 - dim)).view(n, nb, 16)
+        s4 = (mx / 7).double()
+        kb = torch.where(xp.abs().amax(2) > 0, torch.ceil(xp.abs().amax(2) * (255 / mx)).clamp(1, 255), torch.zeros((), device=dev)).double()
+        sb = s4 * kb / 255
+        cb = torch.where(sb[:, :, None] > 0, (xp.double() / sb[:, :, None]).round().clamp(-7, 7), torch.zeros((), device=dev, dtype=torch.float64))
+        xh = (sb[:, :, None] * cb).view(n, nb * 16)[:, :dim]
+        rho4 = (x.double() - xh).norm(dim=1, keepdim=True)
+        eb = torch.nn.functional.pad(qd.abs(), (0, nb * 16 - dim)).view(nq, nb, 16).sum(2) * (0.5 + 2.0 ** -13) \
+            + sq * 0.014 * torch.clamp(dim - 16 * torch.arange(nb, device=dev), 0, 16)
+        up4 = xh @ (sq * (h + l / 254)).T + torch.minimum(sb @ eb.T, rho4 * (qn + e2) + e2 * mxn) + 2.0 ** -19 * (qn + e2) * (mxn + rho4)
         for k in prefixes:
             p5 = up5 >= thr[k] - slack6
             c5[k] += p5.sum(0)
             c6[k] += (p5 & (up6 >= thr[k] - slack6)).sum(0)
+            c4b[k] += (up4 >= thr[k] - slack6).sum(0)
         s8 = (mx / 127).double()
         c = (x * (127 / mx)).round().clamp(-127, 127).double()
         up8 = s8 * (sq.T * (c @ h.T + (c @ l.T) / 254) + e8)
         c8 += (up8 >= thr8 - slack8).sum(0)
-        del x, c, rho, up6, up8, c5c, rho5, up5
-    return {"q6": {k: {"sample_rows": prefixes[k], "q6_stage1": c5[k].tolist(), "q6_stage2": c6[k].tolist()} for k in prefixes},
+        del x, c, rho, up6, up8, c5c, rho5, up5, xp, cb, xh, up4
+    return {"q6": {k: {"sample_rows": prefixes[k], "q6_stage1": c5[k].tolist(), "q6_stage2": c6[k].tolist(),
+                  "q4b_stage1": c4b[k].tolist()} for k in prefixes},
             "int8": c8.tolist(), "int8_sample_rows": sample8}
 
 
