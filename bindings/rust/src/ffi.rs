@@ -102,6 +102,7 @@ extern "C" {
     pub fn qb_comm_check(c: *mut qb_comm) -> qb_status;
     pub fn qb_hnsw_create_plain(s: *mut qb_storage, links_bin: *const u8, n_bytes: u64, m: u32, m0: u32, out: *mut *mut qb_hnsw) -> qb_status;
     pub fn qb_hnsw_create_compressed(s: *mut qb_storage, bytes: *const u8, n_bytes: u64, out: *mut *mut qb_hnsw) -> qb_status;
+    pub fn qb_hnsw_create_with_vectors(quantized: *mut qb_storage, bytes: *const u8, n_bytes: u64, out: *mut *mut qb_hnsw) -> qb_status;
     pub fn qb_hnsw_links(g: *const qb_hnsw, level: u32, ids: *const u32, n_ids: u32, cap: u32, out: *mut u32, counts: *mut u32) -> qb_status;
     pub fn qb_hnsw_destroy(g: *mut qb_hnsw);
     pub fn qb_hnsw_info(g: *const qb_hnsw, n_points: *mut u32, levels: *mut u32, hbm_bytes: *mut u64) -> qb_status;
@@ -112,6 +113,8 @@ extern "C" {
     pub fn qb_hnsw_search_batch_algo(g: *mut qb_hnsw, queries: *const f32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, deleted_bitmap: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters, algorithm: i32) -> qb_status;
     pub fn qb_hnsw_search_batch_device_algo(g: *mut qb_hnsw, dev_queries: *const f32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, dev_out: *mut qb_scored_point, dev_counts: *mut u32, algorithm: i32) -> qb_status;
     pub fn qb_hnsw_stats(g: *mut qb_hnsw, hops: *mut u64, scored_points: *mut u64, reset: i32) -> qb_status;
+    pub fn qb_hnsw_search_with_vectors_batch(g: *mut qb_hnsw, queries: *const f32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, deleted_bitmap: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters) -> qb_status;
+    pub fn qb_hnsw_search_with_vectors_batch_device(g: *mut qb_hnsw, dev_queries: *const f32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, dev_out: *mut qb_scored_point, dev_counts: *mut u32) -> qb_status;
     pub fn qb_hnsw_search_custom_batch(g: *mut qb_hnsw, kind: i32, vectors: *const f32, n_a: u32, n_b: u32, coef: *const f32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, custom_entry_points: *const u32, custom_counts: *const u32, n_custom: u32, deleted_bitmap: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters, algorithm: i32) -> qb_status;
     pub fn qb_hnsw_search_discover_batch(g: *mut qb_hnsw, vectors: *const f32, n_pairs: u32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, deleted_bitmap: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters, algorithm: i32) -> qb_status;
     pub fn qb_search_stats(s: *mut qb_storage, searches: *mut u64, reruns: *mut u64, reset: i32) -> qb_status;

@@ -30,7 +30,16 @@ impl<'a> B200Hnsw<'a> {
         Ok(Self { raw, _storage: std::marker::PhantomData })
     }
 
-    /// `links.bin` in GraphLinksFormat::Compressed; m and m0 come from its header.  CompressedWithVectors is refused.
+    /// `links.bin` in GraphLinksFormat::CompressedWithVectors (inline storage), bound to the segment's SQ8 storage.
+    pub fn from_compressed_links_with_vectors(quantized: &'a B200Storage, links_bin: &[u8]) -> OperationResult<Self> {
+        let mut raw = std::ptr::null_mut();
+        let st = unsafe { qb_hnsw_create_with_vectors(quantized.raw, links_bin.as_ptr(), links_bin.len() as u64, &mut raw) };
+        if st != QB_OK { return Err(OperationError::service_error(last_error())); }
+        Ok(Self { raw, _storage: std::marker::PhantomData })
+    }
+
+    /// `links.bin` in GraphLinksFormat::Compressed; m and m0 come from its header.  CompressedWithVectors is refused (see
+    /// `from_compressed_links_with_vectors`).
     pub fn from_compressed_links(storage: &'a B200Storage, links_bin: &[u8]) -> OperationResult<Self> {
         let mut raw = std::ptr::null_mut();
         let st = unsafe { qb_hnsw_create_compressed(storage.raw, links_bin.as_ptr(), links_bin.len() as u64, &mut raw) };
@@ -76,6 +85,22 @@ impl<'a> B200Hnsw<'a> {
             qb_hnsw_search_batch_algo(self.raw, queries.as_ptr(), n_queries as u32, top as u32, ef as u32, entry.0, entry.1 as u32,
                                       deleted.map_or(std::ptr::null(), |d| d.as_ptr()), std::ptr::null(), out.as_mut_ptr(), counts.as_mut_ptr(),
                                       std::ptr::null_mut(), algo)
+        };
+        assert!(st == QB_OK, "{}", last_error());
+        (0..n_queries).map(|q| out[q * top..q * top + counts[q] as usize].iter().map(|p| ScoredPointOffset { idx: p.idx, score: p.score }).collect()).collect()
+    }
+
+    /// `GraphLayers::search_with_vectors` (graph_layers.rs:564-596) on a `from_compressed_links_with_vectors` graph.  The dispatch of
+    /// hnsw/read_view/search.rs:88-178 stays with the caller: this search when the graph has inline vectors, the search is quantized
+    /// and the algorithm is HNSW, with ef = max(ef, oversampled top); otherwise `search_batch` on the same handle.
+    pub fn search_with_vectors(&self, queries: &[f32], n_queries: usize, top: usize, ef: usize, entry: (PointOffsetType, usize), deleted: Option<&[u64]>)
+                               -> Vec<Vec<ScoredPointOffset>> {
+        let mut out = vec![qb_scored_point::default(); n_queries * top];
+        let mut counts = vec![0u32; n_queries];
+        let st = unsafe {
+            qb_hnsw_search_with_vectors_batch(self.raw, queries.as_ptr(), n_queries as u32, top as u32, ef as u32, entry.0, entry.1 as u32,
+                                              deleted.map_or(std::ptr::null(), |d| d.as_ptr()), std::ptr::null(), out.as_mut_ptr(), counts.as_mut_ptr(),
+                                              std::ptr::null_mut())
         };
         assert!(st == QB_OK, "{}", last_error());
         (0..n_queries).map(|q| out[q * top..q * top + counts[q] as usize].iter().map(|p| ScoredPointOffset { idx: p.idx, score: p.score }).collect()).collect()

@@ -360,8 +360,24 @@ QB_API qb_status qb_hnsw_create_plain(qb_storage* s, const uint8_t* links_bin, u
  * builds (graph_links/header.rs:22-34, view.rs:137-163; hnsw/build.rs:548-562).  m / m0 come from the header.  The file is
  * copied to the device once and decoded there into the arrays qb_hnsw_create_plain uploads; the search is the same.
  * Every value taken from the file is checked before it is followed: a malformed file returns QB_ERR_INVALID and leaves the
- * device usable.  CompressedWithVectors (version word ...FF02, inline storage) and m0 > 64 return QB_ERR_UNSUPPORTED. */
+ * device usable.  CompressedWithVectors (version word ...FF02, inline storage) and m0 > 64 return QB_ERR_UNSUPPORTED: those
+ * graphs load through qb_hnsw_create_with_vectors below. */
 QB_API qb_status qb_hnsw_create_compressed(qb_storage* s, const uint8_t* bytes, uint64_t n_bytes, qb_hnsw** out);
+/* A graph from `links.bin` in GraphLinksFormat::CompressedWithVectors, which the reference writes for an index with
+ * HnswConfig.inline_storage and quantization (graph_links/header.rs:37-70, serializer.rs:91-171, view.rs:165-207,276-352): each
+ * level-0 record holds the point's original vector (base), and every link is followed by that neighbour's quantized vector.
+ *   s   the segment's SQ8 storage: link vectors are its rows ([f32 offset][actual_dim codes], layout alignment 1), and the link
+ *       layout size must be 4 + actual_dim (QB_ERR_INVALID otherwise).  BQ / PQ / dense storages: QB_ERR_UNSUPPORTED.
+ *   base vectors must be f32 (layout size dim * 4); f16 / u8 base layouts return QB_ERR_UNSUPPORTED, any other size QB_ERR_INVALID.
+ *       They live in the file, so the original f32 storage need not be resident.
+ * Every value is checked as qb_hnsw_create_compressed checks it, and every record's count (varint), packed links, padding,
+ * link vectors and (level 0) base vector must end inside the record: a malformed file returns QB_ERR_INVALID and leaves the
+ * device usable; a list of more than 128 links returns QB_ERR_UNSUPPORTED.  The links are decoded into the arrays the other
+ * loaders fill, so qb_hnsw_links, qb_hnsw_export_plain and the regular searches (HNSW, ACORN, custom) work on this handle; the
+ * records stay resident for qb_hnsw_search_with_vectors_batch.  HBM: the records (about dim * 4 + m0 * (actual_dim + 4) bytes per
+ * point: ~28 KB at 768-d and m0 = 32, so ~28 GB per million points), the plain arrays and 8 bytes per entry and per point of
+ * offsets; qb_hnsw_info reports the total.  Synchronous. */
+QB_API qb_status qb_hnsw_create_with_vectors(qb_storage* quantized, const uint8_t* bytes, uint64_t n_bytes, qb_hnsw** out);
 /* GraphLinks::links (view.rs:238-263) for n_ids points on one level, from the device-resident graph of either loader:
  * out[i * cap .. i * cap + min(counts[i], cap)) = point ids[i]'s links in the graph's stored order, counts[i] = their full
  * number.  QB_ERR_INVALID when a point is out of range or its top level is below `level` (view.rs:354-369).  Synchronous. */
@@ -411,7 +427,7 @@ QB_API qb_status qb_hnsw_search_batch_device(qb_hnsw* g, const float* dev_querie
  * The choice stays with the caller, as in hnsw/read_view/search.rs:59-86: ACORN when the request sets
  * SearchParams.acorn.enable, the graph has m0 != 0, there is a filter, and the filter's estimated cardinality over the
  * segment's available points is at most acorn.max_selectivity (default 0.4, types.rs:622); HNSW otherwise.  Searches over a
- * CompressedWithVectors graph never use ACORN (search.rs:91-92); this library does not load those graphs.  ACORN uses the
+ * CompressedWithVectors graph never use ACORN (search.rs:91-92); qb_hnsw_search_with_vectors_batch serves them.  ACORN uses the
  * same visited state as HNSW; its per-hop buffers take up to 16 * m0 * m0 bytes of shared memory per query in flight. */
 typedef enum { QB_HNSW_ALGO_HNSW = 0, QB_HNSW_ALGO_ACORN = 1 } qb_hnsw_algorithm;
 /* qb_hnsw_search_batch / qb_hnsw_search_batch_device with the level-0 algorithm chosen; the two calls above are these with
@@ -423,8 +439,33 @@ QB_API qb_status qb_hnsw_search_batch_algo(qb_hnsw* g, const float* queries, uin
 QB_API qb_status qb_hnsw_search_batch_device_algo(qb_hnsw* g, const float* dev_queries, uint32_t n_queries, uint32_t top, uint32_t ef,
                                                   uint32_t entry_point, uint32_t entry_level, qb_scored_point* dev_out, uint32_t* dev_counts,
                                                   qb_hnsw_algorithm algorithm);
-/* scorer calls (hops) and scored points since the last reset, summed over all searches on this graph (waits for them) */
+/* scorer calls (hops) and scored points since the last reset, summed over all searches on this graph (waits for them).  For
+ * qb_hnsw_search_with_vectors_batch: hops and link-scored points (the entry point's score included); base scores are not
+ * counted here (one per popped candidate; they show in the cpu counter). */
 QB_API qb_status qb_hnsw_stats(qb_hnsw* g, uint64_t* hops, uint64_t* scored_points, int32_t reset);
+/* GraphLayers::search_with_vectors (graph_layers.rs:336-452,564-596) on a qb_hnsw_create_with_vectors handle; the same arguments as
+ * qb_hnsw_search_batch, and QB_ERR_UNSUPPORTED on a handle without inline vectors.  The caller passes ef = max(ef, oversampled top)
+ * as search.rs:128 does; max(top, ef) is used.  Which search a request takes stays with the caller (hnsw/read_view/search.rs:88-178):
+ * this one when the graph has inline vectors, the search is quantized and the algorithm is HNSW; otherwise the regular search on
+ * the same handle.
+ *   - the query is Metric::preprocess-ed for the storage's distance, then SQ8-encoded for the link scores;
+ *   - the entry point is scored from the storage's SQ8 row; upper levels move greedily on the inline link vectors;
+ *   - level 0 runs the beam on link scores (filter, then truncate to m0, then score) and scores every candidate it pops exactly
+ *     from its base vector (the f32 chain of qb_score_points on a dense storage), including the candidate whose pop ends the
+ *     search below the beam's lower bound;
+ *   - the result is the best `top` exact scores, with no rescoring step.
+ * Ties: every level-0 comparison, in both lists, orders by (score desc, id asc).  Duplicate ids within one list are outside the
+ * contract (the first copy is scored).  Counters: cpu = link-scored points (the entry included) * dim + base-scored points * dim * 4;
+ * vector_io_read = the entry's quantized row per query for on-disk storages; inline bytes never count.
+ * Not covered: BQ / PQ link vectors, f16 / u8 base vectors, custom queries (the reference scores recommend / context / discover /
+ * feedback through the inline vectors as well; here they run as the regular device search on this handle, which differs from the
+ * reference on inline segments), ACORN (the reference has none with vectors), writing such files. */
+QB_API qb_status qb_hnsw_search_with_vectors_batch(qb_hnsw* g, const float* queries, uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point,
+                                                   uint32_t entry_level, const uint64_t* deleted_bitmap, const volatile int32_t* is_stopped,
+                                                   qb_scored_point* out, uint32_t* out_counts, qb_hw_counters* counters /* optional */);
+/* same with queries / outputs resident in HBM, enqueued on qb_storage_stream(s); no host synchronisation */
+QB_API qb_status qb_hnsw_search_with_vectors_batch_device(qb_hnsw* g, const float* dev_queries, uint32_t n_queries, uint32_t top, uint32_t ef,
+                                                          uint32_t entry_point, uint32_t entry_level, qb_scored_point* dev_out, uint32_t* dev_counts);
 
 /* Custom queries (recommend, context, feedback) through the device traversal: GraphLayers::search with a custom FilteredScorer
  * (hnsw/read_view/search.rs:181-208).  A point's score is qb_score_points on a qb_scorer_create_custom / qb_scorer_create_feedback

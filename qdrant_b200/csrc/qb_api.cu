@@ -1712,6 +1712,93 @@ extern "C" qb_status qb_hnsw_search_batch_device(qb_hnsw* g, const float* dev_qu
     return qb_hnsw_search_batch_device_algo(g, dev_queries, n_queries, top, ef, entry_point, entry_level, dev_out, dev_counts, QB_HNSW_ALGO_HNSW);
 }
 
+// GraphLayers::search_with_vectors on a graph with inline vectors (qb_hnsw_inline.cu).  Counters as the reference meters its three scorers:
+// the entry point's score_point through the quantized storage (cpu and, on disk, vector_io_read, quantized_query_scorer.rs:95-101),
+// each link score through EncodedVectorsU8::score_bytes (cpu only), each base score through MetricQueryScorer::score_bytes (cpu,
+// dim * 4 per point, metric_query_scorer.rs:43-64,101-104); inline bytes never count vector_io_read.
+static qb_status hnsw_with_vectors_counters(qb_hnsw* g, uint32_t n_queries, cudaStream_t stream, qb_hw_counters* counters) {
+    const uint64_t ev0 = g->evals, bev0 = g->base_evals;
+    QB_TRY(qb_hnsw_read_stats(g, stream));
+    if (counters) {
+        qb_storage* s = g->st;
+        counters->cpu += (g->evals - ev0) * cpu_units_per_point(s) + (g->base_evals - bev0) * (uint64_t)s->dim * 4;
+        counters->vector_io_read += (uint64_t)n_queries * io_units_per_point(s);
+    }
+    return QB_OK;
+}
+
+extern "C" qb_status qb_hnsw_search_with_vectors_batch(qb_hnsw* g, const float* queries, uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point,
+                                                       uint32_t entry_level, const uint64_t* deleted_bitmap, const volatile int32_t* is_stopped,
+                                                       qb_scored_point* out, uint32_t* out_counts, qb_hw_counters* counters) {
+    QB_CHECK(g && out && out_counts, QB_ERR_INVALID, "hnsw_search_with_vectors_batch: null argument");
+    QB_CHECK(n_queries == 0 || queries, QB_ERR_INVALID, "hnsw_search_with_vectors_batch: null queries");
+    QB_CHECK(top >= 1 && top <= 4096, QB_ERR_INVALID, "hnsw_search_with_vectors_batch: top %u outside [1,4096]", top);
+    QB_CHECK(g->d_blob, QB_ERR_UNSUPPORTED, "hnsw_search_with_vectors_batch: the graph has no inline vectors (load it with qb_hnsw_create_with_vectors)");
+    if (n_queries == 0) return QB_OK;
+    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    qb_storage* s = g->st;
+    QB_TRY(use_device(s->device));
+    std::lock_guard<std::mutex> glk(g->mu);
+    QbSearchCtx* c = nullptr;
+    QB_TRY(qb_ctx_acquire(s, &c));
+    struct Rel { qb_storage* s; QbSearchCtx* c; ~Rel() { qb_ctx_release(s, c); } } rel{s, c};
+    cudaStream_t stream = c->stream;
+    const size_t raw_bytes = (size_t)n_queries * s->dim * 4, res_bytes = (size_t)n_queries * top * sizeof(qb_scored_point), cnt_bytes = (size_t)n_queries * 4;
+    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, raw_bytes + res_bytes + cnt_bytes + 16));
+    uint8_t* hs = reinterpret_cast<uint8_t*>(c->h_stage);
+    memcpy(hs, queries, raw_bytes);
+    const size_t pre_off = round_up_u64(raw_bytes, 16);
+    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, pre_off + (size_t)n_queries * pre_stride_f(s) * 4));
+    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)n_queries + 256) * qb_encoded_query_bytes(s)));
+    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)n_queries));
+    QB_TRY(ensure_dev_elems(&c->d_out, &c->out_elems, (size_t)n_queries * top));
+    QB_TRY(ensure_dev_elems(&c->d_out_counts, &c->out_counts_elems, (size_t)n_queries + 4));
+    QB_CUDA(cudaMemcpyAsync(c->d_queries_raw, hs, raw_bytes, cudaMemcpyHostToDevice, stream));
+    float* d_pre = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c->d_queries_raw) + pre_off);
+    QB_TRY(prepare_queries(s, reinterpret_cast<const float*>(c->d_queries_raw), n_queries, d_pre, c->d_queries_enc, c->d_q_off, stream));
+    const uint32_t* d_del2 = nullptr;
+    if (deleted_bitmap) {
+        const uint64_t words64 = ceil_div_u64(s->count, 64);
+        QB_TRY(ensure_dev_elems(&c->d_deleted2, &c->deleted2_words, (size_t)words64 * 2));
+        QB_CUDA(cudaMemcpyAsync(c->d_deleted2, deleted_bitmap, words64 * 8, cudaMemcpyHostToDevice, stream));
+        d_del2 = c->d_deleted2;
+    }
+    QB_TRY(qb_hnsw_inline_launch(g, d_pre, pre_stride_f(s), c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, d_del2, c->d_out,
+                                 c->d_out_counts, stream));
+    QB_CUDA(cudaMemcpyAsync(hs + raw_bytes, c->d_out, res_bytes, cudaMemcpyDeviceToHost, stream));
+    QB_CUDA(cudaMemcpyAsync(hs + raw_bytes + res_bytes, c->d_out_counts, cnt_bytes, cudaMemcpyDeviceToHost, stream));
+    QB_CUDA(cudaStreamSynchronize(stream));
+    memcpy(out, hs + raw_bytes, res_bytes);
+    memcpy(out_counts, hs + raw_bytes + res_bytes, cnt_bytes);
+    QB_TRY(hnsw_with_vectors_counters(g, n_queries, stream, counters));
+    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    return QB_OK;
+}
+
+extern "C" qb_status qb_hnsw_search_with_vectors_batch_device(qb_hnsw* g, const float* dev_queries, uint32_t n_queries, uint32_t top, uint32_t ef,
+                                                              uint32_t entry_point, uint32_t entry_level, qb_scored_point* dev_out, uint32_t* dev_counts) {
+    QB_CHECK(g && dev_queries && dev_out && dev_counts, QB_ERR_INVALID, "hnsw_search_with_vectors_batch_device: null argument");
+    QB_CHECK(top >= 1 && top <= 4096, QB_ERR_INVALID, "hnsw_search_with_vectors_batch_device: top %u outside [1,4096]", top);
+    QB_CHECK(g->d_blob, QB_ERR_UNSUPPORTED, "hnsw_search_with_vectors_batch_device: the graph has no inline vectors (load it with qb_hnsw_create_with_vectors)");
+    if (n_queries == 0) return QB_OK;
+    qb_storage* s = g->st;
+    QB_TRY(use_device(s->device));
+    std::lock_guard<std::mutex> glk(g->mu);
+    QbSearchCtx* c = nullptr;
+    QB_TRY(qb_ctx_device(s, &c));
+    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, (size_t)n_queries * pre_stride_f(s) * 4 + 256));
+    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)n_queries + 256) * qb_encoded_query_bytes(s)));
+    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)n_queries));
+    float* d_pre = reinterpret_cast<float*>(c->d_queries_raw);
+    QB_TRY(prepare_queries(s, dev_queries, n_queries, d_pre, c->d_queries_enc, c->d_q_off, c->stream));
+    cudaEvent_t e0, e1;
+    profile_begin(s, c, c->stream, &e0, &e1);
+    QB_TRY(qb_hnsw_inline_launch(g, d_pre, pre_stride_f(s), c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, nullptr, dev_out,
+                                 dev_counts, c->stream));
+    profile_end(s, c->stream, e0, e1);
+    return QB_OK;
+}
+
 // custom queries through the device traversal; discover_pairs > 0: the two-stage discover of that many pairs (kind = DISCOVER)
 static qb_status hnsw_custom_run(qb_hnsw* g, qb_query_kind kind, const float* vectors, uint32_t n_a, uint32_t n_b, const float* coef, uint32_t n_queries,
                                  uint32_t top, uint32_t ef, uint32_t entry_point, uint32_t entry_level, const uint32_t* cep, const uint32_t* cep_counts,

@@ -210,7 +210,26 @@ __global__ void hnsw_c_counts_kernel(const HcLinks p, const uint32_t* __restrict
 }
 
 // one warp per entry: lane j decodes value j (j + 32, ...) at its own bit position; the sorted part is a warp inclusive scan of
-// the deltas (wrapping u32 adds, PackedLinksIterator::next_sorted) with a carry across passes of 32
+// the deltas (wrapping u32 adds, PackedLinksIterator::next_sorted) with a carry across passes of 32.  bit0: the first sorted value.
+__device__ __forceinline__ void hc_decode_warp(const uint8_t* links, uint64_t bit0, uint32_t bps, uint64_t ns, uint64_t nu, uint32_t bits_unsorted,
+                                               uint32_t* out, uint32_t lane) {
+    uint32_t carry = 0;
+    for (uint64_t k0 = 0; k0 < ns; k0 += 32) {
+        const uint64_t k = k0 + lane;
+        uint32_t v = k < ns ? hc_bits(links, bit0 + k * bps, bps) : 0u;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t o = __shfl_up_sync(0xFFFFFFFFu, v, d);
+            if (lane >= (uint32_t)d) v += o;
+        }
+        v += carry;
+        if (k < ns) out[k] = v;
+        carry = __shfl_sync(0xFFFFFFFFu, v, 31);
+    }
+    const uint64_t bit1 = bit0 + ns * bps;
+    for (uint64_t k = lane; k < nu; k += 32) out[ns + k] = hc_bits(links, bit1 + k * bits_unsorted, bits_unsorted);
+}
+
 __global__ void hnsw_c_links_kernel(const HcLinks p, const uint64_t* __restrict__ offsets, uint32_t* __restrict__ neighbors) {
     const uint32_t lane = threadIdx.x & 31u;
     const uint64_t n_warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
@@ -218,23 +237,7 @@ __global__ void hnsw_c_links_kernel(const HcLinks p, const uint64_t* __restrict_
         const uint64_t s = p.byte_off[e], t = p.byte_off[e + 1];
         uint32_t bps; uint64_t ns, nu;
         hc_shape(p, e, s, t, bps, ns, nu);
-        uint32_t* out = neighbors + offsets[e];
-        const uint64_t bit0 = 8 * s + 5;
-        uint32_t carry = 0;
-        for (uint64_t k0 = 0; k0 < ns; k0 += 32) {
-            const uint64_t k = k0 + lane;
-            uint32_t v = k < ns ? hc_bits(p.links, bit0 + k * bps, bps) : 0u;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const uint32_t o = __shfl_up_sync(0xFFFFFFFFu, v, d);
-                if (lane >= (uint32_t)d) v += o;
-            }
-            v += carry;
-            if (k < ns) out[k] = v;
-            carry = __shfl_sync(0xFFFFFFFFu, v, 31);
-        }
-        const uint64_t bit1 = bit0 + ns * bps;
-        for (uint64_t k = lane; k < nu; k += 32) out[ns + k] = hc_bits(p.links, bit1 + k * p.bits_unsorted, p.bits_unsorted);
+        hc_decode_warp(p.links, 8 * s + 5, bps, ns, nu, p.bits_unsorted, neighbors + offsets[e], lane);
     }
 }
 
@@ -398,6 +401,215 @@ extern "C" qb_status qb_hnsw_create_compressed(qb_storage* s, const uint8_t* byt
     return QB_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ compressed links.bin with vectors
+// GraphLinksFormat::CompressedWithVectors (header.rs:37-70, serializer.rs:32-49,91-171, view.rs:165-207,276-352), written for indexes
+// with inline storage:
+//   HeaderCompressedWithVectors, 80 B: bytes 0-58 as HeaderCompressed (version 0xFFFF_FFFF_FFFF_FF02), then base_vector_layout
+//   {u64 size, u8 align} at 59, link_vector_layout at 68, 3 zero bytes; level offsets, reindex, zero padding up to a FILE offset that
+//   is a multiple of max(base align, link align), total_neighbors_bytes of records, the compressed byte offsets.
+//   A record: [base vector, level 0 only][varint link count][packed links][pad to link align][count x link vector][level 0: pad to
+//   base align]; the alignments are relative to the start of the records.  The count is explicit (packed_links_size uses it).
+// The links are decoded once into the plain arrays the regular traversal reads (so qb_hnsw_links / _export_plain / the HNSW, ACORN
+// and custom searches work on this handle unchanged); the records stay resident for qb_hnsw_search_with_vectors_batch, with each
+// entry's link-vector offset and each point's base-vector offset.
+namespace {
+
+enum : uint32_t { HV_RECORD = 8u, HV_TOO_WIDE = 16u };
+
+struct HvShape {
+    const uint8_t* links;         // the records
+    const uint64_t* byte_off;     // decoded offsets [n_entries + 1]
+    uint64_t n_entries, limit, base_size, link_size;
+    uint32_t n_points, m, m0, bits_unsorted, link_align;
+};
+
+// per entry: link count, where its packed links and link vectors start; every part checked to lie inside the record
+__global__ void hnsw_v_shape_kernel(const HvShape p, const uint32_t* __restrict__ reindex, uint64_t* __restrict__ counts, uint64_t* __restrict__ lstart,
+                                    uint64_t* __restrict__ lvoff, uint32_t* __restrict__ flag) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t e = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; e <= p.n_entries; e += stride) {
+        uint64_t c = 0, ls = 0, lv = 0;
+        if (e < p.n_entries) {
+            const uint64_t s = p.byte_off[e], t = p.byte_off[e + 1];
+            if (t < s) atomicOr(flag, HC_OFFSETS_DECREASE);
+            else if (t <= p.limit) {
+                uint64_t pos = s + (e < p.n_points ? p.base_size : 0);
+                bool ok = pos <= t, done = false;
+                uint64_t cnt = 0;
+                for (uint32_t i = 0; ok && !done && i < 10; ++i) {   // u64::decode_var
+                    if (pos >= t) { ok = false; break; }
+                    const uint32_t b = p.links[pos++];
+                    cnt |= (uint64_t)(b & 127u) << (7 * i);
+                    done = (b & 128u) == 0;
+                }
+                ok = ok && done;
+                const bool wide = ok && cnt > HNSW_MAX_LIST;
+                if (wide) ok = false;
+                else if (ok && cnt) {
+                    if (pos >= t) ok = false;
+                    else {   // packed_links_size (bitpacking_links.rs:112-136)
+                        const uint64_t bps = (p.links[pos] & 31u) + 8u, ns = hc_min(cnt, e < p.n_points ? p.m0 : p.m);
+                        ls = pos;
+                        pos += (5 + ns * bps + (cnt - ns) * p.bits_unsorted + 7) / 8;
+                    }
+                }
+                if (ok) {
+                    pos = (pos + p.link_align - 1) / p.link_align * p.link_align;
+                    ok = pos <= t && cnt * p.link_size <= t - pos;
+                }
+                if (ok) { c = cnt; lv = pos; }
+                else atomicOr(flag, wide ? HV_TOO_WIDE : HV_RECORD);
+            }
+        }
+        counts[e] = c;
+        if (e < p.n_entries) { lstart[e] = ls; lvoff[e] = lv; }
+    }
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n_points; i += stride)
+        if (reindex[i] >= p.n_points) atomicOr(flag, HC_REINDEX);
+}
+
+__global__ void hnsw_v_links_kernel(const HvShape p, const uint64_t* __restrict__ lstart, const uint64_t* __restrict__ offsets, uint32_t* __restrict__ neighbors) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint64_t n_warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+    for (uint64_t e = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; e < p.n_entries; e += n_warps) {
+        const uint64_t cnt = offsets[e + 1] - offsets[e];
+        if (!cnt) continue;
+        const uint64_t ls = lstart[e];
+        const uint64_t ns = hc_min(cnt, e < p.n_points ? p.m0 : p.m);
+        hc_decode_warp(p.links, 8 * ls + 5, (p.links[ls] & 31u) + 8u, ns, cnt - ns, p.bits_unsorted, neighbors + offsets[e], lane);
+    }
+}
+
+}  // namespace
+
+extern "C" qb_status qb_hnsw_create_with_vectors(qb_storage* s, const uint8_t* bytes, uint64_t n_bytes, qb_hnsw** out) {
+    QB_CHECK(s && bytes && out, QB_ERR_INVALID, "hnsw_create_with_vectors: null argument");
+    *out = nullptr;
+    QB_CHECK(n_bytes >= 80, QB_ERR_INVALID, "hnsw_create_with_vectors: %llu bytes is smaller than HeaderCompressedWithVectors", (unsigned long long)n_bytes);
+    auto u64_at = [&](uint64_t o) { uint64_t v; memcpy(&v, bytes + o, 8); return v; };
+    const uint64_t n = u64_at(0), version = u64_at(8), levels = u64_at(16), nb_bytes = u64_at(24), length = u64_at(32), m = u64_at(43), m0 = u64_at(51);
+    const uint32_t base_bits = bytes[40], delta_bits = bytes[41], log2 = bytes[42];
+    const uint64_t base_size = u64_at(59), link_size = u64_at(68);
+    const uint32_t base_align = bytes[67], link_align = bytes[76];
+    QB_CHECK(version == HNSW_VERSION_COMPRESSED_WITH_VECTORS, QB_ERR_INVALID,
+             "hnsw_create_with_vectors: version word %016llx is not HEADER_VERSION_COMPRESSED_WITH_VECTORS (a Compressed or plain links.bin?)",
+             (unsigned long long)version);
+    QB_CHECK(s->kind == QB_KIND_SQ8, QB_ERR_UNSUPPORTED,
+             "hnsw_create_with_vectors: the link vectors are read as rows of the bound storage, which must be scalar-quantized (SQ8)");
+    // Layout::from_size_align (header.rs:63-69): a power-of-two alignment
+    QB_CHECK(base_align && !(base_align & (base_align - 1)) && link_align && !(link_align & (link_align - 1)), QB_ERR_INVALID,
+             "hnsw_create_with_vectors: vector alignments %u / %u are not powers of two", base_align, link_align);
+    QB_CHECK(base_size != 2ull * s->dim && base_size != s->dim, QB_ERR_UNSUPPORTED,
+             "hnsw_create_with_vectors: base vectors of %llu bytes at dim %u are f16 or u8; only f32 base vectors are supported",
+             (unsigned long long)base_size, s->dim);
+    QB_CHECK(base_size == 4ull * s->dim, QB_ERR_INVALID, "hnsw_create_with_vectors: base vectors of %llu bytes, dim %u", (unsigned long long)base_size, s->dim);
+    QB_CHECK(link_size == 4ull + s->actual_dim, QB_ERR_INVALID, "hnsw_create_with_vectors: link vectors of %llu bytes, the storage's rows have %u",
+             (unsigned long long)link_size, 4u + s->actual_dim);
+    QB_CHECK(n == s->count, QB_ERR_INVALID, "hnsw_create_with_vectors: graph has %llu points, storage %llu", (unsigned long long)n, (unsigned long long)s->count);
+    QB_CHECK(n <= 0xFFFFFFFFull, QB_ERR_INVALID, "hnsw_create_with_vectors: %llu points", (unsigned long long)n);
+    QB_CHECK(m >= 1 && m0 >= 1, QB_ERR_INVALID, "hnsw_create_with_vectors: m %llu / m0 %llu", (unsigned long long)m, (unsigned long long)m0);
+    QB_CHECK(m <= HNSW_MAX_LINKS && m0 <= HNSW_MAX_LINKS, QB_ERR_UNSUPPORTED, "hnsw_create_with_vectors: m %llu / m0 %llu outside [1,%u]",
+             (unsigned long long)m, (unsigned long long)m0, HNSW_MAX_LINKS);
+    QB_CHECK(levels <= 64 && (levels >= 1 || n == 0), QB_ERR_INVALID, "hnsw_create_with_vectors: %llu levels", (unsigned long long)levels);
+    QB_CHECK(base_bits >= 1 && base_bits <= 64 && delta_bits >= 1 && delta_bits <= 56 && log2 <= 7, QB_ERR_INVALID,
+             "hnsw_create_with_vectors: offsets parameters base_bits %u delta_bits %u chunk_len_log2 %u", base_bits, delta_bits, log2);
+    const uint64_t align = std::max(base_align, link_align);
+    const uint64_t body = round_up_u64(80 + 8 * levels + 4 * n, align);
+    QB_CHECK(body <= n_bytes && nb_bytes <= n_bytes - body, QB_ERR_INVALID, "hnsw_create_with_vectors: %llu bytes, header describes %llu before the offsets",
+             (unsigned long long)n_bytes, (unsigned long long)(body + nb_bytes));
+    const uint64_t rest = n_bytes - body - nb_bytes;
+    const uint64_t chunk_bytes = ceil_div_u64(base_bits + (uint64_t)delta_bits * ((1ull << log2) - 1), 8);
+    const uint64_t chunks = length / (1ull << log2) + ((length & ((1ull << log2) - 1)) ? 1 : 0);
+    QB_CHECK(length >= 1 && chunks <= rest / chunk_bytes && chunks * chunk_bytes + 7 <= rest, QB_ERR_INVALID,
+             "hnsw_create_with_vectors: %llu offsets do not fit the %llu bytes after the records", (unsigned long long)length, (unsigned long long)rest);
+    const uint64_t used = body + nb_bytes + chunks * chunk_bytes + 7;
+    std::vector<uint64_t> lo(levels + 1);
+    memcpy(lo.data(), bytes + 80, 8 * levels);
+    lo[levels] = length - 1;
+    for (uint64_t l = 0; l < levels; ++l)
+        QB_CHECK(lo[l] <= lo[l + 1] && (l != 0 || (lo[0] == 0 && lo[1] == n)), QB_ERR_INVALID, "hnsw_create_with_vectors: level offset %llu (%llu) out of range",
+                 (unsigned long long)l, (unsigned long long)lo[l]);
+    const uint32_t bits_unsorted = std::max<uint32_t>(8, n > 1 ? 64 - __builtin_clzll(n - 1) : 0);
+
+    cudaError_t ce = cudaSetDevice(s->device);
+    if (ce != cudaSuccess) { qb_set_error("hnsw_create_with_vectors: %s", cudaGetErrorString(ce)); return QB_ERR_CUDA; }
+    qb_hnsw* g = new qb_hnsw();
+    g->st = s; g->n_points = (uint32_t)n; g->m = (uint32_t)m; g->m0 = (uint32_t)m0; g->levels = (uint32_t)levels;
+    g->level_offsets_ext = lo; g->n_offsets = length; g->link_size = (uint32_t)link_size;
+    auto fail = [&](qb_status st, const char* what, cudaError_t e) {
+        qb_set_error("hnsw_create_with_vectors: %s: %s", what, cudaGetErrorString(e));
+        qb_hnsw_destroy(g);
+        return st;
+    };
+    HcScratch tmp;
+    uint8_t* d_file = nullptr; uint64_t *d_byte_off = nullptr, *d_counts = nullptr, *d_lstart = nullptr; uint32_t* d_flag = nullptr;
+    bool ok = cudaMalloc(&g->d_links0, std::max<size_t>((size_t)n * m0 * 4, 256)) == cudaSuccess &&
+              cudaMalloc(&g->d_level_offsets, std::max<size_t>(8 * levels, 256)) == cudaSuccess &&
+              cudaMalloc(&g->d_reindex, std::max<size_t>(4 * n, 256)) == cudaSuccess &&
+              cudaMalloc(&g->d_offsets, 8 * (length + n) + 256) == cudaSuccess && cudaMalloc(&g->d_work, 256) == cudaSuccess &&
+              cudaMalloc(&g->d_stats, 256) == cudaSuccess && cudaMalloc(&g->d_blob, nb_bytes + HC_PAD) == cudaSuccess &&
+              cudaMalloc(&g->d_lvoff, 8 * (length + n) + 256) == cudaSuccess && cudaMalloc(&g->d_boff, std::max<size_t>(8 * n, 256)) == cudaSuccess &&
+              tmp.alloc((void**)&d_file, used + HC_PAD) == cudaSuccess && tmp.alloc((void**)&d_byte_off, 8 * length) == cudaSuccess &&
+              tmp.alloc((void**)&d_counts, 8 * length) == cudaSuccess && tmp.alloc((void**)&d_lstart, 8 * length) == cudaSuccess &&
+              tmp.alloc((void**)&d_flag, 4) == cudaSuccess;
+    if (!ok) return fail(QB_ERR_OOM, "cudaMalloc failed", cudaGetLastError());
+    ce = cudaMemcpy(d_file, bytes, used, cudaMemcpyHostToDevice);
+    if (ce == cudaSuccess) ce = cudaMemset(d_file + used, 0, HC_PAD);
+    if (ce == cudaSuccess) ce = cudaMemcpy(g->d_level_offsets, d_file + 80, 8 * levels, cudaMemcpyDeviceToDevice);
+    if (ce == cudaSuccess) ce = cudaMemcpy(g->d_reindex, d_file + 80 + 8 * levels, 4 * n, cudaMemcpyDeviceToDevice);
+    if (ce == cudaSuccess) ce = cudaMemcpy(g->d_blob, d_file + body, nb_bytes, cudaMemcpyDeviceToDevice);
+    if (ce == cudaSuccess) ce = cudaMemset(g->d_blob + nb_bytes, 0, HC_PAD);
+    if (ce == cudaSuccess) ce = cudaMemset(g->d_lvoff, 0, 8 * (length + n) + 256);
+    if (ce == cudaSuccess) ce = cudaMemset(g->d_stats, 0, 256);
+    if (ce == cudaSuccess) ce = cudaMemset(d_flag, 0, 4);
+    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "upload", ce);
+
+    HcOffsets po{d_file + body + nb_bytes, length, chunk_bytes, nb_bytes, base_bits, delta_bits, log2};
+    hnsw_c_offsets_kernel<<<hc_grid(length, 256, 132 * 16), 256>>>(po, d_byte_off, d_flag);
+    QB_LAUNCHED();
+    HvShape pv{d_file + body, d_byte_off, length - 1, nb_bytes, base_size, link_size, (uint32_t)n, (uint32_t)m, (uint32_t)m0, bits_unsorted, link_align};
+    hnsw_v_shape_kernel<<<hc_grid(std::max<uint64_t>(length, n), 256, 132 * 16), 256>>>(pv, g->d_reindex, d_counts, d_lstart, g->d_lvoff, d_flag);
+    QB_LAUNCHED();
+    size_t scan_bytes = 0;
+    ce = cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_counts, g->d_offsets, (int64_t)length);
+    void* d_scan = nullptr;
+    if (ce == cudaSuccess) ce = tmp.alloc(&d_scan, scan_bytes);
+    if (ce == cudaSuccess) ce = cub::DeviceScan::ExclusiveSum(d_scan, scan_bytes, d_counts, g->d_offsets, (int64_t)length);
+    QB_LAUNCHED();
+    uint32_t flag = 0;
+    uint64_t total = 0;
+    if (ce == cudaSuccess) ce = cudaMemcpy(&flag, d_flag, 4, cudaMemcpyDeviceToHost);
+    if (ce == cudaSuccess) ce = cudaMemcpy(&total, g->d_offsets + (length - 1), 8, cudaMemcpyDeviceToHost);
+    if (ce == cudaSuccess && n) ce = cudaMemcpy(g->d_boff, d_byte_off, 8 * n, cudaMemcpyDeviceToDevice);
+    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "decode", ce);
+    if (flag) {
+        const bool wide = flag == HV_TOO_WIDE;
+        qb_set_error("hnsw_create_with_vectors: %s", (flag & HC_OFFSET_PAST_END) ? "a record offset lies past total_neighbors_bytes"
+                                                    : (flag & HC_OFFSETS_DECREASE) ? "record offsets decrease"
+                                                    : (flag & HC_REINDEX)          ? "a reindex entry is >= point_count"
+                                                    : (flag & HV_RECORD)           ? "a record's count, links or link vectors run past its end"
+                                                                                   : "a list has more than 128 links");
+        qb_hnsw_destroy(g);
+        return wide ? QB_ERR_UNSUPPORTED : QB_ERR_INVALID;
+    }
+    g->n_neighbors = total;
+    g->hbm_bytes = (uint64_t)n * m0 * 4 + 8 * levels + 4 * n + 4 * total + 8 * (length + n) + (nb_bytes + HC_PAD) + 8 * (length + n) + 8 * n;
+    if (cudaMalloc(&g->d_neighbors, std::max<size_t>(4 * total, 256)) != cudaSuccess) return fail(QB_ERR_OOM, "cudaMalloc failed", cudaGetLastError());
+    hnsw_v_links_kernel<<<hc_grid(length - 1, 8, 132 * 32), 256>>>(pv, d_lstart, g->d_offsets, g->d_neighbors);
+    QB_LAUNCHED();
+    hnsw_c_pad_kernel<<<hc_grid(n, 256, 132 * 4), 256>>>(g->d_offsets, length, n);
+    QB_LAUNCHED();
+    if (n) {
+        hnsw_links0_kernel<<<hc_grid(n * m0, 256, 132 * 16), 256>>>(g->d_neighbors, g->d_offsets, (uint32_t)n, (uint32_t)m0, g->d_links0);
+        QB_LAUNCHED();
+    }
+    ce = cudaDeviceSynchronize();
+    if (ce == cudaSuccess) ce = cudaGetLastError();
+    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "decode", ce);
+    *out = g;
+    return QB_OK;
+}
+
 extern "C" qb_status qb_hnsw_links(const qb_hnsw* g, uint32_t level, const uint32_t* ids, uint32_t n_ids, uint32_t cap, uint32_t* out, uint32_t* counts) {
     QB_CHECK(g && (ids || n_ids == 0) && (counts || n_ids == 0) && (out || cap == 0 || n_ids == 0), QB_ERR_INVALID, "hnsw_links: null argument");
     QB_CHECK(level < g->levels, QB_ERR_INVALID, "hnsw_links: level %u but the graph has %u levels", level, g->levels);
@@ -435,6 +647,7 @@ extern "C" void qb_hnsw_destroy(qb_hnsw* g) {
     cudaDeviceSynchronize();
     cudaFree(g->d_links0); cudaFree(g->d_level_offsets); cudaFree(g->d_reindex); cudaFree(g->d_neighbors); cudaFree(g->d_offsets);
     cudaFree(g->d_visited); cudaFree(g->d_vlog); cudaFree(g->d_work); cudaFree(g->d_stats);
+    cudaFree(g->d_blob); cudaFree(g->d_lvoff); cudaFree(g->d_boff);
     cudaGetLastError();
     delete g;
 }
@@ -517,11 +730,11 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
 }
 
 qb_status qb_hnsw_read_stats(qb_hnsw* g, cudaStream_t stream, uint64_t* evals_by_slot) {
-    unsigned long long h[4] = {0, 0, 0, 0};
-    QB_CUDA(cudaMemcpyAsync(h, g->d_stats, 32, cudaMemcpyDeviceToHost, stream));
+    unsigned long long h[7] = {0, 0, 0, 0, 0, 0, 0};
+    QB_CUDA(cudaMemcpyAsync(h, g->d_stats, 56, cudaMemcpyDeviceToHost, stream));
     QB_CUDA(cudaStreamSynchronize(stream));
-    QB_CUDA(cudaMemsetAsync(g->d_stats, 0, 32, stream));
-    g->hops += h[0] + h[2]; g->evals += h[1] + h[3];
+    QB_CUDA(cudaMemsetAsync(g->d_stats, 0, 56, stream));
+    g->hops += h[0] + h[2] + h[4]; g->evals += h[1] + h[3] + h[5]; g->base_evals += h[6];
     if (evals_by_slot) { evals_by_slot[0] = h[1]; evals_by_slot[1] = h[3]; }
     return QB_OK;
 }

@@ -19,6 +19,7 @@ constexpr uint32_t HNSW_MAX_LINKS = 64;      // links scored per hop (m0 <= 64)
 constexpr uint32_t HNSW_EMPTY = 0xFFFFFFFFu;
 constexpr uint32_t HNSW_MAX_EF = 4096;
 constexpr uint32_t HNSW_CUSTOM_SMEM = 48 * 1024;   // custom queries: examples up to this size are staged in shared memory
+constexpr uint32_t HNSW_MAX_LIST = 128;      // widest level list of a graph with inline vectors (qb_hnsw_create_with_vectors)
 
 enum { HK_DENSE_AVX = 0, HK_DENSE_SMALL = 1, HK_SQ8 = 2, HK_SQ8_LANEX = 3 };
 
@@ -154,7 +155,10 @@ __device__ __forceinline__ void prefetch_point(const HnswParams& p, uint32_t id)
     else prefetch_row_l2(p.codes + (size_t)id * p.ad, p.ad);
 }
 
-__device__ __forceinline__ bool hnsw_filtered_out(const HnswParams& p, uint32_t id) {
+// ScorerFilters::check_vector fails: the resident deleted flags or the per-call bitmap (either may be null); P = HnswParams or the
+// inline-vector search's parameters (qb_hnsw_inline.cu)
+template <class P>
+__device__ __forceinline__ bool hnsw_filtered_out(const P& p, uint32_t id) {
     bool d = false;
     if (p.deleted) d = (p.deleted[id >> 5] >> (id & 31)) & 1u;
     if (p.deleted2) d = d || ((p.deleted2[id >> 5] >> (id & 31)) & 1u);

@@ -150,8 +150,11 @@ struct qb_hnsw {
     uint32_t* d_visited = nullptr; uint64_t visited_words = 0; unsigned visited_slots = 0;
     uint32_t* d_vlog = nullptr; uint32_t vlog_cap = 0;
     unsigned int* d_work = nullptr;
-    unsigned long long* d_stats = nullptr;
-    uint64_t hops = 0, evals = 0;
+    unsigned long long* d_stats = nullptr;   // [0..3] the regular searches (two slots), [4..6] the inline-vector search
+    uint64_t hops = 0, evals = 0, base_evals = 0;
+    // inline vectors (qb_hnsw_create_with_vectors): the records, each entry's first link vector and each point's base vector (byte
+    // offsets into d_blob); null for the other loaders
+    uint8_t* d_blob = nullptr; uint64_t* d_lvoff = nullptr; uint64_t* d_boff = nullptr; uint32_t link_size = 0;
 };
 
 // A batch of custom queries for qb_hnsw_launch: query q's examples are the encoded queries ex_first .. ex_first + n_ex of the
@@ -171,7 +174,11 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
 // completes a handle whose plain arrays (d_level_offsets, d_reindex, d_neighbors, d_offsets and the host-side counts) are on the device:
 // the level-0 table and the search scratch (qb_hnsw.cu).  On failure the caller destroys g.  who = the error messages' prefix.
 qb_status qb_hnsw_finish_plain(qb_hnsw* g, const char* who);
-// adds the device counters to g->hops / g->evals and clears them; evals_by_slot (optional, [2]) receives each slot's scored points
+// the inline-vector search (qb_hnsw_inline.cu): queries preprocessed (d_q_pre, pre_stride floats apart) and SQ8-encoded; enqueued on stream
+qb_status qb_hnsw_inline_launch(qb_hnsw* g, const float* d_q_pre, uint32_t pre_stride, const void* d_q_enc, const float* d_q_off, uint32_t nq, uint32_t top,
+                                uint32_t ef, uint32_t entry, uint32_t entry_level, const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts,
+                                cudaStream_t stream);
+// adds the device counters to g->hops / g->evals / g->base_evals and clears them; evals_by_slot (optional, [2]) receives each regular slot's scored points
 qb_status qb_hnsw_read_stats(qb_hnsw* g, cudaStream_t stream, uint64_t* evals_by_slot = nullptr);
 
 // One rank of a sharded search (qb_comm.cu): an exchange buffer every peer maps + the peers' buffers

@@ -129,13 +129,15 @@ __device__ __forceinline__ float score_small(const float* __restrict__ row, cons
 // SQ8 (EncodedVectorsU8): raw integer score of one stored code row against one query code, 8 lanes per row, 16 B per lane per
 // step; every lane of the group returns the value.  l1 = Manhattan on codes (impl_score_l1_avx, cpp/avx2.c:65-122); LANEX =
 // the 8-lane partition + HSUM256_PS tree of impl_score_dot_avx (cpp/avx2.c:7-63) for totals that can leave the f32-exact window.
-template <bool LANEX>
-__device__ __forceinline__ float sq8_raw_group8(const uint4* __restrict__ rp, const uint4* __restrict__ qp, uint32_t n_chunks, int t, int l1) {
+// ld(c) returns the row's 16-B chunk c: sq8_raw_group8 reads an aligned stored row, the HNSW inline-vector search (qb_hnsw_inline.cu)
+// a link vector at any byte address; the arithmetic on the chunks is the same.
+template <bool LANEX, class LD>
+__device__ __forceinline__ float sq8_raw_group8_ld(LD ld, const uint4* __restrict__ qp, uint32_t n_chunks, int t, int l1) {
     float score;
     if (l1) {
         unsigned int acc = 0;
         for (uint32_t c = t; c < n_chunks; c += 8) {
-            uint4 v = __ldg(rp + c), w = qp[c];
+            uint4 v = ld(c), w = qp[c];
             acc += __vsadu4(v.x, w.x) + __vsadu4(v.y, w.y) + __vsadu4(v.z, w.z) + __vsadu4(v.w, w.w);
         }
         acc += __shfl_xor_sync(0xFFFFFFFFu, acc, 1);
@@ -145,7 +147,7 @@ __device__ __forceinline__ float sq8_raw_group8(const uint4* __restrict__ rp, co
     } else if (!LANEX) {
         int acc = 0;
         for (uint32_t c = t; c < n_chunks; c += 8) {
-            uint4 v = __ldg(rp + c), w = qp[c];
+            uint4 v = ld(c), w = qp[c];
             acc = __dp4a((int)v.x, (int)w.x, acc);
             acc = __dp4a((int)v.y, (int)w.y, acc);
             acc = __dp4a((int)v.z, (int)w.z, acc);
@@ -159,7 +161,7 @@ __device__ __forceinline__ float sq8_raw_group8(const uint4* __restrict__ rp, co
         // lane partition of impl_score_dot_avx: byte pair j of every 16-B chunk accumulates into i32 lane j
         int ln[8] = {0, 0, 0, 0, 0, 0, 0, 0};
         for (uint32_t c = t; c < n_chunks; c += 8) {
-            uint4 v = __ldg(rp + c), w = qp[c];
+            uint4 v = ld(c), w = qp[c];
             ln[0] = __dp4a((int)v.x, (int)(w.x & 0x0000FFFFu), ln[0]); ln[1] = __dp4a((int)v.x, (int)(w.x & 0xFFFF0000u), ln[1]);
             ln[2] = __dp4a((int)v.y, (int)(w.y & 0x0000FFFFu), ln[2]); ln[3] = __dp4a((int)v.y, (int)(w.y & 0xFFFF0000u), ln[3]);
             ln[4] = __dp4a((int)v.z, (int)(w.z & 0x0000FFFFu), ln[4]); ln[5] = __dp4a((int)v.z, (int)(w.z & 0xFFFF0000u), ln[5]);
@@ -177,6 +179,10 @@ __device__ __forceinline__ float sq8_raw_group8(const uint4* __restrict__ rp, co
         score = __fadd_rn(__fadd_rn(x0, x2), __fadd_rn(x1, x3));
     }
     return score;
+}
+template <bool LANEX>
+__device__ __forceinline__ float sq8_raw_group8(const uint4* __restrict__ rp, const uint4* __restrict__ qp, uint32_t n_chunks, int t, int l1) {
+    return sq8_raw_group8_ld<LANEX>([rp](uint32_t c) { return __ldg(rp + c); }, qp, n_chunks, t, l1);
 }
 
 }  // namespace qbs

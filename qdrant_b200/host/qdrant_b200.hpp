@@ -209,6 +209,12 @@ public:
         check(qb_hnsw_create_compressed(storage.raw(), links_bin, n_bytes, &h));
         return std::unique_ptr<HnswGraph>(new HnswGraph(h));
     }
+    // a CompressedWithVectors links.bin (inline storage) bound to the segment's SQ8 storage (qb_hnsw_create_with_vectors)
+    static std::unique_ptr<HnswGraph> with_vectors(const VectorStorage& quantized, const uint8_t* links_bin, uint64_t n_bytes) {
+        qb_hnsw* h = nullptr;
+        check(qb_hnsw_create_with_vectors(quantized.raw(), links_bin, n_bytes, &h));
+        return std::unique_ptr<HnswGraph>(new HnswGraph(h));
+    }
     // builds the graph of a dense f32 storage on the device (qb_hnsw_build); levels: one per point, <= 30; batch / serial_points 0 = 512 / 256.
     // The entry point the search starts from is returned in entry_point / entry_level.
     static std::unique_ptr<HnswGraph> build(const VectorStorage& storage, uint32_t m, uint32_t m0, uint32_t ef_construct, const std::vector<uint8_t>& levels,
@@ -245,6 +251,17 @@ public:
         std::vector<uint32_t> counts(n_queries);
         check(qb_hnsw_search_batch_algo(h_, queries, n_queries, top, ef, entry_point, entry_level, deleted, nullptr, flat.data(), counts.data(), nullptr,
                                         static_cast<qb_hnsw_algorithm>(algorithm)));
+        std::vector<std::vector<ScoredPointOffset>> out(n_queries);
+        for (uint32_t q = 0; q < n_queries; ++q) out[q].assign(flat.begin() + (size_t)q * top, flat.begin() + (size_t)q * top + counts[q]);
+        return out;
+    }
+    // GraphLayers::search_with_vectors on a with_vectors() graph (qb_hnsw_search_with_vectors_batch); ef = max(ef, oversampled top)
+    std::vector<std::vector<ScoredPointOffset>> search_with_vectors(const float* queries, uint32_t n_queries, uint32_t top, uint32_t ef,
+                                                                    PointOffsetType entry_point, uint32_t entry_level, const uint64_t* deleted = nullptr) const {
+        std::vector<ScoredPointOffset> flat((size_t)n_queries * top);
+        std::vector<uint32_t> counts(n_queries);
+        check(qb_hnsw_search_with_vectors_batch(h_, queries, n_queries, top, ef, entry_point, entry_level, deleted, nullptr, flat.data(), counts.data(),
+                                                nullptr));
         std::vector<std::vector<ScoredPointOffset>> out(n_queries);
         for (uint32_t q = 0; q < n_queries; ++q) out[q].assign(flat.begin() + (size_t)q * top, flat.begin() + (size_t)q * top + counts[q]);
         return out;

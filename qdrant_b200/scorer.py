@@ -734,6 +734,21 @@ class HnswGraph:
         return self
 
     @classmethod
+    def from_compressed_with_vectors(cls, storage: _Storage, links_bin) -> "HnswGraph":
+        """A graph from `links.bin` in GraphLinksFormat::CompressedWithVectors (inline storage), bound to the segment's SQ8 storage
+        (qb_hnsw_create_with_vectors).  search_with_vectors() runs the reference's search over the inline vectors; search() and the
+        custom searches run the regular traversal on the same handle."""
+        self = cls.__new__(cls)
+        self._storage = storage
+        self._h = vp()
+        blob = np.ascontiguousarray(np.frombuffer(links_bin, dtype=np.uint8) if isinstance(links_bin, (bytes, bytearray)) else links_bin,
+                                    dtype=np.uint8).reshape(-1)
+        h = vp()
+        check(lib().qb_hnsw_create_with_vectors(storage._h, blob.ctypes.data_as(u8p), blob.size, C.byref(h)))
+        self._h = h
+        return self
+
+    @classmethod
     def build(cls, storage: _Storage, m: int = 16, ef_construct: int = 100, levels=None, seed: int = 0, batch: int = 0, serial_points: int = 0,
               m0: Optional[int] = None) -> "HnswGraph":
         """Builds the graph of a dense f32 storage on the device (qb_hnsw_build; m0 defaults to 2m).  levels: one per point (<= 30);
@@ -803,6 +818,25 @@ class HnswGraph:
         check(lib().qb_hnsw_search_batch_algo(self._h, q.ctypes.data_as(f32p), nq, int(top), int(ef), int(entry_point), int(entry_level),
                                               None if bm is None else bm.ctypes.data_as(u64p), None, out.ctypes.data_as(C.POINTER(ScoredPoint)),
                                               counts.ctypes.data_as(u32p), None if counters is None else C.byref(counters), self.ALGORITHMS[algorithm]))
+        return [out[i, : counts[i]].copy() for i in range(nq)]
+
+    def search_with_vectors(self, queries, top: int, ef: int, entry_point: int, entry_level: int, point_deleted=None,
+                            counters: Optional[HwCounters] = None, is_stopped: bool = False):
+        """GraphLayers::search_with_vectors on a from_compressed_with_vectors() graph (qb_hnsw_search_with_vectors_batch): the beam on
+        the inline SQ8 link vectors, every popped candidate scored exactly from its inline f32 vector; the best `top` exact scores.
+        Pass ef = max(ef, oversampled top), as the reference does."""
+        q = np.atleast_2d(_f32(queries))
+        if q.shape[1] != self._storage.dim:
+            raise ValueError(f"queries have dim {q.shape[1]}, storage has {self._storage.dim}")
+        nq = q.shape[0]
+        out = np.zeros((nq, max(top, 1)), dtype=SCORED_POINT_OFFSET)
+        counts = np.zeros(nq, dtype=np.uint32)
+        bm = _bitmap(point_deleted, self._storage.count)
+        stop = C.c_int32(1) if is_stopped else None
+        check(lib().qb_hnsw_search_with_vectors_batch(self._h, q.ctypes.data_as(f32p), nq, int(top), int(ef), int(entry_point), int(entry_level),
+                                                      None if bm is None else bm.ctypes.data_as(u64p), None if stop is None else C.byref(stop),
+                                                      out.ctypes.data_as(C.POINTER(ScoredPoint)), counts.ctypes.data_as(u32p),
+                                                      None if counters is None else C.byref(counters)))
         return [out[i, : counts[i]].copy() for i in range(nq)]
 
     def _examples(self, examples, n_ex: int):
