@@ -1018,6 +1018,59 @@ API float qo_f16_dot_scalar(const uint16_t* a, const uint16_t* b, size_t n) {
     return s;
 }
 
+/* ------------------------------------------------------------------------------------------
+ * Whole-storage scoring for the f16 / u8 datatypes and the query conversions in front of it
+ * ---------------------------------------------------------------------------------------- */
+
+/* Metric<u8>::similarity dispatch: the avx2 kernels for n >= 32, the integer-exact scalar tier below */
+static float u8_similarity(int distance, const uint8_t* q, const uint8_t* v, size_t n) {
+    const int avx = n >= MIN_DIM_SIZE_AVX;
+    switch (distance) {
+        case QO_COSINE: return avx ? qo_u8_cosine_avx(q, v, n) : qo_u8_cosine_scalar(q, v, n);
+        case QO_EUCLID: return avx ? qo_u8_euclid_avx(q, v, n) : qo_u8_euclid_scalar(q, v, n);
+        case QO_MANHATTAN: return avx ? qo_u8_manhattan_avx(q, v, n) : qo_u8_manhattan_scalar(q, v, n);
+        default: return avx ? qo_u8_dot_avx(q, v, n) : qo_u8_dot_scalar(q, v, n);
+    }
+}
+
+/* out[i] = similarity(q, rows[ids ? ids[i] : i]) for i < n; q is already in the storage datatype */
+API void qo_score_rows_f16(int distance, const uint16_t* rows, uint64_t n, uint32_t dim, const uint16_t* q, const uint32_t* ids, float* out) {
+    for (uint64_t i = 0; i < n; i++) out[i] = qo_similarity_f16(distance, q, rows + (uint64_t)(ids ? ids[i] : i) * dim, dim);
+}
+API void qo_score_rows_u8(int distance, const uint8_t* rows, uint64_t n, uint32_t dim, const uint8_t* q, const uint32_t* ids, float* out) {
+    for (uint64_t i = 0; i < n; i++) out[i] = u8_similarity(distance, q, rows + (uint64_t)(ids ? ids[i] : i) * dim, dim);
+}
+
+/* f16::from_f32 (half 2.x): round to nearest, ties to even; overflow to +-inf; subnormal results kept; NaN stays NaN (quiet, top
+ * payload bits kept) */
+static uint16_t f32_to_f16_bits(float f) {
+    uint32_t x;
+    memcpy(&x, &f, 4);
+    const uint16_t sign = (uint16_t)((x >> 16) & 0x8000u);
+    const uint32_t ax = x & 0x7FFFFFFFu;
+    if (ax > 0x7F800000u) return (uint16_t)(sign | 0x7E00u | ((ax & 0x7FFFFFu) >> 13));
+    if (ax >= 0x47800000u) return (uint16_t)(sign | 0x7C00u);                 /* >= 65536 and inf */
+    if (ax >= 0x38800000u)                                                      /* the normal range (>= 2^-14): RNE on the 13 dropped bits */
+        return (uint16_t)(sign | (((ax + 0xFFFu + ((ax >> 13) & 1u)) >> 13) - (112u << 10)));   /* a carry out of 0x7BFF is the inf encoding */
+    if (ax <= 0x33000000u) return sign;                                         /* <= 2^-25: the tie at 2^-25 goes to the even 0 */
+    const uint32_t m = (ax & 0x7FFFFFu) | 0x800000u, shift = 126u - (ax >> 23);  /* units of 2^-24: m * 2^(e - 126) */
+    uint32_t r = m >> shift;
+    const uint32_t rem = m & ((1u << shift) - 1u), half = 1u << (shift - 1u);
+    if (rem > half || (rem == half && (r & 1u))) r++;                           /* may reach 0x400, the smallest normal */
+    return (uint16_t)(sign | r);
+}
+API void qo_f32_to_f16(const float* in, uint64_t n, uint16_t* out) {
+    for (uint64_t i = 0; i < n; i++) out[i] = f32_to_f16_bits(in[i]);
+}
+
+/* `x as u8` (Rust's saturating float -> int cast): NaN -> 0, truncate toward zero, clamp to 0..255 */
+API void qo_f32_to_u8(const float* in, uint64_t n, uint8_t* out) {
+    for (uint64_t i = 0; i < n; i++) {
+        const float x = in[i];
+        out[i] = (x != x || x <= 0.0f) ? 0 : (x >= 255.0f ? 255 : (uint8_t)x);
+    }
+}
+
 /* ------------------------------------------------------------------------------------------------
  * Custom queries: Query::score_by over the similarities of one stored vector to the example vectors
  *   lib/common/common/src/math.rs:7-18                      fast_sigmoid, scaled_fast_sigmoid

@@ -84,6 +84,12 @@ def lib() -> C.CDLL:
             fn = getattr(L, n)
             fn.restype, fn.argtypes = C.c_float, [u16p, u16p, C.c_size_t]
         L.qo_similarity_f16.restype, L.qo_similarity_f16.argtypes = C.c_float, [C.c_int, u16p, u16p, C.c_size_t]
+        L.qo_score_rows_f16.restype = None
+        L.qo_score_rows_f16.argtypes = [C.c_int, u16p, C.c_uint64, C.c_uint32, u16p, u32p, f32p]
+        L.qo_score_rows_u8.restype = None
+        L.qo_score_rows_u8.argtypes = [C.c_int, u8p, C.c_uint64, C.c_uint32, u8p, u32p, f32p]
+        L.qo_f32_to_f16.restype, L.qo_f32_to_f16.argtypes = None, [f32p, C.c_uint64, u16p]
+        L.qo_f32_to_u8.restype, L.qo_f32_to_u8.argtypes = None, [f32p, C.c_uint64, u8p]
         L.qo_sq8_dot_avx.restype, L.qo_sq8_dot_avx.argtypes = C.c_float, [u8p, u8p, C.c_uint32]
         L.qo_sq8_l1_avx.restype, L.qo_sq8_l1_avx.argtypes = C.c_float, [u8p, u8p, C.c_uint32]
         mp = C.POINTER(SQ8Meta)
@@ -234,6 +240,64 @@ def raw_f16(name: str, a, b) -> np.float32:
     a = np.ascontiguousarray(a, dtype=np.float16).view(np.uint16)
     b = np.ascontiguousarray(b, dtype=np.float16).view(np.uint16)
     return np.float32(getattr(lib(), f"qo_f16_{name}")(_p(a, C.c_uint16), _p(b, C.c_uint16), a.size))
+
+
+def to_f16_query(distance: int, q) -> np.ndarray:
+    """The query of an f16 storage: Metric::preprocess in f32, then f16::from_f32 (round to nearest even, overflow to inf)."""
+    pre = preprocess_f32(distance, q)
+    out = np.empty(pre.size, dtype=np.uint16)
+    lib().qo_f32_to_f16(_p(pre, C.c_float), pre.size, _p(out, C.c_uint16))
+    return out.view(np.float16)
+
+
+def to_u8_query(q) -> np.ndarray:
+    """The query of a u8 storage: `x as u8` on the raw f32 values (no preprocess, not even for Cosine): NaN -> 0, truncate, saturate."""
+    q = _f32(q)
+    out = np.empty(q.size, dtype=np.uint8)
+    lib().qo_f32_to_u8(_p(q, C.c_float), q.size, _p(out, C.c_uint8))
+    return out
+
+
+def _score_rows_x(fn, ct, distance: int, rows, q, ids):
+    rows, q = np.ascontiguousarray(rows), np.ascontiguousarray(q)
+    assert rows.ndim == 2 and q.shape == (rows.shape[1],)
+    if ids is not None:
+        ids = np.ascontiguousarray(ids, dtype=np.uint32)
+        assert ids.size == 0 or int(ids.max()) < rows.shape[0]
+    out = np.empty(rows.shape[0] if ids is None else ids.size, dtype=np.float32)
+    fn(distance, _p(rows, ct), out.size, rows.shape[1], _p(q, ct), None if ids is None else _p(ids, C.c_uint32), _p(out, C.c_float))
+    return out
+
+
+def score_rows_f16(distance: int, rows, q_f16, ids=None) -> np.ndarray:
+    """Metric<f16>::similarity(q, row) for every row (or every row listed in ids); q_f16 already converted (to_f16_query)."""
+    rows = np.ascontiguousarray(rows, dtype=np.float16).view(np.uint16)
+    q = np.ascontiguousarray(q_f16, dtype=np.float16).view(np.uint16)
+    return _score_rows_x(lib().qo_score_rows_f16, C.c_uint16, distance, rows, q, ids)
+
+
+def score_rows_u8(distance: int, rows, q_u8, ids=None) -> np.ndarray:
+    """Metric<u8>::similarity(q, row) for every row (or every row listed in ids); q_u8 already converted (to_u8_query)."""
+    return _score_rows_x(lib().qo_score_rows_u8, C.c_uint8, distance, _u8(rows), _u8(q_u8), ids)
+
+
+def _scan_x(score_rows, distance: int, base, queries, top: int, deleted):
+    """peek_top_iter over all rows like scan_f32: rows in order, deleted ones skipped, one heap per query."""
+    live = None
+    if deleted is not None:
+        bits = np.unpackbits(np.ascontiguousarray(deleted, dtype=np.uint64).view(np.uint8), bitorder="little")[: base.shape[0]]
+        live = np.flatnonzero(bits == 0).astype(np.uint32)
+    return [topk(score_rows(distance, base, q, live), top, live) for q in queries]
+
+
+def scan_f16(distance: int, base, queries_f16, top: int, deleted=None):
+    """Top-k of an f16 storage for converted queries ([nq, dim] f16) -> list of SCORED arrays (one per query, descending)."""
+    return _scan_x(score_rows_f16, distance, base, np.atleast_2d(np.asarray(queries_f16, dtype=np.float16)), top, deleted)
+
+
+def scan_u8(distance: int, base, queries_u8, top: int, deleted=None):
+    """Top-k of a u8 storage for converted queries ([nq, dim] u8) -> list of SCORED arrays (one per query, descending)."""
+    return _scan_x(score_rows_u8, distance, base, np.atleast_2d(_u8(queries_u8)), top, deleted)
 
 
 def score_rows_f32(distance: int, rows, q_pre) -> np.ndarray:

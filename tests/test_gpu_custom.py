@@ -20,8 +20,9 @@ def qb():
     return scorer
 
 
-def make_queries(qb, rng, dim):
-    v = lambda: rng.standard_normal(dim).astype(np.float32)  # noqa: E731
+def make_queries(qb, rng, dim, scale=1.0, shift=0.0):
+    """scale / shift: example vectors on the scale of the stored values (u8 storages convert them with `x as u8`)"""
+    v = lambda: (rng.standard_normal(dim) * scale + shift).astype(np.float32)  # noqa: E731
     return [
         qb.RecoBestScoreQuery(qb.RecoQuery([v(), v(), v()], [v(), v()])),
         qb.RecoBestScoreQuery(qb.RecoQuery([v()], [])),
@@ -31,21 +32,21 @@ def make_queries(qb, rng, dim):
         qb.DiscoverQuery(v(), []),
         qb.ContextQuery([qb.ContextPair(v(), v()), qb.ContextPair(v(), v())]),
         qb.RecoSumScoresQuery(qb.RecoQuery([v() for _ in range(12)], [v() for _ in range(9)])),   # 21 examples: beyond the fused-fold scan's 16
-        feedback_query(qb, rng, dim, 4),
-        feedback_query(qb, rng, dim, 1),     # fewer than two feedback items: no pairs, score = a * sim(target)
+        feedback_query(qb, rng, dim, 4, v),
+        feedback_query(qb, rng, dim, 1, v),  # fewer than two feedback items: no pairs, score = a * sim(target)
     ]
 
 
-def feedback_query(qb, rng, dim, n_items):
+def feedback_query(qb, rng, dim, n_items, v):
     """NaiveFeedbackQuery -> FeedbackQuery the way the reference builds it (feedback_query.rs:121-172): every ordered pair of feedback
     items whose score difference is positive becomes a context pair with partial_computation = confidence^b * c."""
     from oracle import oracle as o
 
-    items = [rng.standard_normal(dim).astype(np.float32) for _ in range(n_items)]
+    items = [v() for _ in range(n_items)]
     scores = rng.random(n_items).astype(np.float32)
     a, b, c = 0.9, 1.5, 0.4
     pos, neg, part = o.feedback_pairs(scores, b, c)
-    return qb.FeedbackQuery(rng.standard_normal(dim).astype(np.float32), [qb.ContextPair(items[i], items[j]) for i, j in zip(pos, neg)], part, a)
+    return qb.FeedbackQuery(v(), [qb.ContextPair(items[i], items[j]) for i, j in zip(pos, neg)], part, a)
 
 
 def oracle_scores(oracle, query, sim_rows):
@@ -107,6 +108,28 @@ def test_custom_dense_f32(qb, oracle, dist, n, dim):
     st = qb.DenseVectorStorage(stored, d)
     sim = lambda v: oracle.score_rows_f32(int(d), stored, oracle.preprocess_f32(int(d), v))  # noqa: E731
     check_storage(qb, oracle, st, make_queries(qb, rng, dim), sim, n, f"dense {dist}")
+    st.close()
+
+
+@pytest.mark.parametrize("dist", ["Cosine", "Dot", "Euclid", "Manhattan"])
+@pytest.mark.parametrize("dt", ["f16", "u8"])
+def test_custom_dense_f16_u8(qb, oracle, dt, dist):
+    """Every example is converted the way a plain query is (f16: preprocess, then f16::from_f32; u8: `x as u8`), then scored with the
+    storage's own metric."""
+    d = getattr(qb.Distance, dist)
+    n, dim = 300, 70
+    rng = np.random.default_rng(15)
+    if dt == "u8":
+        stored = rng.integers(0, 256, (n, dim), dtype=np.uint8)
+        st = qb.DenseVectorStorage(stored, d, qb.VectorStorageDatatype.Uint8)
+        sim = lambda v: oracle.score_rows_u8(int(d), stored, oracle.to_u8_query(v))  # noqa: E731
+        queries = make_queries(qb, rng, dim, scale=90.0, shift=120.0)              # some examples saturate or truncate to 0
+    else:
+        stored = oracle.preprocess_rows_f32(int(d), rng.standard_normal((n, dim)).astype(np.float32)).astype(np.float16)
+        st = qb.DenseVectorStorage(stored, d, qb.VectorStorageDatatype.Float16)
+        sim = lambda v: oracle.score_rows_f16(int(d), stored, oracle.to_f16_query(int(d), v))  # noqa: E731
+        queries = make_queries(qb, rng, dim)
+    check_storage(qb, oracle, st, queries, sim, n, f"dense {dt} {dist}")
     st.close()
 
 

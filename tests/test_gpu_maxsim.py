@@ -64,6 +64,47 @@ def test_maxsim_dense_f32(qb, oracle, dist, n_points, max_len, dim, nq):
     st.close()
 
 
+@pytest.mark.parametrize("dist", ["Cosine", "Dot", "Euclid", "Manhattan"])
+@pytest.mark.parametrize("dt", ["f16", "u8"])
+def test_maxsim_dense_f16_u8(qb, oracle, dt, dist):
+    """The MaxSim fold over f16 / u8 token similarities: each query vector converted as a plain query is, scored with the storage's metric."""
+    d = getattr(qb.Distance, dist)
+    rng = np.random.default_rng(23)
+    n_points, dim, nq = 300, 48, 5
+    off = make_points(rng, n_points, 7)
+    n_rows = int(off[-1])
+    if dt == "u8":
+        rows = rng.integers(0, 256, (n_rows, dim), dtype=np.uint8)
+        st = qb.DenseVectorStorage(rows, d, qb.VectorStorageDatatype.Uint8)
+        query = rng.uniform(-20.0, 300.0, (nq, dim)).astype(np.float32)
+        sims = np.stack([oracle.score_rows_u8(int(d), rows, oracle.to_u8_query(q)) for q in query])
+    else:
+        rows = oracle.preprocess_rows_f32(int(d), rng.standard_normal((n_rows, dim)).astype(np.float32)).astype(np.float16)
+        st = qb.DenseVectorStorage(rows, d, qb.VectorStorageDatatype.Float16)
+        query = rng.standard_normal((nq, dim)).astype(np.float32)
+        sims = np.stack([oracle.score_rows_f16(int(d), rows, oracle.to_f16_query(int(d), q)) for q in query])
+    want = oracle.maxsim_fold(sims, off)
+    mv = qb.MultiVectorView(st, off)
+    np.testing.assert_array_equal(mv.score_points(query, np.arange(n_points, dtype=np.uint32)).view(np.uint32), want.view(np.uint32))
+    sub = np.array([7, 0, n_points - 1, 7], np.uint32)
+    np.testing.assert_array_equal(mv.score_points(query, sub).view(np.uint32), want[sub].view(np.uint32))
+    for top in (1, 10):
+        got = mv.search(query, top)
+        order = np.argsort(-want, kind="stable")[:top]
+        ref = np.zeros(order.size, dtype=got.dtype)
+        ref["idx"], ref["score"] = order, want[order]
+        assert_topk_equal(got, ref, want, f"maxsim {dt} {dist} top{top}")
+    deleted = rng.random(n_points) < 0.3
+    got = mv.search(query, 10, point_deleted=deleted)
+    live = np.flatnonzero(~deleted)
+    order = live[np.argsort(-want[live], kind="stable")[:10]]
+    ref = np.zeros(order.size, dtype=got.dtype)
+    ref["idx"], ref["score"] = order, want[order]
+    assert_topk_equal(got, ref, want, f"maxsim {dt} {dist} deleted")
+    assert not np.any(deleted[got["idx"]])
+    st.close()
+
+
 def test_maxsim_sq8(qb, oracle):
     """Quantized multivectors: the same fold over SQ8 similarities (quantized_multivector_storage)."""
     d = qb.Distance.Dot
