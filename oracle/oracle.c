@@ -949,6 +949,22 @@ API void qo_scan_bq(const uint8_t* rows, uint64_t row_begin, uint64_t row_end, u
     free(pqs);
 }
 
+/* Whole-storage quantized scoring: out[i] = the per-row score (qo_sq8_score / qo_pq_score / qo_bq_score) of row ids ? ids[i] : i,
+ * i < n, for one encoded query */
+API void qo_score_rows_sq8(const qo_sq8_meta* m, const uint8_t* rows, uint64_t n, const uint8_t* q_code, float q_off, const uint32_t* ids, float* out) {
+    const size_t stride = 4 + (size_t)m->actual_dim;
+    for (uint64_t i = 0; i < n; i++) out[i] = qo_sq8_score(m, q_code, q_off, rows + (uint64_t)(ids ? ids[i] : i) * stride);
+}
+API void qo_score_rows_pq(const uint8_t* codes, uint64_t n, uint32_t m_chunks, uint32_t n_centroids, const float* lut, const uint32_t* ids, float* out) {
+    for (uint64_t i = 0; i < n; i++) out[i] = qo_pq_score(lut, n_centroids, codes + (uint64_t)(ids ? ids[i] : i) * m_chunks, m_chunks);
+}
+API void qo_score_rows_bq(const uint8_t* rows, uint64_t n, uint32_t dim, int encoding, uint32_t query_bits_count, int distance_type, int invert,
+                          const uint8_t* q_enc, const uint32_t* ids, float* out) {
+    const uint32_t rb = qo_bq_row_bytes(dim, encoding);
+    for (uint64_t i = 0; i < n; i++)
+        out[i] = qo_bq_score(rows + (uint64_t)(ids ? ids[i] : i) * rb, q_enc, dim, encoding, query_bits_count, distance_type, invert);
+}
+
 /* bulk helpers used by tests/bench (score every listed id) */
 API void qo_score_points_f32(int distance, const float* base, uint32_t dim, const float* q_pre,
                              const uint32_t* ids, uint64_t n, float* scores) {

@@ -116,6 +116,12 @@ def lib() -> C.CDLL:
         L.qo_scan_pq.argtypes = [u8p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint32, f32p, C.c_uint32, C.c_uint32, u64p, C.c_void_p, u32p]
         L.qo_scan_bq.restype = None
         L.qo_scan_bq.argtypes = [u8p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int, C.c_uint32, C.c_int, C.c_int, u8p, C.c_uint32, C.c_uint32, C.c_uint32, u64p, C.c_void_p, u32p]
+        L.qo_score_rows_sq8.restype = None
+        L.qo_score_rows_sq8.argtypes = [mp, u8p, C.c_uint64, u8p, C.c_float, u32p, f32p]
+        L.qo_score_rows_pq.restype = None
+        L.qo_score_rows_pq.argtypes = [u8p, C.c_uint64, C.c_uint32, C.c_uint32, f32p, u32p, f32p]
+        L.qo_score_rows_bq.restype = None
+        L.qo_score_rows_bq.argtypes = [u8p, C.c_uint64, C.c_uint32, C.c_int, C.c_uint32, C.c_int, C.c_int, u8p, u32p, f32p]
         L.qo_score_points_f32.restype = None
         L.qo_score_points_f32.argtypes = [C.c_int, f32p, C.c_uint32, f32p, u32p, C.c_uint64, f32p]
         L.qo_score_rows_f32.restype = None
@@ -346,6 +352,15 @@ def topk(scores, top: int, ids=None) -> np.ndarray:
     return out[:n].copy()
 
 
+def _row_ids(ids, count: int):
+    """(kept array, pointer or None, number of scores) for the optional id list of the quantized score_rows"""
+    if ids is None:
+        return None, None, count
+    ids = np.ascontiguousarray(ids, dtype=np.uint32)
+    assert ids.size == 0 or int(ids.max()) < count
+    return ids, _p(ids, C.c_uint32), ids.size
+
+
 # ------------------------------------------------------------------ SQ8
 @dataclass
 class SQ8:
@@ -386,8 +401,17 @@ class SQ8:
         ri, rj = np.ascontiguousarray(self.rows[i]), np.ascontiguousarray(self.rows[j])
         return np.float32(lib().qo_sq8_score_internal(C.byref(self.meta), _p(ri, C.c_uint8), _p(rj, C.c_uint8)))
 
+    def score_rows(self, q_code, q_off, ids=None) -> np.ndarray:
+        """score(q_code, q_off, row) for every row (or every row listed in ids)."""
+        rows, q_code = np.ascontiguousarray(self.rows), _u8(q_code)
+        assert q_code.size == self.meta.actual_dim
+        ids, idp, n = _row_ids(ids, rows.shape[0])
+        out = np.empty(n, dtype=np.float32)
+        lib().qo_score_rows_sq8(C.byref(self.meta), _p(rows, C.c_uint8), n, _p(q_code, C.c_uint8), C.c_float(float(q_off)), idp, _p(out, C.c_float))
+        return out
+
     def score_all(self, q_code, q_off) -> np.ndarray:
-        return np.array([self.score(q_code, q_off, i) for i in range(self.rows.shape[0])], dtype=np.float32)
+        return self.score_rows(q_code, q_off)
 
     def scan(self, q_codes, q_offs, top: int, deleted=None):
         q_codes = np.atleast_2d(_u8(q_codes))
@@ -460,6 +484,15 @@ class PQ:
         code = np.ascontiguousarray(self.codes[row_id])
         lut = _f32(lut)
         return np.float32(lib().qo_pq_score(_p(lut, C.c_float), self.centroids.shape[0], _p(code, C.c_uint8), self.m))
+
+    def score_rows(self, lut, ids=None) -> np.ndarray:
+        """score(lut, row) for every row (or every row listed in ids)."""
+        codes, lut = np.ascontiguousarray(self.codes), _f32(lut)
+        assert lut.shape == (self.m, self.centroids.shape[0])
+        ids, idp, n = _row_ids(ids, codes.shape[0])
+        out = np.empty(n, dtype=np.float32)
+        lib().qo_score_rows_pq(_p(codes, C.c_uint8), n, self.m, self.centroids.shape[0], _p(lut, C.c_float), idp, _p(out, C.c_float))
+        return out
 
     def score_internal(self, i: int, j: int) -> np.float32:
         ci, cj = np.ascontiguousarray(self.codes[i]), np.ascontiguousarray(self.codes[j])
@@ -539,6 +572,16 @@ class BQ:
         q_enc = _u8(q_enc)
         return np.float32(lib().qo_bq_score(_p(row, C.c_uint8), _p(q_enc, C.c_uint8), self.dim, self.encoding, self.query_bits,
                                             self.distance_type, int(self.invert)))
+
+    def score_rows(self, q_enc, ids=None) -> np.ndarray:
+        """score(q_enc, row) for every row (or every row listed in ids)."""
+        rows, q_enc = np.ascontiguousarray(self.rows), _u8(q_enc)
+        assert q_enc.size == (self.rows.shape[1] if self.query_encoding == BQQ_SAME else self.query_bytes)
+        ids, idp, n = _row_ids(ids, rows.shape[0])
+        out = np.empty(n, dtype=np.float32)
+        lib().qo_score_rows_bq(_p(rows, C.c_uint8), n, self.dim, self.encoding, self.query_bits, self.distance_type, int(self.invert),
+                               _p(q_enc, C.c_uint8), idp, _p(out, C.c_float))
+        return out
 
     def scan(self, q_encs, top: int, deleted=None):
         q_encs = np.atleast_2d(_u8(q_encs))

@@ -7,6 +7,7 @@
 #include <stdlib.h>
 
 #include <algorithm>
+#include <cmath>
 
 #include "qb_internal.h"
 
@@ -346,11 +347,17 @@ extern "C" qb_status qb_storage_create_sq8(int32_t device, uint32_t dim, uint64_
         if (cudaMalloc(&d_stage, std::min<uint64_t>(chunk_rows, count) * row_bytes) != cudaSuccess) {
             qb_set_error("create_sq8: staging cudaMalloc failed"); qb_storage_destroy(s); return QB_ERR_OOM;
         }
+        std::vector<float> h_voff;
         for (uint64_t r = 0; r < count; r += chunk_rows) {
             const uint64_t n = std::min<uint64_t>(chunk_rows, count - r);
             cudaError_t e = cudaMemcpy(d_stage, rows + r * row_bytes, n * row_bytes, cudaMemcpyDefault);  // host or device source
             qb_status st = (e == cudaSuccess) ? qb_sq8_repack(s, d_stage, row_bytes, r, n, 0) : QB_ERR_CUDA;
             if (st == QB_OK && cudaDeviceSynchronize() != cudaSuccess) st = QB_ERR_CUDA;
+            // the largest |v_off| (inf once one is not finite) bounds the scores the tensor-core path can produce (qb_sq8_mma_block)
+            h_voff.resize(n);
+            if (st == QB_OK && cudaMemcpy(h_voff.data(), s->d_voff + r, n * 4, cudaMemcpyDeviceToHost) != cudaSuccess) st = QB_ERR_CUDA;
+            if (st == QB_OK)
+                for (const float v : h_voff) s->voff_absmax = std::isfinite(v) ? std::max(s->voff_absmax, std::fabs(v)) : INFINITY;
             if (st != QB_OK) { qb_set_error("create_sq8: upload failed: %s", cudaGetErrorString(cudaGetLastError())); cudaFree(d_stage); qb_storage_destroy(s); return st; }
         }
         cudaFree(d_stage);

@@ -74,6 +74,7 @@ struct qb_storage {
     uint8_t* d_codes = nullptr;      // [count][actual_dim], actual_dim % 16 == 0
     float* d_voff = nullptr;         // [count]
     float alpha = 0, offset = 0, multiplier = 0;
+    float voff_absmax = 0;           // max |v_off| over the rows; inf when one is not finite (qb_sq8_mma_block)
 
     // ---- PQ
     uint32_t pq_m = 0, pq_stride = 0, n_centroids = 0;

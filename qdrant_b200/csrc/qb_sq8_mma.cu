@@ -690,10 +690,21 @@ qb_status launch_mma(const CUtensorMap& map_a, const CUtensorMap& map_b, MmaPara
 
 }  // namespace
 
+// The epilogue's filter (sc >= thr) drops a NaN score, which the CUDA-core scan keeps (OrderedFloat: NaN is the greatest score), so
+// the tensor cores only take storages whose scores are finite: score = multiplier * dot + q_off + v_off with dot <= actual_dim * 127^2,
+// |q_off| <= actual_dim * 127 * |alpha * offset| (dot / cosine) or actual_dim * 127^2 * alpha^2 (L2).  A bound that is not finite or
+// not clear of FLT_MAX (metadata from rows holding +-inf: alpha = inf, every offset 0 * inf = NaN) sends the batch to the CUDA cores.
+static bool sq8_scores_finite(const qb_storage* s) {
+    const double d = (double)s->actual_dim * 127.0 * 127.0, a = fabs((double)s->alpha), o = fabs((double)s->offset);
+    const double q = (s->qdist == QB_QD_L2) ? d * a * a : (double)s->actual_dim * 127.0 * a * o;
+    return fabs((double)s->multiplier) * d + q + (double)s->voff_absmax < 1.0e38;   // false for inf and NaN
+}
+
 // Can this (storage, batch) use the tensor-core path?  Returns the query block width (0 = no).
 uint32_t qb_sq8_mma_block(const qb_storage* s, uint32_t nq) {
     if (s->kind != QB_KIND_SQ8 || s->qdist == QB_QD_L1) return 0;
     if (nq < 32 || s->count < 4 * 128) return 0;
+    if (!sq8_scores_finite(s)) return 0;
     return block_for(s, nq);
 }
 // scratch the filter-mode scan needs (bias rows, bias integers, the batch threshold)

@@ -18,9 +18,16 @@ def qb():
     return scorer
 
 
-@pytest.mark.parametrize("world,nq,top,n,dim", [(2, 1, 10, 150_003, 64), (3, 5, 10, 90_001, 96), (4, 40, 7, 70_000, 32), (8, 1, 10, 80_000, 128),
-                                                (2, 1, 10, 1_200_001, 64)])   # the last one: shards of >= 2^19 rows answer through the shadow-plane scan
-def test_sharded_equals_single_through_the_c_abi(qb, oracle, world, nq, top, n, dim):
+def _case(world, nq, top, n, dim, kind="f32"):
+    return pytest.param(world, nq, top, n, dim, kind, id="-".join(map(str, (world, nq, top, n, dim))) + ("" if kind == "f32" else f"-{kind}"))
+
+
+@pytest.mark.parametrize("world,nq,top,n,dim,kind", [_case(2, 1, 10, 150_003, 64), _case(3, 5, 10, 90_001, 96), _case(4, 40, 7, 70_000, 32),
+                                                     _case(8, 1, 10, 80_000, 128),
+                                                     _case(2, 1, 10, 1_200_001, 64),   # shards of >= 2^19 rows answer through the shadow-plane scan
+                                                     _case(2, 12, 10, 150_002, 128, "pq"),   # pq_scan16_kernel + pq_rescore_kernel per shard
+                                                     _case(2, 12, 10, 150_002, 64, "sq8")])  # SQ8 sample -> threshold -> filter per shard
+def test_sharded_equals_single_through_the_c_abi(qb, oracle, world, nq, top, n, dim, kind):
     import torch
 
     from qdrant_b200._capi import ScoredPoint, check, f32p, lib, u32p, vp
@@ -32,10 +39,20 @@ def test_sharded_equals_single_through_the_c_abi(qb, oracle, world, nq, top, n, 
     rng = np.random.default_rng(world)
     base = oracle.preprocess_rows_f32(oracle.COSINE, rng.standard_normal((n, dim)).astype(np.float32))
     queries = rng.standard_normal((6, nq, dim)).astype(np.float32)          # six consecutive collective calls (parity slots, seq)
-    single = qb.DenseVectorStorage(base, qb.Distance.Cosine)
+    if kind == "pq":     # one codebook and one code array, split by rows: the shards and the single storage score the same bytes
+        cents = (rng.standard_normal((256, dim)) * 0.5).astype(np.float32)
+        codes = rng.integers(0, 256, (n, dim // 4), dtype=np.uint8)
+        make = lambda lo, hi, dev: qb.ProductQuantizedVectors(codes[lo:hi], cents, 4, dim, qb.Distance.Cosine, device=dev)   # noqa: E731
+    elif kind == "sq8":  # one alpha / offset for all shards, as a shard of one encoded storage has
+        sq = oracle.SQ8.encode(base, oracle.QD_DOT, False)
+        make = lambda lo, hi, dev: qb.ScalarQuantizedVectors(sq.rows[lo:hi], dim, sq.meta.alpha, sq.meta.offset, sq.meta.multiplier,   # noqa: E731
+                                                             qb.Distance.Cosine, device=dev)
+    else:
+        make = lambda lo, hi, dev: qb.DenseVectorStorage(base[lo:hi], qb.Distance.Cosine, device=dev)   # noqa: E731
+    single = make(0, n, 0)
     shards, comms = [], (vp * world)()
     for r, (b, e) in enumerate(shard_ranges(n, world)):
-        st = qb.DenseVectorStorage(base[b:e], qb.Distance.Cosine, device=r % n_dev)
+        st = make(b, e, r % n_dev)
         check(lib().qb_storage_set_id_base(st._h, b))
         shards.append(st)
         h = vp()
