@@ -38,6 +38,18 @@ impl<'a> B200Hnsw<'a> {
         Ok(Self { raw, _storage: std::marker::PhantomData })
     }
 
+    /// `links.bin` (Compressed) of a multivector named vector: a graph over POINTS, point p being token rows
+    /// [point_offsets[p], point_offsets[p + 1]) of `tokens` (dense f32 or SQ8).  Search it with `search_maxsim`.
+    pub fn from_compressed_links_multivector(tokens: &'a B200Storage, point_offsets: &[u32], links_bin: &[u8]) -> OperationResult<Self> {
+        let mut raw = std::ptr::null_mut();
+        let n_points = point_offsets.len().saturating_sub(1) as u32;
+        let st = unsafe {
+            qb_hnsw_create_compressed_multivector(tokens.raw, point_offsets.as_ptr(), n_points, links_bin.as_ptr(), links_bin.len() as u64, &mut raw)
+        };
+        if st != QB_OK { return Err(OperationError::service_error(last_error())); }
+        Ok(Self { raw, _storage: std::marker::PhantomData })
+    }
+
     /// `links.bin` in GraphLinksFormat::Compressed; m and m0 come from its header.  CompressedWithVectors is refused (see
     /// `from_compressed_links_with_vectors`).
     pub fn from_compressed_links(storage: &'a B200Storage, links_bin: &[u8]) -> OperationResult<Self> {
@@ -101,6 +113,24 @@ impl<'a> B200Hnsw<'a> {
             qb_hnsw_search_with_vectors_batch(self.raw, queries.as_ptr(), n_queries as u32, top as u32, ef as u32, entry.0, entry.1 as u32,
                                               deleted.map_or(std::ptr::null(), |d| d.as_ptr()), std::ptr::null(), out.as_mut_ptr(), counts.as_mut_ptr(),
                                               std::ptr::null_mut())
+        };
+        assert!(st == QB_OK, "{}", last_error());
+        (0..n_queries).map(|q| out[q * top..q * top + counts[q] as usize].iter().map(|p| ScoredPointOffset { idx: p.idx, score: p.score }).collect()).collect()
+    }
+
+    /// `GraphLayers::search` with a MaxSim `FilteredScorer` (MultiMetricQueryScorer / QuantizedMultivectorStorage) on a
+    /// `from_compressed_links_multivector` graph: query i = rows [query_offsets[i], query_offsets[i + 1]) of `query_vectors` (raw f32 x dim,
+    /// 1..4096 vectors each); `deleted` is a bitmap over points.  Scores equal qb_score_maxsim bit for bit.
+    pub fn search_maxsim(&self, query_vectors: &[f32], query_offsets: &[u32], top: usize, ef: usize, entry: (PointOffsetType, usize),
+                         deleted: Option<&[u64]>, algorithm: SearchAlgorithm) -> Vec<Vec<ScoredPointOffset>> {
+        let n_queries = query_offsets.len().saturating_sub(1);
+        let mut out = vec![qb_scored_point::default(); n_queries * top];
+        let mut counts = vec![0u32; n_queries];
+        let algo = match algorithm { SearchAlgorithm::Hnsw => QB_HNSW_ALGO_HNSW, SearchAlgorithm::Acorn => QB_HNSW_ALGO_ACORN };
+        let st = unsafe {
+            qb_hnsw_search_maxsim_batch(self.raw, query_vectors.as_ptr(), query_offsets.as_ptr(), n_queries as u32, top as u32, ef as u32, entry.0,
+                                        entry.1 as u32, deleted.map_or(std::ptr::null(), |d| d.as_ptr()), std::ptr::null(), out.as_mut_ptr(),
+                                        counts.as_mut_ptr(), std::ptr::null_mut(), algo)
         };
         assert!(st == QB_OK, "{}", last_error());
         (0..n_queries).map(|q| out[q * top..q * top + counts[q] as usize].iter().map(|p| ScoredPointOffset { idx: p.idx, score: p.score }).collect()).collect()

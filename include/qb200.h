@@ -467,6 +467,45 @@ QB_API qb_status qb_hnsw_search_with_vectors_batch(qb_hnsw* g, const float* quer
 QB_API qb_status qb_hnsw_search_with_vectors_batch_device(qb_hnsw* g, const float* dev_queries, uint32_t n_queries, uint32_t top, uint32_t ef,
                                                           uint32_t entry_point, uint32_t entry_level, qb_scored_point* dev_out, uint32_t* dev_counts);
 
+/* A graph over the POINTS of a multivector collection whose token rows live in `tokens` (dense f32 or SQ8; others:
+ * QB_ERR_UNSUPPORTED).  point p = token rows [point_offsets[p], point_offsets[p+1]) — the layout of qb_search_maxsim; the offsets
+ * must ascend and end at or before the storage's count (QB_ERR_INVALID).  The graph's point count must equal n_points
+ * (QB_ERR_INVALID otherwise).  The offsets are copied to the device (4 * (n_points + 1) bytes, in qb_hnsw_info's total).  The files
+ * are read and checked as qb_hnsw_create_plain / qb_hnsw_create_compressed read them; CompressedWithVectors: QB_ERR_UNSUPPORTED.
+ * This is the graph the reference builds for a multivector named vector with an HNSW index (a links.bin like any other), searched
+ * through GraphLayers::search with MultiMetricQueryScorer (query_scorer/multi_metric_query_scorer.rs) for dense tokens and
+ * QuantizedMultivectorStorage::score_point_max_similarity (quantized/quantized_multivector_storage/mod.rs:328-352) for SQ8 tokens.
+ * qb_hnsw_links, qb_hnsw_export_plain, qb_hnsw_info, qb_hnsw_stats and qb_hnsw_destroy work on the handle; the single-vector searches
+ * (qb_hnsw_search_batch*, _custom_, _discover_, _with_vectors_) return QB_ERR_UNSUPPORTED.  Synchronous. */
+QB_API qb_status qb_hnsw_create_plain_multivector(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, const uint8_t* links_bin,
+                                                  uint64_t n_bytes, uint32_t m, uint32_t m0, qb_hnsw** out);
+QB_API qb_status qb_hnsw_create_compressed_multivector(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, const uint8_t* bytes,
+                                                       uint64_t n_bytes, qb_hnsw** out);
+/* GraphLayers::search (graph_layers.rs:530-561) with a MaxSim FilteredScorer, for a batch of multivector queries, on a
+ * qb_hnsw_create_*_multivector handle (QB_ERR_UNSUPPORTED on any other).  Replaces the per-hop qb_score_maxsim boundary.
+ *   query i         rows [query_offsets[i], query_offsets[i+1]) of query_vectors (raw f32 x dim), 1..4096 vectors each
+ *   deleted_points  optional bitmap over POINTS, ceil(n_points / 64) words, as qb_search_maxsim takes it; a point that fails it is
+ *                   neither scored nor traversed.  The token storage's resident deleted flags are per token row and do not apply.
+ *   out             point offsets 0 .. n_points - 1 (the numbering of qb_search_maxsim), descending
+ * The other arguments and the traversal are qb_hnsw_search_batch_algo's (max(ef, top), ef <= 4096, keyed ties, is_stopped).
+ * A point's score equals qb_score_maxsim on that point bit for bit: each query vector prepared as a plain query, every (vector,
+ * token) similarity by the storage's chain, per vector the sequential `sim > max` fold over the point's tokens from -inf (NaN
+ * never wins, the earlier of -0.0 / +0.0 keeps its bits, an empty run stays -inf), the maxima summed in vector order from +0.0.
+ * (For SQ8 tokens the reference sums with Iterator::sum, which starts from -0.0: the two differ only when every maximum is -0.0.)
+ * Counters: cpu += query vectors x token rows x the storage's per-vector units per scored point (dim * 4 for f32, dim for SQ8),
+ * vector_io_read += token rows x the row size on disk.  qb_hnsw_stats counts hops and scored points (points, not token rows). */
+QB_API qb_status qb_hnsw_search_maxsim_batch(qb_hnsw* g, const float* query_vectors, const uint32_t* query_offsets, uint32_t n_queries, uint32_t top,
+                                             uint32_t ef, uint32_t entry_point, uint32_t entry_level, const uint64_t* deleted_points,
+                                             const volatile int32_t* is_stopped, qb_scored_point* out, uint32_t* out_counts,
+                                             qb_hw_counters* counters /* optional */, qb_hnsw_algorithm algorithm);
+/* same with query vectors (n_query_vectors x dim), offsets (n_queries + 1) and outputs resident in HBM, enqueued on
+ * qb_storage_stream(tokens), no host synchronisation and no filter.  max_query_vectors (1..4096) bounds the largest query's vector
+ * count; it sizes the shared-memory staging of the query vectors only (a larger query is read from HBM, with the same results).
+ * Offsets beyond n_query_vectors are clamped to it. */
+QB_API qb_status qb_hnsw_search_maxsim_batch_device(qb_hnsw* g, const float* dev_query_vectors, uint32_t n_query_vectors, const uint32_t* dev_query_offsets,
+                                                    uint32_t n_queries, uint32_t max_query_vectors, uint32_t top, uint32_t ef, uint32_t entry_point,
+                                                    uint32_t entry_level, qb_scored_point* dev_out, uint32_t* dev_counts, qb_hnsw_algorithm algorithm);
+
 /* Custom queries (recommend, context, feedback) through the device traversal: GraphLayers::search with a custom FilteredScorer
  * (hnsw/read_view/search.rs:181-208).  A point's score is qb_score_points on a qb_scorer_create_custom / qb_scorer_create_feedback
  * scorer of the same examples, bit for bit.

@@ -1806,6 +1806,105 @@ extern "C" qb_status qb_hnsw_search_with_vectors_batch_device(qb_hnsw* g, const 
     return QB_OK;
 }
 
+// GraphLayers::search with a MaxSim FilteredScorer on a graph over multivector points (qb_hnsw_create_*_multivector).  Counters as the
+// reference meters MultiMetricQueryScorer (multi_metric_query_scorer.rs:37-79,102-113): cpu += query vectors x token rows x the storage's
+// per-vector units for every scored point (SQ8: the units qb_search_maxsim uses), vector_io_read += token rows x io units on disk.
+extern "C" qb_status qb_hnsw_search_maxsim_batch(qb_hnsw* g, const float* query_vectors, const uint32_t* query_offsets, uint32_t n_queries, uint32_t top,
+                                                 uint32_t ef, uint32_t entry_point, uint32_t entry_level, const uint64_t* deleted_points,
+                                                 const volatile int32_t* is_stopped, qb_scored_point* out, uint32_t* out_counts, qb_hw_counters* counters,
+                                                 qb_hnsw_algorithm algorithm) {
+    QB_CHECK(g && out && out_counts, QB_ERR_INVALID, "hnsw_search_maxsim_batch: null argument");
+    QB_CHECK(n_queries == 0 || (query_vectors && query_offsets), QB_ERR_INVALID, "hnsw_search_maxsim_batch: null queries");
+    QB_CHECK(top >= 1 && top <= 4096, QB_ERR_INVALID, "hnsw_search_maxsim_batch: top %u outside [1,4096]", top);
+    QB_CHECK(g->d_mv_tok, QB_ERR_UNSUPPORTED, "hnsw_search_maxsim_batch: the graph is not over multivector points (load it with qb_hnsw_create_*_multivector)");
+    if (n_queries == 0) return QB_OK;
+    uint32_t max_q = 0;
+    for (uint32_t i = 0; i < n_queries; ++i) {
+        QB_CHECK(query_offsets[i] <= query_offsets[i + 1], QB_ERR_INVALID, "hnsw_search_maxsim_batch: query_offsets not ascending at %u", i);
+        const uint32_t nqv = query_offsets[i + 1] - query_offsets[i];
+        QB_CHECK(nqv >= 1 && nqv <= 4096, QB_ERR_INVALID, "hnsw_search_maxsim_batch: query %u has %u vectors (need 1..4096)", i, nqv);
+        max_q = std::max(max_q, nqv);
+    }
+    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    qb_storage* s = g->st;
+    QB_TRY(use_device(s->device));
+    std::lock_guard<std::mutex> glk(g->mu);
+    QbSearchCtx* c = nullptr;
+    QB_TRY(qb_ctx_acquire(s, &c));
+    struct Rel { qb_storage* s; QbSearchCtx* c; ~Rel() { qb_ctx_release(s, c); } } rel{s, c};
+    cudaStream_t stream = c->stream;
+    const uint32_t nv = query_offsets[n_queries];   // vectors before query_offsets[0] are uploaded and not read
+    const size_t raw_bytes = (size_t)nv * s->dim * 4, res_bytes = (size_t)n_queries * top * sizeof(qb_scored_point), cnt_bytes = (size_t)n_queries * 4;
+    const size_t off_bytes = ((size_t)n_queries + 1) * 4;
+    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, raw_bytes + off_bytes + res_bytes + cnt_bytes + 16));
+    uint8_t* hs = reinterpret_cast<uint8_t*>(c->h_stage);
+    memcpy(hs, query_vectors, raw_bytes);
+    memcpy(hs + raw_bytes, query_offsets, off_bytes);
+    uint8_t* h_res = hs + raw_bytes + off_bytes;
+    const size_t pre_off = round_up_u64(raw_bytes, 16);
+    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, pre_off + (size_t)nv * pre_stride_f(s) * 4));
+    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)nv + 256) * qb_encoded_query_bytes(s)));
+    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)nv));
+    QB_TRY(ensure_dev_elems(&c->d_ids, &c->ids_elems, (size_t)n_queries + 1));
+    QB_TRY(ensure_dev_elems(&c->d_out, &c->out_elems, (size_t)n_queries * top));
+    QB_TRY(ensure_dev_elems(&c->d_out_counts, &c->out_counts_elems, (size_t)n_queries + 4));
+    QB_CUDA(cudaMemcpyAsync(c->d_queries_raw, hs, raw_bytes, cudaMemcpyHostToDevice, stream));
+    QB_CUDA(cudaMemcpyAsync(c->d_ids, hs + raw_bytes, off_bytes, cudaMemcpyHostToDevice, stream));
+    float* d_pre = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c->d_queries_raw) + pre_off);
+    QB_TRY(prepare_queries(s, reinterpret_cast<const float*>(c->d_queries_raw), nv, d_pre, c->d_queries_enc, c->d_q_off, stream));
+    const uint32_t* d_del2 = nullptr;
+    if (deleted_points) {
+        const uint64_t words64 = ceil_div_u64(g->n_points, 64);   // a bitmap over points, as qb_search_maxsim takes it
+        QB_TRY(ensure_dev_elems(&c->d_deleted2, &c->deleted2_words, (size_t)words64 * 2));
+        QB_CUDA(cudaMemcpyAsync(c->d_deleted2, deleted_points, words64 * 8, cudaMemcpyHostToDevice, stream));
+        d_del2 = c->d_deleted2;
+    }
+    const QbHnswMaxsim mv{c->d_ids, nv, max_q};
+    QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, d_del2, c->d_out, c->d_out_counts, stream,
+                          (int)algorithm, nullptr, &mv));
+    QB_CUDA(cudaMemcpyAsync(h_res, c->d_out, res_bytes, cudaMemcpyDeviceToHost, stream));
+    QB_CUDA(cudaMemcpyAsync(h_res + res_bytes, c->d_out_counts, cnt_bytes, cudaMemcpyDeviceToHost, stream));
+    QB_CUDA(cudaStreamSynchronize(stream));
+    memcpy(out, h_res, res_bytes);
+    memcpy(out_counts, h_res + res_bytes, cnt_bytes);
+    if (counters) {
+        const uint64_t rows0 = g->mv_rows, qrows0 = g->mv_qrows;
+        QB_TRY(qb_hnsw_read_stats(g, stream));
+        counters->cpu += (g->mv_qrows - qrows0) * cpu_units_per_point(s);
+        counters->vector_io_read += (g->mv_rows - rows0) * io_units_per_point(s);
+    }
+    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    return QB_OK;
+}
+
+extern "C" qb_status qb_hnsw_search_maxsim_batch_device(qb_hnsw* g, const float* dev_query_vectors, uint32_t n_query_vectors, const uint32_t* dev_query_offsets,
+                                                        uint32_t n_queries, uint32_t max_query_vectors, uint32_t top, uint32_t ef, uint32_t entry_point,
+                                                        uint32_t entry_level, qb_scored_point* dev_out, uint32_t* dev_counts, qb_hnsw_algorithm algorithm) {
+    QB_CHECK(g && dev_query_vectors && dev_query_offsets && dev_out && dev_counts, QB_ERR_INVALID, "hnsw_search_maxsim_batch_device: null argument");
+    QB_CHECK(top >= 1 && top <= 4096, QB_ERR_INVALID, "hnsw_search_maxsim_batch_device: top %u outside [1,4096]", top);
+    QB_CHECK(max_query_vectors >= 1 && max_query_vectors <= 4096, QB_ERR_INVALID, "hnsw_search_maxsim_batch_device: max_query_vectors %u outside [1,4096]",
+             max_query_vectors);
+    QB_CHECK(g->d_mv_tok, QB_ERR_UNSUPPORTED,
+             "hnsw_search_maxsim_batch_device: the graph is not over multivector points (load it with qb_hnsw_create_*_multivector)");
+    if (n_queries == 0) return QB_OK;
+    qb_storage* s = g->st;
+    QB_TRY(use_device(s->device));
+    std::lock_guard<std::mutex> glk(g->mu);
+    QbSearchCtx* c = nullptr;
+    QB_TRY(qb_ctx_device(s, &c));
+    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, (size_t)n_query_vectors * pre_stride_f(s) * 4 + 256));
+    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)n_query_vectors + 256) * qb_encoded_query_bytes(s)));
+    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)n_query_vectors));
+    QB_TRY(prepare_queries(s, dev_query_vectors, n_query_vectors, reinterpret_cast<float*>(c->d_queries_raw), c->d_queries_enc, c->d_q_off, c->stream));
+    cudaEvent_t e0, e1;
+    profile_begin(s, c, c->stream, &e0, &e1);
+    const QbHnswMaxsim mv{dev_query_offsets, n_query_vectors, max_query_vectors};
+    QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, nullptr, dev_out, dev_counts, c->stream,
+                          (int)algorithm, nullptr, &mv));
+    profile_end(s, c->stream, e0, e1);
+    return QB_OK;
+}
+
 // custom queries through the device traversal; discover_pairs > 0: the two-stage discover of that many pairs (kind = DISCOVER)
 static qb_status hnsw_custom_run(qb_hnsw* g, qb_query_kind kind, const float* vectors, uint32_t n_a, uint32_t n_b, const float* coef, uint32_t n_queries,
                                  uint32_t top, uint32_t ef, uint32_t entry_point, uint32_t entry_level, const uint32_t* cep, const uint32_t* cep_counts,

@@ -54,7 +54,9 @@ __global__ void hnsw_links0_kernel(const uint32_t* __restrict__ neighbors, const
     }
 }
 
-extern "C" qb_status qb_hnsw_create_plain(qb_storage* s, const uint8_t* links_bin, uint64_t n_bytes, uint32_t m, uint32_t m0, qb_hnsw** out) {
+// a plain links.bin over `expect` points: the storage's rows, or the points of a multivector collection (`of` names which)
+static qb_status hnsw_create_plain_n(qb_storage* s, uint64_t expect, const char* of, const uint8_t* links_bin, uint64_t n_bytes, uint32_t m, uint32_t m0,
+                                     qb_hnsw** out) {
     QB_CHECK(s && links_bin && out, QB_ERR_INVALID, "hnsw_create_plain: null argument");
     *out = nullptr;
     QB_CHECK(m >= 1 && m0 >= 1 && m0 <= HNSW_MAX_LINKS && m <= HNSW_MAX_LINKS, QB_ERR_UNSUPPORTED, "hnsw_create_plain: m %u / m0 %u outside [1,%u]", m, m0, HNSW_MAX_LINKS);
@@ -62,7 +64,7 @@ extern "C" qb_status qb_hnsw_create_plain(qb_storage* s, const uint8_t* links_bi
     uint64_t hdr[5];
     memcpy(hdr, links_bin, sizeof(hdr));   // point_count, levels_count, total_neighbors_count, total_offset_count, offsets_padding_bytes
     const uint64_t n = hdr[0], levels = hdr[1], n_nb = hdr[2], n_off = hdr[3], pad = hdr[4];
-    QB_CHECK(n == s->count, QB_ERR_INVALID, "hnsw_create_plain: graph has %llu points, storage %llu", (unsigned long long)n, (unsigned long long)s->count);
+    QB_CHECK(n == expect, QB_ERR_INVALID, "hnsw_create_plain: graph has %llu points, %s %llu", (unsigned long long)n, of, (unsigned long long)expect);
     QB_CHECK(pad == 0 || pad == 4, QB_ERR_INVALID, "hnsw_create_plain: offsets padding %llu", (unsigned long long)pad);
     QB_CHECK(levels <= 64 && n_off >= n + 1, QB_ERR_INVALID, "hnsw_create_plain: bad header (levels %llu, offsets %llu)", (unsigned long long)levels, (unsigned long long)n_off);
     const uint64_t need = 64 + 8 * levels + 4 * n + 4 * n_nb + pad + 8 * n_off;
@@ -96,6 +98,10 @@ extern "C" qb_status qb_hnsw_create_plain(qb_storage* s, const uint8_t* links_bi
     if (st != QB_OK) { qb_hnsw_destroy(g); return st; }
     *out = g;
     return QB_OK;
+}
+
+extern "C" qb_status qb_hnsw_create_plain(qb_storage* s, const uint8_t* links_bin, uint64_t n_bytes, uint32_t m, uint32_t m0, qb_hnsw** out) {
+    return hnsw_create_plain_n(s, s ? s->count : 0, "storage", links_bin, n_bytes, m, m0, out);
 }
 
 // the rest of a handle whose plain arrays are on the device (qb_hnsw_create_plain's upload, qb_hnsw_build's finish): the level-0 table
@@ -289,7 +295,8 @@ inline unsigned hc_grid(uint64_t items, uint64_t per_block, uint64_t max_blocks)
 
 }  // namespace
 
-extern "C" qb_status qb_hnsw_create_compressed(qb_storage* s, const uint8_t* bytes, uint64_t n_bytes, qb_hnsw** out) {
+// a compressed links.bin over `expect` points, as hnsw_create_plain_n
+static qb_status hnsw_create_compressed_n(qb_storage* s, uint64_t expect, const char* of, const uint8_t* bytes, uint64_t n_bytes, qb_hnsw** out) {
     QB_CHECK(s && bytes && out, QB_ERR_INVALID, "hnsw_create_compressed: null argument");
     *out = nullptr;
     QB_CHECK(n_bytes >= 64, QB_ERR_INVALID, "hnsw_create_compressed: %llu bytes is smaller than HeaderCompressed", (unsigned long long)n_bytes);
@@ -301,7 +308,7 @@ extern "C" qb_status qb_hnsw_create_compressed(qb_storage* s, const uint8_t* byt
              "(graph_layers.rs:336-388), a different algorithm; this loader takes GraphLinksFormat::Compressed");
     QB_CHECK(version == HNSW_VERSION_COMPRESSED, QB_ERR_INVALID, "hnsw_create_compressed: version word %016llx is not HEADER_VERSION_COMPRESSED (a plain links.bin?)",
              (unsigned long long)version);
-    QB_CHECK(n == s->count, QB_ERR_INVALID, "hnsw_create_compressed: graph has %llu points, storage %llu", (unsigned long long)n, (unsigned long long)s->count);
+    QB_CHECK(n == expect, QB_ERR_INVALID, "hnsw_create_compressed: graph has %llu points, %s %llu", (unsigned long long)n, of, (unsigned long long)expect);
     QB_CHECK(n <= 0xFFFFFFFFull, QB_ERR_INVALID, "hnsw_create_compressed: %llu points", (unsigned long long)n);
     QB_CHECK(m >= 1 && m0 >= 1, QB_ERR_INVALID, "hnsw_create_compressed: m %llu / m0 %llu", (unsigned long long)m, (unsigned long long)m0);
     QB_CHECK(m <= HNSW_MAX_LINKS && m0 <= HNSW_MAX_LINKS, QB_ERR_UNSUPPORTED, "hnsw_create_compressed: m %llu / m0 %llu outside [1,%u]", (unsigned long long)m,
@@ -397,6 +404,63 @@ extern "C" qb_status qb_hnsw_create_compressed(qb_storage* s, const uint8_t* byt
     ce = cudaDeviceSynchronize();
     if (ce == cudaSuccess) ce = cudaGetLastError();
     if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "decode", ce);
+    *out = g;
+    return QB_OK;
+}
+
+extern "C" qb_status qb_hnsw_create_compressed(qb_storage* s, const uint8_t* bytes, uint64_t n_bytes, qb_hnsw** out) {
+    return hnsw_create_compressed_n(s, s ? s->count : 0, "storage", bytes, n_bytes, out);
+}
+
+// ------------------------------------------------------------------------------------------------ graphs over multivector points
+// The graph of a multivector named vector links POINTS; the scorer behind its search is MaxSim over each point's token rows
+// (MultiMetricQueryScorer, multi_metric_query_scorer.rs; QuantizedMultivectorStorage, quantized_multivector_storage/mod.rs:328-352).
+// The loaders are the regular ones with the point count taken from the collection, plus the token offsets on the device.
+static qb_status mv_check(qb_storage* s, const uint32_t* point_offsets, uint32_t n_points, const char* who) {
+    QB_CHECK(s && point_offsets, QB_ERR_INVALID, "%s: null argument", who);
+    QB_CHECK((s->kind == QB_KIND_DENSE && s->dtype == QB_DT_F32) || s->kind == QB_KIND_SQ8, QB_ERR_UNSUPPORTED,
+             "%s: device MaxSim traversal supports dense f32 and SQ8 token storages", who);
+    // the checks qb_search_maxsim makes (maxsim_run)
+    for (uint32_t p = 0; p < n_points; ++p) QB_CHECK(point_offsets[p] <= point_offsets[p + 1], QB_ERR_INVALID, "%s: point_offsets not ascending at %u", who, p);
+    QB_CHECK(point_offsets[n_points] <= s->count, QB_ERR_INVALID, "%s: point_offsets end %u beyond the %llu stored vectors", who, point_offsets[n_points],
+             (unsigned long long)s->count);
+    return QB_OK;
+}
+
+static qb_status mv_attach(qb_hnsw* g, const uint32_t* point_offsets, uint32_t n_points, const char* who) {
+    const size_t bytes = 4ull * ((size_t)n_points + 1);
+    cudaError_t ce = cudaMalloc(&g->d_mv_tok, bytes);
+    if (ce == cudaSuccess) ce = cudaMemcpy(g->d_mv_tok, point_offsets, bytes, cudaMemcpyHostToDevice);
+    if (ce != cudaSuccess) {
+        qb_set_error("%s: offsets upload: %s", who, cudaGetErrorString(ce));
+        return ce == cudaErrorMemoryAllocation ? QB_ERR_OOM : QB_ERR_CUDA;
+    }
+    g->hbm_bytes += bytes;
+    return QB_OK;
+}
+
+extern "C" qb_status qb_hnsw_create_plain_multivector(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, const uint8_t* links_bin,
+                                                      uint64_t n_bytes, uint32_t m, uint32_t m0, qb_hnsw** out) {
+    QB_CHECK(out, QB_ERR_INVALID, "hnsw_create_plain_multivector: null argument");
+    *out = nullptr;
+    QB_TRY(mv_check(tokens, point_offsets, n_points, "hnsw_create_plain_multivector"));
+    qb_hnsw* g = nullptr;
+    QB_TRY(hnsw_create_plain_n(tokens, n_points, "collection", links_bin, n_bytes, m, m0, &g));
+    const qb_status st = mv_attach(g, point_offsets, n_points, "hnsw_create_plain_multivector");
+    if (st != QB_OK) { qb_hnsw_destroy(g); return st; }
+    *out = g;
+    return QB_OK;
+}
+
+extern "C" qb_status qb_hnsw_create_compressed_multivector(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, const uint8_t* bytes,
+                                                           uint64_t n_bytes, qb_hnsw** out) {
+    QB_CHECK(out, QB_ERR_INVALID, "hnsw_create_compressed_multivector: null argument");
+    *out = nullptr;
+    QB_TRY(mv_check(tokens, point_offsets, n_points, "hnsw_create_compressed_multivector"));
+    qb_hnsw* g = nullptr;
+    QB_TRY(hnsw_create_compressed_n(tokens, n_points, "collection", bytes, n_bytes, &g));
+    const qb_status st = mv_attach(g, point_offsets, n_points, "hnsw_create_compressed_multivector");
+    if (st != QB_OK) { qb_hnsw_destroy(g); return st; }
     *out = g;
     return QB_OK;
 }
@@ -647,7 +711,7 @@ extern "C" void qb_hnsw_destroy(qb_hnsw* g) {
     cudaDeviceSynchronize();
     cudaFree(g->d_links0); cudaFree(g->d_level_offsets); cudaFree(g->d_reindex); cudaFree(g->d_neighbors); cudaFree(g->d_offsets);
     cudaFree(g->d_visited); cudaFree(g->d_vlog); cudaFree(g->d_work); cudaFree(g->d_stats);
-    cudaFree(g->d_blob); cudaFree(g->d_lvoff); cudaFree(g->d_boff);
+    cudaFree(g->d_blob); cudaFree(g->d_lvoff); cudaFree(g->d_boff); cudaFree(g->d_mv_tok);
     cudaGetLastError();
     delete g;
 }
@@ -662,8 +726,12 @@ extern "C" qb_status qb_hnsw_info(const qb_hnsw* g, uint32_t* n_points, uint32_t
 
 // queries already encoded (d_q_enc / d_q_off); results to device buffers; enqueued on `stream`, no synchronisation
 qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, uint32_t nq, uint32_t top, uint32_t ef, uint32_t entry, uint32_t entry_level,
-                         const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts, cudaStream_t stream, int algo, const QbHnswCustom* custom) {
+                         const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts, cudaStream_t stream, int algo, const QbHnswCustom* custom,
+                         const QbHnswMaxsim* maxsim) {
     qb_storage* s = g->st;
+    QB_CHECK(!maxsim == !g->d_mv_tok, QB_ERR_UNSUPPORTED,
+             maxsim ? "hnsw_search_maxsim: the graph is not over multivector points (load it with qb_hnsw_create_*_multivector)"
+                    : "hnsw_search: the graph is over multivector points; search it with qb_hnsw_search_maxsim_batch");
     QB_CHECK(algo == ALGO_HNSW || algo == ALGO_ACORN, QB_ERR_INVALID, "hnsw_search: algorithm %d is neither QB_HNSW_ALGO_HNSW nor QB_HNSW_ALGO_ACORN", algo);
     QB_CHECK(entry < g->n_points, QB_ERR_INVALID, "hnsw_search: entry point %u out of range", entry);
     QB_CHECK(entry_level < std::max<uint32_t>(g->levels, 1), QB_ERR_INVALID, "hnsw_search: entry level %u but the graph has %u levels", entry_level, g->levels);
@@ -701,14 +769,26 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
         q_smem = p.ex_smem ? (uint32_t)ex_bytes : 0u;
         p.q_smem = q_smem;
     }
+    if (maxsim) {
+        // points are numbered 0 .. n_points - 1 and filtered by the per-call bitmap over points only: the token storage's resident flags
+        // are per token row
+        p.deleted = nullptr; p.id_base = 0;
+        mv_tok(p) = g->d_mv_tok; mv_qoff(p) = maxsim->d_qoff; mv_nv(p) = maxsim->n_vectors;
+        // a query's vectors are staged in shared memory when the largest query's fit in HNSW_CUSTOM_SMEM, as custom examples are
+        mv_stage_q(p) = (uint64_t)maxsim->max_q * p.q_bytes <= HNSW_CUSTOM_SMEM ? maxsim->max_q : 0u;
+        q_smem = mv_stage_q(p) * p.q_bytes;
+        p.q_smem = q_smem;
+        p.stats = g->d_stats + 8;
+    }
     const size_t smem = acorn ? acorn_smem_bytes(q_smem, ef, p.hop_cap) : hnsw_smem_bytes(q_smem, ef);
     QB_CHECK(smem <= 200 * 1024, QB_ERR_UNSUPPORTED, "hnsw_search: query (%u B) + ef %u need %zu B of shared memory", q_smem, ef, smem);
     // threads per CTA: 256 = one 8-lane group per level-0 link (m0 = 32), fewer queries in flight per SM; 128 (default) = two scoring rounds
     // per hop, twice the resident queries.  The traversal is a chain of dependent memory round trips, so queries in flight is what hides them.
-    // Custom queries are instantiated for 128 threads only.
-    const int nt = custom ? 128 : (qb_opt().hnsw_threads == 256 ? 256 : (qb_opt().hnsw_threads == 64 ? 64 : 128));
-    const int per_sm = custom ? (acorn ? occupancy_dispatch<128, ALGO_ACORN, 1>(kind, metric, smem) : occupancy_dispatch<128, ALGO_HNSW, 1>(kind, metric, smem))
-                              : (acorn ? occupancy_nt<ALGO_ACORN>(nt, kind, metric, smem) : occupancy_nt<ALGO_HNSW>(nt, kind, metric, smem));
+    // Custom and MaxSim queries are instantiated for 128 threads only.
+    const int nt = (custom || maxsim) ? 128 : (qb_opt().hnsw_threads == 256 ? 256 : (qb_opt().hnsw_threads == 64 ? 64 : 128));
+    const int per_sm = maxsim ? (acorn ? occupancy_dispatch<128, ALGO_ACORN, HC_MAXSIM>(kind, metric, smem) : occupancy_dispatch<128, ALGO_HNSW, HC_MAXSIM>(kind, metric, smem))
+                       : custom ? (acorn ? occupancy_dispatch<128, ALGO_ACORN, 1>(kind, metric, smem) : occupancy_dispatch<128, ALGO_HNSW, 1>(kind, metric, smem))
+                                : (acorn ? occupancy_nt<ALGO_ACORN>(nt, kind, metric, smem) : occupancy_nt<ALGO_HNSW>(nt, kind, metric, smem));
     p.prefetch = qb_opt().hnsw_no_prefetch ? 0 : 1;
     const unsigned max_grid = (unsigned)s->sm_count * (unsigned)per_sm;
     const unsigned grid = std::min<unsigned>(max_grid, nq);
@@ -724,17 +804,21 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
     }
     p.visited = g->d_visited; p.visited_words = words; p.vlog = g->d_vlog; p.vlog_cap = g->vlog_cap; p.work = g->d_work;
     QB_CUDA(cudaMemsetAsync(g->d_work, 0, 4, stream));
+    if (maxsim)
+        return acorn ? launch_dispatch<128, ALGO_ACORN, HC_MAXSIM>(kind, metric, p, grid, smem, stream)
+                     : launch_dispatch<128, ALGO_HNSW, HC_MAXSIM>(kind, metric, p, grid, smem, stream);
     if (custom)
         return acorn ? launch_dispatch<128, ALGO_ACORN, 1>(kind, metric, p, grid, smem, stream) : launch_dispatch<128, ALGO_HNSW, 1>(kind, metric, p, grid, smem, stream);
     return acorn ? launch_nt<ALGO_ACORN>(nt, kind, metric, p, grid, smem, stream) : launch_nt<ALGO_HNSW>(nt, kind, metric, p, grid, smem, stream);
 }
 
 qb_status qb_hnsw_read_stats(qb_hnsw* g, cudaStream_t stream, uint64_t* evals_by_slot) {
-    unsigned long long h[7] = {0, 0, 0, 0, 0, 0, 0};
-    QB_CUDA(cudaMemcpyAsync(h, g->d_stats, 56, cudaMemcpyDeviceToHost, stream));
+    unsigned long long h[12] = {};
+    QB_CUDA(cudaMemcpyAsync(h, g->d_stats, sizeof(h), cudaMemcpyDeviceToHost, stream));
     QB_CUDA(cudaStreamSynchronize(stream));
-    QB_CUDA(cudaMemsetAsync(g->d_stats, 0, 56, stream));
-    g->hops += h[0] + h[2] + h[4]; g->evals += h[1] + h[3] + h[5]; g->base_evals += h[6];
+    QB_CUDA(cudaMemsetAsync(g->d_stats, 0, sizeof(h), stream));
+    g->hops += h[0] + h[2] + h[4] + h[8]; g->evals += h[1] + h[3] + h[5] + h[9]; g->base_evals += h[6];
+    g->mv_rows += h[10]; g->mv_qrows += h[11];
     if (evals_by_slot) { evals_by_slot[0] = h[1]; evals_by_slot[1] = h[3]; }
     return QB_OK;
 }

@@ -65,6 +65,18 @@ struct HnswParams {
     const uint32_t* b_pts; uint32_t* b_entry; const uint32_t* b_remap; uint32_t b_insert;
     unsigned long long* b_tkey; uint32_t* b_tval;
 };
+// Multivector MaxSim queries (CUSTOM == HC_MAXSIM) reuse fields that only graph builds and custom queries read, so HnswParams, and with it
+// the code of every other instantiation, stays as it was.  Point p = token rows mv_tok(p)[p] .. [p + 1) of the storage; query q = encoded
+// query vectors mv_qoff(p)[q] .. [q + 1) of q_enc / q_off, clamped to mv_nv(p); a query of at most mv_stage_q(p) vectors is staged in
+// shared memory (q_smem bytes), a larger one is read where it is.
+__host__ __device__ __forceinline__ const uint32_t*& mv_tok(HnswParams& p) { return p.b_pts; }
+__host__ __device__ __forceinline__ const uint32_t*& mv_qoff(HnswParams& p) { return p.b_remap; }
+__host__ __device__ __forceinline__ uint32_t& mv_nv(HnswParams& p) { return p.n_ex; }
+__host__ __device__ __forceinline__ uint32_t& mv_stage_q(HnswParams& p) { return p.ex_smem; }
+__device__ __forceinline__ const uint32_t* mv_tok(const HnswParams& p) { return p.b_pts; }
+__device__ __forceinline__ const uint32_t* mv_qoff(const HnswParams& p) { return p.b_remap; }
+__device__ __forceinline__ uint32_t mv_nv(const HnswParams& p) { return p.n_ex; }
+__device__ __forceinline__ uint32_t mv_stage_q(const HnswParams& p) { return p.ex_smem; }
 
 struct HnswSmem {
     unsigned long long* keys[2];
@@ -76,6 +88,7 @@ struct HnswSmem {
 };
 
 enum { ALGO_HNSW = 0, ALGO_ACORN = 1 };   // qb_hnsw_algorithm
+enum { HC_NEAREST = 0, HC_CUSTOM = 1, HC_MAXSIM = 2 };   // hnsw_search_kernel's CUSTOM: what a query is
 enum { ALGO_BUILD = 2 };                  // an insert of qb_hnsw_build: HNSW level search of a stored point, then its links (qb_hnsw_build.cu)
 
 // ALGO_BUILD: a point's row in its level's table
@@ -111,12 +124,127 @@ __device__ __forceinline__ float score_q(const HnswParams& p, const HnswSmem& sm
     }
 }
 
+// ---- multivector MaxSim (score_max_similarity, query_scorer/mod.rs:77-98; QuantizedMultivectorStorage::score_point_max_similarity,
+// quantized_multivector_storage/mod.rs:328-352).  A point's score is, summed sequentially in query-vector order from +0.0, the maximum
+// over its token rows of each query vector's similarity, that maximum being the sequential `if sim > max` fold from -inf.  The CTA
+// scores the hop's (point, token row) items in parallel, so the fold is restated as a max over keys (mv_key) that picks exactly the
+// value the sequential fold keeps: NaN and -inf never win, -0.0 and +0.0 are equal and the earlier token keeps its own bits.
+constexpr uint32_t MV_PTS = 64;   // points per scoring batch
+constexpr uint32_t MV_NQ = 8;     // query vectors per chunk (score_avx_group8_multi accumulators)
+
+struct MvShared {
+    unsigned long long key[MV_PTS * MV_NQ];   // [point][query vector of the chunk] max keys, 0 = none (-inf)
+    float sum[MV_PTS];                         // running sums over the chunks
+    uint32_t pre[MV_PTS + 1];                  // token-row prefix of the batch's points
+    uint32_t q0, nqv;                          // the query's first encoded vector and its vector count
+    unsigned long long rows;                   // token rows the query scored (the counters)
+};
+// one per CTA; only the MaxSim instantiations reference it
+__device__ __forceinline__ MvShared& mv_shared() {
+    __shared__ MvShared s;
+    return s;
+}
+
+// (canonical value, earliest token) -> an ordered key, with the winner's sign of zero in bit 0
+__device__ __forceinline__ unsigned long long mv_key(float v, uint32_t tok) {
+    if (!(v > __int_as_float(0xff800000))) return 0ull;
+    const uint32_t b = __float_as_uint(v == 0.0f ? 0.0f : v);
+    const uint32_t ord = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+    const uint32_t neg0 = (v == 0.0f) ? (__float_as_uint(v) >> 31) : 0u;
+    return ((unsigned long long)ord << 32) | ((unsigned long long)(0x7FFFFFFFu - tok) << 1) | neg0;
+}
+__device__ __forceinline__ float mv_value(unsigned long long key) {
+    if (!key) return __int_as_float(0xff800000);
+    if (key & 1ull) return -0.0f;
+    const uint32_t ord = (uint32_t)(key >> 32);
+    return __uint_as_float((ord & 0x80000000u) ? (ord & 0x7FFFFFFFu) : ~ord);
+}
+
+// the batch point whose token rows hold item k: pre[i] <= k < pre[i + 1]
+__device__ __forceinline__ uint32_t mv_find(const uint32_t* pre, uint32_t ns, uint32_t k) {
+    uint32_t lo = 0, hi = ns - 1;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (pre[mid + 1] > k) hi = mid; else lo = mid + 1; }
+    return lo;
+}
+
+// MaxSim scores of the points ids[0 .. n) into sc[0 .. n): batches of MV_PTS points, chunks of MV_NQ query vectors; every (point, token
+// row) item of a batch goes to one 8-lane group (dense small dims: one thread), which scores the row against the chunk's vectors by the
+// storage's own chain and folds each similarity into its (point, vector) key.  One thread per point then adds the chunk's maxima in order.
+template <int KIND, int METRIC, int NT>
+__device__ __forceinline__ void maxsim_list(const HnswParams& p, const HnswSmem& sm, uint32_t n) {
+    constexpr uint32_t GROUPS = NT / 8;
+    MvShared& ms = mv_shared();
+    const int tid = threadIdx.x;
+    const uint32_t nqv = ms.nqv;
+    const float* qoff = p.q_off ? p.q_off + ms.q0 : nullptr;
+    for (uint32_t s0 = 0; s0 < n; s0 += MV_PTS) {
+        const uint32_t ns = min(n - s0, MV_PTS);
+        if ((uint32_t)tid < ns) {
+            const uint32_t id = sm.ids[s0 + tid];
+            ms.pre[tid + 1] = mv_tok(p)[id + 1] - mv_tok(p)[id];
+            ms.sum[tid] = 0.0f;
+        }
+        __syncthreads();
+        if (tid == 0) {
+            ms.pre[0] = 0;
+            for (uint32_t i = 0; i < ns; ++i) ms.pre[i + 1] += ms.pre[i];
+            ms.rows += ms.pre[ns];
+        }
+        __syncthreads();
+        const uint32_t items = ms.pre[ns];
+        for (uint32_t c0 = 0; c0 < nqv; c0 += MV_NQ) {
+            const uint32_t nc = min(nqv - c0, MV_NQ);
+            for (uint32_t i = tid; i < ns * MV_NQ; i += NT) ms.key[i] = 0ull;
+            __syncthreads();
+            const uint8_t* qc = sm.q + (size_t)c0 * p.q_bytes;
+            if (KIND == HK_DENSE_SMALL) {
+                for (uint32_t k = tid; k < items; k += NT) {
+                    const uint32_t i = mv_find(ms.pre, ns, k), tok = k - ms.pre[i], row = mv_tok(p)[sm.ids[s0 + i]] + tok;
+                    for (uint32_t j = 0; j < nc; ++j)
+                        atomicMax(&ms.key[i * MV_NQ + j], mv_key(score_one<KIND, METRIC>(p, qc + (size_t)j * p.q_bytes, 0.0f, row, 0), tok));
+                }
+            } else {
+                const int g = tid >> 3, t = tid & 7;
+                for (uint32_t k = g; k < ((items + GROUPS - 1) / GROUPS) * GROUPS; k += GROUPS) {   // whole warps stay converged for the shuffles
+                    const uint32_t kk = k < items ? k : 0;
+                    const uint32_t i = mv_find(ms.pre, ns, kk), tok = kk - ms.pre[i], row = mv_tok(p)[sm.ids[s0 + i]] + tok;
+                    float v[MV_NQ];
+                    if (KIND == HK_DENSE_AVX && nc == MV_NQ) {
+                        score_avx_group8_multi<METRIC, MV_NQ>(reinterpret_cast<const float*>(p.rows + (size_t)row * p.stride), reinterpret_cast<const float*>(qc),
+                                                              p.q_bytes / 4, p.dim, t, v);
+                    } else {
+#pragma unroll
+                        for (uint32_t j = 0; j < MV_NQ; ++j)
+                            if (j < nc) v[j] = score_one<KIND, METRIC>(p, qc + (size_t)j * p.q_bytes, qoff ? qoff[c0 + j] : 0.0f, row, t);
+                    }
+                    if (k < items && t == 0) {
+#pragma unroll
+                        for (uint32_t j = 0; j < MV_NQ; ++j)
+                            if (j < nc) atomicMax(&ms.key[i * MV_NQ + j], mv_key(v[j], tok));
+                    }
+                }
+            }
+            __syncthreads();
+            if ((uint32_t)tid < ns) {
+                float s = ms.sum[tid];
+                for (uint32_t j = 0; j < nc; ++j) s = __fadd_rn(s, mv_value(ms.key[tid * MV_NQ + j]));
+                ms.sum[tid] = s;
+            }
+            __syncthreads();
+        }
+        if ((uint32_t)tid < ns) sm.sc[s0 + tid] = ms.sum[tid];
+        __syncthreads();
+    }
+}
+
 // scores ids[0..n) into sc[0..n): one 8-lane group per id (dense small dims: one thread per id)
 template <int KIND, int METRIC, int NT, int CUSTOM>
 __device__ __forceinline__ void score_list(const HnswParams& p, const HnswSmem& sm, float q_off, uint32_t n, uint32_t q) {
     constexpr int HNSW_GROUPS = NT / 8;
     const int tid = threadIdx.x;
-    if (KIND == HK_DENSE_SMALL) {
+    if constexpr (CUSTOM == HC_MAXSIM) {
+        maxsim_list<KIND, METRIC, NT>(p, sm, n);
+    } else if (KIND == HK_DENSE_SMALL) {
         if ((uint32_t)tid < n) sm.sc[tid] = score_q<KIND, METRIC, CUSTOM>(p, sm, q_off, sm.ids[tid], 0, q);
     } else {
         const int g = tid >> 3, t = tid & 7;
@@ -149,10 +277,19 @@ __device__ __forceinline__ void hnsw_score_rows(const HnswParams& p, const uint8
 __device__ __forceinline__ void prefetch_row_l2(const void* p, uint32_t bytes) {
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
 }
-template <int KIND>
+// MV: a multivector point, whose token rows are consecutive
+template <int KIND, int MV = 0>
 __device__ __forceinline__ void prefetch_point(const HnswParams& p, uint32_t id) {
-    if (KIND == HK_DENSE_AVX || KIND == HK_DENSE_SMALL) prefetch_row_l2(p.rows + (size_t)id * p.stride, p.stride);
-    else prefetch_row_l2(p.codes + (size_t)id * p.ad, p.ad);
+    if constexpr (MV) {
+        const uint32_t r0 = mv_tok(p)[id], r1 = mv_tok(p)[id + 1];
+        if (r1 <= r0) return;
+        if (KIND == HK_DENSE_AVX || KIND == HK_DENSE_SMALL) prefetch_row_l2(p.rows + (size_t)r0 * p.stride, (r1 - r0) * p.stride);
+        else prefetch_row_l2(p.codes + (size_t)r0 * p.ad, (r1 - r0) * p.ad);
+    } else if (KIND == HK_DENSE_AVX || KIND == HK_DENSE_SMALL) {
+        prefetch_row_l2(p.rows + (size_t)id * p.stride, p.stride);
+    } else {
+        prefetch_row_l2(p.codes + (size_t)id * p.ad, p.ad);
+    }
 }
 
 // ScorerFilters::check_vector fails: the resident deleted flags or the per-call bitmap (either may be null); P = HnswParams or the
@@ -204,7 +341,7 @@ __device__ __forceinline__ void hnsw_custom_entry(const HnswParams& p, uint32_t 
 //    filter lookups; here it would cost a second bitmap per CTA and an atomic per filtered-out 2-hop link.
 //  * to_score's order only decides the merge order of distinct keys, which the sorted merge does not depend on.
 // Leaves s_n = |to_score| with the ids in sm.ids, and the marks logged.
-template <int KIND, int NT>
+template <int KIND, int NT, int MV = 0>
 __device__ __forceinline__ void acorn_collect(const HnswParams& p, const HnswSmem& sm, uint32_t* xids, uint32_t cand, uint32_t* visited, uint32_t* vlog,
                                               unsigned int& s_n, unsigned int& s_nx, unsigned int& s_nlog, unsigned int* s_warp_cnt) {
     const int tid = threadIdx.x;
@@ -220,7 +357,7 @@ __device__ __forceinline__ void acorn_collect(const HnswParams& p, const HnswSme
         const uint32_t ps = ((tid >> 5) ? s_warp_cnt[0] : 0u) + __popc(bs & lt);
         const uint32_t px = ((tid >> 5) ? s_warp_cnt[2] : 0u) + __popc(bx & lt);
         if (pass) {
-            if (p.prefetch) prefetch_point<KIND>(p, l);
+            if (p.prefetch) prefetch_point<KIND, MV>(p, l);
             sm.ids[ps] = l;
         } else if (fresh) {
             xids[px] = l;
@@ -244,7 +381,7 @@ __device__ __forceinline__ void acorn_collect(const HnswParams& p, const HnswSme
         if (hnsw_filtered_out(p, l)) continue;
         const uint32_t bit = 1u << (l & 31);
         if (atomicOr(&visited[l >> 5], bit) & bit) continue;                // hop1_visited_list.check, then marked on acceptance
-        if (p.prefetch) prefetch_point<KIND>(p, l);
+        if (p.prefetch) prefetch_point<KIND, MV>(p, l);
         sm.ids[atomicAdd(&s_n, 1u)] = l;
         const uint32_t lp = atomicAdd(&s_nlog, 1u);
         if (lp < p.vlog_cap) vlog[lp] = l;
@@ -280,7 +417,8 @@ __device__ __forceinline__ uint32_t count_greater(const unsigned long long* keys
     return lo;
 }
 
-// CUSTOM = 1: a custom query (recommend / discover / context / feedback) scored through qbf::fold, with per-query custom entry points
+// CUSTOM = HC_CUSTOM: a custom query (recommend / discover / context / feedback) scored through qbf::fold, with per-query custom entry
+// points; HC_MAXSIM: a multivector query over a graph of multivector points, scored by maxsim_list (128 threads)
 template <int KIND, int METRIC, int NT, int ALGO, int CUSTOM>
 __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
     constexpr int HNSW_THREADS = NT;
@@ -309,6 +447,7 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
     uint32_t* visited = p.visited + (size_t)blockIdx.x * p.visited_words;
     uint32_t* vlog = p.vlog + (size_t)blockIdx.x * p.vlog_cap;
     unsigned long long hops = 0, evals = 0;   // thread 0 only
+    unsigned long long mv_rows = 0, mv_qrows = 0;   // HC_MAXSIM, thread 0: token rows scored, and times the query's vector count
 
     for (;;) {
         if (tid == 0) s_q = atomicAdd(p.work, 1u);
@@ -325,6 +464,20 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
             const uint4* src = reinterpret_cast<const uint4*>(p.q_enc + (size_t)q * p.q_bytes);
             uint4* dst = reinterpret_cast<uint4*>(const_cast<uint8_t*>(sm.q));
             for (uint32_t i = tid; i < (p.q_bytes + 15u) / 16u; i += HNSW_THREADS) dst[i] = src[i];
+        } else if constexpr (CUSTOM == HC_MAXSIM) {
+            // the query's vectors: into shared memory when they fit, else read where they are (the same arithmetic either way)
+            MvShared& ms = mv_shared();
+            const uint32_t q1 = min(mv_qoff(p)[q + 1], mv_nv(p)), q0 = min(mv_qoff(p)[q], q1);
+            const uint8_t* src = p.q_enc + (size_t)q0 * p.q_bytes;
+            if (q1 - q0 <= mv_stage_q(p)) {
+                const uint4* s4 = reinterpret_cast<const uint4*>(src);
+                uint4* dst = reinterpret_cast<uint4*>(smem_raw);
+                for (uint32_t i = tid; i < ((q1 - q0) * p.q_bytes) / 16u; i += HNSW_THREADS) dst[i] = s4[i];
+                sm.q = smem_raw;
+            } else {
+                sm.q = src;
+            }
+            if (tid == 0) { ms.q0 = q0; ms.nqv = q1 - q0; ms.rows = 0; }
         } else {
             // the examples: into shared memory when they fit, else read where they are (the same arithmetic either way)
             const size_t first = (size_t)q * p.ex_stride + p.ex_first;
@@ -341,7 +494,7 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
         const float q_off = (!CUSTOM && p.q_off) ? p.q_off[q] : 0.0f;
         if (tid == 0) {
             s_nlog = 0;
-            if constexpr (CUSTOM) {
+            if constexpr (CUSTOM == HC_CUSTOM) {
                 uint32_t e, l;
                 hnsw_custom_entry(p, q, e, l);
                 s_entry = e; s_entry_level = l; sm.ids[0] = e;
@@ -352,17 +505,20 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
             }
         }
         __syncthreads();
-        // `CUSTOM ? s_entry : p.entry` is written out at each use, not bound to a local, so the nearest-query kernels compile as before
+        // `CUSTOM == HC_CUSTOM ? s_entry : p.entry` is written out at each use, not bound to a local, so the nearest-query kernels compile as before
 
         // ---- search_entry: greedy descent from the entry point's level to level 1 (graph_layers.rs:247-316)
         score_list<KIND, METRIC, NT, CUSTOM>(p, sm, q_off, 1, q);      // score_point(entry)
         __syncthreads();
-        if (tid == 0) { s_cur = CUSTOM ? s_entry : (ALGO == ALGO_BUILD ? sm.ids[0] : p.entry); s_cur_score = sm.sc[0]; ++hops; ++evals; }
+        if (tid == 0) { s_cur = CUSTOM == HC_CUSTOM ? s_entry : (ALGO == ALGO_BUILD ? sm.ids[0] : p.entry); s_cur_score = sm.sc[0]; ++hops; ++evals; }
         __syncthreads();
-        for (uint32_t lvl = CUSTOM ? s_entry_level : p.entry_level; lvl >= 1; --lvl) {
+        for (uint32_t lvl = CUSTOM == HC_CUSTOM ? s_entry_level : p.entry_level; lvl >= 1; --lvl) {
             // search_entry_on_level re-scores its entry point on every level (graph_layers.rs:298-301): same value, but the scorer call
             // and the scored point are metered, so they are counted here too
-            if (tid == 0 && lvl != (CUSTOM ? s_entry_level : p.entry_level)) { ++hops; ++evals; }
+            if (tid == 0 && lvl != (CUSTOM == HC_CUSTOM ? s_entry_level : p.entry_level)) {
+                ++hops; ++evals;
+                if constexpr (CUSTOM == HC_MAXSIM) mv_shared().rows += mv_tok(p)[s_cur + 1] - mv_tok(p)[s_cur];
+            }
             for (;;) {
                 const uint32_t cur = s_cur;
                 // links of `cur` on this level: neighbors[offsets[idx] .. offsets[idx + 1]), idx = level_offsets[lvl] + reindex[cur] (view.rs:203-215)
@@ -377,7 +533,7 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
                         const bool keep = l != HNSW_EMPTY && l < p.n_points && !hnsw_filtered_out(p, l);
                         const unsigned int bal = __ballot_sync(0xFFFFFFFFu, keep);
                         const uint32_t pos = cnt + __popc(bal & ((1u << tid) - 1u));
-                        if (keep && pos < p.m && pos < HNSW_MAX_LINKS) { sm.ids[pos] = l; if (p.prefetch) prefetch_point<KIND>(p, l); }
+                        if (keep && pos < p.m && pos < HNSW_MAX_LINKS) { sm.ids[pos] = l; if (p.prefetch) prefetch_point<KIND, CUSTOM == HC_MAXSIM>(p, l); }
                         cnt += __popc(bal);
                     }
                     if (tid == 0) s_n = min(min(cnt, p.m), HNSW_MAX_LINKS);
@@ -454,12 +610,12 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
             const uint32_t cand = qb_key_id(keys[best]);
             if constexpr (ALGO == ALGO_ACORN) {
                 if (tid == 0) flags[best] = 1;
-                acorn_collect<KIND, NT>(p, sm, xids, cand, visited, vlog, s_n, s_nx, s_nlog, s_warp_cnt);
+                acorn_collect<KIND, NT, CUSTOM == HC_MAXSIM>(p, sm, xids, cand, visited, vlog, s_n, s_nx, s_nlog, s_warp_cnt);
                 const uint32_t n = s_n;
                 if (tid == 0) { if (n) { ++hops; evals += n; } s_nvalid = 0; }
                 if (n == 0) { __syncthreads(); continue; }
                 // score_points_unfiltered(to_score)
-                if (KIND == HK_DENSE_SMALL) {
+                if (KIND == HK_DENSE_SMALL && CUSTOM != HC_MAXSIM) {
                     for (uint32_t i = tid; i < n; i += HNSW_THREADS) sm.sc[i] = score_q<KIND, METRIC, CUSTOM>(p, sm, q_off, sm.ids[i], 0, q);
                 } else {
                     score_list<KIND, METRIC, NT, CUSTOM>(p, sm, q_off, n, q);
@@ -510,7 +666,7 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
                 asm volatile("bar.sync 1, 64;" ::: "memory");
                 const uint32_t pos = ((tid >> 5) ? s_warp_cnt[0] : 0u) + __popc(bal & ((1u << (tid & 31)) - 1u));
                 if (keep) {
-                    if (p.prefetch) prefetch_point<KIND>(p, l);          // HBM -> L2 for the whole vector, in flight while the list is published
+                    if (p.prefetch) prefetch_point<KIND, CUSTOM == HC_MAXSIM>(p, l);          // HBM -> L2 for the whole vector, in flight while the list is published
                     sm.ids[pos] = l;
                     const uint32_t lp = s_nlog + pos;
                     if (lp < p.vlog_cap) vlog[lp] = l;
@@ -609,6 +765,9 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
             }
             if (tid == 0) p.out_counts[q] = cnt;
         }
+        if constexpr (CUSTOM == HC_MAXSIM) {
+            if (tid == 0) { const MvShared& ms = mv_shared(); mv_rows += ms.rows; mv_qrows += ms.rows * ms.nqv; }
+        }
         // ---- un-set the visited bits this query set
         {
             const uint32_t nlog = s_nlog;
@@ -621,6 +780,9 @@ __global__ void __launch_bounds__(NT) hnsw_search_kernel(const HnswParams p) {
         __syncthreads();
     }
     if (tid == 0 && p.stats) { atomicAdd(&p.stats[0], hops); atomicAdd(&p.stats[1], evals); }
+    if constexpr (CUSTOM == HC_MAXSIM) {
+        if (tid == 0 && p.stats) { atomicAdd(&p.stats[2], mv_rows); atomicAdd(&p.stats[3], mv_qrows); }
+    }
 }
 
 template <int KIND, int NT, int ALGO, int CUSTOM>

@@ -151,11 +151,21 @@ struct qb_hnsw {
     uint32_t* d_visited = nullptr; uint64_t visited_words = 0; unsigned visited_slots = 0;
     uint32_t* d_vlog = nullptr; uint32_t vlog_cap = 0;
     unsigned int* d_work = nullptr;
-    unsigned long long* d_stats = nullptr;   // [0..3] the regular searches (two slots), [4..6] the inline-vector search
+    unsigned long long* d_stats = nullptr;   // [0..3] the regular searches (two slots), [4..6] the inline-vector search, [8..11] MaxSim
     uint64_t hops = 0, evals = 0, base_evals = 0;
+    uint64_t mv_rows = 0, mv_qrows = 0;      // MaxSim: token rows scored, and those times the query's vector count
     // inline vectors (qb_hnsw_create_with_vectors): the records, each entry's first link vector and each point's base vector (byte
     // offsets into d_blob); null for the other loaders
     uint8_t* d_blob = nullptr; uint64_t* d_lvoff = nullptr; uint64_t* d_boff = nullptr; uint32_t link_size = 0;
+    // a graph over the points of a multivector collection (qb_hnsw_create_*_multivector): point p = token rows d_mv_tok[p] ..
+    // d_mv_tok[p + 1) of st; null for the other loaders.  Only the MaxSim searches run on such a handle.
+    uint32_t* d_mv_tok = nullptr;
+};
+
+// A batch of multivector queries for qb_hnsw_launch: query q = encoded query vectors d_qoff[q] .. d_qoff[q + 1) (device) of the n_vectors
+// that d_q_enc / d_q_off hold; max_q bounds a query's vector count for the shared-memory staging (a larger query is read from HBM)
+struct QbHnswMaxsim {
+    const uint32_t* d_qoff; uint32_t n_vectors, max_q;
 };
 
 // A batch of custom queries for qb_hnsw_launch: query q's examples are the encoded queries ex_first .. ex_first + n_ex of the
@@ -171,7 +181,7 @@ struct QbHnswCustom {
 
 qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, uint32_t nq, uint32_t top, uint32_t ef, uint32_t entry, uint32_t entry_level,
                          const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts, cudaStream_t stream, int algo /* qb_hnsw_algorithm */,
-                         const QbHnswCustom* custom = nullptr);
+                         const QbHnswCustom* custom = nullptr, const QbHnswMaxsim* maxsim = nullptr);
 // completes a handle whose plain arrays (d_level_offsets, d_reindex, d_neighbors, d_offsets and the host-side counts) are on the device:
 // the level-0 table and the search scratch (qb_hnsw.cu).  On failure the caller destroys g.  who = the error messages' prefix.
 qb_status qb_hnsw_finish_plain(qb_hnsw* g, const char* who);
@@ -179,7 +189,7 @@ qb_status qb_hnsw_finish_plain(qb_hnsw* g, const char* who);
 qb_status qb_hnsw_inline_launch(qb_hnsw* g, const float* d_q_pre, uint32_t pre_stride, const void* d_q_enc, const float* d_q_off, uint32_t nq, uint32_t top,
                                 uint32_t ef, uint32_t entry, uint32_t entry_level, const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts,
                                 cudaStream_t stream);
-// adds the device counters to g->hops / g->evals / g->base_evals and clears them; evals_by_slot (optional, [2]) receives each regular slot's scored points
+// adds the device counters to g->hops / g->evals / g->base_evals / g->mv_rows / g->mv_qrows and clears them; evals_by_slot (optional, [2]) receives each regular slot's scored points
 qb_status qb_hnsw_read_stats(qb_hnsw* g, cudaStream_t stream, uint64_t* evals_by_slot = nullptr);
 
 // One rank of a sharded search (qb_comm.cu): an exchange buffer every peer maps + the peers' buffers

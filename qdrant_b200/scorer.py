@@ -749,6 +749,55 @@ class HnswGraph:
         return self
 
     @classmethod
+    def multivector(cls, view: "MultiVectorView", links_bin, m: int, m0: int) -> "HnswGraph":
+        """A plain links.bin over the POINTS of a multivector collection (qb_hnsw_create_plain_multivector); search it with search_maxsim()."""
+        return cls._multivector(view, links_bin, lambda h, blob: lib().qb_hnsw_create_plain_multivector(
+            view.storage._h, view.offsets.ctypes.data_as(u32p), view.n_points, blob.ctypes.data_as(u8p), blob.size, int(m), int(m0), C.byref(h)))
+
+    @classmethod
+    def from_compressed_multivector(cls, view: "MultiVectorView", links_bin) -> "HnswGraph":
+        """A compressed links.bin over the points of a multivector collection (qb_hnsw_create_compressed_multivector)."""
+        return cls._multivector(view, links_bin, lambda h, blob: lib().qb_hnsw_create_compressed_multivector(
+            view.storage._h, view.offsets.ctypes.data_as(u32p), view.n_points, blob.ctypes.data_as(u8p), blob.size, C.byref(h)))
+
+    @classmethod
+    def _multivector(cls, view: "MultiVectorView", links_bin, create) -> "HnswGraph":
+        self = cls.__new__(cls)
+        self._storage = view.storage
+        self._view = view
+        self._h = vp()
+        blob = np.ascontiguousarray(np.frombuffer(links_bin, dtype=np.uint8) if isinstance(links_bin, (bytes, bytearray)) else links_bin,
+                                    dtype=np.uint8).reshape(-1)
+        h = vp()
+        check(create(h, blob))
+        self._h = h
+        return self
+
+    def search_maxsim(self, queries, top: int, ef: int, entry_point: int, entry_level: int, point_deleted=None, counters: Optional[HwCounters] = None,
+                      algorithm: str = "hnsw"):
+        """GraphLayers::search with a MaxSim scorer on a multivector() graph (qb_hnsw_search_maxsim_batch).  queries: a list of
+        [Q_i, dim] arrays (1..4096 vectors each); point_deleted: over points.  Returns one list of point offsets per query; a score
+        equals MultiVectorView.score_points on that point, bit for bit."""
+        if algorithm not in self.ALGORITHMS:
+            raise ValueError(f"algorithm {algorithm!r} is not one of {sorted(self.ALGORITHMS)}")
+        view = getattr(self, "_view", None)
+        mats = [np.atleast_2d(_f32(q)) for q in queries]
+        for m in mats:
+            if m.shape[1] != self._storage.dim:
+                raise ValueError(f"query vectors have dim {m.shape[1]}, storage has {self._storage.dim}")
+        nq = len(mats)
+        vecs = np.ascontiguousarray(np.concatenate(mats) if nq else np.zeros((0, self._storage.dim), np.float32))
+        off = np.concatenate([[0], np.cumsum([m.shape[0] for m in mats])]).astype(np.uint32)
+        out = np.zeros((max(nq, 1), max(top, 1)), dtype=SCORED_POINT_OFFSET)
+        counts = np.zeros(max(nq, 1), dtype=np.uint32)
+        bm = _bitmap(point_deleted, view.n_points if view is not None else self.info()[0])
+        check(lib().qb_hnsw_search_maxsim_batch(self._h, vecs.ctypes.data_as(f32p), off.ctypes.data_as(u32p), nq, int(top), int(ef), int(entry_point),
+                                                int(entry_level), None if bm is None else bm.ctypes.data_as(u64p), None,
+                                                out.ctypes.data_as(C.POINTER(ScoredPoint)), counts.ctypes.data_as(u32p),
+                                                None if counters is None else C.byref(counters), self.ALGORITHMS[algorithm]))
+        return [out[i, : counts[i]].copy() for i in range(nq)]
+
+    @classmethod
     def build(cls, storage: _Storage, m: int = 16, ef_construct: int = 100, levels=None, seed: int = 0, batch: int = 0, serial_points: int = 0,
               m0: Optional[int] = None) -> "HnswGraph":
         """Builds the graph of a dense f32 storage on the device (qb_hnsw_build; m0 defaults to 2m).  levels: one per point (<= 30);
