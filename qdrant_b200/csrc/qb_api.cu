@@ -552,6 +552,81 @@ static qb_status prepare_queries(const qb_storage* s, const float* d_q_raw, uint
     }
 }
 
+// A pooled search context of a storage, given back when the lease goes out of scope.
+struct CtxLease {
+    qb_storage* s = nullptr;
+    QbSearchCtx* c = nullptr;
+    CtxLease() = default;
+    CtxLease(const CtxLease&) = delete;
+    CtxLease& operator=(const CtxLease&) = delete;
+    qb_status acquire(qb_storage* st) { s = st; return qb_ctx_acquire(s, &c); }
+    ~CtxLease() { if (c) qb_ctx_release(s, c); }
+};
+
+// Host f32 vectors (nv rows of dim) to encoded queries in c->d_queries_enc / c->d_q_off, enqueued on c->stream:
+//   pinned stage   [vectors | tail_bytes]   the tail holds what the caller sends or brings back besides the vectors
+//   d_queries_raw  [vectors | pad to 16 | nv rows of pre_stride_f preprocessed floats]
+//   d_queries_enc  nv + 256 rows: the tensor-core SQ8 path reads whole query blocks (rows past nv are masked, never scored)
+// *h_tail: the tail of the stage; *d_pre: the preprocessed rows (dense f32 writes them to d_queries_enc instead).
+static qb_status stage_queries(const qb_storage* s, QbSearchCtx* c, const float* vectors, uint32_t nv, size_t tail_bytes, uint8_t** h_tail,
+                               float** d_pre = nullptr) {
+    const size_t raw_bytes = (size_t)nv * s->dim * 4, pre_off = round_up_u64(raw_bytes, 16);
+    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, raw_bytes + tail_bytes));
+    uint8_t* hs = reinterpret_cast<uint8_t*>(c->h_stage);
+    memcpy(hs, vectors, raw_bytes);
+    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, pre_off + (size_t)nv * pre_stride_f(s) * 4));
+    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)nv + 256) * qb_encoded_query_bytes(s)));
+    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)nv));
+    QB_CUDA(cudaMemcpyAsync(c->d_queries_raw, hs, raw_bytes, cudaMemcpyHostToDevice, c->stream));
+    float* pre = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c->d_queries_raw) + pre_off);
+    QB_TRY(prepare_queries(s, reinterpret_cast<const float*>(c->d_queries_raw), nv, pre, c->d_queries_enc, c->d_q_off, c->stream));
+    *h_tail = hs + raw_bytes;
+    if (d_pre) *d_pre = pre;
+    return QB_OK;
+}
+
+// stage_queries for queries already in device memory: d_queries_raw holds only the nv preprocessed rows
+static qb_status encode_device_queries(const qb_storage* s, QbSearchCtx* c, const float* dev_queries, uint32_t nv, float** d_pre = nullptr) {
+    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, (size_t)nv * pre_stride_f(s) * 4 + 256));
+    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)nv + 256) * qb_encoded_query_bytes(s)));
+    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)nv));
+    float* pre = reinterpret_cast<float*>(c->d_queries_raw);
+    QB_TRY(prepare_queries(s, dev_queries, nv, pre, c->d_queries_enc, c->d_q_off, c->stream));
+    if (d_pre) *d_pre = pre;
+    return QB_OK;
+}
+
+// A host bitmap of n_bits deleted flags (whole u64 words) to c->d_deleted2; *d_bitmap = null when there is none
+static qb_status upload_bitmap(QbSearchCtx* c, const uint64_t* words, uint64_t n_bits, const uint32_t** d_bitmap) {
+    *d_bitmap = nullptr;
+    if (!words) return QB_OK;
+    const uint64_t words64 = ceil_div_u64(n_bits, 64);
+    QB_TRY(ensure_dev_elems(&c->d_deleted2, &c->deleted2_words, (size_t)words64 * 2));
+    QB_CUDA(cudaMemcpyAsync(c->d_deleted2, words, words64 * 8, cudaMemcpyHostToDevice, c->stream));
+    *d_bitmap = c->d_deleted2;
+    return QB_OK;
+}
+
+// n lists of `top` results and their counts back to the host through the stage tail [lists | counts | extra], one synchronisation,
+// then out to the caller.  extra: bytes that follow the counts on the device and come back in the same copy (a flags word).
+static qb_status fetch_lists(QbSearchCtx* c, const qb_scored_point* d_out, const uint32_t* d_counts, uint32_t n, uint32_t top, size_t extra, uint8_t* h_tail,
+                             qb_scored_point* out, uint32_t* out_counts) {
+    const size_t res_bytes = (size_t)n * top * sizeof(qb_scored_point), cnt_bytes = (size_t)n * 4;
+    QB_CUDA(cudaMemcpyAsync(h_tail, d_out, res_bytes, cudaMemcpyDeviceToHost, c->stream));
+    QB_CUDA(cudaMemcpyAsync(h_tail + res_bytes, d_counts, cnt_bytes + extra, cudaMemcpyDeviceToHost, c->stream));
+    QB_CUDA(cudaStreamSynchronize(c->stream));
+    memcpy(out, h_tail, res_bytes);
+    memcpy(out_counts, h_tail + res_bytes, cnt_bytes);
+    return QB_OK;
+}
+
+// a stop flag raised before or during a search: sets the error of QB_ERR_CANCELLED
+static bool cancelled(const volatile int32_t* is_stopped) {
+    if (!is_stopped || !*is_stopped) return false;
+    qb_set_error("search cancelled");
+    return true;
+}
+
 qb_status qb_launch_scan(const qb_storage* s, const QbScanArgs& a, cudaStream_t stream) {
     switch (s->kind) {
         case QB_KIND_DENSE: return s->dtype == QB_DT_F32 ? qb_dense_f32_scan(s, a, stream) : qb_dense_x_scan(s, a, stream);
@@ -709,7 +784,7 @@ static qb_status run_search(qb_storage* s, QbSearchCtx* c, uint32_t nq, uint32_t
     const size_t enc_bytes = qb_encoded_query_bytes(s);
 
     for (uint32_t q0 = 0; q0 < nq; q0 += plan.q_chunk) {
-        if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+        if (cancelled(is_stopped)) return QB_ERR_CANCELLED;
         const uint32_t qn = std::min<uint32_t>(plan.q_chunk, nq - q0);
         QbScanArgs a{};
         a.d_q_enc = reinterpret_cast<const uint8_t*>(c->d_queries_enc) + (size_t)q0 * enc_bytes;
@@ -771,7 +846,7 @@ static qb_status run_search(qb_storage* s, QbSearchCtx* c, uint32_t nq, uint32_t
             QB_CUDA(cudaMemsetAsync(c->d_cnt + q0, 0, (size_t)qn * 4, stream));
             a.row_begin = 0; a.row_end = n_cand;
             a.emit.dense = 0; a.emit.thr = c->d_thr + q0; a.emit.cnt = c->d_cnt + q0;
-            if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+            if (cancelled(is_stopped)) return QB_ERR_CANCELLED;
             profile_begin(s, c, stream, &e0, &e1);
             unsigned long long seg_len = 0;
             if (f32b) {
@@ -790,6 +865,45 @@ static qb_status run_search(qb_storage* s, QbSearchCtx* c, uint32_t nq, uint32_t
             QB_TRY(qb_launch_select(c->d_cand, c->d_cnt + q0, plan.cap, seg_len, qn, top, 0, d_out + (size_t)q0 * top, d_counts + q0, nullptr, d_overflow, stream));
         }
     }
+    return QB_OK;
+}
+
+// run_search, fast path first.  The device reports in a flags word (d_flags) when one of its assumptions did not hold, and the search
+// runs again without it:
+//   1 candidate buffer overflow (threshold admitted too much: mass ties, mostly-deleted sample) -> full materialisation
+//   2 a tensor-core dot product left the f32-exact window (>= 2^24)                           -> lane-exact CUDA-core kernel
+//   8 a per-(query, CTA) survivor segment filled up                                            -> global counters
+// out != null: every attempt brings the lists, the counts and the flags word (d_flags must follow d_counts) back in one round trip
+// through the stage tail h_tail, and the last attempt's lists go to out / out_counts.  out == null: only the flags word comes back,
+// to h_tail, and not at all on the paths that cannot flag, which leaves the call asynchronous.
+static qb_status search_with_reruns(qb_storage* s, QbSearchCtx* c, uint32_t nq, uint32_t top, const uint32_t* d_ids, uint64_t n_ids, const uint32_t* d_del2,
+                                    const volatile int32_t* is_stopped, qb_scored_point* d_out, uint32_t* d_counts, unsigned int* d_flags, uint8_t* h_tail,
+                                    qb_scored_point* out = nullptr, uint32_t* out_counts = nullptr) {
+    const uint8_t* h_flags = out ? h_tail + (size_t)nq * top * sizeof(qb_scored_point) + (size_t)nq * 4 : h_tail;
+    uint32_t rs_flags = 0;
+    for (int attempt = 0; attempt < 4; ++attempt) {
+        QB_CUDA(cudaMemsetAsync(d_flags, 0, 4, c->stream));
+        bool can_flag = true;
+        QB_TRY(run_search(s, c, nq, top, d_ids, n_ids, d_del2, is_stopped, rs_flags, d_out, d_counts, d_flags, &can_flag));
+        if (out) {
+            QB_TRY(fetch_lists(c, d_out, d_counts, nq, top, 4, h_tail, out, out_counts));
+        } else {
+            if (!can_flag) break;  // exact single-pass path: nothing to check
+            QB_CUDA(cudaMemcpyAsync(h_tail, d_flags, 4, cudaMemcpyDeviceToHost, c->stream));
+            QB_CUDA(cudaStreamSynchronize(c->stream));
+        }
+        unsigned int flags = 0;
+        memcpy(&flags, h_flags, 4);
+        uint32_t next = rs_flags;
+        if (flags & 8u) next |= RS_NO_SEGMENTS;
+        if (flags & 2u) next |= RS_NO_MMA;
+        if (flags & 1u) next |= RS_FORCE_DIRECT | RS_NO_MMA;
+        if (next == rs_flags) break;
+        s->n_reruns.fetch_add(1, std::memory_order_relaxed);
+        if (qb_opt().verbose) fprintf(stderr, "[qb200] search rerun: device flags=0x%x, mode 0x%x -> 0x%x\n", flags, rs_flags, next);
+        rs_flags = next;
+    }
+    s->n_searches.fetch_add(1, std::memory_order_relaxed);
     return QB_OK;
 }
 
@@ -822,73 +936,32 @@ extern "C" qb_status qb_search_batch(qb_storage* s, const float* queries, uint32
     QB_CHECK(top >= 1, QB_ERR_INVALID, "search_batch: top must be >= 1 (FixedLengthPriorityQueue::new panics on 0)");
     QB_CHECK(top <= QB_MAX_TOP, QB_ERR_UNSUPPORTED, "search_batch: top %u > %u not supported by the fused selection", top, QB_MAX_TOP);
     if (n_queries == 0) return QB_OK;
-    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    if (cancelled(is_stopped)) return QB_ERR_CANCELLED;
     QB_TRY(use_device(s->device));
-    QbSearchCtx* c = nullptr;
-    QB_TRY(qb_ctx_acquire(s, &c));
-    struct Rel { qb_storage* s; QbSearchCtx* c; ~Rel() { qb_ctx_release(s, c); } } rel{s, c};
-    cudaStream_t stream = c->stream;
-
+    CtxLease lease;
+    QB_TRY(lease.acquire(s));
+    QbSearchCtx* c = lease.c;
+    // stage tail: [results | counts | flags word | candidate ids]; the ids are checked before anything is enqueued
     const size_t raw_bytes = (size_t)n_queries * s->dim * 4;
-    const size_t res_bytes = (size_t)n_queries * top * sizeof(qb_scored_point);
-    const size_t cnt_bytes = (size_t)n_queries * 4;
-    // pinned staging: [queries | results | counts | overflow flag | candidate ids]
-    const size_t ids_off = round_up_u64(raw_bytes + res_bytes + cnt_bytes + 16, 16);
-    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, ids_off + (id_list ? n_ids * 4 : 0)));
-    uint8_t* hs = reinterpret_cast<uint8_t*>(c->h_stage);
-    memcpy(hs, queries, raw_bytes);
-    if (id_list) QB_TRY(localize_ids(s, id_list, n_ids, reinterpret_cast<uint32_t*>(hs + ids_off), "search_batch"));
-    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, raw_bytes + (size_t)n_queries * pre_stride_f(s) * 4));
-    // +256 rows: the tensor-core SQ8 path reads whole query blocks (rows past n_queries are masked, never scored)
-    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)n_queries + 256) * qb_encoded_query_bytes(s)));
-    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)n_queries));
+    const size_t ids_at = (size_t)n_queries * top * sizeof(qb_scored_point) + (size_t)n_queries * 4 + 4;
+    const size_t tail_bytes = ids_at + (id_list ? n_ids * 4 : 0);
+    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, raw_bytes + tail_bytes));
+    uint32_t* h_ids = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(c->h_stage) + raw_bytes + ids_at);
+    if (id_list) QB_TRY(localize_ids(s, id_list, n_ids, h_ids, "search_batch"));
+    uint8_t* h_tail = nullptr;
+    QB_TRY(stage_queries(s, c, queries, n_queries, tail_bytes, &h_tail));
     QB_TRY(ensure_dev_elems(&c->d_out, &c->out_elems, (size_t)n_queries * top));
     QB_TRY(ensure_dev_elems(&c->d_out_counts, &c->out_counts_elems, (size_t)n_queries + 4));
-    QB_CUDA(cudaMemcpyAsync(c->d_queries_raw, hs, raw_bytes, cudaMemcpyHostToDevice, stream));
-    float* d_pre = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c->d_queries_raw) + raw_bytes);
-    QB_TRY(prepare_queries(s, reinterpret_cast<const float*>(c->d_queries_raw), n_queries, d_pre, c->d_queries_enc, c->d_q_off, stream));
-
     const uint32_t* d_del2 = nullptr;
-    if (deleted_bitmap) {
-        const uint64_t words64 = ceil_div_u64(s->count, 64);
-        QB_TRY(ensure_dev_elems(&c->d_deleted2, &c->deleted2_words, (size_t)words64 * 2));
-        QB_CUDA(cudaMemcpyAsync(c->d_deleted2, deleted_bitmap, words64 * 8, cudaMemcpyHostToDevice, stream));
-        d_del2 = c->d_deleted2;
-    }
+    QB_TRY(upload_bitmap(c, deleted_bitmap, s->count, &d_del2));
     const uint32_t* d_ids = nullptr;
     if (id_list) {
         QB_TRY(ensure_dev_elems(&c->d_ids, &c->ids_elems, (size_t)std::max<uint64_t>(n_ids, 1)));
-        QB_CUDA(cudaMemcpyAsync(c->d_ids, hs + ids_off, n_ids * 4, cudaMemcpyHostToDevice, stream));
+        QB_CUDA(cudaMemcpyAsync(c->d_ids, h_ids, n_ids * 4, cudaMemcpyHostToDevice, c->stream));
         d_ids = c->d_ids;
     }
-    unsigned int* d_overflow = reinterpret_cast<unsigned int*>(c->d_out_counts + n_queries);
-    uint8_t* h_res = hs + raw_bytes;
-    uint8_t* h_cnt = h_res + res_bytes;
-    // Fast path first; the device reports (flags word) when one of its assumptions did not hold and the host reruns without it:
-    //   1 candidate buffer overflow (threshold admitted too much: mass ties, mostly-deleted sample) -> full materialisation
-    //   2 a tensor-core dot product left the f32-exact window (>= 2^24)                           -> lane-exact CUDA-core kernel
-    //   8 a per-(query, CTA) survivor segment filled up                                            -> global counters
-    uint32_t rs_flags = 0;
-    for (int attempt = 0; attempt < 4; ++attempt) {
-        QB_CUDA(cudaMemsetAsync(d_overflow, 0, 4, stream));
-        QB_TRY(run_search(s, c, n_queries, top, d_ids, n_ids, d_del2, is_stopped, rs_flags, c->d_out, c->d_out_counts, d_overflow));
-        QB_CUDA(cudaMemcpyAsync(h_res, c->d_out, res_bytes, cudaMemcpyDeviceToHost, stream));
-        QB_CUDA(cudaMemcpyAsync(h_cnt, c->d_out_counts, cnt_bytes + 4, cudaMemcpyDeviceToHost, stream));
-        QB_CUDA(cudaStreamSynchronize(stream));
-        unsigned int flags = 0;
-        memcpy(&flags, h_cnt + cnt_bytes, 4);
-        uint32_t next = rs_flags;
-        if (flags & 8u) next |= RS_NO_SEGMENTS;
-        if (flags & 2u) next |= RS_NO_MMA;
-        if (flags & 1u) next |= RS_FORCE_DIRECT | RS_NO_MMA;
-        if (next == rs_flags) break;
-        s->n_reruns.fetch_add(1, std::memory_order_relaxed);
-        if (qb_opt().verbose) fprintf(stderr, "[qb200] search rerun: device flags=0x%x, mode 0x%x -> 0x%x\n", flags, rs_flags, next);
-        rs_flags = next;
-    }
-    s->n_searches.fetch_add(1, std::memory_order_relaxed);
-    memcpy(out, h_res, res_bytes);
-    memcpy(out_counts, h_cnt, cnt_bytes);
+    unsigned int* d_flags = reinterpret_cast<unsigned int*>(c->d_out_counts + n_queries);
+    QB_TRY(search_with_reruns(s, c, n_queries, top, d_ids, n_ids, d_del2, is_stopped, c->d_out, c->d_out_counts, d_flags, h_tail, out, out_counts));
     if (counters) {
         const uint64_t n_cand = id_list ? n_ids : s->count;
         counters->cpu += n_cand * (uint64_t)n_queries * cpu_units_per_point(s);
@@ -905,36 +978,12 @@ extern "C" qb_status qb_search_batch_device(qb_storage* s, const float* dev_quer
     QB_TRY(use_device(s->device));
     QbSearchCtx* c = nullptr;
     QB_TRY(qb_ctx_device(s, &c));
-    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, (size_t)n_queries * pre_stride_f(s) * 4 + 256));
-    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)n_queries + 256) * qb_encoded_query_bytes(s)));
-    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)n_queries));
+    QB_TRY(encode_device_queries(s, c, dev_queries, n_queries));
     QB_TRY(ensure_dev_elems(&c->d_out_counts, &c->out_counts_elems, (size_t)n_queries + 4));
-    QB_TRY(prepare_queries(s, dev_queries, n_queries, reinterpret_cast<float*>(c->d_queries_raw), c->d_queries_enc, c->d_q_off, c->stream));
-    unsigned int* d_overflow = reinterpret_cast<unsigned int*>(c->d_out_counts + n_queries);
-    // same contract as qb_search_batch: the device reports a broken fast-path assumption in a flags word and the host reruns
-    // without it; reading that word is the one synchronisation of this call
+    unsigned int* d_flags = reinterpret_cast<unsigned int*>(c->d_out_counts + n_queries);
+    // reading the flags word of the reruns is the one synchronisation of this call
     QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, 64));
-    uint32_t rs_flags = 0;
-    for (int attempt = 0; attempt < 4; ++attempt) {
-        QB_CUDA(cudaMemsetAsync(d_overflow, 0, 4, c->stream));
-        bool can_flag = true;
-        QB_TRY(run_search(s, c, n_queries, top, nullptr, 0, nullptr, nullptr, rs_flags, dev_out, dev_counts, d_overflow, &can_flag));
-        if (!can_flag) break;  // exact single-pass path: nothing to check, the call stays asynchronous
-        QB_CUDA(cudaMemcpyAsync(c->h_stage, d_overflow, 4, cudaMemcpyDeviceToHost, c->stream));
-        QB_CUDA(cudaStreamSynchronize(c->stream));
-        unsigned int flags = 0;
-        memcpy(&flags, c->h_stage, 4);
-        uint32_t next = rs_flags;
-        if (flags & 8u) next |= RS_NO_SEGMENTS;
-        if (flags & 2u) next |= RS_NO_MMA;
-        if (flags & 1u) next |= RS_FORCE_DIRECT | RS_NO_MMA;
-        if (next == rs_flags) break;
-        s->n_reruns.fetch_add(1, std::memory_order_relaxed);
-        if (qb_opt().verbose) fprintf(stderr, "[qb200] search rerun: device flags=0x%x, mode 0x%x -> 0x%x\n", flags, rs_flags, next);
-        rs_flags = next;
-    }
-    s->n_searches.fetch_add(1, std::memory_order_relaxed);
-    return QB_OK;
+    return search_with_reruns(s, c, n_queries, top, nullptr, 0, nullptr, nullptr, dev_out, dev_counts, d_flags, reinterpret_cast<uint8_t*>(c->h_stage));
 }
 
 // ------------------------------------------------------------------------------------------------ RawScorer
@@ -1079,35 +1128,26 @@ static qb_status search_custom_impl(qb_storage* s, qb_query_kind kind, const flo
     const bool try_fold = !id_list && s->kind == QB_KIND_DENSE && s->dtype == QB_DT_F32 && s->dim >= 32 && ne <= 16 && n >= 1024;
     QB_CHECK(try_fold || n * (12ull + 4ull * ne) <= (16ull << 30), QB_ERR_UNSUPPORTED, "search_custom: %llu candidates x %u examples exceed the 16 GB scratch budget",
              (unsigned long long)n, ne);
-    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    if (cancelled(is_stopped)) return QB_ERR_CANCELLED;
     QB_TRY(use_device(s->device));
-    QbSearchCtx* c = nullptr;
-    QB_TRY(qb_ctx_acquire(s, &c));
-    struct Rel { qb_storage* s; QbSearchCtx* c; ~Rel() { qb_ctx_release(s, c); } } rel{s, c};
+    CtxLease lease;
+    QB_TRY(lease.acquire(s));
+    QbSearchCtx* c = lease.c;
     cudaStream_t stream = c->stream;
-    const size_t raw_bytes = (size_t)ne * s->dim * 4, res_bytes = (size_t)top * sizeof(qb_scored_point);
-    const size_t ids_off = round_up_u64(raw_bytes + res_bytes + 16, 16);
-    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, ids_off + (id_list ? n_ids * 4 : 0)));
-    uint8_t* hs = reinterpret_cast<uint8_t*>(c->h_stage);
-    memcpy(hs, vectors, raw_bytes);
-    if (id_list) QB_TRY(localize_ids(s, id_list, n_ids, reinterpret_cast<uint32_t*>(hs + ids_off), "search_custom"));
-    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, round_up_u64(raw_bytes, 16) + (size_t)ne * pre_stride_f(s) * 4));
-    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)ne + 256) * qb_encoded_query_bytes(s)));
-    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)ne));
+    // stage tail: [result list | count | candidate ids]; the ids are checked before anything is enqueued
+    const size_t raw_bytes = (size_t)ne * s->dim * 4, ids_at = (size_t)top * sizeof(qb_scored_point) + 4;
+    const size_t tail_bytes = ids_at + (id_list ? n_ids * 4 : 0);
+    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, raw_bytes + tail_bytes));
+    uint32_t* h_ids = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(c->h_stage) + raw_bytes + ids_at);
+    if (id_list) QB_TRY(localize_ids(s, id_list, n_ids, h_ids, "search_custom"));
+    uint8_t* h_tail = nullptr;
+    QB_TRY(stage_queries(s, c, vectors, ne, tail_bytes, &h_tail));
     QB_TRY(ensure_dev_elems(&c->d_out, &c->out_elems, (size_t)top));
     QB_TRY(ensure_dev_elems(&c->d_out_counts, &c->out_counts_elems, (size_t)8));
     QB_TRY(ensure_dev_elems(&c->d_cand, &c->cand_elems, (size_t)n));
     QB_TRY(ensure_dev_elems(&c->d_thr, &c->thr_elems, (size_t)n_coef + 64));
-    QB_CUDA(cudaMemcpyAsync(c->d_queries_raw, hs, raw_bytes, cudaMemcpyHostToDevice, stream));
-    QB_TRY(prepare_queries(s, reinterpret_cast<const float*>(c->d_queries_raw), ne,
-                           reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c->d_queries_raw) + round_up_u64(raw_bytes, 16)), c->d_queries_enc, c->d_q_off, stream));
     const uint32_t* d_del2 = nullptr;
-    if (deleted_bitmap) {
-        const size_t words64 = (size_t)ceil_div_u64(s->count, 64);
-        QB_TRY(ensure_dev_elems(&c->d_deleted2, &c->deleted2_words, words64 * 2));
-        QB_CUDA(cudaMemcpyAsync(c->d_deleted2, deleted_bitmap, words64 * 8, cudaMemcpyHostToDevice, stream));
-        d_del2 = c->d_deleted2;
-    }
+    QB_TRY(upload_bitmap(c, deleted_bitmap, s->count, &d_del2));
     QbEmit emit{};
     emit.cand = c->d_cand; emit.cap = n; emit.dense = 1; emit.dense_base = 0; emit.deleted = s->d_deleted; emit.deleted2 = d_del2; emit.id_base = s->id_base;
     const float* d_coef = nullptr;
@@ -1126,21 +1166,17 @@ static qb_status search_custom_impl(qb_storage* s, qb_query_kind kind, const flo
                  (unsigned long long)n, ne);
         QB_TRY(ensure_dev_elems(&c->d_ids, &c->ids_elems, (size_t)n));
         QB_TRY(qb_ensure_device(&c->d_mma, &c->mma_bytes, (size_t)ne * n * 4 + 256));
-        if (id_list) QB_CUDA(cudaMemcpyAsync(c->d_ids, hs + ids_off, n * 4, cudaMemcpyHostToDevice, stream));
+        if (id_list) QB_CUDA(cudaMemcpyAsync(c->d_ids, h_ids, n * 4, cudaMemcpyHostToDevice, stream));
         else QB_TRY(qb_launch_iota(c->d_ids, n, stream));
         float* d_sims = reinterpret_cast<float*>(c->d_mma);
         for (uint32_t e = 0; e < ne; ++e) {
-            if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+            if (cancelled(is_stopped)) return QB_ERR_CANCELLED;
             QB_TRY(launch_example(s, c->d_queries_enc, c->d_q_off, e, false, c->d_ids, n, d_sims + (size_t)e * n, stream));
         }
         QB_TRY(qb_launch_custom_combine((int)kind, n_a, n_b, d_coef, d_sims, n, n, nullptr, c->d_ids, &emit, stream));
     }
     QB_TRY(qb_launch_select(c->d_cand, nullptr, n, n, 1, top, 0, c->d_out, c->d_out_counts, nullptr, nullptr, stream));
-    QB_CUDA(cudaMemcpyAsync(hs + raw_bytes, c->d_out, res_bytes, cudaMemcpyDeviceToHost, stream));
-    QB_CUDA(cudaMemcpyAsync(hs + raw_bytes + res_bytes, c->d_out_counts, 4, cudaMemcpyDeviceToHost, stream));
-    QB_CUDA(cudaStreamSynchronize(stream));
-    memcpy(out, hs + raw_bytes, res_bytes);
-    memcpy(out_count, hs + raw_bytes + res_bytes, 4);
+    QB_TRY(fetch_lists(c, c->d_out, c->d_out_counts, 1, top, 0, h_tail, out, out_count));
     if (counters) { counters->cpu += n * (uint64_t)ne * cpu_units_per_point(s); counters->vector_io_read += n * (uint64_t)ne * io_units_per_point(s); }
     return QB_OK;
 }
@@ -1193,18 +1229,13 @@ static qb_status maxsim_run(qb_storage* s, const uint32_t* point_offsets, uint32
     QB_CHECK(n_rows * (4ull * nqt + 4) + n_pts * 20 <= (16ull << 30), QB_ERR_UNSUPPORTED, "maxsim: %llu vectors x %u query vectors exceed the 16 GB scratch budget",
              (unsigned long long)n_rows, nqt);
     QB_TRY(use_device(s->device));
-    QbSearchCtx* c = nullptr;
-    QB_TRY(qb_ctx_acquire(s, &c));
-    struct Rel { qb_storage* s; QbSearchCtx* c; ~Rel() { qb_ctx_release(s, c); } } rel{s, c};
+    CtxLease lease;
+    QB_TRY(lease.acquire(s));
+    QbSearchCtx* c = lease.c;
     cudaStream_t stream = c->stream;
-    const size_t raw_bytes = (size_t)nqt * s->dim * 4;
-    const size_t res_bytes = scores ? (size_t)n_pts * 4 : (size_t)top * sizeof(qb_scored_point);
-    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, raw_bytes + res_bytes + 16));
-    uint8_t* hs = reinterpret_cast<uint8_t*>(c->h_stage);
-    memcpy(hs, query_tokens, raw_bytes);
-    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, round_up_u64(raw_bytes, 16) + (size_t)nqt * pre_stride_f(s) * 4));
-    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)nqt + 256) * qb_encoded_query_bytes(s)));
-    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)nqt));
+    // stage tail: the scores, or the result list and its count
+    uint8_t* h_tail = nullptr;
+    QB_TRY(stage_queries(s, c, query_tokens, nqt, scores ? (size_t)n_pts * 4 : (size_t)top * sizeof(qb_scored_point) + 4, &h_tail));
     QB_TRY(ensure_dev_elems(&c->d_ids, &c->ids_elems, (size_t)std::max<uint64_t>(n_rows, 1)));
     // scratch: [similarities nqt x n_rows][column offsets n_pts + 1][point ids n_pts][scores n_pts]
     const size_t sims_bytes = round_up_u64((size_t)nqt * n_rows * 4, 256), off_bytes = round_up_u64((n_pts + 1) * 4, 256), pid_bytes = round_up_u64(n_pts * 4, 256);
@@ -1214,9 +1245,6 @@ static qb_status maxsim_run(qb_storage* s, const uint32_t* point_offsets, uint32
     uint32_t* d_off = reinterpret_cast<uint32_t*>(sc + sims_bytes);
     uint32_t* d_pid = reinterpret_cast<uint32_t*>(sc + sims_bytes + off_bytes);
     float* d_scores = reinterpret_cast<float*>(sc + sims_bytes + off_bytes + pid_bytes);
-    QB_CUDA(cudaMemcpyAsync(c->d_queries_raw, hs, raw_bytes, cudaMemcpyHostToDevice, stream));
-    QB_TRY(prepare_queries(s, reinterpret_cast<const float*>(c->d_queries_raw), nqt,
-                           reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c->d_queries_raw) + round_up_u64(raw_bytes, 16)), c->d_queries_enc, c->d_q_off, stream));
     QB_CUDA(cudaMemcpyAsync(d_off, h_off.data(), (n_pts + 1) * 4, cudaMemcpyHostToDevice, stream));
     if (point_ids) {
         QB_CUDA(cudaMemcpyAsync(d_pid, point_ids, n_pts * 4, cudaMemcpyHostToDevice, stream));
@@ -1227,17 +1255,12 @@ static qb_status maxsim_run(qb_storage* s, const uint32_t* point_offsets, uint32
     for (uint32_t e = 0; e < nqt && n_rows; ++e) QB_TRY(launch_example(s, c->d_queries_enc, c->d_q_off, e, false, c->d_ids, n_rows, d_sims + (size_t)e * n_rows, stream));
     if (scores) {
         QB_TRY(qb_launch_maxsim_fold(d_sims, n_rows, nqt, d_off, nullptr, n_pts, d_scores, nullptr, stream));
-        QB_CUDA(cudaMemcpyAsync(hs + raw_bytes, d_scores, n_pts * 4, cudaMemcpyDeviceToHost, stream));
+        QB_CUDA(cudaMemcpyAsync(h_tail, d_scores, n_pts * 4, cudaMemcpyDeviceToHost, stream));
         QB_CUDA(cudaStreamSynchronize(stream));  // also orders the reads of h_off / h_rows / point_ids before they go out of scope
-        memcpy(scores, hs + raw_bytes, n_pts * 4);
+        memcpy(scores, h_tail, n_pts * 4);
     } else {
         const uint32_t* d_del2 = nullptr;
-        if (deleted_points) {
-            const size_t words64 = (size_t)ceil_div_u64(n_points, 64);
-            QB_TRY(ensure_dev_elems(&c->d_deleted2, &c->deleted2_words, words64 * 2));
-            QB_CUDA(cudaMemcpyAsync(c->d_deleted2, deleted_points, words64 * 8, cudaMemcpyHostToDevice, stream));
-            d_del2 = c->d_deleted2;
-        }
+        QB_TRY(upload_bitmap(c, deleted_points, n_points, &d_del2));
         QB_TRY(ensure_dev_elems(&c->d_cand, &c->cand_elems, (size_t)n_pts));
         QB_TRY(ensure_dev_elems(&c->d_out, &c->out_elems, (size_t)top));
         QB_TRY(ensure_dev_elems(&c->d_out_counts, &c->out_counts_elems, (size_t)8));
@@ -1245,11 +1268,7 @@ static qb_status maxsim_run(qb_storage* s, const uint32_t* point_offsets, uint32
         emit.cand = c->d_cand; emit.cap = n_pts; emit.dense = 1; emit.dense_base = 0; emit.deleted = nullptr; emit.deleted2 = d_del2; emit.id_base = 0;
         QB_TRY(qb_launch_maxsim_fold(d_sims, n_rows, nqt, d_off, nullptr, n_pts, nullptr, &emit, stream));
         QB_TRY(qb_launch_select(c->d_cand, nullptr, n_pts, n_pts, 1, top, 0, c->d_out, c->d_out_counts, nullptr, nullptr, stream));
-        QB_CUDA(cudaMemcpyAsync(hs + raw_bytes, c->d_out, res_bytes, cudaMemcpyDeviceToHost, stream));
-        QB_CUDA(cudaMemcpyAsync(hs + raw_bytes + res_bytes, c->d_out_counts, 4, cudaMemcpyDeviceToHost, stream));
-        QB_CUDA(cudaStreamSynchronize(stream));
-        memcpy(out, hs + raw_bytes, res_bytes);
-        memcpy(out_count, hs + raw_bytes + res_bytes, 4);
+        QB_TRY(fetch_lists(c, c->d_out, c->d_out_counts, 1, top, 0, h_tail, out, out_count));
     }
     if (counters) counters->cpu += n_rows * (uint64_t)nqt * cpu_units_per_point(s);
     return QB_OK;
@@ -1307,20 +1326,16 @@ static qb_status maxsim_custom_run(qb_storage* s, const uint32_t* point_offsets,
     QB_CHECK(max_tok <= 4096, QB_ERR_INVALID, "maxsim_custom: %u vectors in one example (max 4096)", max_tok);
     QB_CHECK(n_rows * (4ull * max_tok + 4) + n_pts * (4ull * ne + 20) <= (16ull << 30), QB_ERR_UNSUPPORTED, "maxsim_custom: scratch budget exceeded");
     QB_TRY(use_device(s->device));
-    QbSearchCtx* c = nullptr;
-    QB_TRY(qb_ctx_acquire(s, &c));
-    struct Rel { qb_storage* s; QbSearchCtx* c; ~Rel() { qb_ctx_release(s, c); } } rel{s, c};
+    CtxLease lease;
+    QB_TRY(lease.acquire(s));
+    QbSearchCtx* c = lease.c;
     cudaStream_t stream = c->stream;
     const uint32_t n_coef = (kind == QB_QUERY_FEEDBACK_NAIVE) ? 1 + n_a : 0;
-    const size_t raw_bytes = (size_t)total_tok * s->dim * 4;
-    const size_t res_bytes = scores ? (size_t)n_pts * 4 : (size_t)top * sizeof(qb_scored_point);
-    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, raw_bytes + res_bytes + (size_t)n_coef * 4 + 16));
-    uint8_t* hs = reinterpret_cast<uint8_t*>(c->h_stage);
-    memcpy(hs, example_vectors, raw_bytes);
-    if (n_coef) memcpy(hs + raw_bytes + res_bytes, coef, (size_t)n_coef * 4);
-    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, round_up_u64(raw_bytes, 16) + (size_t)total_tok * pre_stride_f(s) * 4));
-    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)total_tok + 256) * qb_encoded_query_bytes(s)));
-    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)total_tok));
+    // stage tail: [the scores, or the result list and its count | coefficients]
+    const size_t coef_at = scores ? (size_t)n_pts * 4 : (size_t)top * sizeof(qb_scored_point) + 4;
+    uint8_t* h_tail = nullptr;
+    QB_TRY(stage_queries(s, c, example_vectors, total_tok, coef_at + (size_t)n_coef * 4, &h_tail));
+    if (n_coef) memcpy(h_tail + coef_at, coef, (size_t)n_coef * 4);
     QB_TRY(ensure_dev_elems(&c->d_ids, &c->ids_elems, (size_t)std::max<uint64_t>(n_rows, 1)));
     QB_TRY(ensure_dev_elems(&c->d_thr, &c->thr_elems, (size_t)n_coef + 64));
     // scratch: [token similarities max_tok x n_rows][per-example MaxSim ne x n_pts][column offsets n_pts + 1][final scores n_pts]
@@ -1331,14 +1346,11 @@ static qb_status maxsim_custom_run(qb_storage* s, const uint32_t* point_offsets,
     float* d_ex = reinterpret_cast<float*>(sc + sims_bytes);
     uint32_t* d_off = reinterpret_cast<uint32_t*>(sc + sims_bytes + ex_bytes);
     float* d_scores = reinterpret_cast<float*>(sc + sims_bytes + ex_bytes + off_bytes);
-    QB_CUDA(cudaMemcpyAsync(c->d_queries_raw, hs, raw_bytes, cudaMemcpyHostToDevice, stream));
-    QB_TRY(prepare_queries(s, reinterpret_cast<const float*>(c->d_queries_raw), total_tok,
-                           reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c->d_queries_raw) + round_up_u64(raw_bytes, 16)), c->d_queries_enc, c->d_q_off, stream));
     QB_CUDA(cudaMemcpyAsync(d_off, h_off.data(), (n_pts + 1) * 4, cudaMemcpyHostToDevice, stream));
     if (point_ids) { if (n_rows) QB_CUDA(cudaMemcpyAsync(c->d_ids, h_rows.data(), n_rows * 4, cudaMemcpyHostToDevice, stream)); }
     else QB_TRY(qb_launch_iota(c->d_ids, n_rows, stream));
     const float* d_coef = nullptr;
-    if (n_coef) { QB_CUDA(cudaMemcpyAsync(c->d_thr, hs + raw_bytes + res_bytes, (size_t)n_coef * 4, cudaMemcpyHostToDevice, stream)); d_coef = c->d_thr; }
+    if (n_coef) { QB_CUDA(cudaMemcpyAsync(c->d_thr, h_tail + coef_at, (size_t)n_coef * 4, cudaMemcpyHostToDevice, stream)); d_coef = c->d_thr; }
     for (uint32_t e = 0; e < ne; ++e) {
         const uint32_t t0 = example_offsets[e], nt = example_offsets[e + 1] - t0;
         for (uint32_t t = 0; t < nt && n_rows; ++t) QB_TRY(launch_example(s, c->d_queries_enc, c->d_q_off, t0 + t, false, c->d_ids, n_rows, d_sims + (size_t)t * n_rows, stream));
@@ -1346,17 +1358,12 @@ static qb_status maxsim_custom_run(qb_storage* s, const uint32_t* point_offsets,
     }
     if (scores) {
         QB_TRY(qb_launch_custom_combine((int)kind, n_a, n_b, d_coef, d_ex, n_pts, n_pts, d_scores, nullptr, nullptr, stream));
-        QB_CUDA(cudaMemcpyAsync(hs + raw_bytes, d_scores, n_pts * 4, cudaMemcpyDeviceToHost, stream));
+        QB_CUDA(cudaMemcpyAsync(h_tail, d_scores, n_pts * 4, cudaMemcpyDeviceToHost, stream));
         QB_CUDA(cudaStreamSynchronize(stream));
-        memcpy(scores, hs + raw_bytes, n_pts * 4);
+        memcpy(scores, h_tail, n_pts * 4);
     } else {
         const uint32_t* d_del2 = nullptr;
-        if (deleted_points) {
-            const size_t words64 = (size_t)ceil_div_u64(n_points, 64);
-            QB_TRY(ensure_dev_elems(&c->d_deleted2, &c->deleted2_words, words64 * 2));
-            QB_CUDA(cudaMemcpyAsync(c->d_deleted2, deleted_points, words64 * 8, cudaMemcpyHostToDevice, stream));
-            d_del2 = c->d_deleted2;
-        }
+        QB_TRY(upload_bitmap(c, deleted_points, n_points, &d_del2));
         QB_TRY(ensure_dev_elems(&c->d_cand, &c->cand_elems, (size_t)n_pts));
         QB_TRY(ensure_dev_elems(&c->d_out, &c->out_elems, (size_t)top));
         QB_TRY(ensure_dev_elems(&c->d_out_counts, &c->out_counts_elems, (size_t)8));
@@ -1364,11 +1371,7 @@ static qb_status maxsim_custom_run(qb_storage* s, const uint32_t* point_offsets,
         emit.cand = c->d_cand; emit.cap = n_pts; emit.dense = 1; emit.dense_base = 0; emit.deleted = nullptr; emit.deleted2 = d_del2; emit.id_base = 0;
         QB_TRY(qb_launch_custom_combine((int)kind, n_a, n_b, d_coef, d_ex, n_pts, n_pts, nullptr, nullptr, &emit, stream));
         QB_TRY(qb_launch_select(c->d_cand, nullptr, n_pts, n_pts, 1, top, 0, c->d_out, c->d_out_counts, nullptr, nullptr, stream));
-        QB_CUDA(cudaMemcpyAsync(hs + raw_bytes, c->d_out, res_bytes, cudaMemcpyDeviceToHost, stream));
-        QB_CUDA(cudaMemcpyAsync(hs + raw_bytes + res_bytes + (size_t)n_coef * 4, c->d_out_counts, 4, cudaMemcpyDeviceToHost, stream));
-        QB_CUDA(cudaStreamSynchronize(stream));
-        memcpy(out, hs + raw_bytes, res_bytes);
-        memcpy(out_count, hs + raw_bytes + res_bytes + (size_t)n_coef * 4, 4);
+        QB_TRY(fetch_lists(c, c->d_out, c->d_out_counts, 1, top, 0, h_tail, out, out_count));
     }
     if (counters) { counters->cpu += n_rows * (uint64_t)total_tok * cpu_units_per_point(s); counters->vector_io_read += n_rows * (uint64_t)ne * (s->on_disk ? 1 : 0); }
     return QB_OK;
@@ -1641,47 +1644,30 @@ extern "C" qb_status qb_hnsw_search_batch_algo(qb_hnsw* g, const float* queries,
     QB_CHECK(n_queries == 0 || queries, QB_ERR_INVALID, "hnsw_search_batch: null queries");
     QB_CHECK(top >= 1 && top <= 4096, QB_ERR_INVALID, "hnsw_search_batch: top %u outside [1,4096]", top);
     if (n_queries == 0) return QB_OK;
-    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    if (cancelled(is_stopped)) return QB_ERR_CANCELLED;
     qb_storage* s = g->st;
     QB_TRY(use_device(s->device));
     std::lock_guard<std::mutex> glk(g->mu);
-    QbSearchCtx* c = nullptr;
-    QB_TRY(qb_ctx_acquire(s, &c));
-    struct Rel { qb_storage* s; QbSearchCtx* c; ~Rel() { qb_ctx_release(s, c); } } rel{s, c};
-    cudaStream_t stream = c->stream;
-    const size_t raw_bytes = (size_t)n_queries * s->dim * 4, res_bytes = (size_t)n_queries * top * sizeof(qb_scored_point), cnt_bytes = (size_t)n_queries * 4;
-    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, raw_bytes + res_bytes + cnt_bytes + 16));
-    uint8_t* hs = reinterpret_cast<uint8_t*>(c->h_stage);
-    memcpy(hs, queries, raw_bytes);
-    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, raw_bytes + (size_t)n_queries * pre_stride_f(s) * 4));
-    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)n_queries + 256) * qb_encoded_query_bytes(s)));
-    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)n_queries));
+    CtxLease lease;
+    QB_TRY(lease.acquire(s));
+    QbSearchCtx* c = lease.c;
+    const size_t lists_bytes = (size_t)n_queries * (top * sizeof(qb_scored_point) + 4);
+    uint8_t* h_tail = nullptr;
+    QB_TRY(stage_queries(s, c, queries, n_queries, lists_bytes, &h_tail));
     QB_TRY(ensure_dev_elems(&c->d_out, &c->out_elems, (size_t)n_queries * top));
     QB_TRY(ensure_dev_elems(&c->d_out_counts, &c->out_counts_elems, (size_t)n_queries + 4));
-    QB_CUDA(cudaMemcpyAsync(c->d_queries_raw, hs, raw_bytes, cudaMemcpyHostToDevice, stream));
-    float* d_pre = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c->d_queries_raw) + raw_bytes);
-    QB_TRY(prepare_queries(s, reinterpret_cast<const float*>(c->d_queries_raw), n_queries, d_pre, c->d_queries_enc, c->d_q_off, stream));
     const uint32_t* d_del2 = nullptr;
-    if (deleted_bitmap) {
-        const uint64_t words64 = ceil_div_u64(s->count, 64);
-        QB_TRY(ensure_dev_elems(&c->d_deleted2, &c->deleted2_words, (size_t)words64 * 2));
-        QB_CUDA(cudaMemcpyAsync(c->d_deleted2, deleted_bitmap, words64 * 8, cudaMemcpyHostToDevice, stream));
-        d_del2 = c->d_deleted2;
-    }
-    QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, d_del2, c->d_out, c->d_out_counts, stream,
+    QB_TRY(upload_bitmap(c, deleted_bitmap, s->count, &d_del2));
+    QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, d_del2, c->d_out, c->d_out_counts, c->stream,
                           (int)algorithm));
-    QB_CUDA(cudaMemcpyAsync(hs + raw_bytes, c->d_out, res_bytes, cudaMemcpyDeviceToHost, stream));
-    QB_CUDA(cudaMemcpyAsync(hs + raw_bytes + res_bytes, c->d_out_counts, cnt_bytes, cudaMemcpyDeviceToHost, stream));
-    QB_CUDA(cudaStreamSynchronize(stream));
-    memcpy(out, hs + raw_bytes, res_bytes);
-    memcpy(out_counts, hs + raw_bytes + res_bytes, cnt_bytes);
+    QB_TRY(fetch_lists(c, c->d_out, c->d_out_counts, n_queries, top, 0, h_tail, out, out_counts));
     if (counters) {
         const uint64_t before = g->evals;
-        QB_TRY(qb_hnsw_read_stats(g, stream));
+        QB_TRY(qb_hnsw_read_stats(g, c->stream));
         counters->cpu += (g->evals - before) * cpu_units_per_point(s);
         counters->vector_io_read += (g->evals - before) * io_units_per_point(s);
     }
-    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    if (cancelled(is_stopped)) return QB_ERR_CANCELLED;
     return QB_OK;
 }
 
@@ -1702,10 +1688,7 @@ extern "C" qb_status qb_hnsw_search_batch_device_algo(qb_hnsw* g, const float* d
     std::lock_guard<std::mutex> glk(g->mu);
     QbSearchCtx* c = nullptr;
     QB_TRY(qb_ctx_device(s, &c));
-    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, (size_t)n_queries * pre_stride_f(s) * 4 + 256));
-    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)n_queries + 256) * qb_encoded_query_bytes(s)));
-    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)n_queries));
-    QB_TRY(prepare_queries(s, dev_queries, n_queries, reinterpret_cast<float*>(c->d_queries_raw), c->d_queries_enc, c->d_q_off, c->stream));
+    QB_TRY(encode_device_queries(s, c, dev_queries, n_queries));
     cudaEvent_t e0, e1;
     profile_begin(s, c, c->stream, &e0, &e1);
     QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, nullptr, dev_out, dev_counts, c->stream,
@@ -1742,43 +1725,26 @@ extern "C" qb_status qb_hnsw_search_with_vectors_batch(qb_hnsw* g, const float* 
     QB_CHECK(top >= 1 && top <= 4096, QB_ERR_INVALID, "hnsw_search_with_vectors_batch: top %u outside [1,4096]", top);
     QB_CHECK(g->d_blob, QB_ERR_UNSUPPORTED, "hnsw_search_with_vectors_batch: the graph has no inline vectors (load it with qb_hnsw_create_with_vectors)");
     if (n_queries == 0) return QB_OK;
-    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    if (cancelled(is_stopped)) return QB_ERR_CANCELLED;
     qb_storage* s = g->st;
     QB_TRY(use_device(s->device));
     std::lock_guard<std::mutex> glk(g->mu);
-    QbSearchCtx* c = nullptr;
-    QB_TRY(qb_ctx_acquire(s, &c));
-    struct Rel { qb_storage* s; QbSearchCtx* c; ~Rel() { qb_ctx_release(s, c); } } rel{s, c};
-    cudaStream_t stream = c->stream;
-    const size_t raw_bytes = (size_t)n_queries * s->dim * 4, res_bytes = (size_t)n_queries * top * sizeof(qb_scored_point), cnt_bytes = (size_t)n_queries * 4;
-    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, raw_bytes + res_bytes + cnt_bytes + 16));
-    uint8_t* hs = reinterpret_cast<uint8_t*>(c->h_stage);
-    memcpy(hs, queries, raw_bytes);
-    const size_t pre_off = round_up_u64(raw_bytes, 16);
-    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, pre_off + (size_t)n_queries * pre_stride_f(s) * 4));
-    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)n_queries + 256) * qb_encoded_query_bytes(s)));
-    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)n_queries));
+    CtxLease lease;
+    QB_TRY(lease.acquire(s));
+    QbSearchCtx* c = lease.c;
+    const size_t lists_bytes = (size_t)n_queries * (top * sizeof(qb_scored_point) + 4);
+    uint8_t* h_tail = nullptr;
+    float* d_pre = nullptr;
+    QB_TRY(stage_queries(s, c, queries, n_queries, lists_bytes, &h_tail, &d_pre));
     QB_TRY(ensure_dev_elems(&c->d_out, &c->out_elems, (size_t)n_queries * top));
     QB_TRY(ensure_dev_elems(&c->d_out_counts, &c->out_counts_elems, (size_t)n_queries + 4));
-    QB_CUDA(cudaMemcpyAsync(c->d_queries_raw, hs, raw_bytes, cudaMemcpyHostToDevice, stream));
-    float* d_pre = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c->d_queries_raw) + pre_off);
-    QB_TRY(prepare_queries(s, reinterpret_cast<const float*>(c->d_queries_raw), n_queries, d_pre, c->d_queries_enc, c->d_q_off, stream));
     const uint32_t* d_del2 = nullptr;
-    if (deleted_bitmap) {
-        const uint64_t words64 = ceil_div_u64(s->count, 64);
-        QB_TRY(ensure_dev_elems(&c->d_deleted2, &c->deleted2_words, (size_t)words64 * 2));
-        QB_CUDA(cudaMemcpyAsync(c->d_deleted2, deleted_bitmap, words64 * 8, cudaMemcpyHostToDevice, stream));
-        d_del2 = c->d_deleted2;
-    }
+    QB_TRY(upload_bitmap(c, deleted_bitmap, s->count, &d_del2));
     QB_TRY(qb_hnsw_inline_launch(g, d_pre, pre_stride_f(s), c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, d_del2, c->d_out,
-                                 c->d_out_counts, stream));
-    QB_CUDA(cudaMemcpyAsync(hs + raw_bytes, c->d_out, res_bytes, cudaMemcpyDeviceToHost, stream));
-    QB_CUDA(cudaMemcpyAsync(hs + raw_bytes + res_bytes, c->d_out_counts, cnt_bytes, cudaMemcpyDeviceToHost, stream));
-    QB_CUDA(cudaStreamSynchronize(stream));
-    memcpy(out, hs + raw_bytes, res_bytes);
-    memcpy(out_counts, hs + raw_bytes + res_bytes, cnt_bytes);
-    QB_TRY(hnsw_with_vectors_counters(g, n_queries, stream, counters));
-    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+                                 c->d_out_counts, c->stream));
+    QB_TRY(fetch_lists(c, c->d_out, c->d_out_counts, n_queries, top, 0, h_tail, out, out_counts));
+    QB_TRY(hnsw_with_vectors_counters(g, n_queries, c->stream, counters));
+    if (cancelled(is_stopped)) return QB_ERR_CANCELLED;
     return QB_OK;
 }
 
@@ -1793,11 +1759,8 @@ extern "C" qb_status qb_hnsw_search_with_vectors_batch_device(qb_hnsw* g, const 
     std::lock_guard<std::mutex> glk(g->mu);
     QbSearchCtx* c = nullptr;
     QB_TRY(qb_ctx_device(s, &c));
-    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, (size_t)n_queries * pre_stride_f(s) * 4 + 256));
-    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)n_queries + 256) * qb_encoded_query_bytes(s)));
-    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)n_queries));
-    float* d_pre = reinterpret_cast<float*>(c->d_queries_raw);
-    QB_TRY(prepare_queries(s, dev_queries, n_queries, d_pre, c->d_queries_enc, c->d_q_off, c->stream));
+    float* d_pre = nullptr;
+    QB_TRY(encode_device_queries(s, c, dev_queries, n_queries, &d_pre));
     cudaEvent_t e0, e1;
     profile_begin(s, c, c->stream, &e0, &e1);
     QB_TRY(qb_hnsw_inline_launch(g, d_pre, pre_stride_f(s), c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, nullptr, dev_out,
@@ -1825,55 +1788,36 @@ extern "C" qb_status qb_hnsw_search_maxsim_batch(qb_hnsw* g, const float* query_
         QB_CHECK(nqv >= 1 && nqv <= 4096, QB_ERR_INVALID, "hnsw_search_maxsim_batch: query %u has %u vectors (need 1..4096)", i, nqv);
         max_q = std::max(max_q, nqv);
     }
-    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    if (cancelled(is_stopped)) return QB_ERR_CANCELLED;
     qb_storage* s = g->st;
     QB_TRY(use_device(s->device));
     std::lock_guard<std::mutex> glk(g->mu);
-    QbSearchCtx* c = nullptr;
-    QB_TRY(qb_ctx_acquire(s, &c));
-    struct Rel { qb_storage* s; QbSearchCtx* c; ~Rel() { qb_ctx_release(s, c); } } rel{s, c};
-    cudaStream_t stream = c->stream;
+    CtxLease lease;
+    QB_TRY(lease.acquire(s));
+    QbSearchCtx* c = lease.c;
     const uint32_t nv = query_offsets[n_queries];   // vectors before query_offsets[0] are uploaded and not read
-    const size_t raw_bytes = (size_t)nv * s->dim * 4, res_bytes = (size_t)n_queries * top * sizeof(qb_scored_point), cnt_bytes = (size_t)n_queries * 4;
-    const size_t off_bytes = ((size_t)n_queries + 1) * 4;
-    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, raw_bytes + off_bytes + res_bytes + cnt_bytes + 16));
-    uint8_t* hs = reinterpret_cast<uint8_t*>(c->h_stage);
-    memcpy(hs, query_vectors, raw_bytes);
-    memcpy(hs + raw_bytes, query_offsets, off_bytes);
-    uint8_t* h_res = hs + raw_bytes + off_bytes;
-    const size_t pre_off = round_up_u64(raw_bytes, 16);
-    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, pre_off + (size_t)nv * pre_stride_f(s) * 4));
-    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)nv + 256) * qb_encoded_query_bytes(s)));
-    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)nv));
+    // stage tail: [query offsets | result lists | counts]
+    const size_t off_bytes = ((size_t)n_queries + 1) * 4, lists_bytes = (size_t)n_queries * (top * sizeof(qb_scored_point) + 4);
+    uint8_t* h_tail = nullptr;
+    QB_TRY(stage_queries(s, c, query_vectors, nv, off_bytes + lists_bytes, &h_tail));
+    memcpy(h_tail, query_offsets, off_bytes);
     QB_TRY(ensure_dev_elems(&c->d_ids, &c->ids_elems, (size_t)n_queries + 1));
     QB_TRY(ensure_dev_elems(&c->d_out, &c->out_elems, (size_t)n_queries * top));
     QB_TRY(ensure_dev_elems(&c->d_out_counts, &c->out_counts_elems, (size_t)n_queries + 4));
-    QB_CUDA(cudaMemcpyAsync(c->d_queries_raw, hs, raw_bytes, cudaMemcpyHostToDevice, stream));
-    QB_CUDA(cudaMemcpyAsync(c->d_ids, hs + raw_bytes, off_bytes, cudaMemcpyHostToDevice, stream));
-    float* d_pre = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c->d_queries_raw) + pre_off);
-    QB_TRY(prepare_queries(s, reinterpret_cast<const float*>(c->d_queries_raw), nv, d_pre, c->d_queries_enc, c->d_q_off, stream));
+    QB_CUDA(cudaMemcpyAsync(c->d_ids, h_tail, off_bytes, cudaMemcpyHostToDevice, c->stream));
     const uint32_t* d_del2 = nullptr;
-    if (deleted_points) {
-        const uint64_t words64 = ceil_div_u64(g->n_points, 64);   // a bitmap over points, as qb_search_maxsim takes it
-        QB_TRY(ensure_dev_elems(&c->d_deleted2, &c->deleted2_words, (size_t)words64 * 2));
-        QB_CUDA(cudaMemcpyAsync(c->d_deleted2, deleted_points, words64 * 8, cudaMemcpyHostToDevice, stream));
-        d_del2 = c->d_deleted2;
-    }
+    QB_TRY(upload_bitmap(c, deleted_points, g->n_points, &d_del2));   // a bitmap over points, as qb_search_maxsim takes it
     const QbHnswMaxsim mv{c->d_ids, nv, max_q};
-    QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, d_del2, c->d_out, c->d_out_counts, stream,
+    QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, d_del2, c->d_out, c->d_out_counts, c->stream,
                           (int)algorithm, nullptr, &mv));
-    QB_CUDA(cudaMemcpyAsync(h_res, c->d_out, res_bytes, cudaMemcpyDeviceToHost, stream));
-    QB_CUDA(cudaMemcpyAsync(h_res + res_bytes, c->d_out_counts, cnt_bytes, cudaMemcpyDeviceToHost, stream));
-    QB_CUDA(cudaStreamSynchronize(stream));
-    memcpy(out, h_res, res_bytes);
-    memcpy(out_counts, h_res + res_bytes, cnt_bytes);
+    QB_TRY(fetch_lists(c, c->d_out, c->d_out_counts, n_queries, top, 0, h_tail + off_bytes, out, out_counts));
     if (counters) {
         const uint64_t rows0 = g->mv_rows, qrows0 = g->mv_qrows;
-        QB_TRY(qb_hnsw_read_stats(g, stream));
+        QB_TRY(qb_hnsw_read_stats(g, c->stream));
         counters->cpu += (g->mv_qrows - qrows0) * cpu_units_per_point(s);
         counters->vector_io_read += (g->mv_rows - rows0) * io_units_per_point(s);
     }
-    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    if (cancelled(is_stopped)) return QB_ERR_CANCELLED;
     return QB_OK;
 }
 
@@ -1892,10 +1836,7 @@ extern "C" qb_status qb_hnsw_search_maxsim_batch_device(qb_hnsw* g, const float*
     std::lock_guard<std::mutex> glk(g->mu);
     QbSearchCtx* c = nullptr;
     QB_TRY(qb_ctx_device(s, &c));
-    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, (size_t)n_query_vectors * pre_stride_f(s) * 4 + 256));
-    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)n_query_vectors + 256) * qb_encoded_query_bytes(s)));
-    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)n_query_vectors));
-    QB_TRY(prepare_queries(s, dev_query_vectors, n_query_vectors, reinterpret_cast<float*>(c->d_queries_raw), c->d_queries_enc, c->d_q_off, c->stream));
+    QB_TRY(encode_device_queries(s, c, dev_query_vectors, n_query_vectors));
     cudaEvent_t e0, e1;
     profile_begin(s, c, c->stream, &e0, &e1);
     const QbHnswMaxsim mv{dev_query_offsets, n_query_vectors, max_query_vectors};
@@ -1930,33 +1871,20 @@ static qb_status hnsw_custom_run(qb_hnsw* g, qb_query_kind kind, const float* ve
         }
     }
     if (n_queries == 0) return QB_OK;
-    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    if (cancelled(is_stopped)) return QB_ERR_CANCELLED;
     QB_TRY(use_device(s->device));
     std::lock_guard<std::mutex> glk(g->mu);
-    QbSearchCtx* c = nullptr;
-    QB_TRY(qb_ctx_acquire(s, &c));
-    struct Rel { qb_storage* s; QbSearchCtx* c; ~Rel() { qb_ctx_release(s, c); } } rel{s, c};
+    CtxLease lease;
+    QB_TRY(lease.acquire(s));
+    QbSearchCtx* c = lease.c;
     cudaStream_t stream = c->stream;
-    const size_t nv = (size_t)n_queries * ne;   // example vectors, encoded back to back: query q's are [q * ne, (q + 1) * ne)
-    const size_t raw_bytes = nv * s->dim * 4, res_bytes = (size_t)n_queries * top * sizeof(qb_scored_point), cnt_bytes = (size_t)n_queries * 4;
-    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, raw_bytes + res_bytes + cnt_bytes + 16));
-    uint8_t* hs = reinterpret_cast<uint8_t*>(c->h_stage);
-    memcpy(hs, vectors, raw_bytes);
-    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, raw_bytes + nv * pre_stride_f(s) * 4));
-    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, (nv + 256) * qb_encoded_query_bytes(s)));
-    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, nv));
+    // example vectors, encoded back to back: query q's are [q * ne, (q + 1) * ne)
+    uint8_t* h_tail = nullptr;
+    QB_TRY(stage_queries(s, c, vectors, n_queries * ne, (size_t)n_queries * (top * sizeof(qb_scored_point) + 4), &h_tail));
     QB_TRY(ensure_dev_elems(&c->d_out, &c->out_elems, (size_t)n_queries * top));
     QB_TRY(ensure_dev_elems(&c->d_out_counts, &c->out_counts_elems, (size_t)n_queries + 4));
-    QB_CUDA(cudaMemcpyAsync(c->d_queries_raw, hs, raw_bytes, cudaMemcpyHostToDevice, stream));
-    float* d_pre = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c->d_queries_raw) + raw_bytes);
-    QB_TRY(prepare_queries(s, reinterpret_cast<const float*>(c->d_queries_raw), (uint32_t)nv, d_pre, c->d_queries_enc, c->d_q_off, stream));
     const uint32_t* d_del2 = nullptr;
-    if (deleted_bitmap) {
-        const uint64_t words64 = ceil_div_u64(s->count, 64);
-        QB_TRY(ensure_dev_elems(&c->d_deleted2, &c->deleted2_words, (size_t)words64 * 2));
-        QB_CUDA(cudaMemcpyAsync(c->d_deleted2, deleted_bitmap, words64 * 8, cudaMemcpyHostToDevice, stream));
-        d_del2 = c->d_deleted2;
-    }
+    QB_TRY(upload_bitmap(c, deleted_bitmap, s->count, &d_del2));
     // per-call buffers: coefficients, custom entry points (as scored points: the stage-1 lists of discover have that layout), counts
     constexpr uint32_t DISCOVERY_ENTRY_POINT_COUNT = 10;   // search.rs:325
     const uint32_t n_coef = fb ? 1 + n_a : 0;
@@ -1992,11 +1920,7 @@ static qb_status hnsw_custom_run(qb_hnsw* g, qb_query_kind kind, const float* ve
     QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, d_del2, c->d_out, c->d_out_counts, stream,
                           (int)algorithm, &cq));
     profile_end(s, stream, e0, e1);
-    QB_CUDA(cudaMemcpyAsync(hs + raw_bytes, c->d_out, res_bytes, cudaMemcpyDeviceToHost, stream));
-    QB_CUDA(cudaMemcpyAsync(hs + raw_bytes + res_bytes, c->d_out_counts, cnt_bytes, cudaMemcpyDeviceToHost, stream));
-    QB_CUDA(cudaStreamSynchronize(stream));
-    memcpy(out, hs + raw_bytes, res_bytes);
-    memcpy(out_counts, hs + raw_bytes + res_bytes, cnt_bytes);
+    QB_TRY(fetch_lists(c, c->d_out, c->d_out_counts, n_queries, top, 0, h_tail, out, out_counts));
     if (counters) {
         // per scored point: E similarities of cpu units, one read of the vector (custom_query_scorer.rs:78-111, qb_score_points)
         uint64_t ev[2] = {0, 0};
@@ -2004,7 +1928,7 @@ static qb_status hnsw_custom_run(qb_hnsw* g, qb_query_kind kind, const float* ve
         counters->cpu += (ev[0] * ne + ev[1] * (2ull * n_a)) * cpu_units_per_point(s);
         counters->vector_io_read += (ev[0] + ev[1]) * io_units_per_point(s);
     }
-    if (is_stopped && *is_stopped) { qb_set_error("search cancelled"); return QB_ERR_CANCELLED; }
+    if (cancelled(is_stopped)) return QB_ERR_CANCELLED;
     return QB_OK;
 }
 
@@ -2049,17 +1973,15 @@ extern "C" qb_status qb_multi_search_batch(qb_comm* cm, qb_storage* s, const flo
     if (n_queries == 0) return QB_OK;
     QB_TRY(use_device(s->device));
     std::lock_guard<std::mutex> clk(cm->mu);
-    QbSearchCtx* c = nullptr;
-    QB_TRY(qb_ctx_acquire(s, &c));
-    struct Rel { qb_storage* s; QbSearchCtx* c; ~Rel() { qb_ctx_release(s, c); } } rel{s, c};
+    CtxLease lease;
+    QB_TRY(lease.acquire(s));
+    QbSearchCtx* c = lease.c;
     cudaStream_t stream = c->stream;
-    const size_t raw_bytes = (size_t)n_queries * s->dim * 4, res_bytes = (size_t)n_queries * top * sizeof(qb_scored_point), cnt_bytes = (size_t)n_queries * 4;
-    QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, raw_bytes + res_bytes + cnt_bytes + 32));
-    uint8_t* hs = reinterpret_cast<uint8_t*>(c->h_stage);
-    memcpy(hs, queries, raw_bytes);
-    QB_TRY(qb_ensure_device(&c->d_queries_raw, &c->queries_raw_bytes, raw_bytes + (size_t)n_queries * pre_stride_f(s) * 4));
-    QB_TRY(qb_ensure_device(&c->d_queries_enc, &c->queries_enc_bytes, ((size_t)n_queries + 256) * qb_encoded_query_bytes(s)));
-    QB_TRY(ensure_dev_elems(&c->d_q_off, &c->q_off_elems, (size_t)n_queries));
+    // stage tail: [result lists | counts | flags word | exchange error]
+    const size_t res_bytes = (size_t)n_queries * top * sizeof(qb_scored_point), cnt_bytes = (size_t)n_queries * 4;
+    uint8_t* h_res = nullptr;
+    QB_TRY(stage_queries(s, c, queries, n_queries, res_bytes + cnt_bytes + 8, &h_res));
+    uint8_t* h_cnt = h_res + res_bytes;
     QB_TRY(ensure_dev_elems(&c->d_out, &c->out_elems, (size_t)n_queries * top));
     QB_TRY(ensure_dev_elems(&c->d_out_counts, &c->out_counts_elems, (size_t)n_queries + 4));
     if (cm->local_cap < (size_t)n_queries * top) {
@@ -2068,48 +1990,19 @@ extern "C" qb_status qb_multi_search_batch(qb_comm* cm, qb_storage* s, const flo
         QB_CUDA(cudaMalloc(&cm->d_local_cnt, ((size_t)n_queries * top + 4) * 4));
         cm->local_cap = (size_t)n_queries * top;
     }
-    QB_CUDA(cudaMemcpyAsync(c->d_queries_raw, hs, raw_bytes, cudaMemcpyHostToDevice, stream));
-    float* d_pre = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(c->d_queries_raw) + raw_bytes);
-    QB_TRY(prepare_queries(s, reinterpret_cast<const float*>(c->d_queries_raw), n_queries, d_pre, c->d_queries_enc, c->d_q_off, stream));
     const uint32_t* d_del2 = nullptr;
-    if (deleted_bitmap) {
-        const uint64_t words64 = ceil_div_u64(s->count, 64);
-        QB_TRY(ensure_dev_elems(&c->d_deleted2, &c->deleted2_words, (size_t)words64 * 2));
-        QB_CUDA(cudaMemcpyAsync(c->d_deleted2, deleted_bitmap, words64 * 8, cudaMemcpyHostToDevice, stream));
-        d_del2 = c->d_deleted2;
-    }
-    unsigned int* d_overflow = reinterpret_cast<unsigned int*>(cm->d_local_cnt + (size_t)n_queries * top);
-    uint8_t* h_res = hs + raw_bytes;
-    uint8_t* h_cnt = h_res + res_bytes;
-    uint32_t rs_flags = 0;
-    qb_status st_local = QB_OK;
-    for (int attempt = 0; attempt < 4; ++attempt) {
-        QB_CUDA(cudaMemsetAsync(d_overflow, 0, 4, stream));
-        bool can_flag = true;
-        st_local = run_search(s, c, n_queries, top, nullptr, 0, d_del2, is_stopped, rs_flags, cm->d_local, cm->d_local_cnt, d_overflow, &can_flag);
-        if (st_local != QB_OK || !can_flag) break;
-        QB_CUDA(cudaMemcpyAsync(h_cnt + cnt_bytes, d_overflow, 4, cudaMemcpyDeviceToHost, stream));
-        QB_CUDA(cudaStreamSynchronize(stream));
-        unsigned int flags = 0;
-        memcpy(&flags, h_cnt + cnt_bytes, 4);
-        uint32_t next = rs_flags;
-        if (flags & 8u) next |= RS_NO_SEGMENTS;
-        if (flags & 2u) next |= RS_NO_MMA;
-        if (flags & 1u) next |= RS_FORCE_DIRECT | RS_NO_MMA;
-        if (next == rs_flags) break;
-        s->n_reruns.fetch_add(1, std::memory_order_relaxed);
-        rs_flags = next;
-    }
-    s->n_searches.fetch_add(1, std::memory_order_relaxed);
+    QB_TRY(upload_bitmap(c, deleted_bitmap, s->count, &d_del2));
+    unsigned int* d_flags = reinterpret_cast<unsigned int*>(cm->d_local_cnt + (size_t)n_queries * top);
+    const qb_status st_local = search_with_reruns(s, c, n_queries, top, nullptr, 0, d_del2, is_stopped, cm->d_local, cm->d_local_cnt, d_flags, h_cnt + cnt_bytes);
     // a rank that failed locally still joins the exchange (with empty lists) so that its peers do not wait for it
     if (st_local != QB_OK) QB_CUDA(cudaMemsetAsync(cm->d_local_cnt, 0, (size_t)n_queries * 4, stream));
     QB_TRY(qb_comm_exchange_merge(cm, cm->d_local, cm->d_local_cnt, n_queries, top, c->d_out, c->d_out_counts, stream));
     QB_CUDA(cudaMemcpyAsync(h_res, c->d_out, res_bytes, cudaMemcpyDeviceToHost, stream));
     QB_CUDA(cudaMemcpyAsync(h_cnt, c->d_out_counts, cnt_bytes, cudaMemcpyDeviceToHost, stream));
-    QB_CUDA(cudaMemcpyAsync(h_cnt + cnt_bytes + 8, cm->d_error, 4, cudaMemcpyDeviceToHost, stream));
+    QB_CUDA(cudaMemcpyAsync(h_cnt + cnt_bytes + 4, cm->d_error, 4, cudaMemcpyDeviceToHost, stream));
     QB_CUDA(cudaStreamSynchronize(stream));
     unsigned int xerr = 0;
-    memcpy(&xerr, h_cnt + cnt_bytes + 8, 4);
+    memcpy(&xerr, h_cnt + cnt_bytes + 4, 4);
     QB_CHECK(xerr == 0, QB_ERR_CUDA, "multi_search_batch: a peer rank never joined the exchange (timeout)");
     if (st_local != QB_OK) return st_local;
     memcpy(out, h_res, res_bytes);
