@@ -76,6 +76,25 @@ impl<'a> B200Hnsw<'a> {
         Ok((Self { raw, _storage: std::marker::PhantomData }, (entry, level as usize)))
     }
 
+    /// Builds the graph over the POINTS of a multivector named vector on the device (qb_hnsw_build_multivector): `build`'s schedule
+    /// with MaxSim between stored points, point p being token rows [point_offsets[p], point_offsets[p + 1]) of the dense f32 `tokens`.
+    /// `levels`: one per point; `deleted`: a bitmap over points (not inserted), or None.  Search it with `search_maxsim`.  Returns the
+    /// graph and its entry point (id, level).
+    pub fn build_multivector(tokens: &'a B200Storage, point_offsets: &[u32], m: usize, m0: usize, ef_construct: usize, levels: &[u8],
+                             deleted: Option<&[u64]>, batch: usize, serial_points: usize) -> OperationResult<(Self, (PointOffsetType, usize))> {
+        if point_offsets.len() != levels.len() + 1 {
+            return Err(OperationError::service_error("levels and point_offsets disagree on the point count"));
+        }
+        let mut raw = std::ptr::null_mut();
+        let (mut entry, mut level) = (0u32, 0u32);
+        let st = unsafe {
+            qb_hnsw_build_multivector(tokens.raw, point_offsets.as_ptr(), levels.len() as u32, m as u32, m0 as u32, ef_construct as u32, levels.as_ptr(),
+                                      deleted.map_or(std::ptr::null(), |d| d.as_ptr()), batch as u32, serial_points as u32, &mut raw, &mut entry, &mut level)
+        };
+        if st != QB_OK { return Err(OperationError::service_error(last_error())); }
+        Ok((Self { raw, _storage: std::marker::PhantomData }, (entry, level as usize)))
+    }
+
     /// The graph as a plain `links.bin` (GraphLinksFormat::Plain), whichever way it was made.
     pub fn export_plain(&self) -> OperationResult<Vec<u8>> {
         let mut n = 0u64;

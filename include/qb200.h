@@ -481,6 +481,26 @@ QB_API qb_status qb_hnsw_create_plain_multivector(qb_storage* tokens, const uint
                                                   uint64_t n_bytes, uint32_t m, uint32_t m0, qb_hnsw** out);
 QB_API qb_status qb_hnsw_create_compressed_multivector(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, const uint8_t* bytes,
                                                        uint64_t n_bytes, qb_hnsw** out);
+/* Builds the graph over the POINTS of a multivector collection on the device: qb_hnsw_build's schedule and arithmetic (levels
+ * descending then id, serial_points batches of one, batches of at most `batch` cut where the level changes, two-phase backlinks), so the
+ * graph is a pure function of its inputs, with every score the MaxSim S(a, b) of two stored points: point a's token rows are the
+ * query, scored against point b's rows with the arithmetic of qb_hnsw_search_maxsim_batch (per query row the sequential `sim > max`
+ * fold from -inf, the maxima summed in row order from +0.0).  An insert's search scores S(inserted, p); the heuristic keeps a
+ * candidate c unless S(c, kept) > S(inserted, c) for a kept link; connect_with_heuristic scores S(target, link)
+ * (MultiMetricQueryScorer::score_internal behind FilteredScorer::new_internal, multi_metric_query_scorer.rs:64-121).
+ *   tokens, point_offsets, n_points   the layout qb_hnsw_create_plain_multivector takes, checked the same way (QB_ERR_INVALID)
+ *   deleted_points  optional bitmap over POINTS, ceil(n_points / 64) words: such a point is not inserted, keeps its level and has
+ *                   no links.  The token storage's resident flags are per row and do not apply.
+ * The query is the stored token rows as they are, as qb_scorer_create_internal and qb_hnsw_build use them; the reference passes
+ * them through Metric::preprocess again, which leaves a cosine row unchanged when its squared length is within 1e-6 of 1
+ * (spaces/tools.rs:14-16), so the two agree on rows the storage normalised.  A point with no token rows scores +0.0 against every
+ * point as the query and -inf as the scored point.  Errors: f16 / u8 / SQ8 / PQ / BQ tokens, m or m0 > 64 or ef > 4096:
+ * QB_ERR_UNSUPPORTED (build over the f32 tokens, then bind the exported graph to the quantized storage); bad offsets, a level > 30,
+ * n_points = 0 or every point deleted: QB_ERR_INVALID.  The result is the handle qb_hnsw_create_plain_multivector would make from the
+ * graph's plain links.bin with the same offsets: search it with qb_hnsw_search_maxsim_batch.  Synchronous. */
+QB_API qb_status qb_hnsw_build_multivector(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, uint32_t m, uint32_t m0,
+                                           uint32_t ef_construct, const uint8_t* levels /* n_points */, const uint64_t* deleted_points,
+                                           uint32_t batch, uint32_t serial_points, qb_hnsw** out, uint32_t* entry_point, uint32_t* entry_level);
 /* GraphLayers::search (graph_layers.rs:530-561) with a MaxSim FilteredScorer, for a batch of multivector queries, on a
  * qb_hnsw_create_*_multivector handle (QB_ERR_UNSUPPORTED on any other).  Replaces the per-hop qb_score_maxsim boundary.
  *   query i         rows [query_offsets[i], query_offsets[i+1]) of query_vectors (raw f32 x dim), 1..4096 vectors each

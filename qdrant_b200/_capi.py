@@ -107,6 +107,7 @@ SIGNATURES = {
     "qb_hnsw_search_with_vectors_batch": (C.c_int32, [vp, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, u64p, i32p,
                                                       C.POINTER(ScoredPoint), u32p, C.POINTER(HwCounters)]),
     "qb_hnsw_search_with_vectors_batch_device": (C.c_int32, [vp, vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, vp, vp]),
+    "qb_hnsw_build_multivector": (C.c_int32, [vp, u32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, u8p, u64p, C.c_uint32, C.c_uint32, C.POINTER(vp), u32p, u32p]),
     "qb_hnsw_create_plain_multivector": (C.c_int32, [vp, u32p, C.c_uint32, u8p, C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(vp)]),
     "qb_hnsw_create_compressed_multivector": (C.c_int32, [vp, u32p, C.c_uint32, u8p, C.c_uint64, C.POINTER(vp)]),
     "qb_hnsw_search_maxsim_batch": (C.c_int32, [vp, f32p, u32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, u64p, i32p,

@@ -416,7 +416,7 @@ extern "C" qb_status qb_hnsw_create_compressed(qb_storage* s, const uint8_t* byt
 // The graph of a multivector named vector links POINTS; the scorer behind its search is MaxSim over each point's token rows
 // (MultiMetricQueryScorer, multi_metric_query_scorer.rs; QuantizedMultivectorStorage, quantized_multivector_storage/mod.rs:328-352).
 // The loaders are the regular ones with the point count taken from the collection, plus the token offsets on the device.
-static qb_status mv_check(qb_storage* s, const uint32_t* point_offsets, uint32_t n_points, const char* who) {
+qb_status qb_hnsw_mv_check(qb_storage* s, const uint32_t* point_offsets, uint32_t n_points, const char* who) {
     QB_CHECK(s && point_offsets, QB_ERR_INVALID, "%s: null argument", who);
     QB_CHECK((s->kind == QB_KIND_DENSE && s->dtype == QB_DT_F32) || s->kind == QB_KIND_SQ8, QB_ERR_UNSUPPORTED,
              "%s: device MaxSim traversal supports dense f32 and SQ8 token storages", who);
@@ -443,7 +443,7 @@ extern "C" qb_status qb_hnsw_create_plain_multivector(qb_storage* tokens, const 
                                                       uint64_t n_bytes, uint32_t m, uint32_t m0, qb_hnsw** out) {
     QB_CHECK(out, QB_ERR_INVALID, "hnsw_create_plain_multivector: null argument");
     *out = nullptr;
-    QB_TRY(mv_check(tokens, point_offsets, n_points, "hnsw_create_plain_multivector"));
+    QB_TRY(qb_hnsw_mv_check(tokens, point_offsets, n_points, "hnsw_create_plain_multivector"));
     qb_hnsw* g = nullptr;
     QB_TRY(hnsw_create_plain_n(tokens, n_points, "collection", links_bin, n_bytes, m, m0, &g));
     const qb_status st = mv_attach(g, point_offsets, n_points, "hnsw_create_plain_multivector");
@@ -456,7 +456,7 @@ extern "C" qb_status qb_hnsw_create_compressed_multivector(qb_storage* tokens, c
                                                            uint64_t n_bytes, qb_hnsw** out) {
     QB_CHECK(out, QB_ERR_INVALID, "hnsw_create_compressed_multivector: null argument");
     *out = nullptr;
-    QB_TRY(mv_check(tokens, point_offsets, n_points, "hnsw_create_compressed_multivector"));
+    QB_TRY(qb_hnsw_mv_check(tokens, point_offsets, n_points, "hnsw_create_compressed_multivector"));
     qb_hnsw* g = nullptr;
     QB_TRY(hnsw_create_compressed_n(tokens, n_points, "collection", bytes, n_bytes, &g));
     const qb_status st = mv_attach(g, point_offsets, n_points, "hnsw_create_compressed_multivector");

@@ -21,19 +21,10 @@
 // prefix before the first HNSW_EMPTY).  Level 0 is [n][m0] by id, level l >= 1 [N_l][m] by position in the sorted order (the
 // reference's remap), which is also the plain format's row order, so the finish is a count, a scan and a copy.
 // The insert is hnsw_search_kernel<..., ALGO_BUILD> (qb_hnsw_traverse.cuh): the search kernel's beam search on the level's rows.
-#include <cub/device/device_radix_sort.cuh>
-#include <cub/device/device_scan.cuh>
-
-#include <algorithm>
-#include <vector>
-
-#include "qb_hnsw_traverse.cuh"
+// The host side (the plan, the level loop, the finish) is in qb_hnsw_build.cuh, shared with the multivector build (qb_hnsw_build_mv.cu).
+#include "qb_hnsw_build.cuh"
 
 namespace {
-
-constexpr int HB_THREADS = 128;       // insert kernel: threads per CTA (one point per CTA at a time)
-constexpr int HB_WARPS = 4;           // backlink kernel: warps per CTA (one target per warp at a time)
-constexpr uint32_t HB_MAX_LEVEL = 30; // the highest level a point may have (levels are u8; 30 keeps the per-level tables small)
 
 // connect_with_heuristic (links_container.rs:139-...) of every target in keys[0 .. n) (sorted; key = target << 32 | position, ~0 = none)
 // with its sources vals[] in position order, one warp per target.  A short list appends; a full one is re-scored against the target
@@ -95,59 +86,9 @@ __global__ void __launch_bounds__(HB_WARPS * 32) hnsw_backlink_kernel(const Hnsw
     }
 }
 
-// the build tables of every level, for the finish
-struct HbTables {
-    const uint32_t* t[HB_MAX_LEVEL + 1];
-    uint64_t lo[HB_MAX_LEVEL + 2];   // first row of each level in the plain order; lo[levels] = rows
-    uint32_t levels, m, m0;
-};
-__device__ __forceinline__ const uint32_t* hb_row(const HbTables& tb, uint64_t r, uint32_t& lm) {
-    uint32_t l = 0;
-    while (l + 1 < tb.levels && r >= tb.lo[l + 1]) ++l;
-    lm = l ? tb.m : tb.m0;
-    return tb.t[l] + (r - tb.lo[l]) * lm;
-}
-// links per row (counts[rows] = 0, so the exclusive scan ends on the total)
-__global__ void hnsw_build_counts_kernel(const HbTables tb, uint64_t* __restrict__ counts) {
-    const uint64_t rows = tb.lo[tb.levels];
-    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r <= rows; r += (uint64_t)gridDim.x * blockDim.x) {
-        uint64_t c = 0;
-        if (r < rows) {
-            uint32_t lm;
-            const uint32_t* row = hb_row(tb, r, lm);
-            while (c < lm && row[c] != HNSW_EMPTY) ++c;
-        }
-        counts[r] = c;
-    }
-}
-__global__ void hnsw_build_neighbors_kernel(const HbTables tb, const uint64_t* __restrict__ offsets, uint32_t* __restrict__ neighbors) {
-    const uint64_t rows = tb.lo[tb.levels];
-    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (uint64_t)gridDim.x * blockDim.x) {
-        uint32_t lm;
-        const uint32_t* row = hb_row(tb, r, lm);
-        const uint64_t b = offsets[r], e = offsets[r + 1];
-        for (uint64_t k = 0; k < e - b; ++k) neighbors[b + k] = row[k];
-    }
-}
-
-// device temporaries of one call, freed on every exit path
-struct HbScratch {
-    std::vector<void*> bufs;
-    cudaError_t alloc(void** p, size_t bytes) {
-        *p = nullptr;
-        const cudaError_t e = cudaMalloc(p, std::max<size_t>(bytes, 256));
-        if (e == cudaSuccess) bufs.push_back(*p);
-        return e;
-    }
-    ~HbScratch() { cudaDeviceSynchronize(); for (void* b : bufs) cudaFree(b); }
-};
-
-inline unsigned hb_grid(uint64_t items, uint64_t per_block, uint64_t max_blocks) {
-    return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(ceil_div_u64(items, per_block), max_blocks));
-}
-
 template <int KIND, int METRIC>
 struct HbKernels {
+    using Params = HnswParams;
     static qb_status insert(const HnswParams& p, unsigned grid, size_t smem) {
         hnsw_search_kernel<KIND, METRIC, HB_THREADS, ALGO_BUILD, 0><<<grid, HB_THREADS, smem>>>(p);
         QB_LAUNCHED();
@@ -160,63 +101,13 @@ struct HbKernels {
         QB_CUDA(cudaGetLastError());
         return QB_OK;
     }
-    static qb_status prepare(size_t smem, int* per_sm) {
+    static qb_status prepare(const HnswParams&, size_t smem, int* per_sm) {
         QB_CUDA(cudaFuncSetAttribute(hnsw_search_kernel<KIND, METRIC, HB_THREADS, ALGO_BUILD, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         QB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(per_sm, hnsw_search_kernel<KIND, METRIC, HB_THREADS, ALGO_BUILD, 0>, HB_THREADS, smem));
         if (*per_sm < 1) *per_sm = 1;
         return QB_OK;
     }
 };
-
-// the host-side schedule
-struct HbPlan {
-    std::vector<uint32_t> rest;                       // inserted points after the entry, in the sorted order
-    std::vector<std::pair<uint32_t, uint32_t>> batches;   // [begin, end) in rest
-    std::vector<uint8_t> level_of_rest;
-    uint32_t entry_level = 0, max_batch = 1;
-};
-
-template <int KIND, int METRIC>
-qb_status hb_levels(HnswParams p, const HbPlan& plan, uint32_t m, uint32_t m0, uint32_t* const* tables, const uint32_t* d_remap, uint32_t* d_pts,
-                    uint32_t* d_entry, unsigned long long* d_tkey, uint32_t* d_tval, unsigned long long* d_tkey2, uint32_t* d_tval2, void* d_sort,
-                    size_t sort_bytes, unsigned max_grid, size_t smem, int key_bits) {
-    const uint32_t nr = (uint32_t)plan.rest.size();
-    p.b_tkey = d_tkey; p.b_tval = d_tval;
-    for (int l = (int)plan.entry_level; l >= 0; --l) {
-        const uint32_t lm = l ? m : m0;
-        p.links0 = tables[l]; p.m = lm; p.m0 = lm; p.b_remap = l ? d_remap : nullptr;
-        for (const auto& bt : plan.batches) {
-            if (plan.level_of_rest[bt.first] < (uint32_t)l) continue;
-            const uint32_t np = bt.second - bt.first;
-            p.b_pts = d_pts + bt.first; p.b_entry = d_entry + bt.first; p.nq = np; p.b_insert = 1;
-            QB_CUDA(cudaMemsetAsync(p.work, 0, 4));
-            QB_TRY((HbKernels<KIND, METRIC>::insert(p, std::min<unsigned>(np, max_grid), smem)));
-            size_t bytes = sort_bytes;
-            QB_CUDA(cub::DeviceRadixSort::SortPairs(d_sort, bytes, d_tkey, d_tkey2, d_tval, d_tval2, (int)(np * lm), 0, key_bits));
-            QB_LAUNCHED();
-            QB_TRY((HbKernels<KIND, METRIC>::backlinks(p, d_tkey2, d_tval2, np * lm)));
-        }
-        if (l == 0) break;
-        // the points below l: greedy descent on l, one launch (they follow every insert at l)
-        const uint32_t g0 = (uint32_t)(std::find_if(plan.level_of_rest.begin(), plan.level_of_rest.end(), [&](uint8_t v) { return v < (uint32_t)l; }) -
-                                       plan.level_of_rest.begin());
-        if (g0 < nr) {
-            p.b_pts = d_pts + g0; p.b_entry = d_entry + g0; p.nq = nr - g0; p.b_insert = 0;
-            QB_CUDA(cudaMemsetAsync(p.work, 0, 4));
-            QB_TRY((HbKernels<KIND, METRIC>::insert(p, std::min<unsigned>(nr - g0, max_grid), smem)));
-        }
-    }
-    return QB_OK;
-}
-
-// resident CTAs per SM of the insert kernel
-inline qb_status hb_occupancy(int kind, int metric, size_t smem, int* per_sm) {
-    if (kind == HK_DENSE_AVX)
-        return metric == M_EUCLID ? HbKernels<HK_DENSE_AVX, M_EUCLID>::prepare(smem, per_sm)
-                                  : metric == M_MANHATTAN ? HbKernels<HK_DENSE_AVX, M_MANHATTAN>::prepare(smem, per_sm) : HbKernels<HK_DENSE_AVX, M_DOT>::prepare(smem, per_sm);
-    return metric == M_EUCLID ? HbKernels<HK_DENSE_SMALL, M_EUCLID>::prepare(smem, per_sm)
-                              : metric == M_MANHATTAN ? HbKernels<HK_DENSE_SMALL, M_MANHATTAN>::prepare(smem, per_sm) : HbKernels<HK_DENSE_SMALL, M_DOT>::prepare(smem, per_sm);
-}
 
 }  // namespace
 
@@ -233,153 +124,30 @@ extern "C" qb_status qb_hnsw_build(qb_storage* s, uint32_t m, uint32_t m0, uint3
     const uint32_t ef = std::max(ef_construct, m0);   // gpu_graph_builder.rs:38
     QB_CHECK(ef <= HNSW_MAX_EF, QB_ERR_UNSUPPORTED, "hnsw_build: ef %u > %u", ef, HNSW_MAX_EF);
     const uint32_t n = (uint32_t)s->count;
-    uint32_t top_level = 0;
-    for (uint32_t i = 0; i < n; ++i) {
-        QB_CHECK(levels[i] <= HB_MAX_LEVEL, QB_ERR_INVALID, "hnsw_build: levels[%u] = %u > %u", i, (unsigned)levels[i], HB_MAX_LEVEL);
-        top_level = std::max<uint32_t>(top_level, levels[i]);
-    }
     if (batch == 0) batch = 512;               // GPU_GROUPS_COUNT_DEFAULT, gpu/mod.rs:34
     if (serial_points == 0) serial_points = 256;   // SINGLE_THREADED_HNSW_BUILD_THRESHOLD
     QB_CUDA(cudaSetDevice(s->device));
 
-    // ---- order, rows per level, the schedule
-    const uint32_t L = top_level + 1;
     std::vector<uint32_t> deleted;
     if (s->d_deleted) {
         deleted.resize(ceil_div_u64(n, 32));
         QB_CUDA(cudaMemcpy(deleted.data(), s->d_deleted, 4 * deleted.size(), cudaMemcpyDeviceToHost));
     }
-    std::vector<uint64_t> per_level(L + 1, 0), start(L + 1, 0);
-    for (uint32_t i = 0; i < n; ++i) per_level[levels[i]]++;
-    for (int l = (int)L - 2; l >= 0; --l) start[l] = start[l + 1] + per_level[l + 1];   // level desc, then id (a stable counting sort)
-    std::vector<uint32_t> order(n), pos(n);
-    for (uint32_t i = 0; i < n; ++i) { pos[i] = (uint32_t)start[levels[i]]++; order[pos[i]] = i; }
-    std::vector<uint64_t> rows_on(L);   // N_l: points whose level is >= l = the first N_l of the order
-    for (uint32_t l = 0; l < L; ++l) { uint64_t c = 0; for (uint32_t k = l; k < L; ++k) c += per_level[k]; rows_on[l] = c; }
     HbPlan plan;
-    uint32_t entry = HNSW_EMPTY;
-    for (uint32_t i = 0; i < n; ++i) {
-        const uint32_t id = order[i];
-        if (!deleted.empty() && ((deleted[id >> 5] >> (id & 31)) & 1u)) continue;   // iter_internal_excluding(deleted)
-        if (entry == HNSW_EMPTY) entry = id;
-        else plan.rest.push_back(id);
-    }
-    QB_CHECK(entry != HNSW_EMPTY, QB_ERR_INVALID, "hnsw_build: every point is deleted");
-    plan.entry_level = levels[entry];
-    const uint32_t nr = (uint32_t)plan.rest.size();
-    plan.level_of_rest.resize(nr);
-    for (uint32_t i = 0; i < nr; ++i) plan.level_of_rest[i] = levels[plan.rest[i]];
-    {
-        uint32_t k = 0;
-        for (; k < std::min(serial_points - 1, nr); ++k) plan.batches.push_back({k, k + 1});
-        while (k < nr) {   // build_initial_batches: chunks of `batch` from the first point after the entry, cut where the level changes
-            uint32_t e = (uint32_t)std::min<uint64_t>((uint64_t)(k / batch + 1) * batch, nr);
-            for (uint32_t j = k + 1; j < e; ++j) if (plan.level_of_rest[j] != plan.level_of_rest[k]) { e = j; break; }
-            plan.batches.push_back({k, e});
-            plan.max_batch = std::max(plan.max_batch, e - k);
-            k = e;
-        }
-    }
+    QB_TRY(hb_plan(levels, n, deleted.empty() ? nullptr : deleted.data(), batch, serial_points, "hnsw_build", &plan));
 
-    // ---- device state
     const int kind = s->dim >= 32 ? HK_DENSE_AVX : HK_DENSE_SMALL;
-    const int metric = s->distance == QB_DIST_EUCLID ? M_EUCLID : (s->distance == QB_DIST_MANHATTAN ? M_MANHATTAN : M_DOT);
-    HbScratch tmp;
-    std::vector<uint32_t*> tables(L, nullptr);
-    for (uint32_t l = 0; l < L; ++l) {
-        const size_t bytes = (size_t)rows_on[l] * (l ? m : m0) * 4;
-        QB_CUDA(tmp.alloc((void**)&tables[l], bytes));
-        QB_CUDA(cudaMemset(tables[l], 0xFF, bytes));
-    }
-    uint32_t *d_remap = nullptr, *d_pts = nullptr, *d_entry = nullptr, *d_tval = nullptr, *d_tval2 = nullptr;
-    unsigned long long *d_tkey = nullptr, *d_tkey2 = nullptr;
-    unsigned int* d_work = nullptr;
-    const size_t trip = (size_t)plan.max_batch * m0;
-    QB_CUDA(tmp.alloc((void**)&d_remap, 4ull * n));
-    QB_CUDA(tmp.alloc((void**)&d_pts, 4ull * nr));
-    QB_CUDA(tmp.alloc((void**)&d_entry, 4ull * nr));
-    QB_CUDA(tmp.alloc((void**)&d_tkey, 8 * trip));
-    QB_CUDA(tmp.alloc((void**)&d_tkey2, 8 * trip));
-    QB_CUDA(tmp.alloc((void**)&d_tval, 4 * trip));
-    QB_CUDA(tmp.alloc((void**)&d_tval2, 4 * trip));
-    QB_CUDA(tmp.alloc((void**)&d_work, 4));
-    QB_CUDA(cudaMemcpy(d_remap, pos.data(), 4ull * n, cudaMemcpyHostToDevice));
-    if (nr) QB_CUDA(cudaMemcpy(d_pts, plan.rest.data(), 4ull * nr, cudaMemcpyHostToDevice));
-    {
-        std::vector<uint32_t> ent(nr, entry);   // PointLinkingData::entry starts at the first point
-        if (nr) QB_CUDA(cudaMemcpy(d_entry, ent.data(), 4ull * nr, cudaMemcpyHostToDevice));
-    }
-    const int key_bits = 64;   // target << 32 | position; an empty slot (~0) sorts last
-    size_t sort_bytes = 0;
-    QB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, d_tkey, d_tkey2, d_tval, d_tval2, (int)trip, 0, (int)key_bits));
-    void* d_sort = nullptr;
-    QB_CUDA(tmp.alloc(&d_sort, sort_bytes));
-
+    const int metric = hb_metric(s);
     HnswParams p{};
-    p.n_points = n; p.levels = L;
     p.rows = reinterpret_cast<const uint8_t*>(s->d_rows); p.stride = s->row_stride; p.dim = s->dim;
-    p.q_bytes = s->row_stride; p.ef = ef; p.top = 0; p.entry = 0; p.entry_level = 0;
-    p.prefetch = qb_opt().hnsw_no_prefetch ? 0 : 1;
-    p.work = d_work;
+    p.q_bytes = s->row_stride; p.ef = ef;
     const size_t smem = hnsw_smem_bytes(p.q_bytes, ef);
     QB_CHECK(smem <= 200 * 1024, QB_ERR_UNSUPPORTED, "hnsw_build: a row (%u B) + ef %u need %zu B of shared memory", p.q_bytes, ef, smem);
-    // grid: the resident CTAs, at most one per point of the largest launch; per-CTA visited bitmaps (the kernel leaves them clean) and logs
-    int per_sm = 1;
-    QB_TRY(hb_occupancy(kind, metric, smem, &per_sm));
-    const unsigned grid = std::min<unsigned>((unsigned)s->sm_count * (unsigned)per_sm, std::max<uint32_t>(1, std::max(plan.max_batch, nr)));
-    const uint64_t words = ceil_div_u64(n, 32);
-    p.visited_words = words; p.vlog_cap = 32768;
-    QB_CUDA(tmp.alloc((void**)&p.visited, (size_t)grid * words * 4));
-    QB_CUDA(tmp.alloc((void**)&p.vlog, (size_t)grid * p.vlog_cap * 4));
-    QB_CUDA(cudaMemset(p.visited, 0, (size_t)grid * words * 4));
-#define QB_HB_LEVELS(K, M) hb_levels<K, M>(p, plan, m, m0, tables.data(), d_remap, d_pts, d_entry, d_tkey, d_tval, d_tkey2, d_tval2, d_sort, sort_bytes, grid, smem, key_bits)
-    if (kind == HK_DENSE_AVX) QB_TRY(metric == M_EUCLID ? QB_HB_LEVELS(HK_DENSE_AVX, M_EUCLID) : metric == M_MANHATTAN ? QB_HB_LEVELS(HK_DENSE_AVX, M_MANHATTAN) : QB_HB_LEVELS(HK_DENSE_AVX, M_DOT));
-    else QB_TRY(metric == M_EUCLID ? QB_HB_LEVELS(HK_DENSE_SMALL, M_EUCLID) : metric == M_MANHATTAN ? QB_HB_LEVELS(HK_DENSE_SMALL, M_MANHATTAN) : QB_HB_LEVELS(HK_DENSE_SMALL, M_DOT));
-#undef QB_HB_LEVELS
-
-    // ---- finish: the plain arrays (level offsets, reindex, neighbours, offsets), then the handle as qb_hnsw_create_plain makes it
-    HbTables tb{};
-    tb.levels = L; tb.m = m; tb.m0 = m0;
-    std::vector<uint64_t> lo(L + 1, 0);
-    for (uint32_t l = 0; l < L; ++l) { tb.t[l] = tables[l]; lo[l + 1] = lo[l] + rows_on[l]; }
-    for (uint32_t l = 0; l <= L; ++l) tb.lo[l] = lo[l];
-    const uint64_t rows = lo[L], n_off = rows + 1;
-    uint64_t* d_counts = nullptr;
-    QB_CUDA(tmp.alloc((void**)&d_counts, 8 * n_off));
-    hnsw_build_counts_kernel<<<hb_grid(n_off, 256, 132 * 16), 256>>>(tb, d_counts);
-    QB_LAUNCHED();
-    qb_hnsw* g = new qb_hnsw();
-    g->st = s; g->n_points = n; g->m = m; g->m0 = m0; g->levels = L;
-    g->level_offsets_ext = lo; g->n_offsets = n_off;
-    auto fail = [&](qb_status st, const char* what, cudaError_t e) {
-        qb_set_error("hnsw_build: %s: %s", what, cudaGetErrorString(e));
-        qb_hnsw_destroy(g);
-        return st;
-    };
-    bool ok = cudaMalloc(&g->d_level_offsets, std::max<size_t>(8 * L, 256)) == cudaSuccess && cudaMalloc(&g->d_reindex, std::max<size_t>(4ull * n, 256)) == cudaSuccess &&
-              cudaMalloc(&g->d_offsets, 8 * n_off + 256) == cudaSuccess;
-    if (!ok) return fail(QB_ERR_OOM, "cudaMalloc failed", cudaGetLastError());
-    size_t scan_bytes = 0;
-    cudaError_t ce = cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_counts, g->d_offsets, (int64_t)n_off);
-    void* d_scan = nullptr;
-    if (ce == cudaSuccess) ce = tmp.alloc(&d_scan, scan_bytes);
-    if (ce == cudaSuccess) ce = cub::DeviceScan::ExclusiveSum(d_scan, scan_bytes, d_counts, g->d_offsets, (int64_t)n_off);
-    QB_LAUNCHED();
-    uint64_t total = 0;
-    if (ce == cudaSuccess) ce = cudaMemcpy(&total, g->d_offsets + rows, 8, cudaMemcpyDeviceToHost);
-    if (ce == cudaSuccess) ce = cudaMemcpy(g->d_level_offsets, lo.data(), 8 * L, cudaMemcpyHostToDevice);
-    if (ce == cudaSuccess) ce = cudaMemcpy(g->d_reindex, d_remap, 4ull * n, cudaMemcpyDeviceToDevice);
-    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "build", ce);
-    g->n_neighbors = total;
-    if (cudaMalloc(&g->d_neighbors, std::max<size_t>(4 * total, 256)) != cudaSuccess) return fail(QB_ERR_OOM, "cudaMalloc failed", cudaGetLastError());
-    hnsw_build_neighbors_kernel<<<hb_grid(rows, 256, 132 * 16), 256>>>(tb, g->d_offsets, g->d_neighbors);
-    QB_LAUNCHED();
-    ce = cudaGetLastError();
-    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "build", ce);
-    const qb_status st = qb_hnsw_finish_plain(g, "hnsw_build");
-    if (st != QB_OK) { qb_hnsw_destroy(g); return st; }
-    *out = g;
-    if (entry_point) *entry_point = entry;
+#define QB_HB_RUN(K, M) hb_run<HbKernels<K, M>>(s, p, plan, n, m, m0, smem, "hnsw_build", out)
+    if (kind == HK_DENSE_AVX) QB_TRY(metric == M_EUCLID ? QB_HB_RUN(HK_DENSE_AVX, M_EUCLID) : metric == M_MANHATTAN ? QB_HB_RUN(HK_DENSE_AVX, M_MANHATTAN) : QB_HB_RUN(HK_DENSE_AVX, M_DOT));
+    else QB_TRY(metric == M_EUCLID ? QB_HB_RUN(HK_DENSE_SMALL, M_EUCLID) : metric == M_MANHATTAN ? QB_HB_RUN(HK_DENSE_SMALL, M_MANHATTAN) : QB_HB_RUN(HK_DENSE_SMALL, M_DOT));
+#undef QB_HB_RUN
+    if (entry_point) *entry_point = plan.entry;
     if (entry_level) *entry_level = plan.entry_level;
     return QB_OK;
 }

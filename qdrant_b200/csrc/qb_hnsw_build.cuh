@@ -1,0 +1,251 @@
+// qb_hnsw_build.cuh — the host side of a device graph build, shared by qb_hnsw_build (qb_hnsw_build.cu) and qb_hnsw_build_multivector
+// (qb_hnsw_build_mv.cu): the schedule (hb_plan), the level loop (hb_levels) and the finish into a plain-format handle (hb_run).  The
+// inserts and backlinks are the kernels K of the caller: K::Params, K::insert, K::backlinks, K::prepare.  The schedule is described
+// in qb_hnsw_build.cu's header.
+#pragma once
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
+
+#include <algorithm>
+#include <vector>
+
+#include "qb_hnsw_traverse.cuh"
+
+namespace {
+
+constexpr int HB_THREADS = 128;       // insert kernel: threads per CTA (one point per CTA at a time)
+constexpr int HB_WARPS = 4;           // backlink kernel: warps per CTA (one target per warp at a time)
+constexpr uint32_t HB_MAX_LEVEL = 30; // the highest level a point may have (levels are u8; 30 keeps the per-level tables small)
+
+// the build tables of every level, for the finish
+struct HbTables {
+    const uint32_t* t[HB_MAX_LEVEL + 1];
+    uint64_t lo[HB_MAX_LEVEL + 2];   // first row of each level in the plain order; lo[levels] = rows
+    uint32_t levels, m, m0;
+};
+__device__ __forceinline__ const uint32_t* hb_row(const HbTables& tb, uint64_t r, uint32_t& lm) {
+    uint32_t l = 0;
+    while (l + 1 < tb.levels && r >= tb.lo[l + 1]) ++l;
+    lm = l ? tb.m : tb.m0;
+    return tb.t[l] + (r - tb.lo[l]) * lm;
+}
+// links per row (counts[rows] = 0, so the exclusive scan ends on the total)
+__global__ void hnsw_build_counts_kernel(const HbTables tb, uint64_t* __restrict__ counts) {
+    const uint64_t rows = tb.lo[tb.levels];
+    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r <= rows; r += (uint64_t)gridDim.x * blockDim.x) {
+        uint64_t c = 0;
+        if (r < rows) {
+            uint32_t lm;
+            const uint32_t* row = hb_row(tb, r, lm);
+            while (c < lm && row[c] != HNSW_EMPTY) ++c;
+        }
+        counts[r] = c;
+    }
+}
+__global__ void hnsw_build_neighbors_kernel(const HbTables tb, const uint64_t* __restrict__ offsets, uint32_t* __restrict__ neighbors) {
+    const uint64_t rows = tb.lo[tb.levels];
+    for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += (uint64_t)gridDim.x * blockDim.x) {
+        uint32_t lm;
+        const uint32_t* row = hb_row(tb, r, lm);
+        const uint64_t b = offsets[r], e = offsets[r + 1];
+        for (uint64_t k = 0; k < e - b; ++k) neighbors[b + k] = row[k];
+    }
+}
+
+// device temporaries of one call, freed on every exit path
+struct HbScratch {
+    std::vector<void*> bufs;
+    cudaError_t alloc(void** p, size_t bytes) {
+        *p = nullptr;
+        const cudaError_t e = cudaMalloc(p, std::max<size_t>(bytes, 256));
+        if (e == cudaSuccess) bufs.push_back(*p);
+        return e;
+    }
+    ~HbScratch() { cudaDeviceSynchronize(); for (void* b : bufs) cudaFree(b); }
+};
+
+inline unsigned hb_grid(uint64_t items, uint64_t per_block, uint64_t max_blocks) {
+    return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(ceil_div_u64(items, per_block), max_blocks));
+}
+
+// the host-side schedule
+struct HbPlan {
+    std::vector<uint32_t> rest;                       // inserted points after the entry, in the sorted order
+    std::vector<std::pair<uint32_t, uint32_t>> batches;   // [begin, end) in rest
+    std::vector<uint8_t> level_of_rest;
+    std::vector<uint32_t> pos;                        // each point's position in the sorted order (its row on the levels >= 1)
+    std::vector<uint64_t> rows_on;                    // N_l: points whose level is >= l = the first N_l of the order
+    uint32_t entry = HNSW_EMPTY, entry_level = 0, levels = 1, max_batch = 1;
+};
+
+// the schedule of n points with these levels; deleted: 32-bit words, bit = 1: not inserted (null: none)
+qb_status hb_plan(const uint8_t* levels, uint32_t n, const uint32_t* deleted, uint32_t batch, uint32_t serial_points, const char* who, HbPlan* out) {
+    HbPlan& plan = *out;
+    uint32_t top_level = 0;
+    for (uint32_t i = 0; i < n; ++i) {
+        QB_CHECK(levels[i] <= HB_MAX_LEVEL, QB_ERR_INVALID, "%s: levels[%u] = %u > %u", who, i, (unsigned)levels[i], HB_MAX_LEVEL);
+        top_level = std::max<uint32_t>(top_level, levels[i]);
+    }
+    const uint32_t L = plan.levels = top_level + 1;
+    std::vector<uint64_t> per_level(L + 1, 0), start(L + 1, 0);
+    for (uint32_t i = 0; i < n; ++i) per_level[levels[i]]++;
+    for (int l = (int)L - 2; l >= 0; --l) start[l] = start[l + 1] + per_level[l + 1];   // level desc, then id (a stable counting sort)
+    std::vector<uint32_t> order(n);
+    plan.pos.resize(n);
+    for (uint32_t i = 0; i < n; ++i) { plan.pos[i] = (uint32_t)start[levels[i]]++; order[plan.pos[i]] = i; }
+    plan.rows_on.resize(L);
+    for (uint32_t l = 0; l < L; ++l) { uint64_t c = 0; for (uint32_t k = l; k < L; ++k) c += per_level[k]; plan.rows_on[l] = c; }
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t id = order[i];
+        if (deleted && ((deleted[id >> 5] >> (id & 31)) & 1u)) continue;   // iter_internal_excluding(deleted)
+        if (plan.entry == HNSW_EMPTY) plan.entry = id;
+        else plan.rest.push_back(id);
+    }
+    QB_CHECK(plan.entry != HNSW_EMPTY, QB_ERR_INVALID, "%s: every point is deleted", who);
+    plan.entry_level = levels[plan.entry];
+    const uint32_t nr = (uint32_t)plan.rest.size();
+    plan.level_of_rest.resize(nr);
+    for (uint32_t i = 0; i < nr; ++i) plan.level_of_rest[i] = levels[plan.rest[i]];
+    uint32_t k = 0;
+    for (; k < std::min(serial_points - 1, nr); ++k) plan.batches.push_back({k, k + 1});
+    while (k < nr) {   // build_initial_batches: chunks of `batch` from the first point after the entry, cut where the level changes
+        uint32_t e = (uint32_t)std::min<uint64_t>((uint64_t)(k / batch + 1) * batch, nr);
+        for (uint32_t j = k + 1; j < e; ++j) if (plan.level_of_rest[j] != plan.level_of_rest[k]) { e = j; break; }
+        plan.batches.push_back({k, e});
+        plan.max_batch = std::max(plan.max_batch, e - k);
+        k = e;
+    }
+    return QB_OK;
+}
+
+template <class K>
+qb_status hb_levels(typename K::Params p, const HbPlan& plan, uint32_t m, uint32_t m0, uint32_t* const* tables, const uint32_t* d_remap, uint32_t* d_pts,
+                    uint32_t* d_entry, unsigned long long* d_tkey, uint32_t* d_tval, unsigned long long* d_tkey2, uint32_t* d_tval2, void* d_sort,
+                    size_t sort_bytes, unsigned max_grid, size_t smem, int key_bits) {
+    const uint32_t nr = (uint32_t)plan.rest.size();
+    p.b_tkey = d_tkey; p.b_tval = d_tval;
+    for (int l = (int)plan.entry_level; l >= 0; --l) {
+        const uint32_t lm = l ? m : m0;
+        p.links0 = tables[l]; p.m = lm; p.m0 = lm; p.b_remap = l ? d_remap : nullptr;
+        for (const auto& bt : plan.batches) {
+            if (plan.level_of_rest[bt.first] < (uint32_t)l) continue;
+            const uint32_t np = bt.second - bt.first;
+            p.b_pts = d_pts + bt.first; p.b_entry = d_entry + bt.first; p.nq = np; p.b_insert = 1;
+            QB_CUDA(cudaMemsetAsync(p.work, 0, 4));
+            QB_TRY(K::insert(p, std::min<unsigned>(np, max_grid), smem));
+            size_t bytes = sort_bytes;
+            QB_CUDA(cub::DeviceRadixSort::SortPairs(d_sort, bytes, d_tkey, d_tkey2, d_tval, d_tval2, (int)(np * lm), 0, key_bits));
+            QB_LAUNCHED();
+            QB_TRY(K::backlinks(p, d_tkey2, d_tval2, np * lm));
+        }
+        if (l == 0) break;
+        // the points below l: greedy descent on l, one launch (they follow every insert at l)
+        const uint32_t g0 = (uint32_t)(std::find_if(plan.level_of_rest.begin(), plan.level_of_rest.end(), [&](uint8_t v) { return v < (uint32_t)l; }) -
+                                       plan.level_of_rest.begin());
+        if (g0 < nr) {
+            p.b_pts = d_pts + g0; p.b_entry = d_entry + g0; p.nq = nr - g0; p.b_insert = 0;
+            QB_CUDA(cudaMemsetAsync(p.work, 0, 4));
+            QB_TRY(K::insert(p, std::min<unsigned>(nr - g0, max_grid), smem));
+        }
+    }
+    return QB_OK;
+}
+
+// the build of `plan` with the kernels K, then the handle as qb_hnsw_create_plain makes it from the plain arrays.  p: the storage and
+// query fields (and K's own); smem: the insert kernel's shared memory.
+template <class K>
+qb_status hb_run(qb_storage* s, typename K::Params p, const HbPlan& plan, uint32_t n, uint32_t m, uint32_t m0, size_t smem, const char* who, qb_hnsw** out) {
+    const uint32_t L = plan.levels, nr = (uint32_t)plan.rest.size();
+    HbScratch tmp;
+    std::vector<uint32_t*> tables(L, nullptr);
+    for (uint32_t l = 0; l < L; ++l) {
+        const size_t bytes = (size_t)plan.rows_on[l] * (l ? m : m0) * 4;
+        QB_CUDA(tmp.alloc((void**)&tables[l], bytes));
+        QB_CUDA(cudaMemset(tables[l], 0xFF, bytes));
+    }
+    uint32_t *d_remap = nullptr, *d_pts = nullptr, *d_entry = nullptr, *d_tval = nullptr, *d_tval2 = nullptr;
+    unsigned long long *d_tkey = nullptr, *d_tkey2 = nullptr;
+    unsigned int* d_work = nullptr;
+    const size_t trip = (size_t)plan.max_batch * m0;
+    QB_CUDA(tmp.alloc((void**)&d_remap, 4ull * n));
+    QB_CUDA(tmp.alloc((void**)&d_pts, 4ull * nr));
+    QB_CUDA(tmp.alloc((void**)&d_entry, 4ull * nr));
+    QB_CUDA(tmp.alloc((void**)&d_tkey, 8 * trip));
+    QB_CUDA(tmp.alloc((void**)&d_tkey2, 8 * trip));
+    QB_CUDA(tmp.alloc((void**)&d_tval, 4 * trip));
+    QB_CUDA(tmp.alloc((void**)&d_tval2, 4 * trip));
+    QB_CUDA(tmp.alloc((void**)&d_work, 4));
+    QB_CUDA(cudaMemcpy(d_remap, plan.pos.data(), 4ull * n, cudaMemcpyHostToDevice));
+    if (nr) QB_CUDA(cudaMemcpy(d_pts, plan.rest.data(), 4ull * nr, cudaMemcpyHostToDevice));
+    {
+        std::vector<uint32_t> ent(nr, plan.entry);   // PointLinkingData::entry starts at the first point
+        if (nr) QB_CUDA(cudaMemcpy(d_entry, ent.data(), 4ull * nr, cudaMemcpyHostToDevice));
+    }
+    const int key_bits = 64;   // target << 32 | position; an empty slot (~0) sorts last
+    size_t sort_bytes = 0;
+    QB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, d_tkey, d_tkey2, d_tval, d_tval2, (int)trip, 0, (int)key_bits));
+    void* d_sort = nullptr;
+    QB_CUDA(tmp.alloc(&d_sort, sort_bytes));
+
+    p.n_points = n; p.levels = L;
+    p.prefetch = qb_opt().hnsw_no_prefetch ? 0 : 1;
+    p.work = d_work;
+    // grid: the resident CTAs, at most one per point of the largest launch; per-CTA visited bitmaps (the kernel leaves them clean) and logs
+    int per_sm = 1;
+    QB_TRY(K::prepare(p, smem, &per_sm));
+    const unsigned grid = std::min<unsigned>((unsigned)s->sm_count * (unsigned)per_sm, std::max<uint32_t>(1, std::max(plan.max_batch, nr)));
+    const uint64_t words = ceil_div_u64(n, 32);
+    p.visited_words = words; p.vlog_cap = 32768;
+    QB_CUDA(tmp.alloc((void**)&p.visited, (size_t)grid * words * 4));
+    QB_CUDA(tmp.alloc((void**)&p.vlog, (size_t)grid * p.vlog_cap * 4));
+    QB_CUDA(cudaMemset(p.visited, 0, (size_t)grid * words * 4));
+    QB_TRY(hb_levels<K>(p, plan, m, m0, tables.data(), d_remap, d_pts, d_entry, d_tkey, d_tval, d_tkey2, d_tval2, d_sort, sort_bytes, grid, smem, key_bits));
+
+    // ---- finish: the plain arrays (level offsets, reindex, neighbours, offsets), then the handle as qb_hnsw_create_plain makes it
+    HbTables tb{};
+    tb.levels = L; tb.m = m; tb.m0 = m0;
+    std::vector<uint64_t> lo(L + 1, 0);
+    for (uint32_t l = 0; l < L; ++l) { tb.t[l] = tables[l]; lo[l + 1] = lo[l] + plan.rows_on[l]; }
+    for (uint32_t l = 0; l <= L; ++l) tb.lo[l] = lo[l];
+    const uint64_t rows = lo[L], n_off = rows + 1;
+    uint64_t* d_counts = nullptr;
+    QB_CUDA(tmp.alloc((void**)&d_counts, 8 * n_off));
+    hnsw_build_counts_kernel<<<hb_grid(n_off, 256, 132 * 16), 256>>>(tb, d_counts);
+    QB_LAUNCHED();
+    qb_hnsw* g = new qb_hnsw();
+    g->st = s; g->n_points = n; g->m = m; g->m0 = m0; g->levels = L;
+    g->level_offsets_ext = lo; g->n_offsets = n_off;
+    auto fail = [&](qb_status st, const char* what, cudaError_t e) {
+        qb_set_error("%s: %s: %s", who, what, cudaGetErrorString(e));
+        qb_hnsw_destroy(g);
+        return st;
+    };
+    bool ok = cudaMalloc(&g->d_level_offsets, std::max<size_t>(8 * L, 256)) == cudaSuccess && cudaMalloc(&g->d_reindex, std::max<size_t>(4ull * n, 256)) == cudaSuccess &&
+              cudaMalloc(&g->d_offsets, 8 * n_off + 256) == cudaSuccess;
+    if (!ok) return fail(QB_ERR_OOM, "cudaMalloc failed", cudaGetLastError());
+    size_t scan_bytes = 0;
+    cudaError_t ce = cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_counts, g->d_offsets, (int64_t)n_off);
+    void* d_scan = nullptr;
+    if (ce == cudaSuccess) ce = tmp.alloc(&d_scan, scan_bytes);
+    if (ce == cudaSuccess) ce = cub::DeviceScan::ExclusiveSum(d_scan, scan_bytes, d_counts, g->d_offsets, (int64_t)n_off);
+    QB_LAUNCHED();
+    uint64_t total = 0;
+    if (ce == cudaSuccess) ce = cudaMemcpy(&total, g->d_offsets + rows, 8, cudaMemcpyDeviceToHost);
+    if (ce == cudaSuccess) ce = cudaMemcpy(g->d_level_offsets, lo.data(), 8 * L, cudaMemcpyHostToDevice);
+    if (ce == cudaSuccess) ce = cudaMemcpy(g->d_reindex, d_remap, 4ull * n, cudaMemcpyDeviceToDevice);
+    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "build", ce);
+    g->n_neighbors = total;
+    if (cudaMalloc(&g->d_neighbors, std::max<size_t>(4 * total, 256)) != cudaSuccess) return fail(QB_ERR_OOM, "cudaMalloc failed", cudaGetLastError());
+    hnsw_build_neighbors_kernel<<<hb_grid(rows, 256, 132 * 16), 256>>>(tb, g->d_offsets, g->d_neighbors);
+    QB_LAUNCHED();
+    ce = cudaGetLastError();
+    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "build", ce);
+    const qb_status st = qb_hnsw_finish_plain(g, who);
+    if (st != QB_OK) { qb_hnsw_destroy(g); return st; }
+    *out = g;
+    return QB_OK;
+}
+
+int hb_metric(const qb_storage* s) { return s->distance == QB_DIST_EUCLID ? M_EUCLID : (s->distance == QB_DIST_MANHATTAN ? M_MANHATTAN : M_DOT); }
+
+}  // namespace

@@ -185,6 +185,8 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
 // completes a handle whose plain arrays (d_level_offsets, d_reindex, d_neighbors, d_offsets and the host-side counts) are on the device:
 // the level-0 table and the search scratch (qb_hnsw.cu).  On failure the caller destroys g.  who = the error messages' prefix.
 qb_status qb_hnsw_finish_plain(qb_hnsw* g, const char* who);
+// the checks qb_search_maxsim makes on a multivector collection's token storage and point offsets (qb_hnsw.cu)
+qb_status qb_hnsw_mv_check(qb_storage* s, const uint32_t* point_offsets, uint32_t n_points, const char* who);
 // the inline-vector search (qb_hnsw_inline.cu): queries preprocessed (d_q_pre, pre_stride floats apart) and SQ8-encoded; enqueued on stream
 qb_status qb_hnsw_inline_launch(qb_hnsw* g, const float* d_q_pre, uint32_t pre_stride, const void* d_q_enc, const float* d_q_off, uint32_t nq, uint32_t top,
                                 uint32_t ef, uint32_t entry, uint32_t entry_level, const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts,

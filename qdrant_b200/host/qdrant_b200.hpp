@@ -223,6 +223,18 @@ public:
         check(qb_hnsw_build(storage.raw(), m, m0, ef_construct, levels.data(), batch, serial_points, &h, &entry_point, &entry_level));
         return std::unique_ptr<HnswGraph>(new HnswGraph(h));
     }
+    // builds the graph over the points of a multivector collection on the device (qb_hnsw_build_multivector): point p = token rows
+    // [point_offsets[p], point_offsets[p+1]) of the dense f32 `tokens`; levels: one per point; deleted_points: optional bitmap over points
+    // (ceil(n / 64) words, may be null).  Search it with the MaxSim search.
+    static std::unique_ptr<HnswGraph> build_multivector(const VectorStorage& tokens, const std::vector<uint32_t>& point_offsets, uint32_t m, uint32_t m0,
+                                                        uint32_t ef_construct, const std::vector<uint8_t>& levels, const uint64_t* deleted_points,
+                                                        uint32_t batch, uint32_t serial_points, uint32_t& entry_point, uint32_t& entry_level) {
+        if (point_offsets.empty() || levels.size() + 1 != point_offsets.size()) throw OperationError(QB_ERR_INVALID, "levels and point_offsets disagree on the point count");
+        qb_hnsw* h = nullptr;
+        check(qb_hnsw_build_multivector(tokens.raw(), point_offsets.data(), (uint32_t)levels.size(), m, m0, ef_construct, levels.data(), deleted_points, batch,
+                                        serial_points, &h, &entry_point, &entry_level));
+        return std::unique_ptr<HnswGraph>(new HnswGraph(h));
+    }
     // the graph as a plain links.bin (qb_hnsw_export_plain)
     std::vector<uint8_t> export_plain() const {
         uint64_t n = 0;

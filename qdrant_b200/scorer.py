@@ -804,14 +804,7 @@ class HnswGraph:
         by default round(-ln(U) / ln(m)) with U uniform in (0, 1] from numpy's generator seeded with `seed` (get_random_layer,
         graph_layers_builder.rs:388-396).  batch / serial_points 0 = 512 / 256.  The entry point is in .entry_point / .entry_level."""
         m0 = 2 * m if m0 is None else m0
-        n = storage.count
-        if levels is None:
-            u = 1.0 - np.random.default_rng(seed).random(n)
-            levels = np.minimum(np.round(-np.log(u) / np.log(max(m, 2))), 30)
-        lv = np.ascontiguousarray(levels, dtype=np.int64)
-        if lv.shape != (n,):
-            raise ValueError(f"levels has shape {lv.shape}, storage has {n} points")
-        lv = np.ascontiguousarray(np.clip(lv, 0, 255), dtype=np.uint8)   # a level > 30 is rejected by the library
+        lv = cls._build_levels(levels, storage.count, m, seed)
         self = cls.__new__(cls)
         self._storage = storage
         self._h = vp()
@@ -821,6 +814,40 @@ class HnswGraph:
         self._h = h
         self.entry_point, self.entry_level, self.levels = int(e.value), int(el.value), lv
         return self
+
+    @classmethod
+    def build_multivector(cls, view: "MultiVectorView", m: int = 16, ef_construct: int = 100, levels=None, seed: int = 0, batch: int = 0,
+                          serial_points: int = 0, m0: Optional[int] = None, point_deleted=None) -> "HnswGraph":
+        """Builds the graph over the POINTS of a multivector collection on the device (qb_hnsw_build_multivector): build()'s schedule
+        with MaxSim between stored points.  The view's storage must be dense f32; levels / seed / batch / serial_points / m0 as in
+        build(), one level per point; point_deleted: bool per point (such points are not inserted).  Search it with search_maxsim();
+        the entry point is in .entry_point / .entry_level."""
+        m0 = 2 * m if m0 is None else m0
+        lv = cls._build_levels(levels, view.n_points, m, seed)
+        bm = _bitmap(point_deleted, view.n_points)
+        self = cls.__new__(cls)
+        self._storage = view.storage
+        self._view = view
+        self._h = vp()
+        h, e, el = vp(), C.c_uint32(), C.c_uint32()
+        check(lib().qb_hnsw_build_multivector(view.storage._h, view.offsets.ctypes.data_as(u32p), view.n_points, int(m), int(m0), int(ef_construct),
+                                              lv.ctypes.data_as(u8p), None if bm is None else bm.ctypes.data_as(u64p), int(batch), int(serial_points),
+                                              C.byref(h), C.byref(e), C.byref(el)))
+        self._h = h
+        self.entry_point, self.entry_level, self.levels = int(e.value), int(el.value), lv
+        return self
+
+    @staticmethod
+    def _build_levels(levels, n: int, m: int, seed: int) -> np.ndarray:
+        """levels as u8, one per point; by default round(-ln(U) / ln(m)) with U uniform in (0, 1] from numpy's generator seeded with
+        `seed` (get_random_layer, graph_layers_builder.rs:388-396)"""
+        if levels is None:
+            u = 1.0 - np.random.default_rng(seed).random(n)
+            levels = np.minimum(np.round(-np.log(u) / np.log(max(m, 2))), 30)
+        lv = np.ascontiguousarray(levels, dtype=np.int64)
+        if lv.shape != (n,):
+            raise ValueError(f"levels has shape {lv.shape}, the graph has {n} points")
+        return np.ascontiguousarray(np.clip(lv, 0, 255), dtype=np.uint8)   # a level > 30 is rejected by the library
 
     def export_plain(self) -> np.ndarray:
         """The graph as a plain links.bin (qb_hnsw_export_plain), for any handle."""
