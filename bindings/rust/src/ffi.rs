@@ -107,6 +107,7 @@ extern "C" {
     pub fn qb_hnsw_destroy(g: *mut qb_hnsw);
     pub fn qb_hnsw_info(g: *const qb_hnsw, n_points: *mut u32, levels: *mut u32, hbm_bytes: *mut u64) -> qb_status;
     pub fn qb_hnsw_build(s: *mut qb_storage, m: u32, m0: u32, ef_construct: u32, levels: *const u8, batch: u32, serial_points: u32, out: *mut *mut qb_hnsw, entry_point: *mut u32, entry_level: *mut u32) -> qb_status;
+    pub fn qb_hnsw_build_incremental(s: *mut qb_storage, old: *const qb_hnsw, old_to_new: *const u32, ef_construct: u32, levels: *const u8, batch: u32, serial_points: u32, out: *mut *mut qb_hnsw, entry_point: *mut u32, entry_level: *mut u32) -> qb_status;
     pub fn qb_hnsw_export_plain(g: *const qb_hnsw, out: *mut u8, cap: u64, n_bytes: *mut u64) -> qb_status;
     pub fn qb_hnsw_search_batch(g: *mut qb_hnsw, queries: *const f32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, deleted_bitmap: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters) -> qb_status;
     pub fn qb_hnsw_search_batch_device(g: *mut qb_hnsw, dev_queries: *const f32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, dev_out: *mut qb_scored_point, dev_counts: *mut u32) -> qb_status;

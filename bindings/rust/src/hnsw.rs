@@ -76,6 +76,24 @@ impl<'a> B200Hnsw<'a> {
         Ok((Self { raw, _storage: std::marker::PhantomData }, (entry, level as usize)))
     }
 
+    /// Builds the graph from the old segment's graph on the device (qb_hnsw_build_incremental), in place of the old-index path of
+    /// `HNSWIndex::build` (hnsw/build.rs:225-357): `GraphLayersHealer` heals the lists that link to a removed point,
+    /// `save_into_builder` renumbers them, and only the points the old graph did not have are inserted.  The adapter keeps on the
+    /// host `OldIndexCandidate::evaluate` (whether to reuse `old`, and `old_to_new`: one per old point, `u32::MAX` = not carried
+    /// over) and the level draw for the new points (`levels`: one per point, the reused ones keeping their old level).  `m` / `m0`
+    /// are `old`'s.  Returns the graph and its entry point (id, level).
+    pub fn build_incremental(storage: &'a B200Storage, old: &B200Hnsw<'_>, old_to_new: &[u32], ef_construct: usize, levels: &[u8], batch: usize,
+                             serial_points: usize) -> OperationResult<(Self, (PointOffsetType, usize))> {
+        let mut raw = std::ptr::null_mut();
+        let (mut entry, mut level) = (0u32, 0u32);
+        let st = unsafe {
+            qb_hnsw_build_incremental(storage.raw, old.raw, old_to_new.as_ptr(), ef_construct as u32, levels.as_ptr(), batch as u32, serial_points as u32,
+                                      &mut raw, &mut entry, &mut level)
+        };
+        if st != QB_OK { return Err(OperationError::service_error(last_error())); }
+        Ok((Self { raw, _storage: std::marker::PhantomData }, (entry, level as usize)))
+    }
+
     /// Builds the graph over the POINTS of a multivector named vector on the device (qb_hnsw_build_multivector): `build`'s schedule
     /// with MaxSim between stored points, point p being token rows [point_offsets[p], point_offsets[p + 1]) of the dense f32 `tokens`.
     /// `levels`: one per point; `deleted`: a bitmap over points (not inserted), or None.  Search it with `search_maxsim`.  Returns the

@@ -401,6 +401,37 @@ QB_API qb_status qb_hnsw_info(const qb_hnsw* g, uint32_t* n_points, uint32_t* le
  * quantized storage).  The result is the handle qb_hnsw_create_plain would make from the graph's plain links.bin.  Synchronous. */
 QB_API qb_status qb_hnsw_build(qb_storage* s, uint32_t m, uint32_t m0, uint32_t ef_construct, const uint8_t* levels /* n */, uint32_t batch,
                                uint32_t serial_points, qb_hnsw** out, uint32_t* entry_point, uint32_t* entry_level);
+/* Builds a segment's graph incrementally on the device: the old segment's graph is healed where its points have gone, renumbered into
+ * this storage's ids and extended with the points it did not have (hnsw/build.rs:225-357 with an old index; the reference's own GPU
+ * builder drops the old graph instead, build.rs:259-274).  In the reference's order:
+ *   1. to-heal items: every (point, level) of `old` whose first level_m links (in the handle's stored order) include an unmapped point,
+ *      point ascending, then level ascending (GraphLayersHealer::new over to_edges_impl, graph_layers_healer.rs:33-47,
+ *      graph_links/links.rs:174-186), unmapped points included, as the reference does;
+ *   2. each item is healed as heal_point_on_level does it (graph_layers_healer.rs:82-207): a stack-based search through the unmapped
+ *      points collects the ef_construct best border points, fill_from_sorted_with_heuristic keeps up to level_m - |valid links| of
+ *      them, the valid links follow, and every kept link gets a backlink (connect_with_heuristic) unless it holds the item already.
+ *      The query is the item's stored row in old's storage;
+ *   3. the reference heals in parallel under per-list locks; here each level heals in two phases: every item searches the lists as
+ *      loaded and writes its own list, then the backlinks are applied target by target in item order, the "already linked" test
+ *      made as each is applied.  The graph is a pure function of the inputs;
+ *   4. each mapped point's lists move to its new id without the unmapped links (save_into_builder, :236-256); the entry is the first
+ *      mapped point, in old-offset order, with the strictly highest level (EntryPoints::new_point, entry_points.rs:46-86);
+ *   5. the points of s that are neither mapped nor resident-deleted are inserted with qb_hnsw_build's schedule and arithmetic (ef =
+ *      max(ef_construct, m0)), the first serial_points of them one at a time.  A new point above the top links up to the top from
+ *      the entry and becomes the entry (link_new_point, graph_layers_builder.rs:417-475); batch = 1 equals serial insertion.
+ *   old_to_new  one per old point: its id in s, or 0xFFFFFFFF (not carried over)
+ *   levels      one per point of s, <= 30; a mapped point's must equal its old level (build.rs:235-239)
+ * m / m0 are old's (the reference reuses no graph of another configuration, old_index.rs:67-71); batch / serial_points as for
+ * qb_hnsw_build (0 = 512 / 256).  The decision to reuse a graph (OldIndexCandidate::evaluate, healing_threshold) stays with the
+ * caller.  Errors, checked before any device work: s or old's storage not dense f32, another dim / distance / device, a multivector
+ * or inline-vector (CompressedWithVectors, old_index.rs:72-76) handle, ef > 4096: QB_ERR_UNSUPPORTED; a null argument, ef_construct
+ * = 0, a target >= s's count, two old points on one target, a target with the resident deleted flag, no mapped point (build from
+ * scratch with qb_hnsw_build), a level > 30 or a mapped level that differs: QB_ERR_INVALID.  Healing and inserting read the f32
+ * rows (quantized vectors are out of scope, as for qb_hnsw_build).  The result is the handle qb_hnsw_create_plain would make from
+ * the new graph's plain links.bin, bound to s.  Synchronous. */
+QB_API qb_status qb_hnsw_build_incremental(qb_storage* s, const qb_hnsw* old, const uint32_t* old_to_new /* old n_points */, uint32_t ef_construct,
+                                           const uint8_t* levels /* s->count */, uint32_t batch, uint32_t serial_points, qb_hnsw** out,
+                                           uint32_t* entry_point, uint32_t* entry_level);
 /* The graph of any handle as a plain links.bin (graph_links/header.rs:9-20, serializer.rs:53-200).  *n_bytes = its size; out = NULL
  * asks for the size only, else cap must hold it (QB_ERR_INVALID).  Synchronous. */
 QB_API qb_status qb_hnsw_export_plain(const qb_hnsw* g, uint8_t* out, uint64_t cap, uint64_t* n_bytes);

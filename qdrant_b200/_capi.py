@@ -97,6 +97,7 @@ SIGNATURES = {
     "qb_hnsw_destroy": (None, [vp]),
     "qb_hnsw_info": (C.c_int32, [vp, u32p, u32p, u64p]),
     "qb_hnsw_build": (C.c_int32, [vp, C.c_uint32, C.c_uint32, C.c_uint32, u8p, C.c_uint32, C.c_uint32, C.POINTER(vp), u32p, u32p]),
+    "qb_hnsw_build_incremental": (C.c_int32, [vp, vp, u32p, C.c_uint32, u8p, C.c_uint32, C.c_uint32, C.POINTER(vp), u32p, u32p]),
     "qb_hnsw_export_plain": (C.c_int32, [vp, u8p, C.c_uint64, u64p]),
     "qb_hnsw_search_batch": (C.c_int32, [vp, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, u64p, i32p, C.POINTER(ScoredPoint), u32p,
                                          C.POINTER(HwCounters)]),

@@ -95,6 +95,7 @@ extern "C" qb_status qb_set_option(const char* name, int64_t value) {
     else if (n == "hnsw_threads") o.hnsw_threads = (int)value;
     else if (n == "mma_seg_cap") o.mma_seg_cap = (uint32_t)value;
     else if (n == "hnsw_no_prefetch") o.hnsw_no_prefetch = value != 0;
+    else if (n == "hnsw_heal_stack") o.hnsw_heal_stack = (uint32_t)value;
     else { qb_set_error("set_option: unknown option '%s'", name); return QB_ERR_INVALID; }
     return QB_OK;
 }

@@ -54,6 +54,7 @@ struct QbOptions {
     bool disable_prefilter = false;   // single-query dense f32 searches: always the exact f32 scan (no bf16 shadow plane, qb_prefilter.cu)
     uint32_t mma_seg_cap = 0;      // 0 = 256 survivor slots per (query, CTA) segment of the tensor-core scan
     uint64_t sample_rows = 0;
+    uint32_t hnsw_heal_stack = 0;  // qb_hnsw_build_incremental: DFS stack entries per CTA on the first run (0 = 16384)
 };
 QbOptions& qb_opt();
 

@@ -123,6 +123,11 @@ extern "C" qb_status qb_hnsw_build(qb_storage* s, uint32_t m, uint32_t m0, uint3
     QB_CHECK(m <= HNSW_MAX_LINKS && m0 <= HNSW_MAX_LINKS, QB_ERR_UNSUPPORTED, "hnsw_build: m %u / m0 %u outside [1,%u]", m, m0, HNSW_MAX_LINKS);
     const uint32_t ef = std::max(ef_construct, m0);   // gpu_graph_builder.rs:38
     QB_CHECK(ef <= HNSW_MAX_EF, QB_ERR_UNSUPPORTED, "hnsw_build: ef %u > %u", ef, HNSW_MAX_EF);
+    return qb_hnsw_build_dense(s, m, m0, ef, levels, nullptr, HNSW_EMPTY, batch, serial_points, nullptr, "hnsw_build", out, entry_point, entry_level);
+}
+
+qb_status qb_hnsw_build_dense(qb_storage* s, uint32_t m, uint32_t m0, uint32_t ef, const uint8_t* levels, const uint32_t* given, uint32_t entry, uint32_t batch,
+                              uint32_t serial_points, const HbPrefill& prefill, const char* who, qb_hnsw** out, uint32_t* entry_point, uint32_t* entry_level) {
     const uint32_t n = (uint32_t)s->count;
     if (batch == 0) batch = 512;               // GPU_GROUPS_COUNT_DEFAULT, gpu/mod.rs:34
     if (serial_points == 0) serial_points = 256;   // SINGLE_THREADED_HNSW_BUILD_THRESHOLD
@@ -134,7 +139,7 @@ extern "C" qb_status qb_hnsw_build(qb_storage* s, uint32_t m, uint32_t m0, uint3
         QB_CUDA(cudaMemcpy(deleted.data(), s->d_deleted, 4 * deleted.size(), cudaMemcpyDeviceToHost));
     }
     HbPlan plan;
-    QB_TRY(hb_plan(levels, n, deleted.empty() ? nullptr : deleted.data(), batch, serial_points, "hnsw_build", &plan));
+    QB_TRY(hb_plan(levels, n, deleted.empty() ? nullptr : deleted.data(), batch, serial_points, who, &plan, given, entry));
 
     const int kind = s->dim >= 32 ? HK_DENSE_AVX : HK_DENSE_SMALL;
     const int metric = hb_metric(s);
@@ -142,13 +147,14 @@ extern "C" qb_status qb_hnsw_build(qb_storage* s, uint32_t m, uint32_t m0, uint3
     p.rows = reinterpret_cast<const uint8_t*>(s->d_rows); p.stride = s->row_stride; p.dim = s->dim;
     p.q_bytes = s->row_stride; p.ef = ef;
     const size_t smem = hnsw_smem_bytes(p.q_bytes, ef);
-    QB_CHECK(smem <= 200 * 1024, QB_ERR_UNSUPPORTED, "hnsw_build: a row (%u B) + ef %u need %zu B of shared memory", p.q_bytes, ef, smem);
-#define QB_HB_RUN(K, M) hb_run<HbKernels<K, M>>(s, p, plan, n, m, m0, smem, "hnsw_build", out)
+    QB_CHECK(smem <= 200 * 1024, QB_ERR_UNSUPPORTED, "%s: a row (%u B) + ef %u need %zu B of shared memory", who, p.q_bytes, ef, smem);
+#define QB_HB_RUN(K, M) hb_run<HbKernels<K, M>>(s, p, plan, n, m, m0, smem, who, out, prefill)
     if (kind == HK_DENSE_AVX) QB_TRY(metric == M_EUCLID ? QB_HB_RUN(HK_DENSE_AVX, M_EUCLID) : metric == M_MANHATTAN ? QB_HB_RUN(HK_DENSE_AVX, M_MANHATTAN) : QB_HB_RUN(HK_DENSE_AVX, M_DOT));
     else QB_TRY(metric == M_EUCLID ? QB_HB_RUN(HK_DENSE_SMALL, M_EUCLID) : metric == M_MANHATTAN ? QB_HB_RUN(HK_DENSE_SMALL, M_MANHATTAN) : QB_HB_RUN(HK_DENSE_SMALL, M_DOT));
 #undef QB_HB_RUN
-    if (entry_point) *entry_point = plan.entry;
-    if (entry_level) *entry_level = plan.entry_level;
+    const uint32_t e = plan.lead ? plan.rest[0] : plan.entry;   // entry_points.rs new_point: a new point strictly above the top
+    if (entry_point) *entry_point = e;
+    if (entry_level) *entry_level = levels[e];
     return QB_OK;
 }
 

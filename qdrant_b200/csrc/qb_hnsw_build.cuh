@@ -7,6 +7,7 @@
 #include <cub/device/device_scan.cuh>
 
 #include <algorithm>
+#include <functional>
 #include <vector>
 
 #include "qb_hnsw_traverse.cuh"
@@ -76,10 +77,17 @@ struct HbPlan {
     std::vector<uint32_t> pos;                        // each point's position in the sorted order (its row on the levels >= 1)
     std::vector<uint64_t> rows_on;                    // N_l: points whose level is >= l = the first N_l of the order
     uint32_t entry = HNSW_EMPTY, entry_level = 0, levels = 1, max_batch = 1;
+    // an incremental build whose first new point is above the graph's top level (link_new_point, graph_layers_builder.rs:417-475):
+    // rest[0] links on the levels <= entry_level from `entry`, then it is the entry of every later point, from its own level
+    bool lead = false;
 };
 
-// the schedule of n points with these levels; deleted: 32-bit words, bit = 1: not inserted (null: none)
-qb_status hb_plan(const uint8_t* levels, uint32_t n, const uint32_t* deleted, uint32_t batch, uint32_t serial_points, const char* who, HbPlan* out) {
+// the schedule of n points with these levels; deleted: 32-bit words, bit = 1: not inserted (null: none).  An incremental build passes
+// the points its graph already holds as `given` (same layout; they are not inserted either) and that graph's entry; rest is then every
+// other point, the first serial_points of them one at a time.  Without a given entry the first point of the order is the entry and the
+// first serial_points - 1 after it go one at a time.
+qb_status hb_plan(const uint8_t* levels, uint32_t n, const uint32_t* deleted, uint32_t batch, uint32_t serial_points, const char* who, HbPlan* out,
+                  const uint32_t* given = nullptr, uint32_t entry = HNSW_EMPTY) {
     HbPlan& plan = *out;
     uint32_t top_level = 0;
     for (uint32_t i = 0; i < n; ++i) {
@@ -95,9 +103,11 @@ qb_status hb_plan(const uint8_t* levels, uint32_t n, const uint32_t* deleted, ui
     for (uint32_t i = 0; i < n; ++i) { plan.pos[i] = (uint32_t)start[levels[i]]++; order[plan.pos[i]] = i; }
     plan.rows_on.resize(L);
     for (uint32_t l = 0; l < L; ++l) { uint64_t c = 0; for (uint32_t k = l; k < L; ++k) c += per_level[k]; plan.rows_on[l] = c; }
+    plan.entry = entry;
     for (uint32_t i = 0; i < n; ++i) {
         const uint32_t id = order[i];
         if (deleted && ((deleted[id >> 5] >> (id & 31)) & 1u)) continue;   // iter_internal_excluding(deleted)
+        if (given && ((given[id >> 5] >> (id & 31)) & 1u)) continue;
         if (plan.entry == HNSW_EMPTY) plan.entry = id;
         else plan.rest.push_back(id);
     }
@@ -106,8 +116,9 @@ qb_status hb_plan(const uint8_t* levels, uint32_t n, const uint32_t* deleted, ui
     const uint32_t nr = (uint32_t)plan.rest.size();
     plan.level_of_rest.resize(nr);
     for (uint32_t i = 0; i < nr; ++i) plan.level_of_rest[i] = levels[plan.rest[i]];
+    plan.lead = entry != HNSW_EMPTY && nr && plan.level_of_rest[0] > plan.entry_level;
     uint32_t k = 0;
-    for (; k < std::min(serial_points - 1, nr); ++k) plan.batches.push_back({k, k + 1});
+    for (; k < std::min(entry != HNSW_EMPTY ? serial_points : serial_points - 1, nr); ++k) plan.batches.push_back({k, k + 1});
     while (k < nr) {   // build_initial_batches: chunks of `batch` from the first point after the entry, cut where the level changes
         uint32_t e = (uint32_t)std::min<uint64_t>((uint64_t)(k / batch + 1) * batch, nr);
         for (uint32_t j = k + 1; j < e; ++j) if (plan.level_of_rest[j] != plan.level_of_rest[k]) { e = j; break; }
@@ -151,10 +162,14 @@ qb_status hb_levels(typename K::Params p, const HbPlan& plan, uint32_t m, uint32
     return QB_OK;
 }
 
+// fills the build tables of an incremental build before its inserts: tables[l] as hb_run lays them out, d_remap = the plan's pos
+using HbPrefill = std::function<qb_status(uint32_t* const* tables, const uint32_t* d_remap)>;
+
 // the build of `plan` with the kernels K, then the handle as qb_hnsw_create_plain makes it from the plain arrays.  p: the storage and
-// query fields (and K's own); smem: the insert kernel's shared memory.
+// query fields (and K's own); smem: the insert kernel's shared memory; prefill: the rows the graph already has (null: none).
 template <class K>
-qb_status hb_run(qb_storage* s, typename K::Params p, const HbPlan& plan, uint32_t n, uint32_t m, uint32_t m0, size_t smem, const char* who, qb_hnsw** out) {
+qb_status hb_run(qb_storage* s, typename K::Params p, const HbPlan& plan, uint32_t n, uint32_t m, uint32_t m0, size_t smem, const char* who, qb_hnsw** out,
+                 const HbPrefill& prefill = nullptr) {
     const uint32_t L = plan.levels, nr = (uint32_t)plan.rest.size();
     HbScratch tmp;
     std::vector<uint32_t*> tables(L, nullptr);
@@ -178,7 +193,8 @@ qb_status hb_run(qb_storage* s, typename K::Params p, const HbPlan& plan, uint32
     QB_CUDA(cudaMemcpy(d_remap, plan.pos.data(), 4ull * n, cudaMemcpyHostToDevice));
     if (nr) QB_CUDA(cudaMemcpy(d_pts, plan.rest.data(), 4ull * nr, cudaMemcpyHostToDevice));
     {
-        std::vector<uint32_t> ent(nr, plan.entry);   // PointLinkingData::entry starts at the first point
+        std::vector<uint32_t> ent(nr, plan.lead ? plan.rest[0] : plan.entry);   // PointLinkingData::entry starts at the first point
+        if (plan.lead) ent[0] = plan.entry;
         if (nr) QB_CUDA(cudaMemcpy(d_entry, ent.data(), 4ull * nr, cudaMemcpyHostToDevice));
     }
     const int key_bits = 64;   // target << 32 | position; an empty slot (~0) sorts last
@@ -199,7 +215,17 @@ qb_status hb_run(qb_storage* s, typename K::Params p, const HbPlan& plan, uint32
     QB_CUDA(tmp.alloc((void**)&p.visited, (size_t)grid * words * 4));
     QB_CUDA(tmp.alloc((void**)&p.vlog, (size_t)grid * p.vlog_cap * 4));
     QB_CUDA(cudaMemset(p.visited, 0, (size_t)grid * words * 4));
-    QB_TRY(hb_levels<K>(p, plan, m, m0, tables.data(), d_remap, d_pts, d_entry, d_tkey, d_tval, d_tkey2, d_tval2, d_sort, sort_bytes, grid, smem, key_bits));
+    if (prefill) QB_TRY(prefill(tables.data(), d_remap));
+    if (plan.lead) {   // rest[0] on the levels <= entry_level, then the others from it
+        HbPlan one, others;
+        one.rest = {plan.rest[0]}; one.batches = {{0, 1}}; one.level_of_rest = {plan.level_of_rest[0]}; one.entry_level = plan.entry_level;
+        others.rest = plan.rest; others.level_of_rest = plan.level_of_rest; others.entry_level = plan.level_of_rest[0];
+        others.batches.assign(plan.batches.begin() + 1, plan.batches.end());
+        QB_TRY(hb_levels<K>(p, one, m, m0, tables.data(), d_remap, d_pts, d_entry, d_tkey, d_tval, d_tkey2, d_tval2, d_sort, sort_bytes, grid, smem, key_bits));
+        QB_TRY(hb_levels<K>(p, others, m, m0, tables.data(), d_remap, d_pts, d_entry, d_tkey, d_tval, d_tkey2, d_tval2, d_sort, sort_bytes, grid, smem, key_bits));
+    } else {
+        QB_TRY(hb_levels<K>(p, plan, m, m0, tables.data(), d_remap, d_pts, d_entry, d_tkey, d_tval, d_tkey2, d_tval2, d_sort, sort_bytes, grid, smem, key_bits));
+    }
 
     // ---- finish: the plain arrays (level offsets, reindex, neighbours, offsets), then the handle as qb_hnsw_create_plain makes it
     HbTables tb{};
@@ -249,3 +275,8 @@ qb_status hb_run(qb_storage* s, typename K::Params p, const HbPlan& plan, uint32
 int hb_metric(const qb_storage* s) { return s->distance == QB_DIST_EUCLID ? M_EUCLID : (s->distance == QB_DIST_MANHATTAN ? M_MANHATTAN : M_DOT); }
 
 }  // namespace
+
+// qb_hnsw_build's plan and inserts over a dense f32 storage (qb_hnsw_build.cu), with hb_plan's `given` points and entry and hb_run's
+// prefill: qb_hnsw_build passes none, qb_hnsw_build_incremental (qb_hnsw_heal.cu) the healed graph.  Checks nothing the callers check.
+qb_status qb_hnsw_build_dense(qb_storage* s, uint32_t m, uint32_t m0, uint32_t ef, const uint8_t* levels, const uint32_t* given, uint32_t entry, uint32_t batch,
+                              uint32_t serial_points, const HbPrefill& prefill, const char* who, qb_hnsw** out, uint32_t* entry_point, uint32_t* entry_level);

@@ -223,6 +223,17 @@ public:
         check(qb_hnsw_build(storage.raw(), m, m0, ef_construct, levels.data(), batch, serial_points, &h, &entry_point, &entry_level));
         return std::unique_ptr<HnswGraph>(new HnswGraph(h));
     }
+    // builds the graph of a dense f32 storage from an old segment's graph (qb_hnsw_build_incremental): heals the old graph where points
+    // have gone, renumbers it by old_to_new (one per old point; 0xFFFFFFFF = not carried over) and inserts only the new points.  levels:
+    // one per point of `storage`, a mapped point's equal to its old level; m / m0 are old's; batch / serial_points 0 = 512 / 256.
+    static std::unique_ptr<HnswGraph> build_incremental(const VectorStorage& storage, const HnswGraph& old, const std::vector<uint32_t>& old_to_new,
+                                                        uint32_t ef_construct, const std::vector<uint8_t>& levels, uint32_t batch, uint32_t serial_points,
+                                                        uint32_t& entry_point, uint32_t& entry_level) {
+        qb_hnsw* h = nullptr;
+        check(qb_hnsw_build_incremental(storage.raw(), old.h_, old_to_new.data(), ef_construct, levels.data(), batch, serial_points, &h, &entry_point,
+                                        &entry_level));
+        return std::unique_ptr<HnswGraph>(new HnswGraph(h));
+    }
     // builds the graph over the points of a multivector collection on the device (qb_hnsw_build_multivector): point p = token rows
     // [point_offsets[p], point_offsets[p+1]) of the dense f32 `tokens`; levels: one per point; deleted_points: optional bitmap over points
     // (ceil(n / 64) words, may be null).  Search it with the MaxSim search.

@@ -719,6 +719,7 @@ class HnswGraph:
         h = vp()
         check(lib().qb_hnsw_create_plain(storage._h, blob.ctypes.data_as(u8p), blob.size, int(m), int(m0), C.byref(h)))
         self._h = h
+        self._m = int(m)
 
     @classmethod
     def from_compressed(cls, storage: _Storage, links_bin) -> "HnswGraph":
@@ -812,6 +813,7 @@ class HnswGraph:
         check(lib().qb_hnsw_build(storage._h, int(m), int(m0), int(ef_construct), lv.ctypes.data_as(u8p), int(batch), int(serial_points), C.byref(h),
                                   C.byref(e), C.byref(el)))
         self._h = h
+        self._m = int(m)
         self.entry_point, self.entry_level, self.levels = int(e.value), int(el.value), lv
         return self
 
@@ -836,6 +838,50 @@ class HnswGraph:
         self._h = h
         self.entry_point, self.entry_level, self.levels = int(e.value), int(el.value), lv
         return self
+
+    @classmethod
+    def build_incremental(cls, storage: _Storage, old: "HnswGraph", old_to_new, ef_construct: int = 100, levels=None, seed: int = 0, batch: int = 0,
+                          serial_points: int = 0) -> "HnswGraph":
+        """Builds the graph of a dense f32 storage from an old segment's graph (qb_hnsw_build_incremental): the old graph's lists are
+        healed where points have gone, renumbered, and only the points it did not have are inserted.  old_to_new: one per old point,
+        its id in `storage` or -1 (not carried over).  m / m0 are old's.  levels: one per point; by default a mapped point keeps its old
+        level and the others are drawn as build() draws them (`seed`).  The entry point is in .entry_point / .entry_level."""
+        n_old = old.info()[0]
+        o2n = np.asarray(old_to_new, dtype=np.int64)
+        if o2n.shape != (n_old,):
+            raise ValueError(f"old_to_new has shape {o2n.shape}, the old graph has {n_old} points")
+        o2n = np.ascontiguousarray(np.where(o2n < 0, 0xFFFFFFFF, o2n), dtype=np.uint32)
+        m = getattr(old, "_m", None)
+        if levels is None:
+            if m is None:
+                raise ValueError("the old graph's m is not known here (a compressed links.bin): pass levels")
+            lv = cls._build_levels(None, storage.count, m, seed).copy()
+            keep = (o2n != 0xFFFFFFFF) & (o2n < storage.count)
+            lv[o2n[keep]] = old.point_levels()[keep]
+        else:
+            lv = cls._build_levels(levels, storage.count, m or 2, seed)
+        self = cls.__new__(cls)
+        self._storage = storage
+        self._h = vp()
+        h, e, el = vp(), C.c_uint32(), C.c_uint32()
+        check(lib().qb_hnsw_build_incremental(storage._h, old._h, o2n.ctypes.data_as(u32p), int(ef_construct), lv.ctypes.data_as(u8p), int(batch),
+                                              int(serial_points), C.byref(h), C.byref(e), C.byref(el)))
+        self._h = h
+        self._m = m
+        self.entry_point, self.entry_level, self.levels = int(e.value), int(el.value), lv
+        return self
+
+    def point_levels(self) -> np.ndarray:
+        """Each point's top level (point_level, view.rs:354-369), from the graph's plain links.bin."""
+        b = self.export_plain()
+        n, levels = (int(x) for x in b[:16].view(np.uint64))
+        n_off = int(b[24:32].view(np.uint64)[0])
+        lo = np.append(b[64:64 + 8 * levels].view(np.uint64).astype(np.int64), n_off - 1)
+        reindex = b[64 + 8 * levels:64 + 8 * levels + 4 * n].view(np.uint32).astype(np.int64)
+        out = np.zeros(n, dtype=np.uint8)
+        for lvl in range(1, levels):
+            out[reindex < lo[lvl + 1] - lo[lvl]] = lvl
+        return out
 
     @staticmethod
     def _build_levels(levels, n: int, m: int, seed: int) -> np.ndarray:
