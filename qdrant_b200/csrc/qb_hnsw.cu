@@ -29,9 +29,9 @@
 // The compressed `links.bin` every current index is written in (GraphLinksFormatParam::Compressed, hnsw/build.rs:548-562) is
 // decoded on the device into exactly those arrays (qb_hnsw_create_compressed, below), so one traversal serves both formats.
 // The kernel (hnsw_search_kernel) and its pieces are in qb_hnsw_traverse.cuh, which the graph build (qb_hnsw_build.cu) shares.
-#include <cub/device/device_scan.cuh>
+#include <memory>
 
-#include "qb_hnsw_traverse.cuh"
+#include "qb_hnsw_host.cuh"
 
 // ------------------------------------------------------------------------------------------------ host side
 // ACORN: to_score holds up to m0 * m0 ids (a passing 1-hop links and at most m0 - a explored lists of m0), its keys sorted in a
@@ -79,16 +79,11 @@ static qb_status hnsw_create_plain_n(qb_storage* s, uint64_t expect, const char*
         for (uint64_t l = 0; l < levels; ++l) QB_CHECK(lo[l] < n_off, QB_ERR_INVALID, "hnsw_create_plain: level offset %llu out of range", (unsigned long long)l);
         lo[levels] = n_off - 1;
     }
-    cudaError_t ce = cudaSetDevice(s->device);
-    if (ce != cudaSuccess) { qb_set_error("hnsw_create_plain: %s", cudaGetErrorString(ce)); return QB_ERR_CUDA; }
-    qb_hnsw* g = new qb_hnsw();
-    g->st = s; g->n_points = (uint32_t)n; g->m = m; g->m0 = m0; g->levels = (uint32_t)levels;
-    g->level_offsets_ext = std::move(lo); g->n_offsets = n_off; g->n_neighbors = n_nb;
-    bool ok = cudaMalloc(&g->d_level_offsets, std::max<size_t>(8 * levels, 256)) == cudaSuccess &&
-              cudaMalloc(&g->d_reindex, std::max<size_t>(4 * n, 256)) == cudaSuccess &&
-              cudaMalloc(&g->d_neighbors, std::max<size_t>(4 * n_nb, 256)) == cudaSuccess &&
-              cudaMalloc(&g->d_offsets, 8 * n_off + 256) == cudaSuccess;
-    if (!ok) { qb_set_error("hnsw_create_plain: cudaMalloc failed: %s", cudaGetErrorString(cudaGetLastError())); qb_hnsw_destroy(g); return QB_ERR_OOM; }
+    qb_hnsw* g = nullptr;
+    QB_TRY(qb_hnsw_new(s, (uint32_t)n, m, m0, std::move(lo), n_off, 0, "hnsw_create_plain", &g));
+    g->n_neighbors = n_nb;
+    cudaError_t ce = cudaMalloc(&g->d_neighbors, std::max<size_t>(4 * n_nb, 256));
+    if (ce != cudaSuccess) { qb_set_error("hnsw_create_plain: cudaMalloc failed: %s", cudaGetErrorString(cudaGetLastError())); qb_hnsw_destroy(g); return QB_ERR_OOM; }
     ce = cudaMemcpy(g->d_level_offsets, p_lo, 8 * levels, cudaMemcpyHostToDevice);
     if (ce == cudaSuccess) ce = cudaMemcpy(g->d_reindex, p_re, 4 * n, cudaMemcpyHostToDevice);
     if (ce == cudaSuccess) ce = cudaMemcpy(g->d_neighbors, p_nb, 4 * n_nb, cudaMemcpyHostToDevice);
@@ -104,20 +99,36 @@ extern "C" qb_status qb_hnsw_create_plain(qb_storage* s, const uint8_t* links_bi
     return hnsw_create_plain_n(s, s ? s->count : 0, "storage", links_bin, n_bytes, m, m0, out);
 }
 
-// the rest of a handle whose plain arrays are on the device (qb_hnsw_create_plain's upload, qb_hnsw_build's finish): the level-0 table
-// the traversal reads, the search counters
+qb_status qb_hnsw_new(qb_storage* s, uint32_t n, uint32_t m, uint32_t m0, std::vector<uint64_t> lo, uint64_t n_off, uint64_t tail, const char* who,
+                      qb_hnsw** out) {
+    *out = nullptr;
+    const cudaError_t ce = cudaSetDevice(s->device);
+    if (ce != cudaSuccess) { qb_set_error("%s: %s", who, cudaGetErrorString(ce)); return QB_ERR_CUDA; }
+    qb_hnsw* g = new qb_hnsw();
+    g->st = s; g->n_points = n; g->m = m; g->m0 = m0; g->levels = (uint32_t)(lo.size() - 1);
+    g->level_offsets_ext = std::move(lo); g->n_offsets = n_off;
+    g->hbm_bytes = 8ull * g->levels + 4ull * n + 8 * (n_off + tail);
+    const bool ok = cudaMalloc(&g->d_level_offsets, std::max<size_t>(8ull * g->levels, 256)) == cudaSuccess &&
+                    cudaMalloc(&g->d_reindex, std::max<size_t>(4ull * n, 256)) == cudaSuccess &&
+                    cudaMalloc(&g->d_offsets, 8 * (n_off + tail) + 256) == cudaSuccess;
+    if (!ok) { qb_set_error("%s: cudaMalloc failed: %s", who, cudaGetErrorString(cudaGetLastError())); qb_hnsw_destroy(g); return QB_ERR_OOM; }
+    *out = g;
+    return QB_OK;
+}
+
 qb_status qb_hnsw_finish_plain(qb_hnsw* g, const char* who) {
     const uint64_t n = g->n_points, m0 = g->m0;
     bool ok = cudaMalloc(&g->d_links0, std::max<size_t>((size_t)n * m0 * 4, 256)) == cudaSuccess && cudaMalloc(&g->d_work, 256) == cudaSuccess &&
               cudaMalloc(&g->d_stats, 256) == cudaSuccess;
     if (!ok) { qb_set_error("%s: cudaMalloc failed: %s", who, cudaGetErrorString(cudaGetLastError())); return QB_ERR_OOM; }
-    g->hbm_bytes = n * m0 * 4 + 8ull * g->levels + 4 * n + 4 * g->n_neighbors + 8 * g->n_offsets;
+    g->hbm_bytes += n * m0 * 4 + 4 * g->n_neighbors;
     cudaError_t ce = cudaMemset(g->d_stats, 0, 256);
     if (ce == cudaSuccess && n) {
-        hnsw_links0_kernel<<<(unsigned)std::min<uint64_t>(ceil_div_u64(n * m0, 256), 132 * 16), 256>>>(g->d_neighbors, g->d_offsets, (uint32_t)n, (uint32_t)m0, g->d_links0);
+        hnsw_links0_kernel<<<hnsw_grid(n * m0, 256, 132 * 16), 256>>>(g->d_neighbors, g->d_offsets, (uint32_t)n, (uint32_t)m0, g->d_links0);
         QB_LAUNCHED();
-        ce = cudaDeviceSynchronize();
     }
+    if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
+    if (ce == cudaSuccess) ce = cudaGetLastError();
     if (ce != cudaSuccess) { qb_set_error("%s: upload: %s", who, cudaGetErrorString(ce)); return QB_ERR_CUDA; }
     return QB_OK;
 }
@@ -277,134 +288,115 @@ __global__ void hnsw_links_gather_kernel(const uint32_t* __restrict__ ids, uint3
     }
 }
 
-// device temporaries of one call, freed on every exit path
-struct HcScratch {
-    std::vector<void*> bufs;
-    cudaError_t alloc(void** p, size_t bytes) {
-        *p = nullptr;
-        const cudaError_t e = cudaMalloc(p, std::max<size_t>(bytes, 256));
-        if (e == cudaSuccess) bufs.push_back(*p);
-        return e;
-    }
-    ~HcScratch() { for (void* b : bufs) cudaFree(b); }
+// the fields HeaderCompressed and HeaderCompressedWithVectors share (bytes 0-58), then what hc_check derives from them
+struct HcHeader {
+    uint64_t n, version, levels, nb_bytes, length, m, m0;
+    uint32_t base_bits, delta_bits, log2;
+    uint64_t body, chunk_bytes, used;   // where the links / records start, one chunk of offsets, the bytes the file's parts take
+    uint32_t bits_unsorted;
+    std::vector<uint64_t> lo;           // the level offsets with the extra last element (read_level_offsets, view.rs:381-393)
 };
 
-inline unsigned hc_grid(uint64_t items, uint64_t per_block, uint64_t max_blocks) {
-    return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(ceil_div_u64(items, per_block), max_blocks));
+HcHeader hc_header(const uint8_t* bytes) {
+    auto u64_at = [&](uint64_t o) { uint64_t v; memcpy(&v, bytes + o, 8); return v; };   // the file is little-endian, like every host this builds for
+    HcHeader h{};
+    h.n = u64_at(0); h.version = u64_at(8); h.levels = u64_at(16); h.nb_bytes = u64_at(24); h.length = u64_at(32); h.m = u64_at(43); h.m0 = u64_at(51);
+    h.base_bits = bytes[40]; h.delta_bits = bytes[41]; h.log2 = bytes[42];
+    return h;
+}
+
+// the checks both compressed formats make after their own: the counts, the offsets parameters, the parts' sizes against n_bytes, the level
+// offsets.  head: the header's size; align: the links / records start at a file offset that is a multiple of it; after: what precedes
+// the offsets ("links" / "records"), for the messages
+qb_status hc_check(HcHeader& h, const uint8_t* bytes, uint64_t n_bytes, uint64_t head, uint64_t align, uint64_t expect, const char* of, const char* who,
+                   const char* after) {
+    const uint64_t n = h.n, levels = h.levels, nb_bytes = h.nb_bytes, length = h.length, m = h.m, m0 = h.m0;
+    const uint32_t base_bits = h.base_bits, delta_bits = h.delta_bits, log2 = h.log2;
+    QB_CHECK(n == expect, QB_ERR_INVALID, "%s: graph has %llu points, %s %llu", who, (unsigned long long)n, of, (unsigned long long)expect);
+    QB_CHECK(n <= 0xFFFFFFFFull, QB_ERR_INVALID, "%s: %llu points", who, (unsigned long long)n);
+    QB_CHECK(m >= 1 && m0 >= 1, QB_ERR_INVALID, "%s: m %llu / m0 %llu", who, (unsigned long long)m, (unsigned long long)m0);
+    QB_CHECK(m <= HNSW_MAX_LINKS && m0 <= HNSW_MAX_LINKS, QB_ERR_UNSUPPORTED, "%s: m %llu / m0 %llu outside [1,%u]", who, (unsigned long long)m,
+             (unsigned long long)m0, HNSW_MAX_LINKS);
+    QB_CHECK(levels <= 64 && (levels >= 1 || n == 0), QB_ERR_INVALID, "%s: %llu levels", who, (unsigned long long)levels);
+    // Parameters::validate (bitpacking_ordered.rs:165-180)
+    QB_CHECK(base_bits >= 1 && base_bits <= 64 && delta_bits >= 1 && delta_bits <= 56 && log2 <= 7, QB_ERR_INVALID,
+             "%s: offsets parameters base_bits %u delta_bits %u chunk_len_log2 %u", who, base_bits, delta_bits, log2);
+    const uint64_t body = h.body = round_up_u64(head + 8 * levels + 4 * n, align);
+    QB_CHECK(body <= n_bytes && nb_bytes <= n_bytes - body, QB_ERR_INVALID, "%s: %llu bytes, header describes %llu before the offsets", who,
+             (unsigned long long)n_bytes, (unsigned long long)(body + nb_bytes));
+    const uint64_t rest = n_bytes - body - nb_bytes;
+    const uint64_t chunk_bytes = h.chunk_bytes = ceil_div_u64(base_bits + (uint64_t)delta_bits * ((1ull << log2) - 1), 8);
+    const uint64_t chunks = length / (1ull << log2) + ((length & ((1ull << log2) - 1)) ? 1 : 0);
+    QB_CHECK(length >= 1 && chunks <= rest / chunk_bytes && chunks * chunk_bytes + 7 <= rest, QB_ERR_INVALID,
+             "%s: %llu offsets do not fit the %llu bytes after the %s", who, (unsigned long long)length, (unsigned long long)rest, after);
+    h.used = body + nb_bytes + chunks * chunk_bytes + 7;
+    // level 0 is the first n entries, every level's range inside the table
+    std::vector<uint64_t>& lo = h.lo;
+    lo.resize(levels + 1);
+    memcpy(lo.data(), bytes + head, 8 * levels);
+    lo[levels] = length - 1;
+    for (uint64_t l = 0; l < levels; ++l)
+        QB_CHECK(lo[l] <= lo[l + 1] && (l != 0 || (lo[0] == 0 && lo[1] == n)), QB_ERR_INVALID, "%s: level offset %llu (%llu) out of range", who,
+                 (unsigned long long)l, (unsigned long long)lo[l]);
+    h.bits_unsorted = std::max<uint32_t>(8, n > 1 ? 64 - __builtin_clzll(n - 1) : 0);
+    return QB_OK;
 }
 
 }  // namespace
 
 // a compressed links.bin over `expect` points, as hnsw_create_plain_n
 static qb_status hnsw_create_compressed_n(qb_storage* s, uint64_t expect, const char* of, const uint8_t* bytes, uint64_t n_bytes, qb_hnsw** out) {
+    const char* who = "hnsw_create_compressed";
     QB_CHECK(s && bytes && out, QB_ERR_INVALID, "hnsw_create_compressed: null argument");
     *out = nullptr;
     QB_CHECK(n_bytes >= 64, QB_ERR_INVALID, "hnsw_create_compressed: %llu bytes is smaller than HeaderCompressed", (unsigned long long)n_bytes);
-    auto u64_at = [&](uint64_t o) { uint64_t v; memcpy(&v, bytes + o, 8); return v; };   // the file is little-endian, like every host this builds for
-    const uint64_t n = u64_at(0), version = u64_at(8), levels = u64_at(16), nb_bytes = u64_at(24), length = u64_at(32), m = u64_at(43), m0 = u64_at(51);
-    const uint32_t base_bits = bytes[40], delta_bits = bytes[41], log2 = bytes[42];
-    QB_CHECK(version != HNSW_VERSION_COMPRESSED_WITH_VECTORS, QB_ERR_UNSUPPORTED,
+    HcHeader h = hc_header(bytes);
+    QB_CHECK(h.version != HNSW_VERSION_COMPRESSED_WITH_VECTORS, QB_ERR_UNSUPPORTED,
              "hnsw_create_compressed: CompressedWithVectors (inline storage) graphs are searched from the quantized vectors stored with the links "
              "(graph_layers.rs:336-388), a different algorithm; this loader takes GraphLinksFormat::Compressed");
-    QB_CHECK(version == HNSW_VERSION_COMPRESSED, QB_ERR_INVALID, "hnsw_create_compressed: version word %016llx is not HEADER_VERSION_COMPRESSED (a plain links.bin?)",
-             (unsigned long long)version);
-    QB_CHECK(n == expect, QB_ERR_INVALID, "hnsw_create_compressed: graph has %llu points, %s %llu", (unsigned long long)n, of, (unsigned long long)expect);
-    QB_CHECK(n <= 0xFFFFFFFFull, QB_ERR_INVALID, "hnsw_create_compressed: %llu points", (unsigned long long)n);
-    QB_CHECK(m >= 1 && m0 >= 1, QB_ERR_INVALID, "hnsw_create_compressed: m %llu / m0 %llu", (unsigned long long)m, (unsigned long long)m0);
-    QB_CHECK(m <= HNSW_MAX_LINKS && m0 <= HNSW_MAX_LINKS, QB_ERR_UNSUPPORTED, "hnsw_create_compressed: m %llu / m0 %llu outside [1,%u]", (unsigned long long)m,
-             (unsigned long long)m0, HNSW_MAX_LINKS);
-    QB_CHECK(levels <= 64 && (levels >= 1 || n == 0), QB_ERR_INVALID, "hnsw_create_compressed: %llu levels", (unsigned long long)levels);
-    // Parameters::validate (bitpacking_ordered.rs:165-180)
-    QB_CHECK(base_bits >= 1 && base_bits <= 64 && delta_bits >= 1 && delta_bits <= 56 && log2 <= 7, QB_ERR_INVALID,
-             "hnsw_create_compressed: offsets parameters base_bits %u delta_bits %u chunk_len_log2 %u", base_bits, delta_bits, log2);
-    const uint64_t body = 64 + 8 * levels + 4 * n;
-    QB_CHECK(body <= n_bytes && nb_bytes <= n_bytes - body, QB_ERR_INVALID, "hnsw_create_compressed: %llu bytes, header describes %llu before the offsets",
-             (unsigned long long)n_bytes, (unsigned long long)(body + nb_bytes));
-    const uint64_t rest = n_bytes - body - nb_bytes;
-    const uint64_t chunk_bytes = ceil_div_u64(base_bits + (uint64_t)delta_bits * ((1ull << log2) - 1), 8);
-    const uint64_t chunks = length / (1ull << log2) + ((length & ((1ull << log2) - 1)) ? 1 : 0);
-    QB_CHECK(length >= 1 && chunks <= rest / chunk_bytes && chunks * chunk_bytes + 7 <= rest, QB_ERR_INVALID,
-             "hnsw_create_compressed: %llu offsets do not fit the %llu bytes after the links", (unsigned long long)length, (unsigned long long)rest);
-    const uint64_t used = body + nb_bytes + chunks * chunk_bytes + 7;
-    // level offsets with the extra last element (read_level_offsets, view.rs:381-393): level 0 is the first n entries, every level's
-    // range inside the table
-    std::vector<uint64_t> lo(levels + 1);
-    memcpy(lo.data(), bytes + 64, 8 * levels);
-    lo[levels] = length - 1;
-    for (uint64_t l = 0; l < levels; ++l)
-        QB_CHECK(lo[l] <= lo[l + 1] && (l != 0 || (lo[0] == 0 && lo[1] == n)), QB_ERR_INVALID, "hnsw_create_compressed: level offset %llu (%llu) out of range",
-                 (unsigned long long)l, (unsigned long long)lo[l]);
-    const uint32_t bits_unsorted = std::max<uint32_t>(8, n > 1 ? 64 - __builtin_clzll(n - 1) : 0);
+    QB_CHECK(h.version == HNSW_VERSION_COMPRESSED, QB_ERR_INVALID, "hnsw_create_compressed: version word %016llx is not HEADER_VERSION_COMPRESSED (a plain links.bin?)",
+             (unsigned long long)h.version);
+    QB_TRY(hc_check(h, bytes, n_bytes, 64, 1, expect, of, who, "links"));
+    const uint64_t n = h.n, levels = h.levels, length = h.length;
 
-    cudaError_t ce = cudaSetDevice(s->device);
-    if (ce != cudaSuccess) { qb_set_error("hnsw_create_compressed: %s", cudaGetErrorString(ce)); return QB_ERR_CUDA; }
-    qb_hnsw* g = new qb_hnsw();
-    g->st = s; g->n_points = (uint32_t)n; g->m = (uint32_t)m; g->m0 = (uint32_t)m0; g->levels = (uint32_t)levels;
-    g->level_offsets_ext = lo; g->n_offsets = length;
+    qb_hnsw* g = nullptr;
+    QB_TRY(qb_hnsw_new(s, (uint32_t)n, (uint32_t)h.m, (uint32_t)h.m0, std::move(h.lo), length, n, who, &g));
+    std::unique_ptr<qb_hnsw, decltype(&qb_hnsw_destroy)> guard(g, qb_hnsw_destroy);
     auto fail = [&](qb_status st, const char* what, cudaError_t e) {
         qb_set_error("hnsw_create_compressed: %s: %s", what, cudaGetErrorString(e));
-        qb_hnsw_destroy(g);
         return st;
     };
-    HcScratch tmp;
+    HnswScratch tmp;
     uint8_t* d_file = nullptr; uint64_t* d_byte_off = nullptr; uint64_t* d_counts = nullptr; uint32_t* d_flag = nullptr;
-    bool ok = cudaMalloc(&g->d_links0, std::max<size_t>((size_t)n * m0 * 4, 256)) == cudaSuccess &&
-              cudaMalloc(&g->d_level_offsets, std::max<size_t>(8 * levels, 256)) == cudaSuccess &&
-              cudaMalloc(&g->d_reindex, std::max<size_t>(4 * n, 256)) == cudaSuccess &&
-              cudaMalloc(&g->d_offsets, 8 * (length + n) + 256) == cudaSuccess && cudaMalloc(&g->d_work, 256) == cudaSuccess &&
-              cudaMalloc(&g->d_stats, 256) == cudaSuccess &&
-              tmp.alloc((void**)&d_file, used + HC_PAD) == cudaSuccess && tmp.alloc((void**)&d_byte_off, 8 * length) == cudaSuccess &&
+    bool ok = tmp.alloc((void**)&d_file, h.used + HC_PAD) == cudaSuccess && tmp.alloc((void**)&d_byte_off, 8 * length) == cudaSuccess &&
               tmp.alloc((void**)&d_counts, 8 * length) == cudaSuccess && tmp.alloc((void**)&d_flag, 4) == cudaSuccess;
     if (!ok) return fail(QB_ERR_OOM, "cudaMalloc failed", cudaGetLastError());
     // the file goes to HBM once; everything below reads it there
-    ce = cudaMemcpy(d_file, bytes, used, cudaMemcpyHostToDevice);
-    if (ce == cudaSuccess) ce = cudaMemset(d_file + used, 0, HC_PAD);
+    cudaError_t ce = cudaMemcpy(d_file, bytes, h.used, cudaMemcpyHostToDevice);
+    if (ce == cudaSuccess) ce = cudaMemset(d_file + h.used, 0, HC_PAD);
     if (ce == cudaSuccess) ce = cudaMemcpy(g->d_level_offsets, d_file + 64, 8 * levels, cudaMemcpyDeviceToDevice);
     if (ce == cudaSuccess) ce = cudaMemcpy(g->d_reindex, d_file + 64 + 8 * levels, 4 * n, cudaMemcpyDeviceToDevice);
-    if (ce == cudaSuccess) ce = cudaMemset(g->d_stats, 0, 256);
     if (ce == cudaSuccess) ce = cudaMemset(d_flag, 0, 4);
     if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "upload", ce);
 
-    HcOffsets po{d_file + body + nb_bytes, length, chunk_bytes, nb_bytes, base_bits, delta_bits, log2};
-    hnsw_c_offsets_kernel<<<hc_grid(length, 256, 132 * 16), 256>>>(po, d_byte_off, d_flag);
+    HcOffsets po{d_file + h.body + h.nb_bytes, length, h.chunk_bytes, h.nb_bytes, h.base_bits, h.delta_bits, h.log2};
+    hnsw_c_offsets_kernel<<<hnsw_grid(length, 256, 132 * 16), 256>>>(po, d_byte_off, d_flag);
     QB_LAUNCHED();
-    HcLinks pl{d_file + body, d_byte_off, length - 1, nb_bytes, (uint32_t)n, (uint32_t)m, (uint32_t)m0, bits_unsorted};
-    hnsw_c_counts_kernel<<<hc_grid(std::max<uint64_t>(length, n), 256, 132 * 16), 256>>>(pl, g->d_reindex, d_counts, d_flag);
-    QB_LAUNCHED();
-    // plain element offsets = exclusive scan of the counts
-    size_t scan_bytes = 0;
-    ce = cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_counts, g->d_offsets, (int64_t)length);
-    void* d_scan = nullptr;
-    if (ce == cudaSuccess) ce = tmp.alloc(&d_scan, scan_bytes);
-    if (ce == cudaSuccess) ce = cub::DeviceScan::ExclusiveSum(d_scan, scan_bytes, d_counts, g->d_offsets, (int64_t)length);
+    HcLinks pl{d_file + h.body, d_byte_off, length - 1, h.nb_bytes, (uint32_t)n, (uint32_t)h.m, (uint32_t)h.m0, h.bits_unsorted};
+    hnsw_c_counts_kernel<<<hnsw_grid(std::max<uint64_t>(length, n), 256, 132 * 16), 256>>>(pl, g->d_reindex, d_counts, d_flag);
     QB_LAUNCHED();
     uint32_t flag = 0;
-    uint64_t total = 0;
-    if (ce == cudaSuccess) ce = cudaMemcpy(&flag, d_flag, 4, cudaMemcpyDeviceToHost);
-    if (ce == cudaSuccess) ce = cudaMemcpy(&total, g->d_offsets + (length - 1), 8, cudaMemcpyDeviceToHost);
-    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "decode", ce);
-    if (flag) {
-        qb_set_error("hnsw_create_compressed: %s", (flag & HC_OFFSET_PAST_END) ? "a links offset lies past total_neighbors_bytes"
-                                                   : (flag & HC_OFFSETS_DECREASE) ? "links offsets decrease"
-                                                                                  : "a reindex entry is >= point_count");
-        qb_hnsw_destroy(g);
-        return QB_ERR_INVALID;
-    }
-    g->n_neighbors = total;
-    g->hbm_bytes = (uint64_t)n * m0 * 4 + 8 * levels + 4 * n + 4 * total + 8 * (length + n);
-    if (cudaMalloc(&g->d_neighbors, std::max<size_t>(4 * total, 256)) != cudaSuccess) return fail(QB_ERR_OOM, "cudaMalloc failed", cudaGetLastError());
-    hnsw_c_links_kernel<<<hc_grid(length - 1, 8, 132 * 32), 256>>>(pl, g->d_offsets, g->d_neighbors);
-    QB_LAUNCHED();
-    hnsw_c_pad_kernel<<<hc_grid(n, 256, 132 * 4), 256>>>(g->d_offsets, length, n);
-    QB_LAUNCHED();
-    if (n) {
-        hnsw_links0_kernel<<<hc_grid(n * m0, 256, 132 * 16), 256>>>(g->d_neighbors, g->d_offsets, (uint32_t)n, (uint32_t)m0, g->d_links0);
+    QB_TRY(hnsw_link_offsets(g, d_counts, length, tmp, who, "decode", d_flag, &flag, [&](const uint64_t* d_offsets, uint32_t* d_neighbors) {
+        hnsw_c_links_kernel<<<hnsw_grid(length - 1, 8, 132 * 32), 256>>>(pl, d_offsets, d_neighbors);
         QB_LAUNCHED();
-    }
-    ce = cudaDeviceSynchronize();
-    if (ce == cudaSuccess) ce = cudaGetLastError();
-    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "decode", ce);
-    *out = g;
+    }));
+    QB_CHECK(!flag, QB_ERR_INVALID, "hnsw_create_compressed: %s", (flag & HC_OFFSET_PAST_END) ? "a links offset lies past total_neighbors_bytes"
+                                                                : (flag & HC_OFFSETS_DECREASE) ? "links offsets decrease"
+                                                                                               : "a reindex entry is >= point_count");
+    hnsw_c_pad_kernel<<<hnsw_grid(n, 256, 132 * 4), 256>>>(g->d_offsets, length, n);
+    QB_LAUNCHED();
+    QB_TRY(qb_hnsw_finish_plain(g, who));
+    *out = guard.release();
     return QB_OK;
 }
 
@@ -427,42 +419,51 @@ qb_status qb_hnsw_mv_check(qb_storage* s, const uint32_t* point_offsets, uint32_
     return QB_OK;
 }
 
-static qb_status mv_attach(qb_hnsw* g, const uint32_t* point_offsets, uint32_t n_points, const char* who) {
+qb_status qb_hnsw_mv_upload(const uint32_t* point_offsets, uint32_t n_points, const char* who, uint32_t** d_tok) {
     const size_t bytes = 4ull * ((size_t)n_points + 1);
-    cudaError_t ce = cudaMalloc(&g->d_mv_tok, bytes);
-    if (ce == cudaSuccess) ce = cudaMemcpy(g->d_mv_tok, point_offsets, bytes, cudaMemcpyHostToDevice);
+    *d_tok = nullptr;
+    cudaError_t ce = cudaMalloc(d_tok, bytes);
+    if (ce == cudaSuccess) ce = cudaMemcpy(*d_tok, point_offsets, bytes, cudaMemcpyHostToDevice);
     if (ce != cudaSuccess) {
         qb_set_error("%s: offsets upload: %s", who, cudaGetErrorString(ce));
+        cudaFree(*d_tok);
+        *d_tok = nullptr;
         return ce == cudaErrorMemoryAllocation ? QB_ERR_OOM : QB_ERR_CUDA;
     }
-    g->hbm_bytes += bytes;
+    return QB_OK;
+}
+
+void qb_hnsw_mv_attach(qb_hnsw* g, uint32_t* d_tok, uint32_t n_points) {
+    g->d_mv_tok = d_tok;
+    g->hbm_bytes += 4ull * ((size_t)n_points + 1);
+}
+
+// a loader's graph (create) over the points of a multivector collection, with their token offsets attached
+template <class Create>
+static qb_status hnsw_create_mv(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, const char* who, qb_hnsw** out, Create create) {
+    QB_CHECK(out, QB_ERR_INVALID, "%s: null argument", who);
+    *out = nullptr;
+    QB_TRY(qb_hnsw_mv_check(tokens, point_offsets, n_points, who));
+    qb_hnsw* g = nullptr;
+    QB_TRY(create(&g));
+    uint32_t* d_tok = nullptr;
+    const qb_status st = qb_hnsw_mv_upload(point_offsets, n_points, who, &d_tok);
+    if (st != QB_OK) { qb_hnsw_destroy(g); return st; }
+    qb_hnsw_mv_attach(g, d_tok, n_points);
+    *out = g;
     return QB_OK;
 }
 
 extern "C" qb_status qb_hnsw_create_plain_multivector(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, const uint8_t* links_bin,
                                                       uint64_t n_bytes, uint32_t m, uint32_t m0, qb_hnsw** out) {
-    QB_CHECK(out, QB_ERR_INVALID, "hnsw_create_plain_multivector: null argument");
-    *out = nullptr;
-    QB_TRY(qb_hnsw_mv_check(tokens, point_offsets, n_points, "hnsw_create_plain_multivector"));
-    qb_hnsw* g = nullptr;
-    QB_TRY(hnsw_create_plain_n(tokens, n_points, "collection", links_bin, n_bytes, m, m0, &g));
-    const qb_status st = mv_attach(g, point_offsets, n_points, "hnsw_create_plain_multivector");
-    if (st != QB_OK) { qb_hnsw_destroy(g); return st; }
-    *out = g;
-    return QB_OK;
+    return hnsw_create_mv(tokens, point_offsets, n_points, "hnsw_create_plain_multivector", out,
+                          [&](qb_hnsw** g) { return hnsw_create_plain_n(tokens, n_points, "collection", links_bin, n_bytes, m, m0, g); });
 }
 
 extern "C" qb_status qb_hnsw_create_compressed_multivector(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, const uint8_t* bytes,
                                                            uint64_t n_bytes, qb_hnsw** out) {
-    QB_CHECK(out, QB_ERR_INVALID, "hnsw_create_compressed_multivector: null argument");
-    *out = nullptr;
-    QB_TRY(qb_hnsw_mv_check(tokens, point_offsets, n_points, "hnsw_create_compressed_multivector"));
-    qb_hnsw* g = nullptr;
-    QB_TRY(hnsw_create_compressed_n(tokens, n_points, "collection", bytes, n_bytes, &g));
-    const qb_status st = mv_attach(g, point_offsets, n_points, "hnsw_create_compressed_multivector");
-    if (st != QB_OK) { qb_hnsw_destroy(g); return st; }
-    *out = g;
-    return QB_OK;
+    return hnsw_create_mv(tokens, point_offsets, n_points, "hnsw_create_compressed_multivector", out,
+                          [&](qb_hnsw** g) { return hnsw_create_compressed_n(tokens, n_points, "collection", bytes, n_bytes, g); });
 }
 
 // ------------------------------------------------------------------------------------------------ compressed links.bin with vectors
@@ -550,14 +551,14 @@ extern "C" qb_status qb_hnsw_create_with_vectors(qb_storage* s, const uint8_t* b
     QB_CHECK(s && bytes && out, QB_ERR_INVALID, "hnsw_create_with_vectors: null argument");
     *out = nullptr;
     QB_CHECK(n_bytes >= 80, QB_ERR_INVALID, "hnsw_create_with_vectors: %llu bytes is smaller than HeaderCompressedWithVectors", (unsigned long long)n_bytes);
-    auto u64_at = [&](uint64_t o) { uint64_t v; memcpy(&v, bytes + o, 8); return v; };
-    const uint64_t n = u64_at(0), version = u64_at(8), levels = u64_at(16), nb_bytes = u64_at(24), length = u64_at(32), m = u64_at(43), m0 = u64_at(51);
-    const uint32_t base_bits = bytes[40], delta_bits = bytes[41], log2 = bytes[42];
-    const uint64_t base_size = u64_at(59), link_size = u64_at(68);
+    const char* who = "hnsw_create_with_vectors";
+    HcHeader h = hc_header(bytes);
+    uint64_t base_size, link_size;
+    memcpy(&base_size, bytes + 59, 8); memcpy(&link_size, bytes + 68, 8);
     const uint32_t base_align = bytes[67], link_align = bytes[76];
-    QB_CHECK(version == HNSW_VERSION_COMPRESSED_WITH_VECTORS, QB_ERR_INVALID,
+    QB_CHECK(h.version == HNSW_VERSION_COMPRESSED_WITH_VECTORS, QB_ERR_INVALID,
              "hnsw_create_with_vectors: version word %016llx is not HEADER_VERSION_COMPRESSED_WITH_VECTORS (a Compressed or plain links.bin?)",
-             (unsigned long long)version);
+             (unsigned long long)h.version);
     QB_CHECK(s->kind == QB_KIND_SQ8, QB_ERR_UNSUPPORTED,
              "hnsw_create_with_vectors: the link vectors are read as rows of the bound storage, which must be scalar-quantized (SQ8)");
     // Layout::from_size_align (header.rs:63-69): a power-of-two alignment
@@ -569,108 +570,60 @@ extern "C" qb_status qb_hnsw_create_with_vectors(qb_storage* s, const uint8_t* b
     QB_CHECK(base_size == 4ull * s->dim, QB_ERR_INVALID, "hnsw_create_with_vectors: base vectors of %llu bytes, dim %u", (unsigned long long)base_size, s->dim);
     QB_CHECK(link_size == 4ull + s->actual_dim, QB_ERR_INVALID, "hnsw_create_with_vectors: link vectors of %llu bytes, the storage's rows have %u",
              (unsigned long long)link_size, 4u + s->actual_dim);
-    QB_CHECK(n == s->count, QB_ERR_INVALID, "hnsw_create_with_vectors: graph has %llu points, storage %llu", (unsigned long long)n, (unsigned long long)s->count);
-    QB_CHECK(n <= 0xFFFFFFFFull, QB_ERR_INVALID, "hnsw_create_with_vectors: %llu points", (unsigned long long)n);
-    QB_CHECK(m >= 1 && m0 >= 1, QB_ERR_INVALID, "hnsw_create_with_vectors: m %llu / m0 %llu", (unsigned long long)m, (unsigned long long)m0);
-    QB_CHECK(m <= HNSW_MAX_LINKS && m0 <= HNSW_MAX_LINKS, QB_ERR_UNSUPPORTED, "hnsw_create_with_vectors: m %llu / m0 %llu outside [1,%u]",
-             (unsigned long long)m, (unsigned long long)m0, HNSW_MAX_LINKS);
-    QB_CHECK(levels <= 64 && (levels >= 1 || n == 0), QB_ERR_INVALID, "hnsw_create_with_vectors: %llu levels", (unsigned long long)levels);
-    QB_CHECK(base_bits >= 1 && base_bits <= 64 && delta_bits >= 1 && delta_bits <= 56 && log2 <= 7, QB_ERR_INVALID,
-             "hnsw_create_with_vectors: offsets parameters base_bits %u delta_bits %u chunk_len_log2 %u", base_bits, delta_bits, log2);
-    const uint64_t align = std::max(base_align, link_align);
-    const uint64_t body = round_up_u64(80 + 8 * levels + 4 * n, align);
-    QB_CHECK(body <= n_bytes && nb_bytes <= n_bytes - body, QB_ERR_INVALID, "hnsw_create_with_vectors: %llu bytes, header describes %llu before the offsets",
-             (unsigned long long)n_bytes, (unsigned long long)(body + nb_bytes));
-    const uint64_t rest = n_bytes - body - nb_bytes;
-    const uint64_t chunk_bytes = ceil_div_u64(base_bits + (uint64_t)delta_bits * ((1ull << log2) - 1), 8);
-    const uint64_t chunks = length / (1ull << log2) + ((length & ((1ull << log2) - 1)) ? 1 : 0);
-    QB_CHECK(length >= 1 && chunks <= rest / chunk_bytes && chunks * chunk_bytes + 7 <= rest, QB_ERR_INVALID,
-             "hnsw_create_with_vectors: %llu offsets do not fit the %llu bytes after the records", (unsigned long long)length, (unsigned long long)rest);
-    const uint64_t used = body + nb_bytes + chunks * chunk_bytes + 7;
-    std::vector<uint64_t> lo(levels + 1);
-    memcpy(lo.data(), bytes + 80, 8 * levels);
-    lo[levels] = length - 1;
-    for (uint64_t l = 0; l < levels; ++l)
-        QB_CHECK(lo[l] <= lo[l + 1] && (l != 0 || (lo[0] == 0 && lo[1] == n)), QB_ERR_INVALID, "hnsw_create_with_vectors: level offset %llu (%llu) out of range",
-                 (unsigned long long)l, (unsigned long long)lo[l]);
-    const uint32_t bits_unsorted = std::max<uint32_t>(8, n > 1 ? 64 - __builtin_clzll(n - 1) : 0);
+    QB_TRY(hc_check(h, bytes, n_bytes, 80, std::max(base_align, link_align), s->count, "storage", who, "records"));
+    const uint64_t n = h.n, levels = h.levels, nb_bytes = h.nb_bytes, length = h.length;
 
-    cudaError_t ce = cudaSetDevice(s->device);
-    if (ce != cudaSuccess) { qb_set_error("hnsw_create_with_vectors: %s", cudaGetErrorString(ce)); return QB_ERR_CUDA; }
-    qb_hnsw* g = new qb_hnsw();
-    g->st = s; g->n_points = (uint32_t)n; g->m = (uint32_t)m; g->m0 = (uint32_t)m0; g->levels = (uint32_t)levels;
-    g->level_offsets_ext = lo; g->n_offsets = length; g->link_size = (uint32_t)link_size;
+    qb_hnsw* g = nullptr;
+    QB_TRY(qb_hnsw_new(s, (uint32_t)n, (uint32_t)h.m, (uint32_t)h.m0, std::move(h.lo), length, n, who, &g));
+    std::unique_ptr<qb_hnsw, decltype(&qb_hnsw_destroy)> guard(g, qb_hnsw_destroy);
+    g->link_size = (uint32_t)link_size;
     auto fail = [&](qb_status st, const char* what, cudaError_t e) {
         qb_set_error("hnsw_create_with_vectors: %s: %s", what, cudaGetErrorString(e));
-        qb_hnsw_destroy(g);
         return st;
     };
-    HcScratch tmp;
+    HnswScratch tmp;
     uint8_t* d_file = nullptr; uint64_t *d_byte_off = nullptr, *d_counts = nullptr, *d_lstart = nullptr; uint32_t* d_flag = nullptr;
-    bool ok = cudaMalloc(&g->d_links0, std::max<size_t>((size_t)n * m0 * 4, 256)) == cudaSuccess &&
-              cudaMalloc(&g->d_level_offsets, std::max<size_t>(8 * levels, 256)) == cudaSuccess &&
-              cudaMalloc(&g->d_reindex, std::max<size_t>(4 * n, 256)) == cudaSuccess &&
-              cudaMalloc(&g->d_offsets, 8 * (length + n) + 256) == cudaSuccess && cudaMalloc(&g->d_work, 256) == cudaSuccess &&
-              cudaMalloc(&g->d_stats, 256) == cudaSuccess && cudaMalloc(&g->d_blob, nb_bytes + HC_PAD) == cudaSuccess &&
-              cudaMalloc(&g->d_lvoff, 8 * (length + n) + 256) == cudaSuccess && cudaMalloc(&g->d_boff, std::max<size_t>(8 * n, 256)) == cudaSuccess &&
-              tmp.alloc((void**)&d_file, used + HC_PAD) == cudaSuccess && tmp.alloc((void**)&d_byte_off, 8 * length) == cudaSuccess &&
+    bool ok = cudaMalloc(&g->d_blob, nb_bytes + HC_PAD) == cudaSuccess && cudaMalloc(&g->d_lvoff, 8 * (length + n) + 256) == cudaSuccess &&
+              cudaMalloc(&g->d_boff, std::max<size_t>(8 * n, 256)) == cudaSuccess &&
+              tmp.alloc((void**)&d_file, h.used + HC_PAD) == cudaSuccess && tmp.alloc((void**)&d_byte_off, 8 * length) == cudaSuccess &&
               tmp.alloc((void**)&d_counts, 8 * length) == cudaSuccess && tmp.alloc((void**)&d_lstart, 8 * length) == cudaSuccess &&
               tmp.alloc((void**)&d_flag, 4) == cudaSuccess;
     if (!ok) return fail(QB_ERR_OOM, "cudaMalloc failed", cudaGetLastError());
-    ce = cudaMemcpy(d_file, bytes, used, cudaMemcpyHostToDevice);
-    if (ce == cudaSuccess) ce = cudaMemset(d_file + used, 0, HC_PAD);
+    g->hbm_bytes += (nb_bytes + HC_PAD) + 8 * (length + n) + 8 * n;
+    cudaError_t ce = cudaMemcpy(d_file, bytes, h.used, cudaMemcpyHostToDevice);
+    if (ce == cudaSuccess) ce = cudaMemset(d_file + h.used, 0, HC_PAD);
     if (ce == cudaSuccess) ce = cudaMemcpy(g->d_level_offsets, d_file + 80, 8 * levels, cudaMemcpyDeviceToDevice);
     if (ce == cudaSuccess) ce = cudaMemcpy(g->d_reindex, d_file + 80 + 8 * levels, 4 * n, cudaMemcpyDeviceToDevice);
-    if (ce == cudaSuccess) ce = cudaMemcpy(g->d_blob, d_file + body, nb_bytes, cudaMemcpyDeviceToDevice);
+    if (ce == cudaSuccess) ce = cudaMemcpy(g->d_blob, d_file + h.body, nb_bytes, cudaMemcpyDeviceToDevice);
     if (ce == cudaSuccess) ce = cudaMemset(g->d_blob + nb_bytes, 0, HC_PAD);
     if (ce == cudaSuccess) ce = cudaMemset(g->d_lvoff, 0, 8 * (length + n) + 256);
-    if (ce == cudaSuccess) ce = cudaMemset(g->d_stats, 0, 256);
     if (ce == cudaSuccess) ce = cudaMemset(d_flag, 0, 4);
     if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "upload", ce);
 
-    HcOffsets po{d_file + body + nb_bytes, length, chunk_bytes, nb_bytes, base_bits, delta_bits, log2};
-    hnsw_c_offsets_kernel<<<hc_grid(length, 256, 132 * 16), 256>>>(po, d_byte_off, d_flag);
+    HcOffsets po{d_file + h.body + nb_bytes, length, h.chunk_bytes, nb_bytes, h.base_bits, h.delta_bits, h.log2};
+    hnsw_c_offsets_kernel<<<hnsw_grid(length, 256, 132 * 16), 256>>>(po, d_byte_off, d_flag);
     QB_LAUNCHED();
-    HvShape pv{d_file + body, d_byte_off, length - 1, nb_bytes, base_size, link_size, (uint32_t)n, (uint32_t)m, (uint32_t)m0, bits_unsorted, link_align};
-    hnsw_v_shape_kernel<<<hc_grid(std::max<uint64_t>(length, n), 256, 132 * 16), 256>>>(pv, g->d_reindex, d_counts, d_lstart, g->d_lvoff, d_flag);
-    QB_LAUNCHED();
-    size_t scan_bytes = 0;
-    ce = cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_counts, g->d_offsets, (int64_t)length);
-    void* d_scan = nullptr;
-    if (ce == cudaSuccess) ce = tmp.alloc(&d_scan, scan_bytes);
-    if (ce == cudaSuccess) ce = cub::DeviceScan::ExclusiveSum(d_scan, scan_bytes, d_counts, g->d_offsets, (int64_t)length);
+    HvShape pv{d_file + h.body, d_byte_off, length - 1, nb_bytes, base_size, link_size, (uint32_t)n, (uint32_t)h.m, (uint32_t)h.m0, h.bits_unsorted, link_align};
+    hnsw_v_shape_kernel<<<hnsw_grid(std::max<uint64_t>(length, n), 256, 132 * 16), 256>>>(pv, g->d_reindex, d_counts, d_lstart, g->d_lvoff, d_flag);
     QB_LAUNCHED();
     uint32_t flag = 0;
-    uint64_t total = 0;
-    if (ce == cudaSuccess) ce = cudaMemcpy(&flag, d_flag, 4, cudaMemcpyDeviceToHost);
-    if (ce == cudaSuccess) ce = cudaMemcpy(&total, g->d_offsets + (length - 1), 8, cudaMemcpyDeviceToHost);
-    if (ce == cudaSuccess && n) ce = cudaMemcpy(g->d_boff, d_byte_off, 8 * n, cudaMemcpyDeviceToDevice);
-    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "decode", ce);
+    QB_TRY(hnsw_link_offsets(g, d_counts, length, tmp, who, "decode", d_flag, &flag, [&](const uint64_t* d_offsets, uint32_t* d_neighbors) {
+        hnsw_v_links_kernel<<<hnsw_grid(length - 1, 8, 132 * 32), 256>>>(pv, d_lstart, d_offsets, d_neighbors);
+        QB_LAUNCHED();
+    }));
     if (flag) {
-        const bool wide = flag == HV_TOO_WIDE;
         qb_set_error("hnsw_create_with_vectors: %s", (flag & HC_OFFSET_PAST_END) ? "a record offset lies past total_neighbors_bytes"
                                                     : (flag & HC_OFFSETS_DECREASE) ? "record offsets decrease"
                                                     : (flag & HC_REINDEX)          ? "a reindex entry is >= point_count"
                                                     : (flag & HV_RECORD)           ? "a record's count, links or link vectors run past its end"
                                                                                    : "a list has more than 128 links");
-        qb_hnsw_destroy(g);
-        return wide ? QB_ERR_UNSUPPORTED : QB_ERR_INVALID;
+        return flag == HV_TOO_WIDE ? QB_ERR_UNSUPPORTED : QB_ERR_INVALID;
     }
-    g->n_neighbors = total;
-    g->hbm_bytes = (uint64_t)n * m0 * 4 + 8 * levels + 4 * n + 4 * total + 8 * (length + n) + (nb_bytes + HC_PAD) + 8 * (length + n) + 8 * n;
-    if (cudaMalloc(&g->d_neighbors, std::max<size_t>(4 * total, 256)) != cudaSuccess) return fail(QB_ERR_OOM, "cudaMalloc failed", cudaGetLastError());
-    hnsw_v_links_kernel<<<hc_grid(length - 1, 8, 132 * 32), 256>>>(pv, d_lstart, g->d_offsets, g->d_neighbors);
+    if (n && (ce = cudaMemcpy(g->d_boff, d_byte_off, 8 * n, cudaMemcpyDeviceToDevice)) != cudaSuccess) return fail(QB_ERR_CUDA, "decode", ce);
+    hnsw_c_pad_kernel<<<hnsw_grid(n, 256, 132 * 4), 256>>>(g->d_offsets, length, n);
     QB_LAUNCHED();
-    hnsw_c_pad_kernel<<<hc_grid(n, 256, 132 * 4), 256>>>(g->d_offsets, length, n);
-    QB_LAUNCHED();
-    if (n) {
-        hnsw_links0_kernel<<<hc_grid(n * m0, 256, 132 * 16), 256>>>(g->d_neighbors, g->d_offsets, (uint32_t)n, (uint32_t)m0, g->d_links0);
-        QB_LAUNCHED();
-    }
-    ce = cudaDeviceSynchronize();
-    if (ce == cudaSuccess) ce = cudaGetLastError();
-    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "decode", ce);
-    *out = g;
+    QB_TRY(qb_hnsw_finish_plain(g, who));
+    *out = guard.release();
     return QB_OK;
 }
 
@@ -684,7 +637,7 @@ extern "C" qb_status qb_hnsw_links(const qb_hnsw* g, uint32_t level, const uint3
     uint64_t on_level = ~0ull;
     for (uint32_t l = 1; l <= level; ++l) on_level = std::min<uint64_t>(on_level, lo[l + 1] >= lo[l] ? lo[l + 1] - lo[l] : 0);
     QB_CUDA(cudaSetDevice(g->st->device));
-    HcScratch tmp;
+    HnswScratch tmp;
     uint32_t *d_ids = nullptr, *d_out = nullptr, *d_counts = nullptr, *d_flag = nullptr;
     QB_CUDA(tmp.alloc((void**)&d_ids, 4ull * n_ids));
     QB_CUDA(tmp.alloc((void**)&d_out, 4ull * n_ids * cap));
@@ -692,7 +645,7 @@ extern "C" qb_status qb_hnsw_links(const qb_hnsw* g, uint32_t level, const uint3
     QB_CUDA(tmp.alloc((void**)&d_flag, 4));
     QB_CUDA(cudaMemcpy(d_ids, ids, 4ull * n_ids, cudaMemcpyHostToDevice));
     QB_CUDA(cudaMemset(d_flag, 0, 4));
-    hnsw_links_gather_kernel<<<hc_grid(n_ids, 128, 132 * 8), 128>>>(d_ids, n_ids, level, level ? lo[level] : 0, on_level, g->d_reindex, g->d_offsets, g->n_offsets,
+    hnsw_links_gather_kernel<<<hnsw_grid(n_ids, 128, 132 * 8), 128>>>(d_ids, n_ids, level, level ? lo[level] : 0, on_level, g->d_reindex, g->d_offsets, g->n_offsets,
                                                                     g->d_neighbors, g->n_neighbors, cap, d_out, d_counts, d_flag);
     QB_LAUNCHED();
     QB_CUDA(cudaGetLastError());

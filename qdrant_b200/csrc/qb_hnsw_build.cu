@@ -96,7 +96,7 @@ struct HbKernels {
         return QB_OK;
     }
     static qb_status backlinks(const HnswParams& p, const unsigned long long* keys, const uint32_t* vals, uint32_t n) {
-        hnsw_backlink_kernel<KIND, METRIC><<<hb_grid(n, HB_WARPS, 132 * 16), HB_WARPS * 32>>>(p, keys, vals, n);
+        hnsw_backlink_kernel<KIND, METRIC><<<hnsw_grid(n, HB_WARPS, 132 * 16), HB_WARPS * 32>>>(p, keys, vals, n);
         QB_LAUNCHED();
         QB_CUDA(cudaGetLastError());
         return QB_OK;

@@ -4,13 +4,13 @@
 // in qb_hnsw_build.cu's header.
 #pragma once
 #include <cub/device/device_radix_sort.cuh>
-#include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <functional>
+#include <memory>
 #include <vector>
 
-#include "qb_hnsw_traverse.cuh"
+#include "qb_hnsw_host.cuh"
 
 namespace {
 
@@ -51,22 +51,6 @@ __global__ void hnsw_build_neighbors_kernel(const HbTables tb, const uint64_t* _
         const uint64_t b = offsets[r], e = offsets[r + 1];
         for (uint64_t k = 0; k < e - b; ++k) neighbors[b + k] = row[k];
     }
-}
-
-// device temporaries of one call, freed on every exit path
-struct HbScratch {
-    std::vector<void*> bufs;
-    cudaError_t alloc(void** p, size_t bytes) {
-        *p = nullptr;
-        const cudaError_t e = cudaMalloc(p, std::max<size_t>(bytes, 256));
-        if (e == cudaSuccess) bufs.push_back(*p);
-        return e;
-    }
-    ~HbScratch() { cudaDeviceSynchronize(); for (void* b : bufs) cudaFree(b); }
-};
-
-inline unsigned hb_grid(uint64_t items, uint64_t per_block, uint64_t max_blocks) {
-    return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(ceil_div_u64(items, per_block), max_blocks));
 }
 
 // the host-side schedule
@@ -171,7 +155,7 @@ template <class K>
 qb_status hb_run(qb_storage* s, typename K::Params p, const HbPlan& plan, uint32_t n, uint32_t m, uint32_t m0, size_t smem, const char* who, qb_hnsw** out,
                  const HbPrefill& prefill = nullptr) {
     const uint32_t L = plan.levels, nr = (uint32_t)plan.rest.size();
-    HbScratch tmp;
+    HnswScratch tmp;
     std::vector<uint32_t*> tables(L, nullptr);
     for (uint32_t l = 0; l < L; ++l) {
         const size_t bytes = (size_t)plan.rows_on[l] * (l ? m : m0) * 4;
@@ -236,39 +220,22 @@ qb_status hb_run(qb_storage* s, typename K::Params p, const HbPlan& plan, uint32
     const uint64_t rows = lo[L], n_off = rows + 1;
     uint64_t* d_counts = nullptr;
     QB_CUDA(tmp.alloc((void**)&d_counts, 8 * n_off));
-    hnsw_build_counts_kernel<<<hb_grid(n_off, 256, 132 * 16), 256>>>(tb, d_counts);
+    hnsw_build_counts_kernel<<<hnsw_grid(n_off, 256, 132 * 16), 256>>>(tb, d_counts);
     QB_LAUNCHED();
-    qb_hnsw* g = new qb_hnsw();
-    g->st = s; g->n_points = n; g->m = m; g->m0 = m0; g->levels = L;
-    g->level_offsets_ext = lo; g->n_offsets = n_off;
-    auto fail = [&](qb_status st, const char* what, cudaError_t e) {
-        qb_set_error("%s: %s: %s", who, what, cudaGetErrorString(e));
-        qb_hnsw_destroy(g);
-        return st;
-    };
-    bool ok = cudaMalloc(&g->d_level_offsets, std::max<size_t>(8 * L, 256)) == cudaSuccess && cudaMalloc(&g->d_reindex, std::max<size_t>(4ull * n, 256)) == cudaSuccess &&
-              cudaMalloc(&g->d_offsets, 8 * n_off + 256) == cudaSuccess;
-    if (!ok) return fail(QB_ERR_OOM, "cudaMalloc failed", cudaGetLastError());
-    size_t scan_bytes = 0;
-    cudaError_t ce = cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, d_counts, g->d_offsets, (int64_t)n_off);
-    void* d_scan = nullptr;
-    if (ce == cudaSuccess) ce = tmp.alloc(&d_scan, scan_bytes);
-    if (ce == cudaSuccess) ce = cub::DeviceScan::ExclusiveSum(d_scan, scan_bytes, d_counts, g->d_offsets, (int64_t)n_off);
-    QB_LAUNCHED();
-    uint64_t total = 0;
-    if (ce == cudaSuccess) ce = cudaMemcpy(&total, g->d_offsets + rows, 8, cudaMemcpyDeviceToHost);
-    if (ce == cudaSuccess) ce = cudaMemcpy(g->d_level_offsets, lo.data(), 8 * L, cudaMemcpyHostToDevice);
+    qb_hnsw* g = nullptr;
+    QB_TRY(qb_hnsw_new(s, n, m, m0, std::move(lo), n_off, 0, who, &g));
+    std::unique_ptr<qb_hnsw, decltype(&qb_hnsw_destroy)> guard(g, qb_hnsw_destroy);
+    cudaError_t ce = cudaMemcpy(g->d_level_offsets, g->level_offsets_ext.data(), 8 * L, cudaMemcpyHostToDevice);
     if (ce == cudaSuccess) ce = cudaMemcpy(g->d_reindex, d_remap, 4ull * n, cudaMemcpyDeviceToDevice);
-    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "build", ce);
-    g->n_neighbors = total;
-    if (cudaMalloc(&g->d_neighbors, std::max<size_t>(4 * total, 256)) != cudaSuccess) return fail(QB_ERR_OOM, "cudaMalloc failed", cudaGetLastError());
-    hnsw_build_neighbors_kernel<<<hb_grid(rows, 256, 132 * 16), 256>>>(tb, g->d_offsets, g->d_neighbors);
-    QB_LAUNCHED();
+    if (ce != cudaSuccess) { qb_set_error("%s: build: %s", who, cudaGetErrorString(ce)); return QB_ERR_CUDA; }
+    QB_TRY(hnsw_link_offsets(g, d_counts, n_off, tmp, who, "build", nullptr, nullptr, [&](const uint64_t* d_offsets, uint32_t* d_neighbors) {
+        hnsw_build_neighbors_kernel<<<hnsw_grid(rows, 256, 132 * 16), 256>>>(tb, d_offsets, d_neighbors);
+        QB_LAUNCHED();
+    }));
     ce = cudaGetLastError();
-    if (ce != cudaSuccess) return fail(QB_ERR_CUDA, "build", ce);
-    const qb_status st = qb_hnsw_finish_plain(g, who);
-    if (st != QB_OK) { qb_hnsw_destroy(g); return st; }
-    *out = g;
+    if (ce != cudaSuccess) { qb_set_error("%s: build: %s", who, cudaGetErrorString(ce)); return QB_ERR_CUDA; }
+    QB_TRY(qb_hnsw_finish_plain(g, who));
+    *out = guard.release();
     return QB_OK;
 }
 

@@ -89,7 +89,7 @@ struct HbMvKernels {
         return QB_OK;
     }
     static qb_status backlinks(const HnswMvBuildParams& p, const unsigned long long* keys, const uint32_t* vals, uint32_t n) {
-        hnsw_backlink_mv_kernel<KIND, METRIC><<<hb_grid(n, 1, 132 * 16), HB_THREADS, p.q_smem>>>(p, keys, vals, n);
+        hnsw_backlink_mv_kernel<KIND, METRIC><<<hnsw_grid(n, 1, 132 * 16), HB_THREADS, p.q_smem>>>(p, keys, vals, n);
         QB_LAUNCHED();
         QB_CUDA(cudaGetLastError());
         return QB_OK;
@@ -139,10 +139,8 @@ extern "C" qb_status qb_hnsw_build_multivector(qb_storage* tokens, const uint32_
     QB_CHECK(smem <= 200 * 1024, QB_ERR_UNSUPPORTED, "%s: a query (%u B) + ef %u need %zu B of shared memory", who, p.q_smem, ef, smem);
     // the token offsets, kept by the handle (d_mv_tok) once the build succeeds
     uint32_t* d_tok = nullptr;
-    const size_t tok_bytes = 4ull * ((size_t)n_points + 1);
-    QB_CUDA(cudaMalloc(&d_tok, tok_bytes));
+    QB_TRY(qb_hnsw_mv_upload(point_offsets, n_points, who, &d_tok));
     std::unique_ptr<uint32_t, decltype(&cudaFree)> tok_guard(d_tok, cudaFree);
-    QB_CUDA(cudaMemcpy(d_tok, point_offsets, tok_bytes, cudaMemcpyHostToDevice));
     p.tok = d_tok;
 
     const int kind = tokens->dim >= 32 ? HK_DENSE_AVX : HK_DENSE_SMALL;
@@ -152,8 +150,7 @@ extern "C" qb_status qb_hnsw_build_multivector(qb_storage* tokens, const uint32_
     if (kind == HK_DENSE_AVX) QB_TRY(metric == M_EUCLID ? QB_HB_RUN(HK_DENSE_AVX, M_EUCLID) : metric == M_MANHATTAN ? QB_HB_RUN(HK_DENSE_AVX, M_MANHATTAN) : QB_HB_RUN(HK_DENSE_AVX, M_DOT));
     else QB_TRY(metric == M_EUCLID ? QB_HB_RUN(HK_DENSE_SMALL, M_EUCLID) : metric == M_MANHATTAN ? QB_HB_RUN(HK_DENSE_SMALL, M_MANHATTAN) : QB_HB_RUN(HK_DENSE_SMALL, M_DOT));
 #undef QB_HB_RUN
-    g->d_mv_tok = tok_guard.release();
-    g->hbm_bytes += tok_bytes;
+    qb_hnsw_mv_attach(g, tok_guard.release(), n_points);
     *out = g;
     if (entry_point) *entry_point = plan.entry;
     if (entry_level) *entry_level = plan.entry_level;

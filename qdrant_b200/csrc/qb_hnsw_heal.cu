@@ -330,7 +330,7 @@ struct HealKernels {
         return QB_OK;
     }
     static qb_status backlinks(const HnswParams& p, const unsigned long long* keys, const uint32_t* vals, uint32_t n) {
-        hnsw_heal_backlink_kernel<KIND, METRIC><<<hb_grid(n, HB_WARPS, 132 * 16), HB_WARPS * 32>>>(p, keys, vals, n);
+        hnsw_heal_backlink_kernel<KIND, METRIC><<<hnsw_grid(n, HB_WARPS, 132 * 16), HB_WARPS * 32>>>(p, keys, vals, n);
         QB_LAUNCHED();
         QB_CUDA(cudaGetLastError());
         return QB_OK;
@@ -348,7 +348,7 @@ struct HealJob {
 };
 
 template <int KIND, int METRIC>
-qb_status heal_levels(HbScratch& tmp, const HealJob& job, const std::vector<uint32_t*>& tabs, const std::vector<uint32_t*>& old_tabs, unsigned sm_count,
+qb_status heal_levels(HnswScratch& tmp, const HealJob& job, const std::vector<uint32_t*>& tabs, const std::vector<uint32_t*>& old_tabs, unsigned sm_count,
                       const char* who) {
     using K = HealKernels<KIND, METRIC>;
     const qb_hnsw* g = job.old;
@@ -498,7 +498,7 @@ extern "C" qb_status qb_hnsw_build_incremental(qb_storage* s, const qb_hnsw* old
     }
 
     // the old graph's level tables, as loaded and to be healed; the to-heal items
-    HbScratch tmp;
+    HnswScratch tmp;
     uint32_t* d_o2n = nullptr;
     QB_CUDA(tmp.alloc((void**)&d_o2n, 4ull * n_old));
     QB_CUDA(cudaMemcpy(d_o2n, old_to_new, 4ull * n_old, cudaMemcpyHostToDevice));
@@ -512,10 +512,10 @@ extern "C" qb_status qb_hnsw_build_incremental(qb_storage* s, const qb_hnsw* old
         const size_t bytes = (size_t)rows_old[l] * lm * 4;
         QB_CUDA(tmp.alloc((void**)&old_tabs[l], bytes));
         QB_CUDA(tmp.alloc((void**)&tabs[l], bytes));
-        hnsw_heal_table_kernel<<<hb_grid(rows_old[l], 256, 132 * 16), 256>>>(old->d_offsets, old->d_neighbors, old->level_offsets_ext[l], rows_old[l], lm, old_tabs[l]);
+        hnsw_heal_table_kernel<<<hnsw_grid(rows_old[l], 256, 132 * 16), 256>>>(old->d_offsets, old->d_neighbors, old->level_offsets_ext[l], rows_old[l], lm, old_tabs[l]);
         QB_LAUNCHED();
         QB_CUDA(cudaMemcpyAsync(tabs[l], old_tabs[l], bytes, cudaMemcpyDeviceToDevice));
-        hnsw_heal_flags_kernel<<<hb_grid(rows_old[l], 256, 132 * 16), 256>>>(old_tabs[l], rows_old[l], lm, d_o2n, d_flags, 1u << l);
+        hnsw_heal_flags_kernel<<<hnsw_grid(rows_old[l], 256, 132 * 16), 256>>>(old_tabs[l], rows_old[l], lm, d_o2n, d_flags, 1u << l);
         QB_LAUNCHED();
         QB_CUDA(cudaGetLastError());
     }
@@ -541,7 +541,7 @@ extern "C" qb_status qb_hnsw_build_incremental(qb_storage* s, const qb_hnsw* old
     QB_CUDA(cudaMemcpy(d_old_level, job.old_level.data(), n_old, cudaMemcpyHostToDevice));
     auto prefill = [&](uint32_t* const* tables, const uint32_t* d_remap) -> qb_status {
         for (uint32_t l = 0; l < std::min(L_old, top_new + 1); ++l) {   // the mapped points keep their levels: none is above top_new
-            hnsw_heal_renumber_kernel<<<hb_grid(n_old, 256, 132 * 16), 256>>>(tabs[l], old->d_reindex, d_old_level, d_o2n, n_old, l, l ? m : m0, d_remap, tables[l]);
+            hnsw_heal_renumber_kernel<<<hnsw_grid(n_old, 256, 132 * 16), 256>>>(tabs[l], old->d_reindex, d_old_level, d_o2n, n_old, l, l ? m : m0, d_remap, tables[l]);
             QB_LAUNCHED();
         }
         QB_CUDA(cudaGetLastError());

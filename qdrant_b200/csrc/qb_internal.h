@@ -182,11 +182,20 @@ struct QbHnswCustom {
 qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, uint32_t nq, uint32_t top, uint32_t ef, uint32_t entry, uint32_t entry_level,
                          const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts, cudaStream_t stream, int algo /* qb_hnsw_algorithm */,
                          const QbHnswCustom* custom = nullptr, const QbHnswMaxsim* maxsim = nullptr);
-// completes a handle whose plain arrays (d_level_offsets, d_reindex, d_neighbors, d_offsets and the host-side counts) are on the device:
-// the level-0 table and the search scratch (qb_hnsw.cu).  On failure the caller destroys g.  who = the error messages' prefix.
+// A handle over n points bound to s, with the plain arrays every loader and build fills allocated (qb_hnsw.cu): d_level_offsets (lo: their
+// host copy with the extra last element, so lo.size() - 1 levels), d_reindex, and d_offsets with n_off entries plus `tail` more (the
+// compressed formats pad the table, hnsw_c_pad_kernel).  hbm_bytes counts these.  who = the error messages' prefix.
+qb_status qb_hnsw_new(qb_storage* s, uint32_t n, uint32_t m, uint32_t m0, std::vector<uint64_t> lo, uint64_t n_off, uint64_t tail, const char* who,
+                      qb_hnsw** out);
+// completes a handle from qb_hnsw_new whose plain arrays are filled (d_neighbors and n_neighbors included): the level-0 table and the search
+// counters, added to hbm_bytes (qb_hnsw.cu).  On failure the caller destroys g.  who = the error messages' prefix.
 qb_status qb_hnsw_finish_plain(qb_hnsw* g, const char* who);
 // the checks qb_search_maxsim makes on a multivector collection's token storage and point offsets (qb_hnsw.cu)
 qb_status qb_hnsw_mv_check(qb_storage* s, const uint32_t* point_offsets, uint32_t n_points, const char* who);
+// a multivector collection's point offsets [n_points + 1] uploaded to *d_tok, which the caller frees or hands to qb_hnsw_mv_attach (qb_hnsw.cu)
+qb_status qb_hnsw_mv_upload(const uint32_t* point_offsets, uint32_t n_points, const char* who, uint32_t** d_tok);
+// makes g a graph over those points: g takes d_tok over as d_mv_tok and counts it in hbm_bytes
+void qb_hnsw_mv_attach(qb_hnsw* g, uint32_t* d_tok, uint32_t n_points);
 // the inline-vector search (qb_hnsw_inline.cu): queries preprocessed (d_q_pre, pre_stride floats apart) and SQ8-encoded; enqueued on stream
 qb_status qb_hnsw_inline_launch(qb_hnsw* g, const float* d_q_pre, uint32_t pre_stride, const void* d_q_enc, const float* d_q_off, uint32_t nq, uint32_t top,
                                 uint32_t ef, uint32_t entry, uint32_t entry_level, const uint32_t* d_deleted2, qb_scored_point* d_out, uint32_t* d_counts,

@@ -239,16 +239,38 @@ def test_malformed_files_are_refused_and_the_device_stays_usable(qb, oracle):
         "level 0 not the first n entries": _rebuild(comp, lo=[1] + list(r.level_offsets[1:-1])),
         "reindex out of range": _rebuild(comp, reindex=np.r_[np.uint32(n + 5), r.reindex[1:]]),
     }
+    # the full message of each refusal
+    message = {
+        "truncated header": "hnsw_create_compressed: 40 bytes is smaller than HeaderCompressed",
+        "truncated body": "hnsw_create_compressed: 100 bytes, header describes 13537 before the offsets",
+        "truncated tail": "hnsw_create_compressed: 617 offsets do not fit the 708 bytes after the links",
+        "plain file": "hnsw_create_compressed: version word 0000000000000004 is not HEADER_VERSION_COMPRESSED (a plain links.bin?)",
+        "wrong point count": "hnsw_create_compressed: graph has 499 points, storage 500",
+        "delta_bits 0": "hnsw_create_compressed: offsets parameters base_bits 14 delta_bits 0 chunk_len_log2 3",
+        "delta_bits 57": "hnsw_create_compressed: offsets parameters base_bits 14 delta_bits 57 chunk_len_log2 3",
+        "chunk_len_log2 8": "hnsw_create_compressed: offsets parameters base_bits 14 delta_bits 8 chunk_len_log2 8",
+        "base_bits 0": "hnsw_create_compressed: offsets parameters base_bits 0 delta_bits 8 chunk_len_log2 3",
+        "m 0": "hnsw_create_compressed: m 0 / m0 32",
+        "offsets decrease": "hnsw_create_compressed: links offsets decrease",
+        "offset past total_neighbors_bytes": "hnsw_create_compressed: a links offset lies past total_neighbors_bytes",
+        "level offset >= length": "hnsw_create_compressed: level offset 3 (620) out of range",
+        "level 0 not the first n entries": "hnsw_create_compressed: level offset 0 (1) out of range",
+        "reindex out of range": "hnsw_create_compressed: a reindex entry is >= point_count",
+        "CompressedWithVectors": "hnsw_create_compressed: CompressedWithVectors (inline storage) graphs are searched from the quantized vectors stored with the links (graph_layers.rs:336-388), a different algorithm; this loader takes GraphLinksFormat::Compressed",
+        "m0 65": "hnsw_create_compressed: m 16 / m0 65 outside [1,64]",
+    }
     for what, blob in bad.items():
         with pytest.raises(qb.QbError) as ei:
             qb.HnswGraph.from_compressed(st, blob)
         assert ei.value.status == -1, (what, str(ei.value))
+        assert str(ei.value) == f"qb_status -1: {message[what]}", what
     with_vectors = patched(8, gl.VERSION_COMPRESSED_WITH_VECTORS.to_bytes(8, "little"))
     for what, blob in {"CompressedWithVectors": with_vectors, "m0 65": patched(51, (65).to_bytes(8, "little"))}.items():
         with pytest.raises(qb.QbError) as ei:
             qb.HnswGraph.from_compressed(st, blob)
         assert ei.value.status == -3, (what, str(ei.value))
         assert what != "CompressedWithVectors" or "CompressedWithVectors" in str(ei.value)
+        assert str(ei.value) == f"qb_status -3: {message[what]}", what
     torch.cuda.synchronize()
     # the rebuilt file itself is valid: only the planted values were wrong
     hc = qb.HnswGraph.from_compressed(st, _rebuild(comp))

@@ -200,10 +200,34 @@ def test_malformed_and_unsupported(qb, oracle):
         "offset past the end": _rebuild(blob, boff=boff[:-1] + [boff[-1] + 9]),
         "reindex out of range": _rebuild(blob, reindex=np.r_[np.uint32(n + 5), r.reindex[1:]]),
     }
+    # the full message of each refusal
+    message = {
+        "truncated header": "hnsw_create_with_vectors: 60 bytes is smaller than HeaderCompressedWithVectors",
+        "truncated body": "hnsw_create_with_vectors: 200 bytes, header describes 260096 before the offsets",
+        "truncated tail": "hnsw_create_with_vectors: 550 offsets do not fit the 972 bytes after the records",
+        "plain file": "hnsw_create_with_vectors: version word 0000000000000005 is not HEADER_VERSION_COMPRESSED_WITH_VECTORS (a Compressed or plain links.bin?)",
+        "compressed file": "hnsw_create_with_vectors: version word ffffffffffffff01 is not HEADER_VERSION_COMPRESSED_WITH_VECTORS (a Compressed or plain links.bin?)",
+        "wrong point count": "hnsw_create_with_vectors: graph has 399 points, storage 400",
+        "delta_bits 0": "hnsw_create_with_vectors: offsets parameters base_bits 18 delta_bits 0 chunk_len_log2 2",
+        'link size': "hnsw_create_with_vectors: link vectors of 37 bytes, the storage's rows have 36",
+        "base size": "hnsw_create_with_vectors: base vectors of 100 bytes, dim 24",
+        "alignment 3": "hnsw_create_with_vectors: vector alignments 4 / 3 are not powers of two",
+        'varint past the record': "hnsw_create_with_vectors: a record's count, links or link vectors run past its end",
+        'link vectors past the record': "hnsw_create_with_vectors: a record's count, links or link vectors run past its end",
+        'base vector past the record': "hnsw_create_with_vectors: a record's count, links or link vectors run past its end",
+        'packed links past the record': "hnsw_create_with_vectors: a record's count, links or link vectors run past its end",
+        "offsets decrease": "hnsw_create_with_vectors: record offsets decrease",
+        "offset past the end": "hnsw_create_with_vectors: a record offset lies past total_neighbors_bytes",
+        "reindex out of range": "hnsw_create_with_vectors: a reindex entry is >= point_count",
+        "f16 base": "hnsw_create_with_vectors: base vectors of 48 bytes at dim 24 are f16 or u8; only f32 base vectors are supported",
+        "u8 base": "hnsw_create_with_vectors: base vectors of 24 bytes at dim 24 are f16 or u8; only f32 base vectors are supported",
+        "list of 129 links": "hnsw_create_with_vectors: a list has more than 128 links",
+    }
     for what, b in bad.items():
         with pytest.raises(qb.QbError) as ei:
             qb.HnswGraph.from_compressed_with_vectors(st, b)
         assert ei.value.status == -1, (what, str(ei.value))
+        assert str(ei.value) == f"qb_status -1: {message[what]}", what
     wide = [[list(lv[0]) + [x for x in range(n) if x not in lv[0]][:129 - len(lv[0])]] + lv[1:] if p == 5 else lv for p, lv in enumerate(edges)]
     unsupported = {
         "f16 base": patched(59, (dim * 2).to_bytes(8, "little")),
@@ -214,6 +238,7 @@ def test_malformed_and_unsupported(qb, oracle):
         with pytest.raises(qb.QbError) as ei:
             qb.HnswGraph.from_compressed_with_vectors(st, b)
         assert ei.value.status == -3, (what, str(ei.value))
+        assert str(ei.value) == f"qb_status -3: {message[what]}", what
     dense = qb.DenseVectorStorage(base, qb.Distance.Dot)
     pq = oracle.PQ.encode(base, 4, rng.standard_normal((256, dim)).astype(np.float32), oracle.QD_DOT, False)
     pqs = qb.ProductQuantizedVectors(pq.codes, rng.standard_normal((256, dim)).astype(np.float32), 4, dim, qb.Distance.Dot)
@@ -223,6 +248,7 @@ def test_malformed_and_unsupported(qb, oracle):
         with pytest.raises(qb.QbError) as ei:
             qb.HnswGraph.from_compressed_with_vectors(other, blob)
         assert ei.value.status == -3
+        assert str(ei.value) == 'qb_status -3: hnsw_create_with_vectors: the link vectors are read as rows of the bound storage, which must be scalar-quantized (SQ8)'
     pqs.close(); bqs.close()
     hc = qb.HnswGraph.from_compressed(st, gl.serialize_compressed(edges, m, m0))
     with pytest.raises(qb.QbError) as ei:
