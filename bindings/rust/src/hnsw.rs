@@ -60,7 +60,7 @@ impl<'a> B200Hnsw<'a> {
     }
 
     /// Builds the graph on the device, in place of `build_hnsw_on_gpu` (gpu/gpu_graph_builder.rs) and of the CPU
-    /// `GraphLayersBuilder::link_new_point` pool (hnsw/build.rs:285-355) for a dense f32 storage.  The adapter keeps on the host:
+    /// `GraphLayersBuilder::link_new_point` pool (hnsw/build.rs:285-355) for a dense f32 or Uint8 storage.  The adapter keeps on the host:
     /// the level draw (`GraphLayersBuilder::get_random_layer`, one u8 per point), the mapping between point offsets and the
     /// storage's rows, the deleted flags (set on the storage beforehand), and writing `links.bin` in the compressed format from
     /// `export_plain` (GraphLinksSerializer).  Returns the graph and its entry point (id, level).

@@ -352,8 +352,9 @@ QB_API qb_status qb_comm_check(qb_comm* c);
  *
  * links_bin = the bytes of the segment's `links.bin` in GraphLinksFormat::Plain (graph_links/header.rs:9-20,
  * graph_links/view.rs:121-135): HeaderPlain, level offsets, reindex, neighbors, padding, offsets.  m / m0 = HnswM
- * (hnsw_index/mod.rs:34-40), both <= 64.  The graph is bound to `s` (dense f32 or SQ8; the quantized storage when the
- * segment searches quantized) and must outlive neither it nor its searches. */
+ * (hnsw_index/mod.rs:34-40), both <= 64.  The graph is bound to `s` (dense f32, dense Uint8 or SQ8; the quantized storage when
+ * the segment searches quantized) and must outlive neither it nor its searches.  Float16 storages load but are not searched on the
+ * device (QB_ERR_UNSUPPORTED). */
 typedef struct qb_hnsw qb_hnsw;
 QB_API qb_status qb_hnsw_create_plain(qb_storage* s, const uint8_t* links_bin, uint64_t n_bytes, uint32_t m, uint32_t m0, qb_hnsw** out);
 /* The same graph from `links.bin` in GraphLinksFormat::Compressed, the format the reference writes for every HNSW index it
@@ -385,7 +386,7 @@ QB_API qb_status qb_hnsw_links(const qb_hnsw* g, uint32_t level, const uint32_t*
                                uint32_t* counts);
 QB_API void qb_hnsw_destroy(qb_hnsw* g);
 QB_API qb_status qb_hnsw_info(const qb_hnsw* g, uint32_t* n_points, uint32_t* levels, uint64_t* hbm_bytes);
-/* Builds the HNSW graph of a dense f32 storage on the device, with the schedule of the reference's GPU builder
+/* Builds the HNSW graph of a dense f32 or Uint8 storage on the device, with the schedule of the reference's GPU builder
  * (gpu/gpu_graph_builder.rs:19-101, gpu_level_builder.rs:12-96, batched_points.rs:36-163) and the CPU builder's per-point
  * arithmetic (search_on_level with ef = max(ef_construct, m0), fill_from_sorted_with_heuristic, connect_with_heuristic):
  *   - points sorted by level descending, then id; the first is the entry point (returned in entry_point / entry_level);
@@ -397,8 +398,12 @@ QB_API qb_status qb_hnsw_info(const qb_hnsw* g, uint32_t* n_points, uint32_t* le
  *   levels    one per point, <= 30: the reference draws them from an unseeded RNG (get_random_layer), the caller draws them here
  * Points with the storage's resident deleted flag (qb_storage_set_deleted) are not inserted (iter_internal_excluding(deleted)): they keep
  * their level and have no links.  m, m0 <= 64 and ef <= 4096 (else QB_ERR_UNSUPPORTED); a level > 30, an empty storage or no point left
- * to insert: QB_ERR_INVALID.  Other storages: QB_ERR_UNSUPPORTED (build over the original vectors, then bind the exported graph to the
- * quantized storage).  The result is the handle qb_hnsw_create_plain would make from the graph's plain links.bin.  Synchronous. */
+ * to insert: QB_ERR_INVALID.  Other storages (Float16 included): QB_ERR_UNSUPPORTED (build over the original vectors, then bind the
+ * exported graph to the quantized storage).  The result is the handle qb_hnsw_create_plain would make from the graph's plain links.bin.
+ * Uint8: an insert's query is the point's stored row, and every score is Metric<u8>::similarity of two stored rows (score_internal),
+ * as both reference builders score u8 (FilteredScorer::new_internal, run_insert_vector.comp:41).  Its Dot / Euclid / Manhattan scores
+ * are integers, so ties are common: the graph equals the reference's build with every level-0 comparison of the inserts' searches on
+ * (score desc, id asc) keys; the greedy descent through the upper levels moves only to a strictly greater score.  Synchronous. */
 QB_API qb_status qb_hnsw_build(qb_storage* s, uint32_t m, uint32_t m0, uint32_t ef_construct, const uint8_t* levels /* n */, uint32_t batch,
                                uint32_t serial_points, qb_hnsw** out, uint32_t* entry_point, uint32_t* entry_level);
 /* Builds a segment's graph incrementally on the device: the old segment's graph is healed where its points have gone, renumbered into
@@ -423,12 +428,14 @@ QB_API qb_status qb_hnsw_build(qb_storage* s, uint32_t m, uint32_t m0, uint32_t 
  *   levels      one per point of s, <= 30; a mapped point's must equal its old level (build.rs:235-239)
  * m / m0 are old's (the reference reuses no graph of another configuration, old_index.rs:67-71); batch / serial_points as for
  * qb_hnsw_build (0 = 512 / 256).  The decision to reuse a graph (OldIndexCandidate::evaluate, healing_threshold) stays with the
- * caller.  Errors, checked before any device work: s or old's storage not dense f32, another dim / distance / device, a multivector
+ * caller.  Errors, checked before any device work: s not dense f32 or Uint8, old's storage not of s's datatype (f32 and Uint8 do not
+ * mix), another dim / distance / device, a multivector
  * or inline-vector (CompressedWithVectors, old_index.rs:72-76) handle, ef > 4096: QB_ERR_UNSUPPORTED; a null argument, ef_construct
  * = 0, a target >= s's count, two old points on one target, a target with the resident deleted flag, no mapped point (build from
- * scratch with qb_hnsw_build), a level > 30 or a mapped level that differs: QB_ERR_INVALID.  Healing and inserting read the f32
- * rows (quantized vectors are out of scope, as for qb_hnsw_build).  The result is the handle qb_hnsw_create_plain would make from
- * the new graph's plain links.bin, bound to s.  Synchronous. */
+ * scratch with qb_hnsw_build), a level > 30 or a mapped level that differs: QB_ERR_INVALID.  Healing and inserting read the stored
+ * f32 or Uint8 rows (quantized vectors are out of scope, as for qb_hnsw_build).  Uint8: the keyed tie contract of qb_hnsw_build, in
+ * the inserts and in the heal's `nearest` (the heal's stack test stays score-only, as in the reference).  The result is the handle
+ * qb_hnsw_create_plain would make from the new graph's plain links.bin, bound to s.  Synchronous. */
 QB_API qb_status qb_hnsw_build_incremental(qb_storage* s, const qb_hnsw* old, const uint32_t* old_to_new /* old n_points */, uint32_t ef_construct,
                                            const uint8_t* levels /* s->count */, uint32_t batch, uint32_t serial_points, qb_hnsw** out,
                                            uint32_t* entry_point, uint32_t* entry_level);
@@ -442,7 +449,11 @@ QB_API qb_status qb_hnsw_export_plain(const qb_hnsw* g, uint8_t* out, uint64_t c
  *   deleted_bitmap  optional filter (bit = 1: point fails ScorerFilters::check_vector), OR-ed with the resident flags;
  *                   filtered-out links are neither scored nor traversed (point_scorer.rs:270-277)
  *   out             n_queries x top, descending; out_counts[q] valid entries
- * Result lists equal the reference traversal's whenever scores are distinct (ties are ordered by id). */
+ * Result lists equal the reference traversal's whenever scores are distinct (ties are ordered by id).  Storages: dense f32, dense
+ * Uint8 (queries `x as u8` after Metric<u8>::preprocess, the identity even for Cosine; counters cpu += dim per scored point,
+ * vector_io_read += dim on disk) and SQ8; Float16: QB_ERR_UNSUPPORTED (qb_score_points per hop).  Uint8 Dot / Euclid / Manhattan
+ * scores are integers, so ties are common there: lists equal the reference traversal with every level-0 comparison on (score desc,
+ * id asc) keys; the greedy upper-level descent moves only to a strictly greater score. */
 QB_API qb_status qb_hnsw_search_batch(qb_hnsw* g, const float* queries, uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point,
                                       uint32_t entry_level, const uint64_t* deleted_bitmap, const volatile int32_t* is_stopped,
                                       qb_scored_point* out, uint32_t* out_counts, qb_hw_counters* counters /* optional */);
@@ -571,7 +582,7 @@ QB_API qb_status qb_hnsw_search_maxsim_batch_device(qb_hnsw* g, const float* dev
  *                   the filter, the one with the highest point level, the LAST of several equal maxima (Iterator::max_by_key); if
  *                   none passes, entry_point / entry_level
  *   counters        cpu += scored points x E x cpu units, vector_io_read += scored points x io units (custom_query_scorer.rs:78-111)
- * The rest is as for qb_hnsw_search_batch_algo.  Dense f32 and SQ8 storages only (QB_ERR_UNSUPPORTED otherwise).
+ * The rest is as for qb_hnsw_search_batch_algo.  Dense f32, dense Uint8 and SQ8 storages only (QB_ERR_UNSUPPORTED otherwise).
  *
  * Ties.  Context scores are sums of fast_sigmoid(min(d, 0)): every point that satisfies all pairs scores exactly 0.0, so custom
  * scores tie often.  The device orders equal scores by id (score desc, id asc) in every comparison of the level-0 search:

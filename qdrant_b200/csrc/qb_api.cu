@@ -1862,8 +1862,8 @@ static qb_status hnsw_custom_run(qb_hnsw* g, qb_query_kind kind, const float* ve
     QB_CHECK(fb == (coef != nullptr), QB_ERR_INVALID, "%s: coef is required for feedback queries and must be NULL otherwise", what);
     QB_CHECK(!cep || (cep_counts && n_custom >= 1), QB_ERR_INVALID, "%s: custom_entry_points need custom_counts and n_custom >= 1", what);
     qb_storage* s = g->st;
-    QB_CHECK((s->kind == QB_KIND_DENSE && s->dtype == QB_DT_F32) || s->kind == QB_KIND_SQ8, QB_ERR_UNSUPPORTED,
-             "%s: device traversal supports dense f32 and SQ8 storages (others go through qb_score_points per hop)", what);
+    QB_CHECK((s->kind == QB_KIND_DENSE && (s->dtype == QB_DT_F32 || s->dtype == QB_DT_U8)) || s->kind == QB_KIND_SQ8, QB_ERR_UNSUPPORTED,
+             "%s: device traversal supports dense f32, Uint8 and SQ8 storages (others go through qb_score_points per hop)", what);
     if (cep) {
         for (uint32_t q = 0; q < n_queries; ++q) {
             QB_CHECK(cep_counts[q] <= n_custom, QB_ERR_INVALID, "%s: custom_counts[%u] = %u > n_custom %u", what, q, cep_counts[q], n_custom);

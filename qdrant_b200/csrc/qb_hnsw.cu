@@ -693,8 +693,13 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
     int kind;
     if (s->kind == QB_KIND_DENSE && s->dtype == QB_DT_F32) kind = s->dim >= 32 ? HK_DENSE_AVX : HK_DENSE_SMALL;
     else if (s->kind == QB_KIND_SQ8) kind = ((uint64_t)s->actual_dim * 127ull * 127ull >= (1ull << 24)) ? HK_SQ8_LANEX : HK_SQ8;
-    else { qb_set_error("hnsw_search: device traversal supports dense f32 and SQ8 storages (others go through qb_score_points per hop)"); return QB_ERR_UNSUPPORTED; }
-    const int metric = s->distance == QB_DIST_EUCLID ? M_EUCLID : (s->distance == QB_DIST_MANHATTAN ? M_MANHATTAN : M_DOT);
+    else if (s->kind == QB_KIND_DENSE && s->dtype == QB_DT_U8 && !maxsim) kind = s->dim >= 32 ? HK_U8 : HK_U8_SMALL;
+    else {
+        qb_set_error("hnsw_search: device traversal supports dense f32, Uint8 and SQ8 storages, MaxSim dense f32 and SQ8 tokens (others go through "
+                     "qb_score_points per hop)");
+        return QB_ERR_UNSUPPORTED;
+    }
+    const int metric = hnsw_metric(s);
     HnswParams p{};
     p.links0 = g->d_links0; p.level_offsets = g->d_level_offsets; p.reindex = g->d_reindex; p.neighbors = g->d_neighbors; p.offsets = g->d_offsets;
     p.n_points = g->n_points; p.m = g->m; p.m0 = g->m0; p.levels = g->levels;

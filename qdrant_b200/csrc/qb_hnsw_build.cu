@@ -1,4 +1,5 @@
-// qb_hnsw_build.cu — HNSW graph construction on the device for dense f32 storages (qb_hnsw_build), and the plain `links.bin` export.
+// qb_hnsw_build.cu — HNSW graph construction on the device for dense f32 and Uint8 storages (qb_hnsw_build), and the plain `links.bin` export.
+// A Uint8 storage's inserts and backlinks are the same kernels instantiated for the u8 kinds (HK_U8, HK_U8_SMALL; DESIGN §3.13d).
 //
 // Schedule: the reference's GPU builder (gpu/gpu_graph_builder.rs:19-101, gpu_level_builder.rs:12-96, batched_points.rs:36-163).
 // Points sorted by level descending, then id; the first is the entry point.  The rest are cut into batches of at most `batch` points,
@@ -109,14 +110,27 @@ struct HbKernels {
     }
 };
 
+// hb_run over a Uint8 storage, with its four metrics
+template <int KIND>
+qb_status hb_run_u8(int metric, qb_storage* s, const HnswParams& p, const HbPlan& plan, uint32_t n, uint32_t m, uint32_t m0, size_t smem, const char* who,
+                    qb_hnsw** out, const HbPrefill& prefill) {
+    switch (metric) {
+        case M_EUCLID: return hb_run<HbKernels<KIND, M_EUCLID>>(s, p, plan, n, m, m0, smem, who, out, prefill);
+        case M_MANHATTAN: return hb_run<HbKernels<KIND, M_MANHATTAN>>(s, p, plan, n, m, m0, smem, who, out, prefill);
+        case M_COSINE: return hb_run<HbKernels<KIND, M_COSINE>>(s, p, plan, n, m, m0, smem, who, out, prefill);
+        default: return hb_run<HbKernels<KIND, M_DOT>>(s, p, plan, n, m, m0, smem, who, out, prefill);
+    }
+}
+
 }  // namespace
 
 extern "C" qb_status qb_hnsw_build(qb_storage* s, uint32_t m, uint32_t m0, uint32_t ef_construct, const uint8_t* levels, uint32_t batch, uint32_t serial_points,
                                    qb_hnsw** out, uint32_t* entry_point, uint32_t* entry_level) {
     QB_CHECK(s && levels && out, QB_ERR_INVALID, "hnsw_build: null argument");
     *out = nullptr;
-    QB_CHECK(s->kind == QB_KIND_DENSE && s->dtype == QB_DT_F32, QB_ERR_UNSUPPORTED,
-             "hnsw_build: graphs are built over dense f32 storages only (build over the original vectors, then bind the graph to the quantized storage)");
+    QB_CHECK(s->kind == QB_KIND_DENSE && (s->dtype == QB_DT_F32 || s->dtype == QB_DT_U8), QB_ERR_UNSUPPORTED,
+             "hnsw_build: graphs are built over dense f32 and Uint8 storages only (build over the original vectors, then bind the graph to the quantized "
+             "storage)");
     QB_CHECK(s->count >= 1, QB_ERR_INVALID, "hnsw_build: empty storage");
     QB_CHECK(s->count < 0xFFFFFFFFull, QB_ERR_UNSUPPORTED, "hnsw_build: %llu points", (unsigned long long)s->count);
     QB_CHECK(m >= 1 && m0 >= 1, QB_ERR_INVALID, "hnsw_build: m %u / m0 %u", m, m0);
@@ -141,8 +155,9 @@ qb_status qb_hnsw_build_dense(qb_storage* s, uint32_t m, uint32_t m0, uint32_t e
     HbPlan plan;
     QB_TRY(hb_plan(levels, n, deleted.empty() ? nullptr : deleted.data(), batch, serial_points, who, &plan, given, entry));
 
-    const int kind = s->dim >= 32 ? HK_DENSE_AVX : HK_DENSE_SMALL;
-    const int metric = hb_metric(s);
+    const bool u8 = s->dtype == QB_DT_U8;
+    const int kind = s->dim >= 32 ? (u8 ? HK_U8 : HK_DENSE_AVX) : (u8 ? HK_U8_SMALL : HK_DENSE_SMALL);
+    const int metric = hnsw_metric(s);
     HnswParams p{};
     p.rows = reinterpret_cast<const uint8_t*>(s->d_rows); p.stride = s->row_stride; p.dim = s->dim;
     p.q_bytes = s->row_stride; p.ef = ef;
@@ -150,7 +165,9 @@ qb_status qb_hnsw_build_dense(qb_storage* s, uint32_t m, uint32_t m0, uint32_t e
     QB_CHECK(smem <= 200 * 1024, QB_ERR_UNSUPPORTED, "%s: a row (%u B) + ef %u need %zu B of shared memory", who, p.q_bytes, ef, smem);
 #define QB_HB_RUN(K, M) hb_run<HbKernels<K, M>>(s, p, plan, n, m, m0, smem, who, out, prefill)
     if (kind == HK_DENSE_AVX) QB_TRY(metric == M_EUCLID ? QB_HB_RUN(HK_DENSE_AVX, M_EUCLID) : metric == M_MANHATTAN ? QB_HB_RUN(HK_DENSE_AVX, M_MANHATTAN) : QB_HB_RUN(HK_DENSE_AVX, M_DOT));
-    else QB_TRY(metric == M_EUCLID ? QB_HB_RUN(HK_DENSE_SMALL, M_EUCLID) : metric == M_MANHATTAN ? QB_HB_RUN(HK_DENSE_SMALL, M_MANHATTAN) : QB_HB_RUN(HK_DENSE_SMALL, M_DOT));
+    else if (kind == HK_DENSE_SMALL) QB_TRY(metric == M_EUCLID ? QB_HB_RUN(HK_DENSE_SMALL, M_EUCLID) : metric == M_MANHATTAN ? QB_HB_RUN(HK_DENSE_SMALL, M_MANHATTAN) : QB_HB_RUN(HK_DENSE_SMALL, M_DOT));
+    else if (kind == HK_U8) QB_TRY(hb_run_u8<HK_U8>(metric, s, p, plan, n, m, m0, smem, who, out, prefill));
+    else QB_TRY(hb_run_u8<HK_U8_SMALL>(metric, s, p, plan, n, m, m0, smem, who, out, prefill));
 #undef QB_HB_RUN
     const uint32_t e = plan.lead ? plan.rest[0] : plan.entry;   // entry_points.rs new_point: a new point strictly above the top
     if (entry_point) *entry_point = e;

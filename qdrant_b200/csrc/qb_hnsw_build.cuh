@@ -239,11 +239,9 @@ qb_status hb_run(qb_storage* s, typename K::Params p, const HbPlan& plan, uint32
     return QB_OK;
 }
 
-int hb_metric(const qb_storage* s) { return s->distance == QB_DIST_EUCLID ? M_EUCLID : (s->distance == QB_DIST_MANHATTAN ? M_MANHATTAN : M_DOT); }
-
 }  // namespace
 
-// qb_hnsw_build's plan and inserts over a dense f32 storage (qb_hnsw_build.cu), with hb_plan's `given` points and entry and hb_run's
+// qb_hnsw_build's plan and inserts over a dense f32 or Uint8 storage (qb_hnsw_build.cu), with hb_plan's `given` points and entry and hb_run's
 // prefill: qb_hnsw_build passes none, qb_hnsw_build_incremental (qb_hnsw_heal.cu) the healed graph.  Checks nothing the callers check.
 qb_status qb_hnsw_build_dense(qb_storage* s, uint32_t m, uint32_t m0, uint32_t ef, const uint8_t* levels, const uint32_t* given, uint32_t entry, uint32_t batch,
                               uint32_t serial_points, const HbPrefill& prefill, const char* who, qb_hnsw** out, uint32_t* entry_point, uint32_t* entry_level);

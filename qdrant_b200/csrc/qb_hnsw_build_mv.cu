@@ -144,7 +144,7 @@ extern "C" qb_status qb_hnsw_build_multivector(qb_storage* tokens, const uint32_
     p.tok = d_tok;
 
     const int kind = tokens->dim >= 32 ? HK_DENSE_AVX : HK_DENSE_SMALL;
-    const int metric = hb_metric(tokens);
+    const int metric = hnsw_metric(tokens);
     qb_hnsw* g = nullptr;
 #define QB_HB_RUN(K, M) hb_run<HbMvKernels<K, M>>(tokens, p, plan, n_points, m, m0, smem, who, &g)
     if (kind == HK_DENSE_AVX) QB_TRY(metric == M_EUCLID ? QB_HB_RUN(HK_DENSE_AVX, M_EUCLID) : metric == M_MANHATTAN ? QB_HB_RUN(HK_DENSE_AVX, M_MANHATTAN) : QB_HB_RUN(HK_DENSE_AVX, M_DOT));

@@ -435,6 +435,18 @@ qb_status heal_levels(HnswScratch& tmp, const HealJob& job, const std::vector<ui
     return QB_OK;
 }
 
+// heal_levels over a Uint8 storage, with its four metrics
+template <int KIND>
+qb_status heal_levels_u8(int metric, HnswScratch& tmp, const HealJob& job, const std::vector<uint32_t*>& tabs, const std::vector<uint32_t*>& old_tabs,
+                         unsigned sm_count, const char* who) {
+    switch (metric) {
+        case M_EUCLID: return heal_levels<KIND, M_EUCLID>(tmp, job, tabs, old_tabs, sm_count, who);
+        case M_MANHATTAN: return heal_levels<KIND, M_MANHATTAN>(tmp, job, tabs, old_tabs, sm_count, who);
+        case M_COSINE: return heal_levels<KIND, M_COSINE>(tmp, job, tabs, old_tabs, sm_count, who);
+        default: return heal_levels<KIND, M_DOT>(tmp, job, tabs, old_tabs, sm_count, who);
+    }
+}
+
 }  // namespace
 
 extern "C" qb_status qb_hnsw_build_incremental(qb_storage* s, const qb_hnsw* old, const uint32_t* old_to_new, uint32_t ef_construct, const uint8_t* levels,
@@ -442,10 +454,12 @@ extern "C" qb_status qb_hnsw_build_incremental(qb_storage* s, const qb_hnsw* old
     const char* who = "hnsw_build_incremental";
     QB_CHECK(s && old && old_to_new && levels && out, QB_ERR_INVALID, "%s: null argument", who);
     *out = nullptr;
-    QB_CHECK(s->kind == QB_KIND_DENSE && s->dtype == QB_DT_F32, QB_ERR_UNSUPPORTED,
-             "%s: graphs are built over dense f32 storages only (build over the original vectors, then bind the graph to the quantized storage)", who);
+    QB_CHECK(s->kind == QB_KIND_DENSE && (s->dtype == QB_DT_F32 || s->dtype == QB_DT_U8), QB_ERR_UNSUPPORTED,
+             "%s: graphs are built over dense f32 and Uint8 storages only (build over the original vectors, then bind the graph to the quantized storage)",
+             who);
     const qb_storage* os = old->st;
-    QB_CHECK(os && os->kind == QB_KIND_DENSE && os->dtype == QB_DT_F32, QB_ERR_UNSUPPORTED, "%s: the old graph is bound to a storage that is not dense f32", who);
+    QB_CHECK(os && os->kind == QB_KIND_DENSE && os->dtype == s->dtype, QB_ERR_UNSUPPORTED,
+             "%s: the old graph is bound to a storage that is not dense of the new storage's datatype (f32 or Uint8)", who);
     QB_CHECK(os->dim == s->dim && os->distance == s->distance && os->device == s->device, QB_ERR_UNSUPPORTED,
              "%s: the old graph's storage has another dim, distance or device", who);
     QB_CHECK(!old->d_mv_tok, QB_ERR_UNSUPPORTED, "%s: the old graph is over multivector points", who);
@@ -527,12 +541,15 @@ extern "C" qb_status qb_hnsw_build_incremental(qb_storage* s, const qb_hnsw* old
         for (uint32_t l = 0; l <= job.old_level[o]; ++l)
             if ((flags[l ? reindex[o] : o] >> l) & 1u) job.items[l].push_back(o);
 
-    const int kind = s->dim >= 32 ? HK_DENSE_AVX : HK_DENSE_SMALL;
-    const int metric = hb_metric(s);
+    const bool u8 = s->dtype == QB_DT_U8;
+    const int kind = s->dim >= 32 ? (u8 ? HK_U8 : HK_DENSE_AVX) : (u8 ? HK_U8_SMALL : HK_DENSE_SMALL);
+    const int metric = hnsw_metric(s);
     const unsigned sms = (unsigned)os->sm_count;
 #define QB_HEAL(K, M) heal_levels<K, M>(tmp, job, tabs, old_tabs, sms, who)
     if (kind == HK_DENSE_AVX) QB_TRY(metric == M_EUCLID ? QB_HEAL(HK_DENSE_AVX, M_EUCLID) : metric == M_MANHATTAN ? QB_HEAL(HK_DENSE_AVX, M_MANHATTAN) : QB_HEAL(HK_DENSE_AVX, M_DOT));
-    else QB_TRY(metric == M_EUCLID ? QB_HEAL(HK_DENSE_SMALL, M_EUCLID) : metric == M_MANHATTAN ? QB_HEAL(HK_DENSE_SMALL, M_MANHATTAN) : QB_HEAL(HK_DENSE_SMALL, M_DOT));
+    else if (kind == HK_DENSE_SMALL) QB_TRY(metric == M_EUCLID ? QB_HEAL(HK_DENSE_SMALL, M_EUCLID) : metric == M_MANHATTAN ? QB_HEAL(HK_DENSE_SMALL, M_MANHATTAN) : QB_HEAL(HK_DENSE_SMALL, M_DOT));
+    else if (kind == HK_U8) QB_TRY(heal_levels_u8<HK_U8>(metric, tmp, job, tabs, old_tabs, sms, who));
+    else QB_TRY(heal_levels_u8<HK_U8_SMALL>(metric, tmp, job, tabs, old_tabs, sms, who));
 #undef QB_HEAL
 
     // renumber into the build's tables, then insert the new points

@@ -201,7 +201,7 @@
                 if (tid == 0) { if (n) { ++hops; evals += n; } s_nvalid = 0; }
                 if (n == 0) { __syncthreads(); continue; }
                 // score_points_unfiltered(to_score)
-                if (KIND == HK_DENSE_SMALL && CUSTOM != HC_MAXSIM) {
+                if (hk_one_thread(KIND) && CUSTOM != HC_MAXSIM) {
                     for (uint32_t i = tid; i < n; i += HNSW_THREADS) sm.sc[i] = score_q<KIND, METRIC, CUSTOM>(p, sm, q_off, sm.ids[i], 0, q);
                 } else {
                     score_list<KIND, METRIC, NT, CUSTOM>(p, sm, q_off, n, q);

@@ -21,7 +21,12 @@ constexpr uint32_t HNSW_MAX_EF = 4096;
 constexpr uint32_t HNSW_CUSTOM_SMEM = 48 * 1024;   // custom queries: examples up to this size are staged in shared memory
 constexpr uint32_t HNSW_MAX_LIST = 128;      // widest level list of a graph with inline vectors (qb_hnsw_create_with_vectors)
 
-enum { HK_DENSE_AVX = 0, HK_DENSE_SMALL = 1, HK_SQ8 = 2, HK_SQ8_LANEX = 3 };
+// HK_U8 / HK_U8_SMALL: Uint8 storages (rows / stride / dim as dense f32), dim >= 32 in 8-lane groups (GPU lane t = AVX lane t) and dim < 32
+// one thread per id, integer-exact; appended so the other kinds' values stay as they were
+enum { HK_DENSE_AVX = 0, HK_DENSE_SMALL = 1, HK_SQ8 = 2, HK_SQ8_LANEX = 3, HK_U8 = 4, HK_U8_SMALL = 5 };
+// kinds whose rows are dense rows of `stride` bytes, and kinds that score one id per thread rather than per 8-lane group
+__host__ __device__ constexpr bool hk_rows(int kind) { return kind == HK_DENSE_AVX || kind == HK_DENSE_SMALL || kind == HK_U8 || kind == HK_U8_SMALL; }
+__host__ __device__ constexpr bool hk_one_thread(int kind) { return kind == HK_DENSE_SMALL || kind == HK_U8_SMALL; }
 
 struct HnswParams {
     // graph
@@ -108,6 +113,10 @@ __device__ __forceinline__ float score_one(const HnswParams& p, const uint8_t* q
         return score_avx_group8<METRIC>(reinterpret_cast<const float*>(p.rows + (size_t)id * p.stride), reinterpret_cast<const float*>(q_smem), p.dim, t);
     } else if (KIND == HK_DENSE_SMALL) {
         return score_small<METRIC>(reinterpret_cast<const float*>(p.rows + (size_t)id * p.stride), reinterpret_cast<const float*>(q_smem), p.dim);
+    } else if (KIND == HK_U8) {
+        return u8_score_avx_group8(METRIC, p.rows + (size_t)id * p.stride, q_smem, p.dim, t);
+    } else if (KIND == HK_U8_SMALL) {
+        return u8_score_small(METRIC, p.rows + (size_t)id * p.stride, q_smem, p.dim);
     } else {
         const float raw = sq8_raw_group8<KIND == HK_SQ8_LANEX>(reinterpret_cast<const uint4*>(p.codes + (size_t)id * p.ad), reinterpret_cast<const uint4*>(q_smem),
                                                                p.ad >> 4, t, p.l1);
@@ -252,7 +261,7 @@ __device__ __forceinline__ void score_list(const P& p, const HnswSmem& sm, float
     const int tid = threadIdx.x;
     if constexpr (CUSTOM == HC_MAXSIM) {
         maxsim_list<KIND, METRIC, NT>(p, sm, n);
-    } else if (KIND == HK_DENSE_SMALL) {
+    } else if (hk_one_thread(KIND)) {
         if ((uint32_t)tid < n) sm.sc[tid] = score_q<KIND, METRIC, CUSTOM>(p, sm, q_off, sm.ids[tid], 0, q);
     } else {
         const int g = tid >> 3, t = tid & 7;
@@ -269,7 +278,7 @@ __device__ __forceinline__ void score_list(const P& p, const HnswSmem& sm, float
 // lane per id.  All GROUPS * 8 lanes must call it (the groups' shuffles span whole warps).
 template <int KIND, int METRIC, int GROUPS, class F>
 __device__ __forceinline__ void hnsw_score_rows(const HnswParams& p, const uint8_t* qrow, const uint32_t* ids, uint32_t n, int lid, F f) {
-    if (KIND == HK_DENSE_SMALL) {
+    if (hk_one_thread(KIND)) {
         for (uint32_t j = lid; j < n; j += GROUPS * 8) f(j, score_one<KIND, METRIC>(p, qrow, 0.0f, ids[j], 0));
     } else {
         const int g = lid >> 3, t = lid & 7;
@@ -293,7 +302,7 @@ __device__ __forceinline__ void prefetch_point(const P& p, uint32_t id) {
         if (r1 <= r0) return;
         if (KIND == HK_DENSE_AVX || KIND == HK_DENSE_SMALL) prefetch_row_l2(p.rows + (size_t)r0 * p.stride, (r1 - r0) * p.stride);
         else prefetch_row_l2(p.codes + (size_t)r0 * p.ad, (r1 - r0) * p.ad);
-    } else if (KIND == HK_DENSE_AVX || KIND == HK_DENSE_SMALL) {
+    } else if (hk_rows(KIND)) {
         prefetch_row_l2(p.rows + (size_t)id * p.stride, p.stride);
     } else {
         prefetch_row_l2(p.codes + (size_t)id * p.ad, p.ad);
@@ -460,6 +469,7 @@ qb_status launch_kind(int metric, const HnswParams& p, unsigned grid, size_t sme
     if (KIND == HK_SQ8 || KIND == HK_SQ8_LANEX) QB_HNSW_LAUNCH(M_DOT);
     else if (metric == M_EUCLID) QB_HNSW_LAUNCH(M_EUCLID);
     else if (metric == M_MANHATTAN) QB_HNSW_LAUNCH(M_MANHATTAN);
+    else if constexpr (KIND == HK_U8 || KIND == HK_U8_SMALL) { if (metric == M_COSINE) QB_HNSW_LAUNCH(M_COSINE); else QB_HNSW_LAUNCH(M_DOT); }
     else QB_HNSW_LAUNCH(M_DOT);
 #undef QB_HNSW_LAUNCH
     QB_LAUNCHED();
@@ -474,8 +484,22 @@ int occupancy_of(size_t smem) {
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, hnsw_search_kernel<KIND, METRIC, NT, ALGO, CUSTOM>, NT, smem) != cudaSuccess) nb = 1;
     return nb < 1 ? 1 : nb;
 }
+// the u8 kinds have a fourth metric (M_COSINE); they are not instantiated for MaxSim (qb_hnsw_mv_check rejects u8 token storages)
+template <int KIND, int NT, int ALGO, int CUSTOM>
+int occupancy_u8(int metric, size_t smem) {
+    switch (metric) {
+        case M_EUCLID: return occupancy_of<KIND, M_EUCLID, NT, ALGO, CUSTOM>(smem);
+        case M_MANHATTAN: return occupancy_of<KIND, M_MANHATTAN, NT, ALGO, CUSTOM>(smem);
+        case M_COSINE: return occupancy_of<KIND, M_COSINE, NT, ALGO, CUSTOM>(smem);
+        default: return occupancy_of<KIND, M_DOT, NT, ALGO, CUSTOM>(smem);
+    }
+}
 template <int NT, int ALGO, int CUSTOM>
 int occupancy_dispatch(int kind, int metric, size_t smem) {
+    if (kind == HK_U8 || kind == HK_U8_SMALL) {
+        if constexpr (CUSTOM == HC_MAXSIM) return 1;
+        else return kind == HK_U8 ? occupancy_u8<HK_U8, NT, ALGO, CUSTOM>(metric, smem) : occupancy_u8<HK_U8_SMALL, NT, ALGO, CUSTOM>(metric, smem);
+    }
     switch (kind) {
         case HK_DENSE_AVX: return metric == M_EUCLID ? occupancy_of<HK_DENSE_AVX, M_EUCLID, NT, ALGO, CUSTOM>(smem) : metric == M_MANHATTAN ? occupancy_of<HK_DENSE_AVX, M_MANHATTAN, NT, ALGO, CUSTOM>(smem) : occupancy_of<HK_DENSE_AVX, M_DOT, NT, ALGO, CUSTOM>(smem);
         case HK_DENSE_SMALL: return metric == M_EUCLID ? occupancy_of<HK_DENSE_SMALL, M_EUCLID, NT, ALGO, CUSTOM>(smem) : metric == M_MANHATTAN ? occupancy_of<HK_DENSE_SMALL, M_MANHATTAN, NT, ALGO, CUSTOM>(smem) : occupancy_of<HK_DENSE_SMALL, M_DOT, NT, ALGO, CUSTOM>(smem);
@@ -485,6 +509,14 @@ int occupancy_dispatch(int kind, int metric, size_t smem) {
 }
 template <int NT, int ALGO, int CUSTOM>
 qb_status launch_dispatch(int kind, int metric, const HnswParams& p, unsigned grid, size_t smem, cudaStream_t stream) {
+    if (kind == HK_U8 || kind == HK_U8_SMALL) {
+        if constexpr (CUSTOM == HC_MAXSIM) {
+            qb_set_error("hnsw_search_maxsim: MaxSim over Uint8 token storages is not supported");
+            return QB_ERR_UNSUPPORTED;
+        } else {
+            return kind == HK_U8 ? launch_kind<HK_U8, NT, ALGO, CUSTOM>(metric, p, grid, smem, stream) : launch_kind<HK_U8_SMALL, NT, ALGO, CUSTOM>(metric, p, grid, smem, stream);
+        }
+    }
     switch (kind) {
         case HK_DENSE_AVX: return launch_kind<HK_DENSE_AVX, NT, ALGO, CUSTOM>(metric, p, grid, smem, stream);
         case HK_DENSE_SMALL: return launch_kind<HK_DENSE_SMALL, NT, ALGO, CUSTOM>(metric, p, grid, smem, stream);
@@ -502,6 +534,16 @@ qb_status launch_nt(int nt, int kind, int metric, const HnswParams& p, unsigned 
                      : (nt == 64 ? launch_dispatch<64, ALGO, 0>(kind, metric, p, grid, smem, stream) : launch_dispatch<256, ALGO, 0>(kind, metric, p, grid, smem, stream));
 }
 
+
+// the METRIC a storage's rows are scored with: f32 cosine rows are normalised (M_DOT), Uint8 cosine is its own chain
+inline int hnsw_metric(const qb_storage* s) {
+    switch (s->distance) {
+        case QB_DIST_EUCLID: return M_EUCLID;
+        case QB_DIST_MANHATTAN: return M_MANHATTAN;
+        case QB_DIST_COSINE: return (s->kind == QB_KIND_DENSE && s->dtype == QB_DT_U8) ? M_COSINE : M_DOT;
+        default: return M_DOT;
+    }
+}
 
 // shared memory of one CTA of hnsw_search_kernel with HNSW level 0 (also ALGO_BUILD): query, two key buffers, the hop's lists, two flag buffers
 inline size_t hnsw_smem_bytes(uint32_t q_bytes, uint32_t ef) {

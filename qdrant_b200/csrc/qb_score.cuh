@@ -6,7 +6,8 @@
 
 namespace qbs {
 
-enum { M_DOT = 0, M_EUCLID = 1, M_MANHATTAN = 2 };
+// M_COSINE: Uint8 storages only (their cosine is its own chain); f32 cosine rows are normalised and scored with M_DOT
+enum { M_DOT = 0, M_EUCLID = 1, M_MANHATTAN = 2, M_COSINE = 3 };
 
 __device__ __forceinline__ float4 shfl_xor4(float4 v, int m) {
     v.x = __shfl_xor_sync(0xFFFFFFFFu, v.x, m);
@@ -125,6 +126,74 @@ __device__ __forceinline__ float score_small(const float* __restrict__ row, cons
     return (METRIC == M_DOT) ? r : -r;
 }
 
+// Uint8 storages (Metric<u8>::similarity, metric_uint/avx2/*.rs, simple_*.rs), shared by the scan (qb_dtype.cu) and the HNSW
+// traversal.  dim >= 32: eight i32 lanes, lane i sums bytes 4i..4i+3 of every 32-B block; manhattan uses sad_epu8 (even lanes =
+// 8-byte sums, odd = 0); the lanes are converted to f32 and added with hsum256_ps_avx; the n % 32 tail is an integer sum converted
+// once.  GPU lane t of an 8-lane group IS AVX lane t.  dim < 32: integer-exact totals.  Rows and query are 4-B aligned.
+__device__ __forceinline__ float hsum8(float f) {  // hsum256_ps_avx over the 8 lanes of a group
+    f = __fadd_rn(f, __shfl_xor_sync(0xFFFFFFFFu, f, 4));  // lr[i] = f[i+4] + f[i]
+    f = __fadd_rn(f, __shfl_xor_sync(0xFFFFFFFFu, f, 1));  // lr0+lr1 | lr2+lr3
+    f = __fadd_rn(f, __shfl_xor_sync(0xFFFFFFFFu, f, 2));
+    return f;
+}
+
+__device__ __forceinline__ float u8_score_avx_group8(int metric, const uint8_t* __restrict__ row, const uint8_t* __restrict__ qry, uint32_t dim, int t) {
+    const uint32_t nblk = dim >> 5;
+    unsigned int acc = 0, n1 = 0, n2 = 0;
+    for (uint32_t b = 0; b < nblk; ++b) {
+        const unsigned int v = *reinterpret_cast<const unsigned int*>(row + b * 32 + 4 * t);
+        const unsigned int q = *reinterpret_cast<const unsigned int*>(qry + b * 32 + 4 * t);
+        if (metric == M_DOT) acc = __dp4a(q, v, acc);
+        else if (metric == M_COSINE) { acc = __dp4a(q, v, acc); n1 = __dp4a(q, q, n1); n2 = __dp4a(v, v, n2); }
+        else if (metric == M_EUCLID) { const unsigned int d = __vabsdiffu4(q, v); acc = __dp4a(d, d, acc); }
+        else acc += __vsadu4(q, v);
+    }
+    if (metric == M_MANHATTAN) {  // sad_epu8: even lanes hold 8-byte sums, odd lanes 0 (avx2/manhattan.rs:33-35)
+        const unsigned int pair = acc + __shfl_xor_sync(0xFFFFFFFFu, acc, 1);
+        acc = (t & 1) ? 0u : pair;
+    }
+    float score = hsum8((float)(int)acc);
+    float f1 = 0.f, f2 = 0.f;
+    if (metric == M_COSINE) { f1 = hsum8((float)(int)n1); f2 = hsum8((float)(int)n2); }
+    const uint32_t rem0 = nblk << 5;
+    if (rem0 < dim) {
+        int rd = 0, r1 = 0, r2 = 0;
+        for (uint32_t i = rem0; i < dim; ++i) {
+            const int x = qry[i], y = row[i];
+            if (metric == M_DOT) rd += x * y;
+            else if (metric == M_COSINE) { rd += x * y; r1 += x * x; r2 += y * y; }
+            else if (metric == M_EUCLID) rd += (x - y) * (x - y);
+            else rd += abs(x - y);
+        }
+        score = __fadd_rn(score, (float)rd);
+        if (metric == M_COSINE) { f1 = __fadd_rn(f1, (float)r1); f2 = __fadd_rn(f2, (float)r2); }
+    }
+    if (metric == M_DOT) return score;
+    if (metric == M_COSINE) {  // avx2/cosine.rs:97-104
+        const float denom = __fmul_rn(f1, f2);
+        if (denom == 0.0f) return 0.0f;
+        return __fdiv_rn(score, __fsqrt_rn(denom));
+    }
+    return -score;
+}
+
+__device__ __forceinline__ float u8_score_small(int metric, const uint8_t* __restrict__ row, const uint8_t* __restrict__ qry, uint32_t dim) {
+    int rd = 0, r1 = 0, r2 = 0;
+    for (uint32_t i = 0; i < dim; ++i) {
+        const int x = qry[i], y = row[i];
+        if (metric == M_DOT) rd += x * y;
+        else if (metric == M_COSINE) { rd += x * y; r1 += x * x; r2 += y * y; }
+        else if (metric == M_EUCLID) rd += (x - y) * (x - y);
+        else rd += abs(x - y);
+    }
+    if (metric == M_DOT) return (float)rd;
+    if (metric == M_COSINE) {
+        const float denom = __fmul_rn((float)r1, (float)r2);
+        if (denom == 0.0f) return 0.0f;
+        return __fdiv_rn((float)rd, __fsqrt_rn(denom));
+    }
+    return -(float)rd;
+}
 
 // SQ8 (EncodedVectorsU8): raw integer score of one stored code row against one query code, 8 lanes per row, 16 B per lane per
 // step; every lane of the group returns the value.  l1 = Manhattan on codes (impl_score_l1_avx, cpp/avx2.c:65-122); LANEX =

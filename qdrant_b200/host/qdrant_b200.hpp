@@ -215,7 +215,7 @@ public:
         check(qb_hnsw_create_with_vectors(quantized.raw(), links_bin, n_bytes, &h));
         return std::unique_ptr<HnswGraph>(new HnswGraph(h));
     }
-    // builds the graph of a dense f32 storage on the device (qb_hnsw_build); levels: one per point, <= 30; batch / serial_points 0 = 512 / 256.
+    // builds the graph of a dense f32 or Uint8 storage on the device (qb_hnsw_build); levels: one per point, <= 30; batch / serial_points 0 = 512 / 256.
     // The entry point the search starts from is returned in entry_point / entry_level.
     static std::unique_ptr<HnswGraph> build(const VectorStorage& storage, uint32_t m, uint32_t m0, uint32_t ef_construct, const std::vector<uint8_t>& levels,
                                             uint32_t batch, uint32_t serial_points, uint32_t& entry_point, uint32_t& entry_level) {
@@ -223,7 +223,7 @@ public:
         check(qb_hnsw_build(storage.raw(), m, m0, ef_construct, levels.data(), batch, serial_points, &h, &entry_point, &entry_level));
         return std::unique_ptr<HnswGraph>(new HnswGraph(h));
     }
-    // builds the graph of a dense f32 storage from an old segment's graph (qb_hnsw_build_incremental): heals the old graph where points
+    // builds the graph of a dense f32 or Uint8 storage from an old segment's graph of the same datatype (qb_hnsw_build_incremental): heals the old graph where points
     // have gone, renumbers it by old_to_new (one per old point; 0xFFFFFFFF = not carried over) and inserts only the new points.  levels:
     // one per point of `storage`, a mapped point's equal to its old level; m / m0 are old's; batch / serial_points 0 = 512 / 256.
     static std::unique_ptr<HnswGraph> build_incremental(const VectorStorage& storage, const HnswGraph& old, const std::vector<uint32_t>& old_to_new,

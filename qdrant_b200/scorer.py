@@ -709,7 +709,7 @@ def set_option(name: str, value: int) -> None:
 
 class HnswGraph:
     """GraphLayers::search with the traversal on the device (qb_hnsw_*): a graph in the reference's plain links.bin layout
-    bound to a storage (dense f32 or SQ8); search() answers a batch of queries in one call.  from_compressed() takes the
+    bound to a storage (dense f32, dense Uint8 or SQ8); search() answers a batch of queries in one call.  from_compressed() takes the
     compressed links.bin the reference writes for every index it builds."""
 
     def __init__(self, storage: _Storage, links_bin, m: int, m0: int):
@@ -801,7 +801,7 @@ class HnswGraph:
     @classmethod
     def build(cls, storage: _Storage, m: int = 16, ef_construct: int = 100, levels=None, seed: int = 0, batch: int = 0, serial_points: int = 0,
               m0: Optional[int] = None) -> "HnswGraph":
-        """Builds the graph of a dense f32 storage on the device (qb_hnsw_build; m0 defaults to 2m).  levels: one per point (<= 30);
+        """Builds the graph of a dense f32 or Uint8 storage on the device (qb_hnsw_build; m0 defaults to 2m).  levels: one per point (<= 30);
         by default round(-ln(U) / ln(m)) with U uniform in (0, 1] from numpy's generator seeded with `seed` (get_random_layer,
         graph_layers_builder.rs:388-396).  batch / serial_points 0 = 512 / 256.  The entry point is in .entry_point / .entry_level."""
         m0 = 2 * m if m0 is None else m0
@@ -842,7 +842,7 @@ class HnswGraph:
     @classmethod
     def build_incremental(cls, storage: _Storage, old: "HnswGraph", old_to_new, ef_construct: int = 100, levels=None, seed: int = 0, batch: int = 0,
                           serial_points: int = 0) -> "HnswGraph":
-        """Builds the graph of a dense f32 storage from an old segment's graph (qb_hnsw_build_incremental): the old graph's lists are
+        """Builds the graph of a dense f32 or Uint8 storage from an old segment's graph over the same datatype (qb_hnsw_build_incremental): the old graph's lists are
         healed where points have gone, renumbered, and only the points it did not have are inserted.  old_to_new: one per old point,
         its id in `storage` or -1 (not carried over).  m / m0 are old's.  levels: one per point; by default a mapped point keeps its old
         level and the others are drawn as build() draws them (`seed`).  The entry point is in .entry_point / .entry_level."""
