@@ -121,6 +121,8 @@ extern "C" {
     pub fn qb_hnsw_build_multivector(tokens: *mut qb_storage, point_offsets: *const u32, n_points: u32, m: u32, m0: u32, ef_construct: u32, levels: *const u8, deleted_points: *const u64, batch: u32, serial_points: u32, out: *mut *mut qb_hnsw, entry_point: *mut u32, entry_level: *mut u32) -> qb_status;
     pub fn qb_hnsw_search_maxsim_batch(g: *mut qb_hnsw, query_vectors: *const f32, query_offsets: *const u32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, deleted_points: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters, algorithm: i32) -> qb_status;
     pub fn qb_hnsw_search_maxsim_batch_device(g: *mut qb_hnsw, dev_query_vectors: *const f32, n_query_vectors: u32, dev_query_offsets: *const u32, n_queries: u32, max_query_vectors: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, dev_out: *mut qb_scored_point, dev_counts: *mut u32, algorithm: i32) -> qb_status;
+    pub fn qb_hnsw_search_maxsim_custom_batch(g: *mut qb_hnsw, kind: i32, example_vectors: *const f32, example_offsets: *const u32, n_a: u32, n_b: u32, coef: *const f32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, custom_entry_points: *const u32, custom_counts: *const u32, n_custom: u32, deleted_points: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters, algorithm: i32) -> qb_status;
+    pub fn qb_hnsw_search_maxsim_discover_batch(g: *mut qb_hnsw, example_vectors: *const f32, example_offsets: *const u32, n_pairs: u32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, deleted_points: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters, algorithm: i32) -> qb_status;
     pub fn qb_hnsw_search_custom_batch(g: *mut qb_hnsw, kind: i32, vectors: *const f32, n_a: u32, n_b: u32, coef: *const f32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, custom_entry_points: *const u32, custom_counts: *const u32, n_custom: u32, deleted_bitmap: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters, algorithm: i32) -> qb_status;
     pub fn qb_hnsw_search_discover_batch(g: *mut qb_hnsw, vectors: *const f32, n_pairs: u32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, deleted_bitmap: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters, algorithm: i32) -> qb_status;
     pub fn qb_search_stats(s: *mut qb_storage, searches: *mut u64, reruns: *mut u64, reset: i32) -> qb_status;

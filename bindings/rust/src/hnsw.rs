@@ -173,6 +173,43 @@ impl<'a> B200Hnsw<'a> {
         (0..n_queries).map(|q| out[q * top..q * top + counts[q] as usize].iter().map(|p| ScoredPointOffset { idx: p.idx, score: p.score }).collect()).collect()
     }
 
+    /// `GraphLayers::search` with a MultiCustomQueryScorer on a multivector graph: custom queries whose examples are multivectors, one kind
+    /// and shape per call (`kind`, `n_a`, `n_b` as qb_scorer_create_custom takes them, E examples per query in its order).  Example j of
+    /// query q = rows [example_offsets[q * E + j], example_offsets[q * E + j + 1]) of `example_vectors` (raw f32 x dim, 1..4096 vectors
+    /// each); `coef`: [a, partial...] per query for feedback.  QB_QUERY_DISCOVER runs both stages of discover_search_with_graph in one
+    /// call (qb_hnsw_search_maxsim_discover_batch); the other kinds go through qb_hnsw_search_maxsim_custom_batch with
+    /// `custom_entry_points` (n_queries x n_custom, `custom_counts[q]` valid).  `deleted` is a bitmap over points.  Scores equal
+    /// qb_score_maxsim_custom bit for bit.
+    pub fn search_maxsim_custom(&self, kind: i32, example_vectors: &[f32], example_offsets: &[u32], n_a: usize, n_b: usize, coef: Option<&[f32]>,
+                                top: usize, ef: usize, entry: (PointOffsetType, usize), custom_entry_points: Option<(&[PointOffsetType], &[u32], usize)>,
+                                deleted: Option<&[u64]>, algorithm: SearchAlgorithm, hc: &HardwareCounterCell)
+                                -> OperationResult<Vec<Vec<ScoredPointOffset>>> {
+        let n_ex = match kind { QB_QUERY_RECO_BEST_SCORE | QB_QUERY_RECO_SUM_SCORES => n_a + n_b, QB_QUERY_CONTEXT => 2 * n_a, _ => 1 + 2 * n_a };
+        let n_queries = example_offsets.len().saturating_sub(1) / n_ex.max(1);
+        let mut out = vec![qb_scored_point::default(); n_queries * top];
+        let mut counts = vec![0u32; n_queries];
+        let mut counters = qb_hw_counters::default();
+        let algo = match algorithm { SearchAlgorithm::Hnsw => QB_HNSW_ALGO_HNSW, SearchAlgorithm::Acorn => QB_HNSW_ALGO_ACORN };
+        let del = deleted.map_or(std::ptr::null(), |d| d.as_ptr());
+        let st = unsafe {
+            if kind == QB_QUERY_DISCOVER {
+                qb_hnsw_search_maxsim_discover_batch(self.raw, example_vectors.as_ptr(), example_offsets.as_ptr(), n_a as u32, n_queries as u32, top as u32,
+                                                     ef as u32, entry.0, entry.1 as u32, del, std::ptr::null(), out.as_mut_ptr(), counts.as_mut_ptr(),
+                                                     &mut counters, algo)
+            } else {
+                let (cep, cep_counts, n_custom) = custom_entry_points.map_or((std::ptr::null(), std::ptr::null(), 0), |(c, n, w)| (c.as_ptr(), n.as_ptr(), w));
+                qb_hnsw_search_maxsim_custom_batch(self.raw, kind, example_vectors.as_ptr(), example_offsets.as_ptr(), n_a as u32, n_b as u32,
+                                                   coef.map_or(std::ptr::null(), |c| c.as_ptr()), n_queries as u32, top as u32, ef as u32, entry.0,
+                                                   entry.1 as u32, cep, cep_counts, n_custom as u32, del, std::ptr::null(), out.as_mut_ptr(),
+                                                   counts.as_mut_ptr(), &mut counters, algo)
+            }
+        };
+        if st != QB_OK { return Err(OperationError::service_error(last_error())); }
+        hc.cpu_counter().incr_delta(counters.cpu as usize);
+        hc.vector_io_read().incr_delta(counters.vector_io_read as usize);
+        Ok((0..n_queries).map(|q| out[q * top..q * top + counts[q] as usize].iter().map(|p| ScoredPointOffset { idx: p.idx, score: p.score }).collect()).collect())
+    }
+
     /// `GraphLayers::search` with a custom `FilteredScorer` for ONE query vector of `search_vectors_with_graph`
     /// (hnsw/read_view/search.rs:181-208): RecommendBestScore / RecommendSumScores / Context through qb_hnsw_search_custom_batch,
     /// Discover through qb_hnsw_search_discover_batch (both stages of discover_search_with_graph, :314-349, in one call).

@@ -518,7 +518,9 @@ QB_API qb_status qb_hnsw_search_with_vectors_batch_device(qb_hnsw* g, const floa
  * through GraphLayers::search with MultiMetricQueryScorer (query_scorer/multi_metric_query_scorer.rs) for dense tokens and
  * QuantizedMultivectorStorage::score_point_max_similarity (quantized/quantized_multivector_storage/mod.rs:328-352) for SQ8 tokens.
  * qb_hnsw_links, qb_hnsw_export_plain, qb_hnsw_info, qb_hnsw_stats and qb_hnsw_destroy work on the handle; the single-vector searches
- * (qb_hnsw_search_batch*, _custom_, _discover_, _with_vectors_) return QB_ERR_UNSUPPORTED.  Synchronous. */
+ * (qb_hnsw_search_batch*, _custom_, _discover_, _with_vectors_) return QB_ERR_UNSUPPORTED.  Search it with qb_hnsw_search_maxsim_batch
+ * (nearest queries) and qb_hnsw_search_maxsim_custom_batch / qb_hnsw_search_maxsim_discover_batch (custom queries with multivector
+ * examples).  Synchronous. */
 QB_API qb_status qb_hnsw_create_plain_multivector(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, const uint8_t* links_bin,
                                                   uint64_t n_bytes, uint32_t m, uint32_t m0, qb_hnsw** out);
 QB_API qb_status qb_hnsw_create_compressed_multivector(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, const uint8_t* bytes,
@@ -567,6 +569,37 @@ QB_API qb_status qb_hnsw_search_maxsim_batch(qb_hnsw* g, const float* query_vect
 QB_API qb_status qb_hnsw_search_maxsim_batch_device(qb_hnsw* g, const float* dev_query_vectors, uint32_t n_query_vectors, const uint32_t* dev_query_offsets,
                                                     uint32_t n_queries, uint32_t max_query_vectors, uint32_t top, uint32_t ef, uint32_t entry_point,
                                                     uint32_t entry_level, qb_scored_point* dev_out, uint32_t* dev_counts, qb_hnsw_algorithm algorithm);
+/* Custom queries whose examples are multivectors, through the device traversal of a graph over multivector points: GraphLayers::search
+ * with a MultiCustomQueryScorer (hnsw/read_view/search.rs:181-208, query_scorer/multi_custom_query_scorer.rs).  Only
+ * qb_hnsw_create_*_multivector and qb_hnsw_build_multivector handles (QB_ERR_UNSUPPORTED on any other); dense f32 and SQ8 tokens.
+ *   kind, n_a, n_b   one kind and one shape per call, as qb_hnsw_search_custom_batch takes them; query q has E =
+ *                    qb_custom_examples(kind, n_a, n_b) examples in the qb_scorer_create_custom order
+ *   example_vectors, example_offsets   example j of query q is rows [example_offsets[q*E + j], example_offsets[q*E + j + 1]) of
+ *                    example_vectors (raw f32 x dim): n_queries*E + 1 ascending offsets, 1..4096 vectors per example (QB_ERR_INVALID)
+ *   coef, custom_entry_points, custom_counts, n_custom   as qb_hnsw_search_custom_batch takes them (get_entry_point included)
+ *   deleted_points, out   over POINTS, as qb_hnsw_search_maxsim_batch takes and returns them; the token storage's resident flags do
+ *                    not apply
+ * The traversal is qb_hnsw_search_batch_algo's (max(ef, top), ef <= 4096 else QB_ERR_UNSUPPORTED, HNSW or ACORN-1, is_stopped) with
+ * the keyed tie contract of qb_hnsw_search_custom_batch.  A point's score equals qb_score_maxsim_custom on that point bit for bit: per
+ * example the MaxSim of qb_hnsw_search_maxsim_batch (the sequential `sim > max` fold from -inf per example vector, the maxima summed in
+ * vector order from +0.0; a point with no token rows scores -inf), then the E values folded by Query::score_by.
+ * Counters (multi_custom_query_scorer.rs:90-133): per scored point of T token rows, cpu += (the vectors of all E examples) x T x the
+ * storage's per-vector units (as qb_hnsw_search_maxsim_batch), vector_io_read += T x io units.  qb_hnsw_stats counts hops and
+ * scored points (points, not token rows). */
+QB_API qb_status qb_hnsw_search_maxsim_custom_batch(qb_hnsw* g, qb_query_kind kind, const float* example_vectors, const uint32_t* example_offsets,
+                                                    uint32_t n_a, uint32_t n_b, const float* coef, uint32_t n_queries, uint32_t top, uint32_t ef,
+                                                    uint32_t entry_point, uint32_t entry_level, const uint32_t* custom_entry_points,
+                                                    const uint32_t* custom_counts, uint32_t n_custom, const uint64_t* deleted_points,
+                                                    const volatile int32_t* is_stopped, qb_scored_point* out, uint32_t* out_counts,
+                                                    qb_hw_counters* counters /* optional */, qb_hnsw_algorithm algorithm);
+/* Discover with multivector examples as one call: the two stages of qb_hnsw_search_discover_batch over the examples above (E = 1 +
+ * 2 n_pairs: the target, then the pairs; n_pairs >= 1).  Stage 1 is a context search over examples 1 .. 2 n_pairs for the top 10
+ * with the same ef, filter, algorithm and entry point; stage 2 the discover search from that list as custom entry points.  Scores,
+ * ties and counters as qb_hnsw_search_maxsim_custom_batch; hops, scored points and counters sum both stages. */
+QB_API qb_status qb_hnsw_search_maxsim_discover_batch(qb_hnsw* g, const float* example_vectors, const uint32_t* example_offsets, uint32_t n_pairs,
+                                                      uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point, uint32_t entry_level,
+                                                      const uint64_t* deleted_points, const volatile int32_t* is_stopped, qb_scored_point* out,
+                                                      uint32_t* out_counts, qb_hw_counters* counters /* optional */, qb_hnsw_algorithm algorithm);
 
 /* Custom queries (recommend, context, feedback) through the device traversal: GraphLayers::search with a custom FilteredScorer
  * (hnsw/read_view/search.rs:181-208).  A point's score is qb_score_points on a qb_scorer_create_custom / qb_scorer_create_feedback

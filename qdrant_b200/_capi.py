@@ -115,6 +115,11 @@ SIGNATURES = {
                                                 C.POINTER(ScoredPoint), u32p, C.POINTER(HwCounters), C.c_int32]),
     "qb_hnsw_search_maxsim_batch_device": (C.c_int32, [vp, vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                                        vp, vp, C.c_int32]),
+    "qb_hnsw_search_maxsim_custom_batch": (C.c_int32, [vp, C.c_int, f32p, u32p, C.c_uint32, C.c_uint32, f32p, C.c_uint32, C.c_uint32, C.c_uint32,
+                                                       C.c_uint32, C.c_uint32, u32p, u32p, C.c_uint32, u64p, i32p, C.POINTER(ScoredPoint), u32p,
+                                                       C.POINTER(HwCounters), C.c_int32]),
+    "qb_hnsw_search_maxsim_discover_batch": (C.c_int32, [vp, f32p, u32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, u64p,
+                                                         i32p, C.POINTER(ScoredPoint), u32p, C.POINTER(HwCounters), C.c_int32]),
     "qb_hnsw_stats": (C.c_int32, [vp, u64p, u64p, C.c_int32]),
     "qb_hnsw_search_custom_batch": (C.c_int32, [vp, C.c_int, f32p, C.c_uint32, C.c_uint32, f32p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
                                                 u32p, u32p, C.c_uint32, u64p, i32p, C.POINTER(ScoredPoint), u32p, C.POINTER(HwCounters), C.c_int32]),

@@ -1847,11 +1847,15 @@ extern "C" qb_status qb_hnsw_search_maxsim_batch_device(qb_hnsw* g, const float*
     return QB_OK;
 }
 
-// custom queries through the device traversal; discover_pairs > 0: the two-stage discover of that many pairs (kind = DISCOVER)
-static qb_status hnsw_custom_run(qb_hnsw* g, qb_query_kind kind, const float* vectors, uint32_t n_a, uint32_t n_b, const float* coef, uint32_t n_queries,
-                                 uint32_t top, uint32_t ef, uint32_t entry_point, uint32_t entry_level, const uint32_t* cep, const uint32_t* cep_counts,
-                                 uint32_t n_custom, const uint64_t* deleted_bitmap, const volatile int32_t* is_stopped, qb_scored_point* out,
-                                 uint32_t* out_counts, qb_hw_counters* counters, qb_hnsw_algorithm algorithm, bool discover, const char* what) {
+// custom queries through the device traversal; discover: the two-stage discover of n_a pairs (kind = DISCOVER).  example_offsets = null:
+// dense examples, query q's are vectors [q * E, (q + 1) * E); else multivector examples on a graph over multivector points, example j of
+// query q being vectors [example_offsets[q * E + j], example_offsets[q * E + j + 1]).
+static qb_status hnsw_custom_run(qb_hnsw* g, qb_query_kind kind, const float* vectors, const uint32_t* example_offsets, uint32_t n_a, uint32_t n_b,
+                                 const float* coef, uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point, uint32_t entry_level,
+                                 const uint32_t* cep, const uint32_t* cep_counts, uint32_t n_custom, const uint64_t* deleted_bitmap,
+                                 const volatile int32_t* is_stopped, qb_scored_point* out, uint32_t* out_counts, qb_hw_counters* counters,
+                                 qb_hnsw_algorithm algorithm, bool discover, const char* what) {
+    const bool mv = example_offsets != nullptr;
     QB_CHECK(g && out && out_counts, QB_ERR_INVALID, "%s: null argument", what);
     QB_CHECK(n_queries == 0 || vectors, QB_ERR_INVALID, "%s: null vectors", what);
     QB_CHECK(top >= 1 && top <= 4096, QB_ERR_INVALID, "%s: top %u outside [1,4096]", what, top);
@@ -1871,6 +1875,19 @@ static qb_status hnsw_custom_run(qb_hnsw* g, qb_query_kind kind, const float* ve
                 QB_CHECK(cep[(size_t)q * n_custom + i] < g->n_points, QB_ERR_INVALID, "%s: custom entry point %u out of range", what, cep[(size_t)q * n_custom + i]);
         }
     }
+    // multivector examples: 1..4096 vectors each (qb_search_maxsim_custom's limit); max_q = the most vectors of one query's examples
+    uint32_t max_q = 0;
+    if (mv) {
+        QB_CHECK(g->d_mv_tok, QB_ERR_UNSUPPORTED, "%s: the graph is not over multivector points (load it with qb_hnsw_create_*_multivector)", what);
+        for (uint32_t q = 0; q < n_queries; ++q) {
+            for (uint32_t j = 0; j < ne; ++j) {
+                const uint32_t a = example_offsets[(size_t)q * ne + j], b = example_offsets[(size_t)q * ne + j + 1];
+                QB_CHECK(a <= b, QB_ERR_INVALID, "%s: example_offsets not ascending at query %u example %u", what, q, j);
+                QB_CHECK(b - a >= 1 && b - a <= 4096, QB_ERR_INVALID, "%s: query %u example %u has %u vectors (need 1..4096)", what, q, j, b - a);
+            }
+            max_q = std::max(max_q, example_offsets[(size_t)(q + 1) * ne] - example_offsets[(size_t)q * ne]);
+        }
+    }
     if (n_queries == 0) return QB_OK;
     if (cancelled(is_stopped)) return QB_ERR_CANCELLED;
     QB_TRY(use_device(s->device));
@@ -1879,50 +1896,63 @@ static qb_status hnsw_custom_run(qb_hnsw* g, qb_query_kind kind, const float* ve
     QB_TRY(lease.acquire(s));
     QbSearchCtx* c = lease.c;
     cudaStream_t stream = c->stream;
-    // example vectors, encoded back to back: query q's are [q * ne, (q + 1) * ne)
+    // example vectors, encoded back to back (multivector: vectors before example_offsets[0] are uploaded and not read)
+    const uint32_t nv = mv ? example_offsets[(size_t)n_queries * ne] : n_queries * ne;
     uint8_t* h_tail = nullptr;
-    QB_TRY(stage_queries(s, c, vectors, n_queries * ne, (size_t)n_queries * (top * sizeof(qb_scored_point) + 4), &h_tail));
+    QB_TRY(stage_queries(s, c, vectors, nv, (size_t)n_queries * (top * sizeof(qb_scored_point) + 4), &h_tail));
     QB_TRY(ensure_dev_elems(&c->d_out, &c->out_elems, (size_t)n_queries * top));
     QB_TRY(ensure_dev_elems(&c->d_out_counts, &c->out_counts_elems, (size_t)n_queries + 4));
     const uint32_t* d_del2 = nullptr;
-    QB_TRY(upload_bitmap(c, deleted_bitmap, s->count, &d_del2));
-    // per-call buffers: coefficients, custom entry points (as scored points: the stage-1 lists of discover have that layout), counts
+    QB_TRY(upload_bitmap(c, deleted_bitmap, mv ? g->n_points : s->count, &d_del2));   // multivector: a bitmap over points
+    // per-call buffers: coefficients, custom entry points (as scored points: the stage-1 lists of discover have that layout), counts,
+    // example offsets
     constexpr uint32_t DISCOVERY_ENTRY_POINT_COUNT = 10;   // search.rs:325
     const uint32_t n_coef = fb ? 1 + n_a : 0;
     const uint32_t n_cep = discover ? DISCOVERY_ENTRY_POINT_COUNT : (cep ? n_custom : 0);
     const size_t coef_bytes = round_up_u64((size_t)n_queries * n_coef * 4, 256), cep_bytes = round_up_u64((size_t)n_queries * n_cep * sizeof(qb_scored_point), 256);
-    std::vector<uint8_t> h_extra(coef_bytes + cep_bytes + (size_t)n_queries * 4, 0);
+    const size_t cnt_bytes = round_up_u64((size_t)n_queries * 4, 256), exo_bytes = mv ? ((size_t)n_queries * ne + 1) * 4 : 0;
+    std::vector<uint8_t> h_extra(coef_bytes + cep_bytes + cnt_bytes + exo_bytes, 0);
     if (fb) memcpy(h_extra.data(), coef, (size_t)n_queries * n_coef * 4);
     if (cep && !discover) {
         qb_scored_point* hp = reinterpret_cast<qb_scored_point*>(h_extra.data() + coef_bytes);
         for (size_t i = 0; i < (size_t)n_queries * n_cep; ++i) hp[i].idx = cep[i];
         memcpy(h_extra.data() + coef_bytes + cep_bytes, cep_counts, (size_t)n_queries * 4);
     }
+    if (mv) memcpy(h_extra.data() + coef_bytes + cep_bytes + cnt_bytes, example_offsets, exo_bytes);
     struct Scratch { void* p = nullptr; ~Scratch() { cudaFree(p); } } extra;
     QB_CUDA(cudaMalloc(&extra.p, h_extra.size() + 256));
     uint8_t* d_extra = reinterpret_cast<uint8_t*>(extra.p);
-    if (fb || (cep && !discover)) QB_CUDA(cudaMemcpyAsync(d_extra, h_extra.data(), h_extra.size(), cudaMemcpyHostToDevice, stream));
+    if (fb || (cep && !discover) || mv) QB_CUDA(cudaMemcpyAsync(d_extra, h_extra.data(), h_extra.size(), cudaMemcpyHostToDevice, stream));
     QbHnswCustom cq{};
     cq.kind = (int)kind; cq.n_a = n_a; cq.n_b = n_b; cq.n_ex = ne; cq.ex_first = 0; cq.ex_stride = ne;
     cq.d_coef = fb ? reinterpret_cast<const float*>(d_extra) : nullptr; cq.n_coef = n_coef;
     qb_scored_point* d_cep = reinterpret_cast<qb_scored_point*>(d_extra + coef_bytes);
     uint32_t* d_cep_counts = reinterpret_cast<uint32_t*>(d_extra + coef_bytes + cep_bytes);
     if (n_cep) { cq.d_cep = d_cep; cq.d_cep_counts = d_cep_counts; cq.n_cep = n_cep; }
+    const QbHnswMaxsim mve{reinterpret_cast<const uint32_t*>(d_extra + coef_bytes + cep_bytes + cnt_bytes), nv, max_q};
+    const QbHnswMaxsim* mvp = mv ? &mve : nullptr;
+    const uint64_t rows0 = g->mv_rows, qrows0 = g->mv_qrows;
     cudaEvent_t e0, e1;
     profile_begin(s, c, stream, &e0, &e1);   // qb_profile_*: the traversal kernels (both stages of discover)
     if (discover) {
-        // stage 1: the context search over the pairs (encoded examples 1 .. 2 n_pairs of each query), top 10, its lists left on the device
+        // stage 1: the context search over the pairs (examples 1 .. 2 n_pairs of each query), top 10, its lists left on the device
         QbHnswCustom ctx{};
         ctx.kind = QB_QUERY_CONTEXT; ctx.n_a = n_a; ctx.n_b = 0; ctx.n_ex = 2 * n_a; ctx.ex_first = 1; ctx.ex_stride = ne;
         ctx.stats_slot = 1; ctx.internal_out = true;
         QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, DISCOVERY_ENTRY_POINT_COUNT, ef, entry_point, entry_level, d_del2, d_cep,
-                              d_cep_counts, stream, (int)algorithm, &ctx));
+                              d_cep_counts, stream, (int)algorithm, &ctx, mvp));
     }
     QB_TRY(qb_hnsw_launch(g, c->d_queries_enc, c->d_q_off, n_queries, top, ef, entry_point, entry_level, d_del2, c->d_out, c->d_out_counts, stream,
-                          (int)algorithm, &cq));
+                          (int)algorithm, &cq, mvp));
     profile_end(s, stream, e0, e1);
     QB_TRY(fetch_lists(c, c->d_out, c->d_out_counts, n_queries, top, 0, h_tail, out, out_counts));
-    if (counters) {
+    if (counters && mv) {
+        // MultiCustomQueryScorer (multi_custom_query_scorer.rs:90-133): per scored point, the examples' vectors x its token rows of cpu
+        // units, its token rows read once
+        QB_TRY(qb_hnsw_read_stats(g, stream));
+        counters->cpu += (g->mv_qrows - qrows0) * cpu_units_per_point(s);
+        counters->vector_io_read += (g->mv_rows - rows0) * io_units_per_point(s);
+    } else if (counters) {
         // per scored point: E similarities of cpu units, one read of the vector (custom_query_scorer.rs:78-111, qb_score_points)
         uint64_t ev[2] = {0, 0};
         QB_TRY(qb_hnsw_read_stats(g, stream, ev));
@@ -1938,16 +1968,38 @@ extern "C" qb_status qb_hnsw_search_custom_batch(qb_hnsw* g, qb_query_kind kind,
                                                  const uint32_t* custom_entry_points, const uint32_t* custom_counts, uint32_t n_custom,
                                                  const uint64_t* deleted_bitmap, const volatile int32_t* is_stopped, qb_scored_point* out,
                                                  uint32_t* out_counts, qb_hw_counters* counters, qb_hnsw_algorithm algorithm) {
-    return hnsw_custom_run(g, kind, vectors, n_a, n_b, coef, n_queries, top, ef, entry_point, entry_level, custom_entry_points, custom_counts, n_custom,
-                           deleted_bitmap, is_stopped, out, out_counts, counters, algorithm, false, "hnsw_search_custom_batch");
+    return hnsw_custom_run(g, kind, vectors, nullptr, n_a, n_b, coef, n_queries, top, ef, entry_point, entry_level, custom_entry_points, custom_counts,
+                           n_custom, deleted_bitmap, is_stopped, out, out_counts, counters, algorithm, false, "hnsw_search_custom_batch");
 }
 
 extern "C" qb_status qb_hnsw_search_discover_batch(qb_hnsw* g, const float* vectors, uint32_t n_pairs, uint32_t n_queries, uint32_t top, uint32_t ef,
                                                    uint32_t entry_point, uint32_t entry_level, const uint64_t* deleted_bitmap,
                                                    const volatile int32_t* is_stopped, qb_scored_point* out, uint32_t* out_counts,
                                                    qb_hw_counters* counters, qb_hnsw_algorithm algorithm) {
-    return hnsw_custom_run(g, QB_QUERY_DISCOVER, vectors, n_pairs, 0, nullptr, n_queries, top, ef, entry_point, entry_level, nullptr, nullptr, 0,
+    return hnsw_custom_run(g, QB_QUERY_DISCOVER, vectors, nullptr, n_pairs, 0, nullptr, n_queries, top, ef, entry_point, entry_level, nullptr, nullptr, 0,
                            deleted_bitmap, is_stopped, out, out_counts, counters, algorithm, true, "hnsw_search_discover_batch");
+}
+
+extern "C" qb_status qb_hnsw_search_maxsim_custom_batch(qb_hnsw* g, qb_query_kind kind, const float* example_vectors, const uint32_t* example_offsets,
+                                                        uint32_t n_a, uint32_t n_b, const float* coef, uint32_t n_queries, uint32_t top, uint32_t ef,
+                                                        uint32_t entry_point, uint32_t entry_level, const uint32_t* custom_entry_points,
+                                                        const uint32_t* custom_counts, uint32_t n_custom, const uint64_t* deleted_points,
+                                                        const volatile int32_t* is_stopped, qb_scored_point* out, uint32_t* out_counts,
+                                                        qb_hw_counters* counters, qb_hnsw_algorithm algorithm) {
+    QB_CHECK(example_offsets, QB_ERR_INVALID, "hnsw_search_maxsim_custom_batch: null example_offsets");   // n_queries * E + 1 entries, one at least
+    return hnsw_custom_run(g, kind, example_vectors, example_offsets, n_a, n_b, coef, n_queries, top, ef, entry_point, entry_level,
+                           custom_entry_points, custom_counts, n_custom, deleted_points, is_stopped, out, out_counts, counters, algorithm, false,
+                           "hnsw_search_maxsim_custom_batch");
+}
+
+extern "C" qb_status qb_hnsw_search_maxsim_discover_batch(qb_hnsw* g, const float* example_vectors, const uint32_t* example_offsets, uint32_t n_pairs,
+                                                          uint32_t n_queries, uint32_t top, uint32_t ef, uint32_t entry_point, uint32_t entry_level,
+                                                          const uint64_t* deleted_points, const volatile int32_t* is_stopped, qb_scored_point* out,
+                                                          uint32_t* out_counts, qb_hw_counters* counters, qb_hnsw_algorithm algorithm) {
+    QB_CHECK(example_offsets, QB_ERR_INVALID, "hnsw_search_maxsim_discover_batch: null example_offsets");   // n_queries * E + 1 entries, one at least
+    return hnsw_custom_run(g, QB_QUERY_DISCOVER, example_vectors, example_offsets, n_pairs, 0, nullptr, n_queries, top, ef,
+                           entry_point, entry_level, nullptr, nullptr, 0, deleted_points, is_stopped, out, out_counts, counters, algorithm, true,
+                           "hnsw_search_maxsim_discover_batch");
 }
 
 extern "C" qb_status qb_hnsw_stats(qb_hnsw* g, uint64_t* hops, uint64_t* scored_points, int32_t reset) {

@@ -684,7 +684,8 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
     qb_storage* s = g->st;
     QB_CHECK(!maxsim == !g->d_mv_tok, QB_ERR_UNSUPPORTED,
              maxsim ? "hnsw_search_maxsim: the graph is not over multivector points (load it with qb_hnsw_create_*_multivector)"
-                    : "hnsw_search: the graph is over multivector points; search it with qb_hnsw_search_maxsim_batch");
+                    : "hnsw_search: the graph is over multivector points; search it with qb_hnsw_search_maxsim_batch / _maxsim_custom_batch");
+    const bool mv_custom = custom && maxsim;
     QB_CHECK(algo == ALGO_HNSW || algo == ALGO_ACORN, QB_ERR_INVALID, "hnsw_search: algorithm %d is neither QB_HNSW_ALGO_HNSW nor QB_HNSW_ALGO_ACORN", algo);
     QB_CHECK(entry < g->n_points, QB_ERR_INVALID, "hnsw_search: entry point %u out of range", entry);
     QB_CHECK(entry_level < std::max<uint32_t>(g->levels, 1), QB_ERR_INVALID, "hnsw_search: entry level %u but the graph has %u levels", entry_level, g->levels);
@@ -727,7 +728,15 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
         q_smem = p.ex_smem ? (uint32_t)ex_bytes : 0u;
         p.q_smem = q_smem;
     }
-    if (maxsim) {
+    if (mv_custom) {
+        // multivector examples: points and filter as for a MaxSim query; all of a query's example vectors are staged in shared memory
+        // when the largest query's fit in HNSW_CUSTOM_SMEM
+        p.deleted = nullptr; p.id_base = 0;
+        p.ex_smem = (uint64_t)maxsim->max_q * p.q_bytes <= HNSW_CUSTOM_SMEM ? 1u : 0u;
+        q_smem = p.ex_smem ? maxsim->max_q * p.q_bytes : 0u;
+        p.q_smem = q_smem;
+        p.stats = g->d_stats + 8;
+    } else if (maxsim) {
         // points are numbered 0 .. n_points - 1 and filtered by the per-call bitmap over points only: the token storage's resident flags
         // are per token row
         p.deleted = nullptr; p.id_base = 0;
@@ -744,7 +753,9 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
     // per hop, twice the resident queries.  The traversal is a chain of dependent memory round trips, so queries in flight is what hides them.
     // Custom and MaxSim queries are instantiated for 128 threads only.
     const int nt = (custom || maxsim) ? 128 : (qb_opt().hnsw_threads == 256 ? 256 : (qb_opt().hnsw_threads == 64 ? 64 : 128));
-    const int per_sm = maxsim ? (acorn ? occupancy_dispatch<128, ALGO_ACORN, HC_MAXSIM>(kind, metric, smem) : occupancy_dispatch<128, ALGO_HNSW, HC_MAXSIM>(kind, metric, smem))
+    int per_sm = 1;
+    if (mv_custom) QB_TRY(qb_hnsw_mv_custom_launch(&p, g->d_mv_tok, maxsim->d_qoff, kind, metric, algo, 0, smem, stream, &per_sm));
+    else per_sm = maxsim ? (acorn ? occupancy_dispatch<128, ALGO_ACORN, HC_MAXSIM>(kind, metric, smem) : occupancy_dispatch<128, ALGO_HNSW, HC_MAXSIM>(kind, metric, smem))
                        : custom ? (acorn ? occupancy_dispatch<128, ALGO_ACORN, 1>(kind, metric, smem) : occupancy_dispatch<128, ALGO_HNSW, 1>(kind, metric, smem))
                                 : (acorn ? occupancy_nt<ALGO_ACORN>(nt, kind, metric, smem) : occupancy_nt<ALGO_HNSW>(nt, kind, metric, smem));
     p.prefetch = qb_opt().hnsw_no_prefetch ? 0 : 1;
@@ -762,6 +773,7 @@ qb_status qb_hnsw_launch(qb_hnsw* g, const void* d_q_enc, const float* d_q_off, 
     }
     p.visited = g->d_visited; p.visited_words = words; p.vlog = g->d_vlog; p.vlog_cap = g->vlog_cap; p.work = g->d_work;
     QB_CUDA(cudaMemsetAsync(g->d_work, 0, 4, stream));
+    if (mv_custom) return qb_hnsw_mv_custom_launch(&p, g->d_mv_tok, maxsim->d_qoff, kind, metric, algo, grid, smem, stream, nullptr);
     if (maxsim)
         return acorn ? launch_dispatch<128, ALGO_ACORN, HC_MAXSIM>(kind, metric, p, grid, smem, stream)
                      : launch_dispatch<128, ALGO_HNSW, HC_MAXSIM>(kind, metric, p, grid, smem, stream);

@@ -1,6 +1,7 @@
 // qb_hnsw_search_body.cuh — the body of hnsw_search_kernel (qb_hnsw_traverse.cuh), included inside the braces of a kernel that defines
 // KIND, METRIC, NT, ALGO and CUSTOM and takes its parameters as `p`: hnsw_search_kernel (p: HnswParams) and the inserts of a multivector
-// build, hnsw_build_mv_kernel (qb_hnsw_build_mv.cu; p: HnswMvBuildParams).  Not a standalone header.  The kernels keep the body in their
+// build, hnsw_build_mv_kernel (qb_hnsw_build_mv.cu; p: HnswMvBuildParams), and the custom queries with multivector examples,
+// hnsw_mv_custom_kernel (qb_hnsw_mv_custom.cu; p: HnswMvCustomParams).  Not a standalone header.  The kernels keep the body in their
 // own braces, rather than calling a shared device function, so that every hnsw_search_kernel instantiation compiles to the machine
 // code it had before the multivector build was added.
     constexpr int HNSW_THREADS = NT;
@@ -29,7 +30,7 @@
     uint32_t* visited = p.visited + (size_t)blockIdx.x * p.visited_words;
     uint32_t* vlog = p.vlog + (size_t)blockIdx.x * p.vlog_cap;
     unsigned long long hops = 0, evals = 0;   // thread 0 only
-    unsigned long long mv_rows = 0, mv_qrows = 0;   // HC_MAXSIM, thread 0: token rows scored, and times the query's vector count
+    unsigned long long mv_rows = 0, mv_qrows = 0;   // MaxSim, thread 0: token rows scored, and times the query's (examples') vector count
 
     for (;;) {
         if (tid == 0) s_q = atomicAdd(p.work, 1u);
@@ -64,6 +65,21 @@
                 sm.q = src;
             }
             if (tid == 0) { ms.q0 = q0; ms.nqv = q1 - q0; ms.rows = 0; }
+        } else if constexpr (CUSTOM == HC_MAXSIM_CUSTOM) {
+            // all of the query's example vectors: into shared memory when they fit, else read where they are; ms.nqv = their count (the counters)
+            MvShared& ms = mv_shared();
+            const uint32_t* eo = mv_ex_off<CUSTOM>(p) + (size_t)q * p.ex_stride + p.ex_first;
+            const uint32_t v0 = eo[0], v1 = eo[p.n_ex];
+            const uint8_t* src = p.q_enc + (size_t)v0 * p.q_bytes;
+            if (p.ex_smem) {
+                const uint4* s4 = reinterpret_cast<const uint4*>(src);
+                uint4* dst = reinterpret_cast<uint4*>(smem_raw);
+                for (uint32_t i = tid; i < ((v1 - v0) * p.q_bytes) / 16u; i += HNSW_THREADS) dst[i] = s4[i];
+                sm.q = smem_raw;
+            } else {
+                sm.q = src;
+            }
+            if (tid == 0) { ms.q0 = v0; ms.nqv = v1 - v0; ms.rows = 0; }
         } else {
             // the examples: into shared memory when they fit, else read where they are (the same arithmetic either way)
             const size_t first = (size_t)q * p.ex_stride + p.ex_first;
@@ -80,7 +96,7 @@
         const float q_off = (!CUSTOM && p.q_off) ? p.q_off[q] : 0.0f;
         if (tid == 0) {
             s_nlog = 0;
-            if constexpr (CUSTOM == HC_CUSTOM) {
+            if constexpr (hc_entry_points(CUSTOM)) {
                 uint32_t e, l;
                 hnsw_custom_entry(p, q, e, l);
                 s_entry = e; s_entry_level = l; sm.ids[0] = e;
@@ -91,19 +107,19 @@
             }
         }
         __syncthreads();
-        // `CUSTOM == HC_CUSTOM ? s_entry : p.entry` is written out at each use, not bound to a local, so the nearest-query kernels compile as before
+        // `hc_entry_points(CUSTOM) ? s_entry : p.entry` is written out at each use, not bound to a local, so the nearest-query kernels compile as before
 
         // ---- search_entry: greedy descent from the entry point's level to level 1 (graph_layers.rs:247-316)
         score_list<KIND, METRIC, NT, CUSTOM>(p, sm, q_off, 1, q);      // score_point(entry)
         __syncthreads();
-        if (tid == 0) { s_cur = CUSTOM == HC_CUSTOM ? s_entry : (ALGO == ALGO_BUILD ? sm.ids[0] : p.entry); s_cur_score = sm.sc[0]; ++hops; ++evals; }
+        if (tid == 0) { s_cur = hc_entry_points(CUSTOM) ? s_entry : (ALGO == ALGO_BUILD ? sm.ids[0] : p.entry); s_cur_score = sm.sc[0]; ++hops; ++evals; }
         __syncthreads();
-        for (uint32_t lvl = CUSTOM == HC_CUSTOM ? s_entry_level : p.entry_level; lvl >= 1; --lvl) {
+        for (uint32_t lvl = hc_entry_points(CUSTOM) ? s_entry_level : p.entry_level; lvl >= 1; --lvl) {
             // search_entry_on_level re-scores its entry point on every level (graph_layers.rs:298-301): same value, but the scorer call
             // and the scored point are metered, so they are counted here too
-            if (tid == 0 && lvl != (CUSTOM == HC_CUSTOM ? s_entry_level : p.entry_level)) {
+            if (tid == 0 && lvl != (hc_entry_points(CUSTOM) ? s_entry_level : p.entry_level)) {
                 ++hops; ++evals;
-                if constexpr (CUSTOM == HC_MAXSIM) mv_shared().rows += mv_tok(p)[s_cur + 1] - mv_tok(p)[s_cur];
+                if constexpr (hc_multivector(CUSTOM)) mv_shared().rows += mv_tok(p)[s_cur + 1] - mv_tok(p)[s_cur];
             }
             for (;;) {
                 const uint32_t cur = s_cur;
@@ -119,7 +135,7 @@
                         const bool keep = l != HNSW_EMPTY && l < p.n_points && !hnsw_filtered_out(p, l);
                         const unsigned int bal = __ballot_sync(0xFFFFFFFFu, keep);
                         const uint32_t pos = cnt + __popc(bal & ((1u << tid) - 1u));
-                        if (keep && pos < p.m && pos < HNSW_MAX_LINKS) { sm.ids[pos] = l; if (p.prefetch) prefetch_point<KIND, CUSTOM == HC_MAXSIM>(p, l); }
+                        if (keep && pos < p.m && pos < HNSW_MAX_LINKS) { sm.ids[pos] = l; if (p.prefetch) prefetch_point<KIND, hc_multivector(CUSTOM)>(p, l); }
                         cnt += __popc(bal);
                     }
                     if (tid == 0) s_n = min(min(cnt, p.m), HNSW_MAX_LINKS);
@@ -196,12 +212,12 @@
             const uint32_t cand = qb_key_id(keys[best]);
             if constexpr (ALGO == ALGO_ACORN) {
                 if (tid == 0) flags[best] = 1;
-                acorn_collect<KIND, NT, CUSTOM == HC_MAXSIM>(p, sm, xids, cand, visited, vlog, s_n, s_nx, s_nlog, s_warp_cnt);
+                acorn_collect<KIND, NT, hc_multivector(CUSTOM)>(p, sm, xids, cand, visited, vlog, s_n, s_nx, s_nlog, s_warp_cnt);
                 const uint32_t n = s_n;
                 if (tid == 0) { if (n) { ++hops; evals += n; } s_nvalid = 0; }
                 if (n == 0) { __syncthreads(); continue; }
                 // score_points_unfiltered(to_score)
-                if (hk_one_thread(KIND) && CUSTOM != HC_MAXSIM) {
+                if (hk_one_thread(KIND) && !hc_multivector(CUSTOM)) {
                     for (uint32_t i = tid; i < n; i += HNSW_THREADS) sm.sc[i] = score_q<KIND, METRIC, CUSTOM>(p, sm, q_off, sm.ids[i], 0, q);
                 } else {
                     score_list<KIND, METRIC, NT, CUSTOM>(p, sm, q_off, n, q);
@@ -252,7 +268,7 @@
                 asm volatile("bar.sync 1, 64;" ::: "memory");
                 const uint32_t pos = ((tid >> 5) ? s_warp_cnt[0] : 0u) + __popc(bal & ((1u << (tid & 31)) - 1u));
                 if (keep) {
-                    if (p.prefetch) prefetch_point<KIND, CUSTOM == HC_MAXSIM>(p, l);          // HBM -> L2 for the whole vector, in flight while the list is published
+                    if (p.prefetch) prefetch_point<KIND, hc_multivector(CUSTOM)>(p, l);          // HBM -> L2 for the whole vector, in flight while the list is published
                     sm.ids[pos] = l;
                     const uint32_t lp = s_nlog + pos;
                     if (lp < p.vlog_cap) vlog[lp] = l;
@@ -361,7 +377,7 @@
             }
             if (tid == 0) p.out_counts[q] = cnt;
         }
-        if constexpr (CUSTOM == HC_MAXSIM) {
+        if constexpr (hc_multivector(CUSTOM)) {
             if (tid == 0) { const MvShared& ms = mv_shared(); mv_rows += ms.rows; mv_qrows += ms.rows * ms.nqv; }
         }
         // ---- un-set the visited bits this query set
@@ -376,6 +392,6 @@
         __syncthreads();
     }
     if (tid == 0 && p.stats) { atomicAdd(&p.stats[0], hops); atomicAdd(&p.stats[1], evals); }
-    if constexpr (CUSTOM == HC_MAXSIM) {
+    if constexpr (hc_multivector(CUSTOM)) {
         if (tid == 0 && p.stats) { atomicAdd(&p.stats[2], mv_rows); atomicAdd(&p.stats[3], mv_qrows); }
     }

@@ -90,6 +90,19 @@ struct HnswMvBuildParams : HnswParams {
     const uint32_t* tok;   // point p = token rows tok[p] .. tok[p + 1) of the storage
 };
 __device__ __forceinline__ const uint32_t* mv_tok(const HnswMvBuildParams& p) { return p.tok; }
+// A custom query whose examples are multivectors, over a graph of multivector points (CUSTOM == HC_MAXSIM_CUSTOM, hnsw_mv_custom_kernel in
+// qb_hnsw_mv_custom.cu).  Every custom-query field of HnswParams keeps its meaning (kind and shape, n_ex / ex_first / ex_stride, coef,
+// custom entry points), counted in examples rather than encoded vectors: example e of query q is the encoded vectors
+// ex_off[q * ex_stride + ex_first + e] .. [+ 1) of q_enc / q_off.  ex_smem = 1: all of a query's examples are staged in shared memory
+// (q_smem bytes); 0: they are read where they are.
+struct HnswMvCustomParams : HnswParams {
+    const uint32_t* tok;      // point p = token rows tok[p] .. tok[p + 1) of the storage
+    const uint32_t* ex_off;   // [nq * ex_stride + 1] example offsets, ascending
+};
+__device__ __forceinline__ const uint32_t* mv_tok(const HnswMvCustomParams& p) { return p.tok; }
+// the example offsets, named through CUSTOM so that only the HC_MAXSIM_CUSTOM instantiations of the search body read the field
+template <int CUSTOM, class P>
+__device__ __forceinline__ const uint32_t* mv_ex_off(const P& p) { return p.ex_off; }
 
 struct HnswSmem {
     unsigned long long* keys[2];
@@ -101,7 +114,11 @@ struct HnswSmem {
 };
 
 enum { ALGO_HNSW = 0, ALGO_ACORN = 1 };   // qb_hnsw_algorithm
-enum { HC_NEAREST = 0, HC_CUSTOM = 1, HC_MAXSIM = 2 };   // hnsw_search_kernel's CUSTOM: what a query is
+// hnsw_search_kernel's CUSTOM: what a query is.  HC_MAXSIM_CUSTOM: a custom query with multivector examples (HnswMvCustomParams)
+enum { HC_NEAREST = 0, HC_CUSTOM = 1, HC_MAXSIM = 2, HC_MAXSIM_CUSTOM = 3 };
+// queries that take custom entry points (get_entry_point), and queries scored by MaxSim over multivector points
+__host__ __device__ constexpr bool hc_entry_points(int custom) { return custom == HC_CUSTOM || custom == HC_MAXSIM_CUSTOM; }
+__host__ __device__ constexpr bool hc_multivector(int custom) { return custom == HC_MAXSIM || custom == HC_MAXSIM_CUSTOM; }
 enum { ALGO_BUILD = 2 };                  // an insert of qb_hnsw_build: HNSW level search of a stored point, then its links (qb_hnsw_build.cu)
 
 // ALGO_BUILD: a point's row in its level's table
@@ -184,9 +201,67 @@ __device__ __forceinline__ uint32_t mv_find(const uint32_t* pre, uint32_t ns, ui
     return lo;
 }
 
-// MaxSim scores of the points ids[0 .. n) into sc[0 .. n): batches of MV_PTS points, chunks of MV_NQ query vectors; every (point, token
-// row) item of a batch goes to one 8-lane group (dense small dims: one thread), which scores the row against the chunk's vectors by the
-// storage's own chain and folds each similarity into its (point, vector) key.  One thread per point then adds the chunk's maxima in order.
+// The two halves of a MaxSim scoring batch, shared by maxsim_list and maxsim_custom_list as macros, so that maxsim_list expands to the
+// code it had before the custom queries with multivector examples were added.  In scope: p, sm, tid, ms (MvShared&), GROUPS (NT / 8).
+// QB_MV_BATCH(S0, NS): the batch ids[S0 .. S0 + NS): its token-row prefix into ms.pre, its rows counted in ms.rows, ms.sum zeroed.
+#define QB_MV_BATCH(S0, NS)                                                  \
+    if ((uint32_t)tid < (NS)) {                                             \
+        const uint32_t id = sm.ids[(S0) + tid];                             \
+        ms.pre[tid + 1] = mv_tok(p)[id + 1] - mv_tok(p)[id];                \
+        ms.sum[tid] = 0.0f;                                                 \
+    }                                                                       \
+    __syncthreads();                                                        \
+    if (tid == 0) {                                                         \
+        ms.pre[0] = 0;                                                      \
+        for (uint32_t i = 0; i < (NS); ++i) ms.pre[i + 1] += ms.pre[i];     \
+        ms.rows += ms.pre[NS];                                              \
+    }                                                                       \
+    __syncthreads();
+// QB_MV_CHUNKS(Q, QOFF, NQV, S0, NS, ITEMS): the batch's MaxSim against the NQV query vectors at Q (their SQ8 offsets at QOFF, or null)
+// added to ms.sum in vector order: chunks of MV_NQ vectors; every (point, token row) item of the batch goes to one 8-lane group (dense
+// small dims: one thread), which scores the row against the chunk's vectors by the storage's own chain and folds each similarity into its
+// (point, vector) key.  One thread per point then adds the chunk's maxima in order.
+#define QB_MV_CHUNKS(Q, QOFF, NQV, S0, NS, ITEMS)                                                                                         \
+    for (uint32_t c0 = 0; c0 < (NQV); c0 += MV_NQ) {                                                                                      \
+        const uint32_t nc = min((NQV) - c0, MV_NQ);                                                                                       \
+        for (uint32_t i = tid; i < (NS) * MV_NQ; i += NT) ms.key[i] = 0ull;                                                               \
+        __syncthreads();                                                                                                                  \
+        const uint8_t* qc = (Q) + (size_t)c0 * p.q_bytes;                                                                                 \
+        if (KIND == HK_DENSE_SMALL) {                                                                                                     \
+            for (uint32_t k = tid; k < (ITEMS); k += NT) {                                                                                \
+                const uint32_t i = mv_find(ms.pre, (NS), k), tok = k - ms.pre[i], row = mv_tok(p)[sm.ids[(S0) + i]] + tok;                \
+                for (uint32_t j = 0; j < nc; ++j)                                                                                         \
+                    atomicMax(&ms.key[i * MV_NQ + j], mv_key(score_one<KIND, METRIC>(p, qc + (size_t)j * p.q_bytes, 0.0f, row, 0), tok)); \
+            }                                                                                                                             \
+        } else {                                                                                                                          \
+            const int g = tid >> 3, t = tid & 7;                                                                                          \
+            for (uint32_t k = g; k < (((ITEMS) + GROUPS - 1) / GROUPS) * GROUPS; k += GROUPS) { /* whole warps stay converged */         \
+                const uint32_t kk = k < (ITEMS) ? k : 0;                                                                                  \
+                const uint32_t i = mv_find(ms.pre, (NS), kk), tok = kk - ms.pre[i], row = mv_tok(p)[sm.ids[(S0) + i]] + tok;              \
+                float v[MV_NQ];                                                                                                           \
+                if (KIND == HK_DENSE_AVX && nc == MV_NQ) {                                                                                \
+                    score_avx_group8_multi<METRIC, MV_NQ>(reinterpret_cast<const float*>(p.rows + (size_t)row * p.stride),                \
+                                                          reinterpret_cast<const float*>(qc), p.q_bytes / 4, p.dim, t, v);                \
+                } else {                                                                                                                  \
+                    _Pragma("unroll") for (uint32_t j = 0; j < MV_NQ; ++j)                                                                \
+                        if (j < nc) v[j] = score_one<KIND, METRIC>(p, qc + (size_t)j * p.q_bytes, (QOFF) ? (QOFF)[c0 + j] : 0.0f, row, t);\
+                }                                                                                                                         \
+                if (k < (ITEMS) && t == 0) {                                                                                              \
+                    _Pragma("unroll") for (uint32_t j = 0; j < MV_NQ; ++j)                                                                \
+                        if (j < nc) atomicMax(&ms.key[i * MV_NQ + j], mv_key(v[j], tok));                                                 \
+                }                                                                                                                         \
+            }                                                                                                                             \
+        }                                                                                                                                 \
+        __syncthreads();                                                                                                                  \
+        if ((uint32_t)tid < (NS)) {                                                                                                       \
+            float s = ms.sum[tid];                                                                                                        \
+            for (uint32_t j = 0; j < nc; ++j) s = __fadd_rn(s, mv_value(ms.key[tid * MV_NQ + j]));                                        \
+            ms.sum[tid] = s;                                                                                                              \
+        }                                                                                                                                 \
+        __syncthreads();                                                                                                                  \
+    }
+
+// MaxSim scores of the points ids[0 .. n) into sc[0 .. n), in batches of MV_PTS points
 template <int KIND, int METRIC, int NT, class P>
 __device__ __forceinline__ void maxsim_list(const P& p, const HnswSmem& sm, uint32_t n) {
     constexpr uint32_t GROUPS = NT / 8;
@@ -196,60 +271,51 @@ __device__ __forceinline__ void maxsim_list(const P& p, const HnswSmem& sm, uint
     const float* qoff = p.q_off ? p.q_off + ms.q0 : nullptr;
     for (uint32_t s0 = 0; s0 < n; s0 += MV_PTS) {
         const uint32_t ns = min(n - s0, MV_PTS);
-        if ((uint32_t)tid < ns) {
-            const uint32_t id = sm.ids[s0 + tid];
-            ms.pre[tid + 1] = mv_tok(p)[id + 1] - mv_tok(p)[id];
-            ms.sum[tid] = 0.0f;
-        }
-        __syncthreads();
-        if (tid == 0) {
-            ms.pre[0] = 0;
-            for (uint32_t i = 0; i < ns; ++i) ms.pre[i + 1] += ms.pre[i];
-            ms.rows += ms.pre[ns];
-        }
-        __syncthreads();
+        QB_MV_BATCH(s0, ns)
         const uint32_t items = ms.pre[ns];
-        for (uint32_t c0 = 0; c0 < nqv; c0 += MV_NQ) {
-            const uint32_t nc = min(nqv - c0, MV_NQ);
-            for (uint32_t i = tid; i < ns * MV_NQ; i += NT) ms.key[i] = 0ull;
-            __syncthreads();
-            const uint8_t* qc = sm.q + (size_t)c0 * p.q_bytes;
-            if (KIND == HK_DENSE_SMALL) {
-                for (uint32_t k = tid; k < items; k += NT) {
-                    const uint32_t i = mv_find(ms.pre, ns, k), tok = k - ms.pre[i], row = mv_tok(p)[sm.ids[s0 + i]] + tok;
-                    for (uint32_t j = 0; j < nc; ++j)
-                        atomicMax(&ms.key[i * MV_NQ + j], mv_key(score_one<KIND, METRIC>(p, qc + (size_t)j * p.q_bytes, 0.0f, row, 0), tok));
-                }
-            } else {
-                const int g = tid >> 3, t = tid & 7;
-                for (uint32_t k = g; k < ((items + GROUPS - 1) / GROUPS) * GROUPS; k += GROUPS) {   // whole warps stay converged for the shuffles
-                    const uint32_t kk = k < items ? k : 0;
-                    const uint32_t i = mv_find(ms.pre, ns, kk), tok = kk - ms.pre[i], row = mv_tok(p)[sm.ids[s0 + i]] + tok;
-                    float v[MV_NQ];
-                    if (KIND == HK_DENSE_AVX && nc == MV_NQ) {
-                        score_avx_group8_multi<METRIC, MV_NQ>(reinterpret_cast<const float*>(p.rows + (size_t)row * p.stride), reinterpret_cast<const float*>(qc),
-                                                              p.q_bytes / 4, p.dim, t, v);
-                    } else {
-#pragma unroll
-                        for (uint32_t j = 0; j < MV_NQ; ++j)
-                            if (j < nc) v[j] = score_one<KIND, METRIC>(p, qc + (size_t)j * p.q_bytes, qoff ? qoff[c0 + j] : 0.0f, row, t);
-                    }
-                    if (k < items && t == 0) {
-#pragma unroll
-                        for (uint32_t j = 0; j < MV_NQ; ++j)
-                            if (j < nc) atomicMax(&ms.key[i * MV_NQ + j], mv_key(v[j], tok));
-                    }
-                }
-            }
-            __syncthreads();
-            if ((uint32_t)tid < ns) {
-                float s = ms.sum[tid];
-                for (uint32_t j = 0; j < nc; ++j) s = __fadd_rn(s, mv_value(ms.key[tid * MV_NQ + j]));
-                ms.sum[tid] = s;
-            }
-            __syncthreads();
-        }
+        QB_MV_CHUNKS(sm.q, qoff, nqv, s0, ns, items)
         if ((uint32_t)tid < ns) sm.sc[s0 + tid] = ms.sum[tid];
+        __syncthreads();
+    }
+}
+
+// ---- custom queries with multivector examples (MultiCustomQueryScorer, multi_custom_query_scorer.rs:88-104): a point's similarity to
+// example e is the MaxSim of e's vectors against its token rows, exactly as maxsim_list computes it; Query::score_by folds the E values
+// (qbf::fold).  A batch keeps every point's E MaxSims in mv_custom_tab() as [point][e], so it holds at most MV_TAB / E points.
+constexpr uint32_t MV_TAB = 4096;   // floats of the [point][example] table: 16 KB, one point at E = 4096
+__host__ __device__ constexpr uint32_t mv_custom_batch(uint32_t n_ex) { return n_ex * MV_PTS <= MV_TAB ? MV_PTS : MV_TAB / n_ex; }
+// one per CTA; only the HC_MAXSIM_CUSTOM instantiations reference it
+__device__ __forceinline__ float* mv_custom_tab() {
+    __shared__ float tab[MV_TAB];
+    return tab;
+}
+
+// the scores of the points ids[0 .. n) for custom query q into sc[0 .. n); sm.q holds the query's first example from its first vector on
+template <int KIND, int METRIC, int NT>
+__device__ __forceinline__ void maxsim_custom_list(const HnswMvCustomParams& p, const HnswSmem& sm, uint32_t n, uint32_t q) {
+    constexpr uint32_t GROUPS = NT / 8;
+    MvShared& ms = mv_shared();
+    float* tab = mv_custom_tab();
+    const int tid = threadIdx.x;
+    const uint32_t ne = p.n_ex, bp = mv_custom_batch(ne);
+    const uint32_t* eo = p.ex_off + (size_t)q * p.ex_stride + p.ex_first;
+    const uint32_t v0 = eo[0];
+    for (uint32_t s0 = 0; s0 < n; s0 += bp) {
+        const uint32_t ns = min(n - s0, bp);
+        QB_MV_BATCH(s0, ns)
+        const uint32_t items = ms.pre[ns];
+        for (uint32_t e = 0; e < ne; ++e) {
+            const uint32_t a = eo[e], nv = eo[e + 1] - a;
+            const uint8_t* qe = sm.q + (size_t)(a - v0) * p.q_bytes;
+            const float* qoff = p.q_off ? p.q_off + a : nullptr;
+            if ((uint32_t)tid < ns) ms.sum[tid] = 0.0f;   // ordered before the sums by the chunks' first barrier
+            QB_MV_CHUNKS(qe, qoff, nv, s0, ns, items)
+            if ((uint32_t)tid < ns) tab[tid * ne + e] = ms.sum[tid];
+        }
+        if ((uint32_t)tid < ns) {
+            const float* row = tab + tid * ne;
+            sm.sc[s0 + tid] = qbf::fold(p.ckind, p.n_a, p.n_b, p.coef ? p.coef + (size_t)q * p.n_coef : nullptr, [&](uint32_t e) { return row[e]; });
+        }
         __syncthreads();
     }
 }
@@ -261,6 +327,8 @@ __device__ __forceinline__ void score_list(const P& p, const HnswSmem& sm, float
     const int tid = threadIdx.x;
     if constexpr (CUSTOM == HC_MAXSIM) {
         maxsim_list<KIND, METRIC, NT>(p, sm, n);
+    } else if constexpr (CUSTOM == HC_MAXSIM_CUSTOM) {
+        maxsim_custom_list<KIND, METRIC, NT>(p, sm, n, q);
     } else if (hk_one_thread(KIND)) {
         if ((uint32_t)tid < n) sm.sc[tid] = score_q<KIND, METRIC, CUSTOM>(p, sm, q_off, sm.ids[tid], 0, q);
     } else {
@@ -551,3 +619,9 @@ inline size_t hnsw_smem_bytes(uint32_t q_bytes, uint32_t ef) {
 }
 
 }  // namespace
+
+// The custom queries with multivector examples (qb_hnsw_mv_custom.cu): `params` is qb_hnsw_launch's HnswParams in this header's layout,
+// passed untyped because the type has internal linkage; the kernel's HnswMvCustomParams add d_tok and d_ex_off to it.  per_sm != null:
+// nothing is launched, *per_sm receives the kernel's resident CTAs per SM at smem bytes of dynamic shared memory.
+qb_status qb_hnsw_mv_custom_launch(const void* params, const uint32_t* d_tok, const uint32_t* d_ex_off, int kind, int metric, int algo, unsigned grid,
+                                   size_t smem, cudaStream_t stream, int* per_sm);

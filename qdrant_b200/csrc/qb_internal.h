@@ -163,7 +163,9 @@ struct qb_hnsw {
 };
 
 // A batch of multivector queries for qb_hnsw_launch: query q = encoded query vectors d_qoff[q] .. d_qoff[q + 1) (device) of the n_vectors
-// that d_q_enc / d_q_off hold; max_q bounds a query's vector count for the shared-memory staging (a larger query is read from HBM)
+// that d_q_enc / d_q_off hold; max_q bounds a query's vector count for the shared-memory staging (a larger query is read from HBM).
+// Given together with a QbHnswCustom, the batch is of custom queries with multivector examples: example e of query q is the encoded vectors
+// d_qoff[q * ex_stride + e] .. [+ 1), and max_q bounds the vectors of all of one query's examples.
 struct QbHnswMaxsim {
     const uint32_t* d_qoff; uint32_t n_vectors, max_q;
 };
@@ -175,7 +177,7 @@ struct QbHnswCustom {
     uint32_t n_ex, ex_first, ex_stride;
     const float* d_coef; uint32_t n_coef;        // feedback: [a, partial...] per query, else null / 0
     const qb_scored_point* d_cep; const uint32_t* d_cep_counts; uint32_t n_cep;
-    uint32_t stats_slot;                         // hops / scored points go to stats slot 0 or 1 (qb_hnsw_read_stats)
+    uint32_t stats_slot;                         // hops / scored points go to stats slot 0 or 1 (qb_hnsw_read_stats); multivector examples: the MaxSim slot
     bool internal_out;                           // results as point offsets, without the storage's id_base (discover's context stage)
 };
 

@@ -313,6 +313,32 @@ public:
                                             nullptr, static_cast<qb_hnsw_algorithm>(algorithm)));
         return split(flat, counts, top);
     }
+    // custom queries whose examples are multivectors, on a multivector graph (qb_hnsw_search_maxsim_custom_batch): example j of query q =
+    // rows [example_offsets[q * E + j], example_offsets[q * E + j + 1]) of example_vectors; the rest as search_custom; deleted: over points
+    std::vector<std::vector<ScoredPointOffset>> search_maxsim_custom(qb_query_kind kind, const float* example_vectors, const uint32_t* example_offsets,
+                                                                     uint32_t n_a, uint32_t n_b, const float* coef, uint32_t n_queries, uint32_t top,
+                                                                     uint32_t ef, PointOffsetType entry_point, uint32_t entry_level,
+                                                                     const uint32_t* custom_entry_points = nullptr, const uint32_t* custom_counts = nullptr,
+                                                                     uint32_t n_custom = 0, const uint64_t* deleted = nullptr,
+                                                                     SearchAlgorithm algorithm = SearchAlgorithm::Hnsw) const {
+        std::vector<ScoredPointOffset> flat((size_t)n_queries * top);
+        std::vector<uint32_t> counts(n_queries);
+        check(qb_hnsw_search_maxsim_custom_batch(h_, kind, example_vectors, example_offsets, n_a, n_b, coef, n_queries, top, ef, entry_point, entry_level,
+                                                 custom_entry_points, custom_counts, n_custom, deleted, nullptr, flat.data(), counts.data(), nullptr,
+                                                 static_cast<qb_hnsw_algorithm>(algorithm)));
+        return split(flat, counts, top);
+    }
+    // discover with multivector examples, both stages in one call (qb_hnsw_search_maxsim_discover_batch); E = 1 + 2 n_pairs
+    std::vector<std::vector<ScoredPointOffset>> search_maxsim_discover(const float* example_vectors, const uint32_t* example_offsets, uint32_t n_pairs,
+                                                                       uint32_t n_queries, uint32_t top, uint32_t ef, PointOffsetType entry_point,
+                                                                       uint32_t entry_level, const uint64_t* deleted = nullptr,
+                                                                       SearchAlgorithm algorithm = SearchAlgorithm::Hnsw) const {
+        std::vector<ScoredPointOffset> flat((size_t)n_queries * top);
+        std::vector<uint32_t> counts(n_queries);
+        check(qb_hnsw_search_maxsim_discover_batch(h_, example_vectors, example_offsets, n_pairs, n_queries, top, ef, entry_point, entry_level, deleted,
+                                                   nullptr, flat.data(), counts.data(), nullptr, static_cast<qb_hnsw_algorithm>(algorithm)));
+        return split(flat, counts, top);
+    }
 
 private:
     static std::vector<std::vector<ScoredPointOffset>> split(const std::vector<ScoredPointOffset>& flat, const std::vector<uint32_t>& counts, uint32_t top) {

@@ -564,6 +564,25 @@ def postprocess_search_result(search_result: np.ndarray, original: DenseVectorSt
 
 
 # ------------------------------------------------------------------------------------------------ multivectors
+def _multi_rows(vectors, dim: int) -> np.ndarray:
+    q = np.atleast_2d(_f32(vectors))
+    if q.shape[1] != dim:
+        raise ValueError(f"query vectors have dim {q.shape[1]}, storage has {dim}")
+    return np.ascontiguousarray(q)
+
+
+def _flat_multi(query, dim: int):
+    """a custom query whose examples are 2-D arrays (vectors x dim) -> (example vectors, example offsets, n_a, n_b, coef or None), the
+    examples in the qb_scorer_create_custom order"""
+    examples, n_a, n_b = query.flat()
+    mats = [_multi_rows(e, dim) for e in examples]
+    off = np.concatenate([[0], np.cumsum([m.shape[0] for m in mats])]).astype(np.uint32)
+    coef = None
+    if query.kind == QueryKind.FeedbackNaive:
+        coef = np.concatenate([[np.float32(query.a)], query.partial]).astype(np.float32)
+    return np.ascontiguousarray(np.concatenate(mats)), off, n_a, n_b, coef
+
+
 class MultiVectorView:
     """A multivector collection over a token-level storage: point p = rows [offsets[p], offsets[p+1]) (the flattened layout of
     vector_storage/multi_dense).  Scores are ColBERT MaxSim (score_max_similarity, query_scorer/mod.rs:77-98)."""
@@ -575,10 +594,7 @@ class MultiVectorView:
         self.n_points = self.offsets.size - 1
 
     def _query(self, query_vectors) -> np.ndarray:
-        q = np.atleast_2d(_f32(query_vectors))
-        if q.shape[1] != self.storage.dim:
-            raise ValueError(f"query vectors have dim {q.shape[1]}, storage has {self.storage.dim}")
-        return np.ascontiguousarray(q)
+        return _multi_rows(query_vectors, self.storage.dim)
 
     def search(self, query_vectors, top: int, point_deleted=None, counters: Optional[HwCounters] = None) -> np.ndarray:
         q = self._query(query_vectors)
@@ -601,13 +617,7 @@ class MultiVectorView:
     # ---- custom queries whose examples are multivectors (MultiCustomQueryScorer, multi_custom_query_scorer.rs:88-104).  `query` is one of the
     # query classes above with 2-D arrays (vectors x dim) in place of vectors.
     def _flat_multi(self, query):
-        examples, n_a, n_b = query.flat()
-        mats = [self._query(e) for e in examples]
-        off = np.concatenate([[0], np.cumsum([m.shape[0] for m in mats])]).astype(np.uint32)
-        coef = None
-        if query.kind == QueryKind.FeedbackNaive:
-            coef = np.concatenate([[np.float32(query.a)], query.partial]).astype(np.float32)
-        return np.ascontiguousarray(np.concatenate(mats)), off, n_a, n_b, coef
+        return _flat_multi(query, self.storage.dim)
 
     def search_custom(self, query, top: int, point_deleted=None) -> np.ndarray:
         vecs, off, n_a, n_b, coef = self._flat_multi(query)
@@ -982,17 +992,7 @@ class HnswGraph:
         ex = self._examples(examples, n_ex) if n_ex else _f32(examples)
         nq = ex.shape[0] if n_ex else 0
         cf = None if coef is None else np.ascontiguousarray(_f32(coef).reshape(nq, -1))
-        cep_arr = cep_cnt = None
-        width = 0
-        if custom_entry_points is not None:
-            if len(custom_entry_points) != nq:
-                raise ValueError(f"custom_entry_points has {len(custom_entry_points)} lists for {nq} queries")
-            width = max(1, max((len(c) for c in custom_entry_points), default=1))
-            cep_arr = np.zeros((nq, width), np.uint32)
-            cep_cnt = np.zeros(nq, np.uint32)
-            for i, c in enumerate(custom_entry_points):
-                cep_arr[i, : len(c)] = np.asarray(c, dtype=np.uint32)
-                cep_cnt[i] = len(c)
+        cep_arr, cep_cnt, width = self._entry_lists(custom_entry_points, nq)
         out = np.zeros((max(nq, 1), max(top, 1)), dtype=SCORED_POINT_OFFSET)
         counts = np.zeros(max(nq, 1), dtype=np.uint32)
         bm = _bitmap(point_deleted, self._storage.count)
@@ -1001,6 +1001,79 @@ class HnswGraph:
                                                 None if cep_arr is None else cep_arr.ctypes.data_as(u32p), None if cep_cnt is None else cep_cnt.ctypes.data_as(u32p),
                                                 width, None if bm is None else bm.ctypes.data_as(u64p), None, out.ctypes.data_as(C.POINTER(ScoredPoint)),
                                                 counts.ctypes.data_as(u32p), None if counters is None else C.byref(counters), self.ALGORITHMS[algorithm]))
+        return [out[i, : counts[i]].copy() for i in range(nq)]
+
+    @staticmethod
+    def _entry_lists(custom_entry_points, nq: int):
+        """one sequence of point offsets per query -> ([nq, width] u32, counts u32, width), or (None, None, 0)"""
+        if custom_entry_points is None:
+            return None, None, 0
+        if len(custom_entry_points) != nq:
+            raise ValueError(f"custom_entry_points has {len(custom_entry_points)} lists for {nq} queries")
+        width = max(1, max((len(c) for c in custom_entry_points), default=1))
+        cep_arr = np.zeros((nq, width), np.uint32)
+        cep_cnt = np.zeros(nq, np.uint32)
+        for i, c in enumerate(custom_entry_points):
+            cep_arr[i, : len(c)] = np.asarray(c, dtype=np.uint32)
+            cep_cnt[i] = len(c)
+        return cep_arr, cep_cnt, width
+
+    def _multi_batch(self, queries):
+        """custom queries with multivector examples -> (kind, n_a, n_b, example vectors, example offsets, coef [nq, 1 + n_a] or None);
+        one kind and one shape per batch"""
+        flat = [_flat_multi(q, self._storage.dim) for q in queries]
+        if not flat:
+            return int(QueryKind.RecommendBestScore), 1, 0, np.zeros((0, self._storage.dim), np.float32), np.zeros(1, np.uint32), None
+        kind, n_a, n_b = int(queries[0].kind), flat[0][2], flat[0][3]
+        for q, f in zip(queries, flat):
+            if int(q.kind) != kind or (f[2], f[3]) != (n_a, n_b):
+                raise ValueError("one query kind and one shape (n_a, n_b) per call")
+        base = np.cumsum([0] + [f[0].shape[0] for f in flat[:-1]])
+        off = np.concatenate([f[1][:-1] + b for f, b in zip(flat, base)] + [[base[-1] + flat[-1][1][-1]]]).astype(np.uint32)
+        coef = np.stack([f[4] for f in flat]) if kind == QueryKind.FeedbackNaive else None
+        return kind, n_a, n_b, np.ascontiguousarray(np.concatenate([f[0] for f in flat])), off, coef
+
+    def search_maxsim_custom(self, queries, top: int, ef: int, entry_point: int, entry_level: int, point_deleted=None,
+                             counters: Optional[HwCounters] = None, custom_entry_points=None, algorithm: str = "hnsw"):
+        """Custom queries whose examples are multivectors, on a multivector() graph (qb_hnsw_search_maxsim_custom_batch).  queries: a list of
+        RecoBestScoreQuery / RecoSumScoresQuery / ContextQuery / FeedbackQuery / DiscoverQuery (one discover search) whose vectors are
+        [vectors, dim] arrays, all of one kind and shape; custom_entry_points: one sequence of point offsets per query, or None;
+        point_deleted: over points.  Returns one list of point offsets per query; a score equals MultiVectorView.score_points_custom."""
+        if algorithm not in self.ALGORITHMS:
+            raise ValueError(f"algorithm {algorithm!r} is not one of {sorted(self.ALGORITHMS)}")
+        kind, n_a, n_b, vecs, off, coef = self._multi_batch(queries)
+        nq = len(queries)
+        cep_arr, cep_cnt, width = self._entry_lists(custom_entry_points, nq)
+        out = np.zeros((max(nq, 1), max(top, 1)), dtype=SCORED_POINT_OFFSET)
+        counts = np.zeros(max(nq, 1), dtype=np.uint32)
+        bm = _bitmap(point_deleted, self.info()[0])
+        check(lib().qb_hnsw_search_maxsim_custom_batch(self._h, kind, vecs.ctypes.data_as(f32p), off.ctypes.data_as(u32p), int(n_a), int(n_b),
+                                                       None if coef is None else coef.ctypes.data_as(f32p), nq, int(top), int(ef), int(entry_point),
+                                                       int(entry_level), None if cep_arr is None else cep_arr.ctypes.data_as(u32p),
+                                                       None if cep_cnt is None else cep_cnt.ctypes.data_as(u32p), width,
+                                                       None if bm is None else bm.ctypes.data_as(u64p), None, out.ctypes.data_as(C.POINTER(ScoredPoint)),
+                                                       counts.ctypes.data_as(u32p), None if counters is None else C.byref(counters),
+                                                       self.ALGORITHMS[algorithm]))
+        return [out[i, : counts[i]].copy() for i in range(nq)]
+
+    def search_maxsim_discover(self, queries, top: int, ef: int, entry_point: int, entry_level: int, point_deleted=None,
+                               counters: Optional[HwCounters] = None, algorithm: str = "hnsw"):
+        """Discover with multivector examples as the reference runs it on an indexed segment (qb_hnsw_search_maxsim_discover_batch): a
+        context search over the pairs for 10 entry points, then the discover search from them, in one call.  queries: DiscoverQuery
+        objects with [vectors, dim] arrays, all with the same number of pairs."""
+        if algorithm not in self.ALGORITHMS:
+            raise ValueError(f"algorithm {algorithm!r} is not one of {sorted(self.ALGORITHMS)}")
+        if any(int(q.kind) != QueryKind.Discover for q in queries):
+            raise ValueError("search_maxsim_discover takes DiscoverQuery objects")
+        _, n_pairs, _, vecs, off, _ = self._multi_batch(queries)
+        nq = len(queries)
+        out = np.zeros((max(nq, 1), max(top, 1)), dtype=SCORED_POINT_OFFSET)
+        counts = np.zeros(max(nq, 1), dtype=np.uint32)
+        bm = _bitmap(point_deleted, self.info()[0])
+        check(lib().qb_hnsw_search_maxsim_discover_batch(self._h, vecs.ctypes.data_as(f32p), off.ctypes.data_as(u32p), int(n_pairs), nq, int(top), int(ef),
+                                                         int(entry_point), int(entry_level), None if bm is None else bm.ctypes.data_as(u64p), None,
+                                                         out.ctypes.data_as(C.POINTER(ScoredPoint)), counts.ctypes.data_as(u32p),
+                                                         None if counters is None else C.byref(counters), self.ALGORITHMS[algorithm]))
         return [out[i, : counts[i]].copy() for i in range(nq)]
 
     def search_discover(self, examples, n_pairs: int, top: int = 10, ef: int = 64, entry_point: int = 0, entry_level: int = 0, point_deleted=None,
