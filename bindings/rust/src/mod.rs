@@ -4,3 +4,4 @@ pub mod raw_scorer;      // impl RawScorer / RawScorerBuilder
 pub mod batch_searcher;  // BatchFilteredSearcher::peek_top_* + oversample / rescore
 pub mod hnsw;            // GraphLayers::search, batched, traversal on the device
 pub mod sharded;         // per-GPU segments + device-side BatchResultAggregator
+pub mod mmr;             // maximal marginal relevance reranking

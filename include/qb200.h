@@ -644,6 +644,41 @@ QB_API qb_status qb_hnsw_search_discover_batch(qb_hnsw* g, const float* vectors,
                                                const volatile int32_t* is_stopped, qb_scored_point* out, uint32_t* out_counts,
                                                qb_hw_counters* counters /* optional */, qb_hnsw_algorithm algorithm);
 
+/* ---------------------------------------------------------------- MMR reranking ---------------------- */
+/* Maximal marginal relevance, the diversity rerank of the universal query API, for dense vectors: mmr_from_points_with_vector +
+ * maximal_marginal_relevance (lib/shard/src/query/mmr/mod.rs:42-279) with its LazyMatrix (lazy_matrix.rs:25-68).
+ *   s           the storage of the candidates' vectors: dense f32 of the collection's distance, rows as they are (the reference's volatile
+ *               storage does not preprocess them, volatile_dense_vector_storage.rs:170-182) — a temporary storage the caller fills with
+ *               the candidates' vectors, or the resident segment storage whose rows are the vectors `with_vector` returns.  Others:
+ *               QB_ERR_UNSUPPORTED
+ *   queries     n_queries x dim raw f32 (Metric::preprocess on the device, as qb_scorer_create)
+ *   lambdas     one per query: 1 - diversity, in [0, 1] (NaN or outside: QB_ERR_INVALID)
+ *   candidates  n_queries x max_candidates, candidate_counts[q] of them valid: the layout qb_search_batch* / qb_hnsw_search_batch* return
+ *               with top = max_candidates.  Ids in the storage's numbering (id_base included); max_candidates <= 16384 (candidates_limit's
+ *               cap, api/src/rest/schema.rs:771), else QB_ERR_UNSUPPORTED
+ *   out         n_queries x limit: the selected candidates in selection order with their ORIGINAL scores; out_counts[q] of them
+ * Per query: unique_by(id) keeps the first occurrence; 0 or 1 candidates left are returned as they are (no scoring, no truncation).
+ * Otherwise rel[i] = sim(preprocess(query), v_i) (qb_score_points on qb_scorer_create(s, query)), pair(c, t) = sim(preprocess(v_c), v_t)
+ * (candidate c's scorer, lazy_matrix.rs:45-52), the first pick is the argmax of rel, and each later pick the argmax over the remaining
+ * candidates of lambda * rel - (1 - lambda) * (max over the picks so far, in pick order, of pair(c, pick)), four f32 operations each
+ * rounded; until `limit` picks or none remain.  Every max / argmax is max_by_key(OrderedFloat): the last maximal element wins, NaN is above
+ * everything and equal to NaN, -0.0 equals +0.0.  Remaining candidates are in IndexSet order and a pick is swap_remove-d (the last
+ * remaining one takes its position), so ties go to the later current position.  Scores are bit-exact with the reference's f32 chains.
+ * Counters: cpu += dim * 4 * (n + sum over k = 1 .. L-1 of (n - k)) per query of n >= 2 unique candidates and L picks (the relevance
+ * pass, then one pair per remaining candidate and later pick); vector_io_read += 0 (the volatile storage is never on disk).
+ * Errors, checked before any device work: a null argument, limit = 0, a lambda outside [0, 1], candidate_counts[q] > max_candidates or
+ * an id outside the storage: QB_ERR_INVALID.  Synchronous. */
+QB_API qb_status qb_mmr_batch(qb_storage* s, const float* queries, uint32_t n_queries, const float* lambdas, const qb_scored_point* candidates,
+                              const uint32_t* candidate_counts, uint32_t max_candidates, uint32_t limit, qb_scored_point* out, uint32_t* out_counts,
+                              qb_hw_counters* counters /* optional */);
+/* same with every array resident in HBM, enqueued on qb_storage_stream(s) with no host synchronisation, so it chains after
+ * qb_search_batch_device / qb_hnsw_search_batch_device on the same storage (top = max_candidates).  The host checks the storage,
+ * max_candidates and limit; lambdas and ids stay on the device unchecked: a count above max_candidates is clamped to it and an id outside
+ * the storage is dropped from its list.  dev_out is n_queries x limit. */
+QB_API qb_status qb_mmr_batch_device(qb_storage* s, const float* dev_queries, uint32_t n_queries, const float* dev_lambdas,
+                                     const qb_scored_point* dev_candidates, const uint32_t* dev_candidate_counts, uint32_t max_candidates,
+                                     uint32_t limit, qb_scored_point* dev_out, uint32_t* dev_out_counts);
+
 /* ---------------------------------------------------------------- profiling hooks ------------------- */
 /* Fused searches run a fast path first and rerun without it when the device reports that one of its assumptions did not
  * hold (candidate buffer overflow, a dot product outside the f32-exact window, a survivor segment full).  searches =

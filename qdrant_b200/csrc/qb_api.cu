@@ -213,7 +213,7 @@ static void ctx_destroy(QbSearchCtx* c) {
     if (!c) return;
     if (c->stream) cudaStreamSynchronize(c->stream);
     cudaFree(c->d_queries_raw); cudaFree(c->d_queries_enc); cudaFree(c->d_q_off); cudaFree(c->d_thr); cudaFree(c->d_cnt); cudaFree(c->d_done);
-    cudaFree(c->d_cand); cudaFree(c->d_out); cudaFree(c->d_out_counts); cudaFree(c->d_deleted2); cudaFree(c->d_ids); cudaFree(c->d_mma); cudaFree(c->d_pf); cudaFree(c->d_pf_up5);
+    cudaFree(c->d_cand); cudaFree(c->d_out); cudaFree(c->d_out_counts); cudaFree(c->d_deleted2); cudaFree(c->d_ids); cudaFree(c->d_mma); cudaFree(c->d_pf); cudaFree(c->d_pf_up5); cudaFree(c->d_mmr);
     if (c->h_stage) cudaFreeHost(c->h_stage);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
@@ -985,6 +985,114 @@ extern "C" qb_status qb_search_batch_device(qb_storage* s, const float* dev_quer
     // reading the flags word of the reruns is the one synchronisation of this call
     QB_TRY(qb_ensure_pinned(&c->h_stage, &c->h_stage_bytes, 64));
     return search_with_reruns(s, c, n_queries, top, nullptr, 0, nullptr, nullptr, dev_out, dev_counts, d_flags, reinterpret_cast<uint8_t*>(c->h_stage));
+}
+
+// ------------------------------------------------------------------------------------------------ MMR reranking
+constexpr uint32_t QB_MMR_MAX_CANDIDATES = 16384;   // candidates_limit's cap (api/src/rest/schema.rs:771); positions are u16 on the device
+
+// the checks both MMR entries make on the host before any device work
+static qb_status mmr_check(const qb_storage* s, uint32_t max_candidates, uint32_t limit, const char* who) {
+    QB_CHECK(s->kind == QB_KIND_DENSE && s->dtype == QB_DT_F32, QB_ERR_UNSUPPORTED, "%s: the storage must be dense f32 (the reference scores MMR on a volatile f32 storage)", who);
+    QB_CHECK(max_candidates <= QB_MMR_MAX_CANDIDATES, QB_ERR_UNSUPPORTED, "%s: max_candidates %u > %u", who, max_candidates, QB_MMR_MAX_CANDIDATES);
+    QB_CHECK(limit >= 1, QB_ERR_INVALID, "%s: limit must be >= 1", who);
+    return QB_OK;
+}
+
+// c->d_mmr = [out counts nq | unique counts nq | candidates nq x max | counts nq | lambdas nq | selections nq x out_stride | Cosine scratch]
+struct MmrLayout {
+    size_t cand_at, counts_at, lambdas_at, out_at, scratch_at, bytes;
+    MmrLayout(const qb_storage* s, uint32_t nq, uint32_t max_cand, uint32_t out_stride) {
+        cand_at = round_up_u64((size_t)nq * 8, 16);
+        counts_at = cand_at + (size_t)nq * max_cand * sizeof(qb_scored_point);
+        lambdas_at = counts_at + (size_t)nq * 4;
+        out_at = round_up_u64(lambdas_at + (size_t)nq * 4, 16);
+        scratch_at = round_up_u64(out_at + (size_t)nq * out_stride * sizeof(qb_scored_point), 256);
+        bytes = scratch_at + qb_mmr_scratch_bytes(s, nq, max_cand);
+    }
+};
+
+// cpu units of one query's MMR (mod.rs:82-98): n relevance scores, then one pair score per remaining candidate and later pick (the lazy
+// matrix computes each (candidate, newest pick) pair once); nothing for fewer than two candidates
+static uint64_t mmr_cpu_units(const qb_storage* s, uint64_t n, uint64_t picked) {
+    if (n < 2) return 0;
+    const uint64_t pairs = picked > 1 ? (picked - 1) * n - (picked - 1) * picked / 2 : 0;
+    return (uint64_t)s->dim * 4 * (n + pairs);
+}
+
+extern "C" qb_status qb_mmr_batch(qb_storage* s, const float* queries, uint32_t n_queries, const float* lambdas, const qb_scored_point* candidates,
+                                  const uint32_t* candidate_counts, uint32_t max_candidates, uint32_t limit, qb_scored_point* out, uint32_t* out_counts,
+                                  qb_hw_counters* counters) {
+    QB_CHECK(s && out_counts && (out || n_queries == 0), QB_ERR_INVALID, "mmr_batch: null argument");
+    QB_CHECK(n_queries == 0 || (queries && lambdas && candidate_counts && (candidates || max_candidates == 0)), QB_ERR_INVALID, "mmr_batch: null argument");
+    QB_TRY(mmr_check(s, max_candidates, limit, "mmr_batch"));
+    uint32_t n_max = 0;
+    for (uint32_t q = 0; q < n_queries; ++q) {
+        const float l = lambdas[q];
+        QB_CHECK(l >= 0.0f && l <= 1.0f, QB_ERR_INVALID, "mmr_batch: lambda %g of query %u outside [0, 1]", (double)l, q);
+        QB_CHECK(candidate_counts[q] <= max_candidates, QB_ERR_INVALID, "mmr_batch: %u candidates for query %u > max_candidates %u", candidate_counts[q], q, max_candidates);
+        n_max = std::max(n_max, candidate_counts[q]);
+        for (uint32_t i = 0; i < candidate_counts[q]; ++i) {
+            const uint32_t id = candidates[(size_t)q * max_candidates + i].idx;
+            QB_CHECK(id >= s->id_base && (uint64_t)(id - s->id_base) < s->count, QB_ERR_INVALID, "mmr_batch: id %u out of range [%u, %llu)", id, s->id_base,
+                     (unsigned long long)s->id_base + s->count);
+        }
+    }
+    if (n_queries == 0) return QB_OK;
+    QB_TRY(use_device(s->device));
+    CtxLease lease;
+    QB_TRY(lease.acquire(s));
+    QbSearchCtx* c = lease.c;
+    const uint32_t out_stride = std::max<uint32_t>(1, std::min(limit, max_candidates));
+    const MmrLayout lay(s, n_queries, max_candidates, out_stride);
+    // stage tail: the inputs [candidates | counts | lambdas] going up, then [selections | out counts | unique counts] coming back
+    const size_t up = lay.out_at - lay.cand_at, down = (size_t)n_queries * out_stride * sizeof(qb_scored_point) + (size_t)n_queries * 8;
+    uint8_t* h_tail = nullptr;
+    QB_TRY(stage_queries(s, c, queries, n_queries, std::max(up, down), &h_tail));
+    const size_t cand_bytes = (size_t)n_queries * max_candidates * sizeof(qb_scored_point);
+    if (cand_bytes) memcpy(h_tail, candidates, cand_bytes);
+    memcpy(h_tail + (lay.counts_at - lay.cand_at), candidate_counts, (size_t)n_queries * 4);
+    memcpy(h_tail + (lay.lambdas_at - lay.cand_at), lambdas, (size_t)n_queries * 4);
+    QB_TRY(qb_ensure_device(&c->d_mmr, &c->mmr_bytes, lay.bytes));
+    uint8_t* d = reinterpret_cast<uint8_t*>(c->d_mmr);
+    QB_CUDA(cudaMemcpyAsync(d + lay.cand_at, h_tail, up, cudaMemcpyHostToDevice, c->stream));
+    uint32_t* d_counts = reinterpret_cast<uint32_t*>(d);
+    QB_TRY(qb_mmr_launch(s, reinterpret_cast<const float*>(c->d_queries_enc), n_queries, reinterpret_cast<const float*>(d + lay.lambdas_at),
+                         reinterpret_cast<const qb_scored_point*>(d + lay.cand_at), reinterpret_cast<const uint32_t*>(d + lay.counts_at), max_candidates, n_max,
+                         limit, reinterpret_cast<qb_scored_point*>(d + lay.out_at), out_stride, d_counts, d_counts + n_queries,
+                         reinterpret_cast<float*>(d + lay.scratch_at), c->stream));
+    const size_t res_bytes = (size_t)n_queries * out_stride * sizeof(qb_scored_point);
+    QB_CUDA(cudaMemcpyAsync(h_tail, d + lay.out_at, res_bytes, cudaMemcpyDeviceToHost, c->stream));
+    QB_CUDA(cudaMemcpyAsync(h_tail + res_bytes, d_counts, (size_t)n_queries * 8, cudaMemcpyDeviceToHost, c->stream));
+    QB_CUDA(cudaStreamSynchronize(c->stream));
+    const qb_scored_point* h_res = reinterpret_cast<const qb_scored_point*>(h_tail);
+    const uint32_t* h_cnt = reinterpret_cast<const uint32_t*>(h_tail + res_bytes);
+    for (uint32_t q = 0; q < n_queries; ++q) {
+        out_counts[q] = h_cnt[q];
+        memcpy(out + (size_t)q * limit, h_res + (size_t)q * out_stride, (size_t)h_cnt[q] * sizeof(qb_scored_point));
+        if (counters) counters->cpu += mmr_cpu_units(s, h_cnt[n_queries + q], h_cnt[q]);   // vector_io_read: the volatile storage is never on disk
+    }
+    return QB_OK;
+}
+
+extern "C" qb_status qb_mmr_batch_device(qb_storage* s, const float* dev_queries, uint32_t n_queries, const float* dev_lambdas,
+                                         const qb_scored_point* dev_candidates, const uint32_t* dev_candidate_counts, uint32_t max_candidates, uint32_t limit,
+                                         qb_scored_point* dev_out, uint32_t* dev_out_counts) {
+    QB_CHECK(s, QB_ERR_INVALID, "mmr_batch_device: null argument");
+    QB_CHECK(n_queries == 0 || (dev_queries && dev_lambdas && dev_candidate_counts && dev_out && dev_out_counts && (dev_candidates || max_candidates == 0)),
+             QB_ERR_INVALID, "mmr_batch_device: null argument");
+    QB_TRY(mmr_check(s, max_candidates, limit, "mmr_batch_device"));
+    if (n_queries == 0) return QB_OK;
+    QB_TRY(use_device(s->device));
+    QbSearchCtx* c = nullptr;
+    QB_TRY(qb_ctx_device(s, &c));
+    QB_TRY(encode_device_queries(s, c, dev_queries, n_queries));
+    // c->d_mmr = [unique counts nq | Cosine scratch]; the counts are not read back
+    const size_t scratch_at = round_up_u64((size_t)n_queries * 4, 256);
+    QB_TRY(qb_ensure_device(&c->d_mmr, &c->mmr_bytes, scratch_at + qb_mmr_scratch_bytes(s, n_queries, max_candidates)));
+    uint8_t* d = reinterpret_cast<uint8_t*>(c->d_mmr);
+    return qb_mmr_launch(s, reinterpret_cast<const float*>(c->d_queries_enc), n_queries, dev_lambdas, dev_candidates, dev_candidate_counts, max_candidates,
+                         max_candidates, limit, dev_out, limit, dev_out_counts, reinterpret_cast<uint32_t*>(d), reinterpret_cast<float*>(d + scratch_at),
+                         c->stream);
 }
 
 // ------------------------------------------------------------------------------------------------ RawScorer

@@ -34,6 +34,7 @@ struct QbSearchCtx {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     bool in_use = false;
     unsigned int* d_done = nullptr;      // arrival counter of the single-query in-kernel top-k (zeroed once, the kernel resets it)
+    void* d_mmr = nullptr;           size_t mmr_bytes = 0;           // MMR reranking (qb_mmr.cu): host inputs / outputs and Cosine scratch
 };
 
 struct qb_storage {
@@ -279,6 +280,14 @@ qb_status qb_launch_select(const unsigned long long* d_cand, const unsigned int*
                            qb_scored_point* d_out, uint32_t* d_out_counts, float* d_thr, unsigned int* d_overflow,
                            cudaStream_t stream);
 qb_status qb_launch_fill_u32(unsigned int* p, unsigned int v, size_t n, cudaStream_t stream);
+
+// MMR reranking (qb_mmr.cu): nq lists of up to max_cand candidates (n_max bounds the counts), queries preprocessed ([nq][row_stride / 4]);
+// selections to d_out[q * out_stride ..), their number to d_out_counts, the candidates left after the dedup to d_n_unique.  d_scratch:
+// qb_mmr_scratch_bytes (Cosine: preprocessed candidate rows, the batch in chunks of a fixed budget)
+size_t qb_mmr_scratch_bytes(const qb_storage* s, uint32_t nq, uint32_t max_cand);
+qb_status qb_mmr_launch(const qb_storage* s, const float* d_q_pre, uint32_t nq, const float* d_lambdas, const qb_scored_point* d_cand,
+                        const uint32_t* d_cand_counts, uint32_t max_cand, uint32_t n_max, uint32_t limit, qb_scored_point* d_out, uint32_t out_stride,
+                        uint32_t* d_out_counts, uint32_t* d_n_unique, float* d_scratch, cudaStream_t stream);
 
 // dense preprocess of rows in place (qb_dense.cu)
 qb_status qb_launch_preprocess_rows(qb_distance distance, uint32_t dim, uint64_t n, const float* in, uint64_t in_stride_f,

@@ -12,6 +12,7 @@
 // Same names, argument meaning and error behaviour: construction may fail (OperationError -> std::runtime_error),
 // scoring is infallible apart from device failures (which throw, the analogue of the reference's `expect`).
 #pragma once
+#include <algorithm>
 #include <atomic>
 #include <cstdint>
 #include <functional>
@@ -111,6 +112,17 @@ public:
         qb_scorer* sc = nullptr;
         check(qb_scorer_create_internal(h_, point, &sc));
         return std::make_unique<B200RawScorer>(sc);
+    }
+    // mmr_from_points_with_vector (shard/src/query/mmr/mod.rs:42-279) over candidates whose vectors are this storage's rows: one query of
+    // dim raw f32, (id, score) candidates in the storage's numbering, lambda = 1 - diversity -> the selection, with the input scores
+    std::vector<qb_scored_point> mmr(const float* query, const std::vector<qb_scored_point>& candidates, float lambda, uint32_t limit,
+                                     qb_hw_counters* counters = nullptr) const {
+        std::vector<qb_scored_point> out(std::max<uint32_t>(limit, 1));
+        const uint32_t n = (uint32_t)candidates.size();
+        uint32_t count = 0;
+        check(qb_mmr_batch(h_, query, 1, &lambda, candidates.data(), &n, n, limit, out.data(), &count, counters));
+        out.resize(count);
+        return out;
     }
     uint64_t count() const {
         uint64_t c = 0;

@@ -384,6 +384,31 @@ class DenseVectorStorage(_Storage):
         r = np.ascontiguousarray(rows)
         check(lib().qb_storage_write_rows(self._h, first_row, r.shape[0], r.ctypes.data_as(vp), r.strides[0]))
 
+    def mmr(self, queries, candidates, lambdas, limit: int, counters: Optional[HwCounters] = None):
+        """Maximal marginal relevance (mmr_from_points_with_vector, shard/src/query/mmr/mod.rs:42-279) over candidates whose vectors are
+        this storage's rows: queries [nq, dim] raw f32; candidates = one SCORED_POINT_OFFSET array per query (what the searches return);
+        lambdas = one per query (1 - diversity) or one for all -> list (one per query) of the selected candidates with their input scores."""
+        q = np.atleast_2d(_f32(queries))
+        if q.shape[1] != self.dim:
+            raise ValueError(f"queries have dim {q.shape[1]}, storage has {self.dim}")
+        nq = q.shape[0]
+        if len(candidates) != nq:
+            raise ValueError(f"{len(candidates)} candidate lists for {nq} queries")
+        lam = np.ascontiguousarray(np.broadcast_to(np.asarray(lambdas, np.float32), (nq,)))
+        max_c = max((len(c) for c in candidates), default=0)
+        cand = np.zeros((nq, max(max_c, 1)), dtype=SCORED_POINT_OFFSET)
+        counts = np.zeros(nq, dtype=np.uint32)
+        for i, c in enumerate(candidates):
+            c = np.asarray(c, dtype=SCORED_POINT_OFFSET)
+            cand[i, : c.size] = c
+            counts[i] = c.size
+        out = np.zeros((nq, max(int(limit), 1)), dtype=SCORED_POINT_OFFSET)
+        out_counts = np.zeros(nq, dtype=np.uint32)
+        check(lib().qb_mmr_batch(self._h, q.ctypes.data_as(f32p), nq, lam.ctypes.data_as(f32p), cand.ctypes.data_as(C.POINTER(ScoredPoint)),
+                                 counts.ctypes.data_as(u32p), cand.shape[1] if max_c else 0, int(limit), out.ctypes.data_as(C.POINTER(ScoredPoint)),
+                                 out_counts.ctypes.data_as(u32p), None if counters is None else C.byref(counters)))
+        return [out[i, : out_counts[i]].copy() for i in range(nq)]
+
     def get_dense(self, ids) -> np.ndarray:
         ids = _ids(ids)
         np_dt = {VectorStorageDatatype.Float32: np.float32, VectorStorageDatatype.Float16: np.float16, VectorStorageDatatype.Uint8: np.uint8}[self.datatype]
