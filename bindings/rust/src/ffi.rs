@@ -127,6 +127,8 @@ extern "C" {
     pub fn qb_hnsw_search_discover_batch(g: *mut qb_hnsw, vectors: *const f32, n_pairs: u32, n_queries: u32, top: u32, ef: u32, entry_point: u32, entry_level: u32, deleted_bitmap: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters, algorithm: i32) -> qb_status;
     pub fn qb_mmr_batch(s: *mut qb_storage, queries: *const f32, n_queries: u32, lambdas: *const f32, candidates: *const qb_scored_point, candidate_counts: *const u32, max_candidates: u32, limit: u32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters) -> qb_status;
     pub fn qb_mmr_batch_device(s: *mut qb_storage, dev_queries: *const f32, n_queries: u32, dev_lambdas: *const f32, dev_candidates: *const qb_scored_point, dev_candidate_counts: *const u32, max_candidates: u32, limit: u32, dev_out: *mut qb_scored_point, dev_out_counts: *mut u32) -> qb_status;
+    pub fn qb_mmr_maxsim_batch(tokens: *mut qb_storage, point_offsets: *const u32, n_points: u32, query_vectors: *const f32, query_offsets: *const u32, n_queries: u32, lambdas: *const f32, candidates: *const qb_scored_point, candidate_counts: *const u32, max_candidates: u32, limit: u32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters) -> qb_status;
+    pub fn qb_mmr_maxsim_batch_device(tokens: *mut qb_storage, point_offsets: *const u32, n_points: u32, dev_query_vectors: *const f32, n_query_vectors: u32, dev_query_offsets: *const u32, n_queries: u32, max_query_vectors: u32, dev_lambdas: *const f32, dev_candidates: *const qb_scored_point, dev_candidate_counts: *const u32, max_candidates: u32, limit: u32, dev_out: *mut qb_scored_point, dev_out_counts: *mut u32) -> qb_status;
     pub fn qb_search_stats(s: *mut qb_storage, searches: *mut u64, reruns: *mut u64, reset: i32) -> qb_status;
     pub fn qb_profile_enable(s: *mut qb_storage, on: i32) -> qb_status;
     pub fn qb_profile_read(s: *mut qb_storage, launches: *mut u64, total_ms: *mut f64, reset: i32) -> qb_status;

@@ -679,6 +679,50 @@ QB_API qb_status qb_mmr_batch_device(qb_storage* s, const float* dev_queries, ui
                                      const qb_scored_point* dev_candidates, const uint32_t* dev_candidate_counts, uint32_t max_candidates,
                                      uint32_t limit, qb_scored_point* dev_out, uint32_t* dev_out_counts);
 
+/* The same rerank over a multivector named vector (ColBERT MaxSim): mmr_from_points_with_vector (mod.rs:42-125) puts the candidates'
+ * multivectors into a volatile multi-dense f32 storage, which does not preprocess them (volatile_multi_dense_vector_storage.rs:138-148),
+ * and its LazyMatrix scores pairs with MultiMetricQueryScorer.
+ *   tokens, point_offsets, n_points   dense f32 token rows (others, e.g. f16 / u8 / SQ8: QB_ERR_UNSUPPORTED), point p = rows
+ *               [point_offsets[p], point_offsets[p+1]) used as they are — the layout qb_search_maxsim takes; the offsets must ascend and
+ *               end within the storage.  Candidate ids are point offsets 0 .. n_points - 1, the numbering the MaxSim searches return
+ *   query q     rows [query_offsets[q], query_offsets[q+1]) of query_vectors: 1..4096 raw f32 vectors, each prepared with
+ *               Metric::preprocess (MultiMetricQueryScorer::new)
+ *   lambdas, candidates, candidate_counts, max_candidates (<= 16384, else QB_ERR_UNSUPPORTED), limit, out, out_counts   as qb_mmr_batch
+ * MaxSim(A, B) = for each vector a of A in order, the sequential `sim > max` fold from -inf over B's vectors (NaN never wins, an empty run
+ * stays -inf, the earlier of -0.0 / +0.0 keeps its bits), the maxima summed sequentially in f32 from +0.0 — qb_score_maxsim's rule.
+ *   rel[i]     = MaxSim(preprocess(Q), P_i), equal to qb_score_maxsim on that point bit for bit
+ *   pair(c, s) = MaxSim(preprocess(P_c), P_s): candidate c's tokens are the query side, the pick's the stored side (lazy_matrix.rs:45-52);
+ *                MaxSim is not symmetric
+ * The selection is qb_mmr_batch's: unique_by(id) keeps the first occurrence, fewer than two are returned as they are, every max / argmax
+ * keeps the last maximum under OrderedFloat, mmr = lambda * rel - (1 - lambda) * maxsim in four rounded f32 operations, picks are
+ * swap_remove-d, the output keeps the input scores in pick order.
+ * Counters (MultiMetricQueryScorer: dim * 4 per vector pair of a MaxSim): per query of n >= 2 unique candidates and L picks,
+ * cpu += dim * 4 * (T_q * sum_i T_i + sum over picks k = 1 .. L-1 of T_pick_k * (sum of T_c over the candidates remaining after pick k));
+ * vector_io_read += 0.
+ * Errors, checked before any device work: a null argument, limit = 0, a lambda NaN or outside [0, 1], a count above max_candidates, an id
+ * >= n_points, offsets that do not ascend or end past the storage, a query with 0 or more than 4096 vectors, or a candidate point with no
+ * token rows (the reference cannot hold an empty multivector): QB_ERR_INVALID.
+ * Device scratch: for Cosine, every candidate's preprocessed token rows, max_candidates x (the longest candidate's row count) x the row
+ * size per query, the batch in chunks of at most 512 MB (one query per chunk when a query needs more); nothing for the other distances.
+ * Synchronous. */
+QB_API qb_status qb_mmr_maxsim_batch(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, const float* query_vectors,
+                                     const uint32_t* query_offsets, uint32_t n_queries, const float* lambdas, const qb_scored_point* candidates,
+                                     const uint32_t* candidate_counts, uint32_t max_candidates, uint32_t limit, qb_scored_point* out, uint32_t* out_counts,
+                                     qb_hw_counters* counters /* optional */);
+/* same with the query vectors (n_query_vectors x dim), their offsets (n_queries + 1), lambdas, candidates and outputs resident in HBM,
+ * enqueued on qb_storage_stream(tokens) with no host synchronisation, so it chains after qb_hnsw_search_maxsim_batch_device on the same
+ * token storage (top = max_candidates).  point_offsets stay in HOST memory: they are the offsets the caller created the graph from, checked
+ * here as the host form checks them and copied to the device in stream order (4 * (n_points + 1) bytes per call).  max_query_vectors
+ * (1..4096) bounds the largest query's vector count; it sizes the shared-memory staging only.  Query offsets beyond n_query_vectors are
+ * clamped to it (a query left with no vectors scores +0.0 relevance).  The host checks the storage, the offsets, max_candidates and
+ * limit; lambdas and ids stay on the device unchecked: a count above max_candidates is clamped, and ids outside the points or points
+ * without token rows are dropped from their list.  The Cosine scratch bound uses the longest point's row count, never the storage's
+ * size.  dev_out is n_queries x limit. */
+QB_API qb_status qb_mmr_maxsim_batch_device(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, const float* dev_query_vectors,
+                                            uint32_t n_query_vectors, const uint32_t* dev_query_offsets, uint32_t n_queries, uint32_t max_query_vectors,
+                                            const float* dev_lambdas, const qb_scored_point* dev_candidates, const uint32_t* dev_candidate_counts,
+                                            uint32_t max_candidates, uint32_t limit, qb_scored_point* dev_out, uint32_t* dev_out_counts);
+
 /* ---------------------------------------------------------------- profiling hooks ------------------- */
 /* Fused searches run a fast path first and rerun without it when the device reports that one of its assumptions did not
  * hold (candidate buffer overflow, a dot product outside the f32-exact window, a survivor segment full).  searches =

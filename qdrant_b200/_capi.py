@@ -128,6 +128,10 @@ SIGNATURES = {
     "qb_mmr_batch": (C.c_int32, [vp, f32p, C.c_uint32, f32p, C.POINTER(ScoredPoint), u32p, C.c_uint32, C.c_uint32, C.POINTER(ScoredPoint), u32p,
                                  C.POINTER(HwCounters)]),
     "qb_mmr_batch_device": (C.c_int32, [vp, vp, C.c_uint32, vp, vp, vp, C.c_uint32, C.c_uint32, vp, vp]),
+    "qb_mmr_maxsim_batch": (C.c_int32, [vp, u32p, C.c_uint32, f32p, u32p, C.c_uint32, f32p, C.POINTER(ScoredPoint), u32p, C.c_uint32, C.c_uint32,
+                                        C.POINTER(ScoredPoint), u32p, C.POINTER(HwCounters)]),
+    "qb_mmr_maxsim_batch_device": (C.c_int32, [vp, u32p, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, vp, vp, vp, C.c_uint32, C.c_uint32, vp,
+                                               vp]),
     "qb_profile_enable": (C.c_int32, [vp, C.c_int32]),
     "qb_profile_read": (C.c_int32, [vp, u64p, C.POINTER(C.c_double), C.c_int32]),
 }

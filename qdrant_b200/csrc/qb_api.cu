@@ -1095,6 +1095,143 @@ extern "C" qb_status qb_mmr_batch_device(qb_storage* s, const float* dev_queries
                          c->stream);
 }
 
+// ------------------------------------------------------------------------------------------------ MMR reranking over multivectors
+// the checks both MaxSim MMR entries make on the host: the token storage, max_candidates, limit and the point offsets (ascending, ending
+// within the storage); *max_tokens = the longest point's row count
+static qb_status mmr_maxsim_check(const qb_storage* s, const uint32_t* point_offsets, uint32_t n_points, uint32_t max_candidates, uint32_t limit,
+                                  const char* who, uint32_t* max_tokens) {
+    QB_CHECK(point_offsets, QB_ERR_INVALID, "%s: null point_offsets", who);
+    QB_TRY(mmr_check(s, max_candidates, limit, who));
+    uint32_t mt = 0;
+    for (uint32_t p = 0; p < n_points; ++p) {
+        QB_CHECK(point_offsets[p] <= point_offsets[p + 1], QB_ERR_INVALID, "%s: point_offsets not ascending at %u", who, p);
+        mt = std::max(mt, point_offsets[p + 1] - point_offsets[p]);
+    }
+    QB_CHECK(point_offsets[n_points] <= s->count, QB_ERR_INVALID, "%s: point_offsets end %u beyond the %llu stored vectors", who, point_offsets[n_points],
+             (unsigned long long)s->count);
+    *max_tokens = std::max<uint32_t>(mt, 1);
+    return QB_OK;
+}
+
+// c->d_mmr = [out counts nq | pairs nq (u64) | candidates nq x max | counts nq | lambdas nq | query offsets nq + 1 | point offsets n_points + 1 |
+//             selections nq x out_stride | Cosine scratch]
+struct MmsLayout {
+    size_t pairs_at, cand_at, counts_at, lambdas_at, qoff_at, tok_at, out_at, scratch_at, bytes;
+    MmsLayout(const qb_storage* s, uint32_t nq, uint32_t max_cand, uint32_t n_points, uint32_t max_tokens, uint32_t out_stride) {
+        pairs_at = round_up_u64((size_t)nq * 4, 8);
+        cand_at = round_up_u64(pairs_at + (size_t)nq * 8, 16);
+        counts_at = cand_at + (size_t)nq * max_cand * sizeof(qb_scored_point);
+        lambdas_at = counts_at + (size_t)nq * 4;
+        qoff_at = lambdas_at + (size_t)nq * 4;
+        tok_at = qoff_at + ((size_t)nq + 1) * 4;
+        out_at = round_up_u64(tok_at + ((size_t)n_points + 1) * 4, 16);
+        scratch_at = round_up_u64(out_at + (size_t)nq * out_stride * sizeof(qb_scored_point), 256);
+        bytes = scratch_at + qb_mmr_maxsim_scratch_bytes(s, nq, max_cand, max_tokens);
+    }
+};
+
+extern "C" qb_status qb_mmr_maxsim_batch(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, const float* query_vectors,
+                                         const uint32_t* query_offsets, uint32_t n_queries, const float* lambdas, const qb_scored_point* candidates,
+                                         const uint32_t* candidate_counts, uint32_t max_candidates, uint32_t limit, qb_scored_point* out, uint32_t* out_counts,
+                                         qb_hw_counters* counters) {
+    qb_storage* s = tokens;
+    QB_CHECK(s && out_counts && (out || n_queries == 0), QB_ERR_INVALID, "mmr_maxsim_batch: null argument");
+    QB_CHECK(n_queries == 0 || (query_vectors && query_offsets && lambdas && candidate_counts && (candidates || max_candidates == 0)), QB_ERR_INVALID,
+             "mmr_maxsim_batch: null argument");
+    uint32_t max_tok_all = 0;
+    QB_TRY(mmr_maxsim_check(s, point_offsets, n_points, max_candidates, limit, "mmr_maxsim_batch", &max_tok_all));
+    uint32_t n_max = 0, max_qv = 1, max_tokens = 1;
+    for (uint32_t q = 0; q < n_queries; ++q) {
+        const float l = lambdas[q];
+        QB_CHECK(l >= 0.0f && l <= 1.0f, QB_ERR_INVALID, "mmr_maxsim_batch: lambda %g of query %u outside [0, 1]", (double)l, q);
+        QB_CHECK(query_offsets[q] <= query_offsets[q + 1], QB_ERR_INVALID, "mmr_maxsim_batch: query_offsets not ascending at %u", q);
+        const uint32_t nqv = query_offsets[q + 1] - query_offsets[q];
+        QB_CHECK(nqv >= 1 && nqv <= 4096, QB_ERR_INVALID, "mmr_maxsim_batch: query %u has %u vectors (need 1..4096)", q, nqv);
+        max_qv = std::max(max_qv, nqv);
+        QB_CHECK(candidate_counts[q] <= max_candidates, QB_ERR_INVALID, "mmr_maxsim_batch: %u candidates for query %u > max_candidates %u", candidate_counts[q],
+                 q, max_candidates);
+        n_max = std::max(n_max, candidate_counts[q]);
+        for (uint32_t i = 0; i < candidate_counts[q]; ++i) {
+            const uint32_t id = candidates[(size_t)q * max_candidates + i].idx;
+            QB_CHECK(id < n_points, QB_ERR_INVALID, "mmr_maxsim_batch: point id %u out of range [0, %u)", id, n_points);
+            const uint32_t t = point_offsets[id + 1] - point_offsets[id];
+            QB_CHECK(t > 0, QB_ERR_INVALID, "mmr_maxsim_batch: point %u has no token rows", id);
+            max_tokens = std::max(max_tokens, t);
+        }
+    }
+    if (n_queries == 0) return QB_OK;
+    QB_TRY(use_device(s->device));
+    CtxLease lease;
+    QB_TRY(lease.acquire(s));
+    QbSearchCtx* c = lease.c;
+    const uint32_t out_stride = std::max<uint32_t>(1, std::min(limit, max_candidates));
+    const MmsLayout lay(s, n_queries, max_candidates, n_points, max_tokens, out_stride);
+    const uint32_t nv = query_offsets[n_queries];   // vectors before query_offsets[0] are uploaded and not read
+    // stage tail: the inputs [candidates | counts | lambdas | query offsets | point offsets] going up, then [selections | out counts | pairs]
+    const size_t up = lay.out_at - lay.cand_at, res_bytes = (size_t)n_queries * out_stride * sizeof(qb_scored_point);
+    const size_t down = res_bytes + lay.cand_at;
+    uint8_t* h_tail = nullptr;
+    QB_TRY(stage_queries(s, c, query_vectors, nv, std::max(up, down), &h_tail));
+    const size_t cand_bytes = (size_t)n_queries * max_candidates * sizeof(qb_scored_point);
+    if (cand_bytes) memcpy(h_tail, candidates, cand_bytes);
+    memcpy(h_tail + (lay.counts_at - lay.cand_at), candidate_counts, (size_t)n_queries * 4);
+    memcpy(h_tail + (lay.lambdas_at - lay.cand_at), lambdas, (size_t)n_queries * 4);
+    memcpy(h_tail + (lay.qoff_at - lay.cand_at), query_offsets, ((size_t)n_queries + 1) * 4);
+    memcpy(h_tail + (lay.tok_at - lay.cand_at), point_offsets, ((size_t)n_points + 1) * 4);
+    QB_TRY(qb_ensure_device(&c->d_mmr, &c->mmr_bytes, lay.bytes));
+    uint8_t* d = reinterpret_cast<uint8_t*>(c->d_mmr);
+    QB_CUDA(cudaMemcpyAsync(d + lay.cand_at, h_tail, up, cudaMemcpyHostToDevice, c->stream));
+    QB_TRY(qb_mmr_maxsim_launch(s, reinterpret_cast<const uint32_t*>(d + lay.tok_at), n_points, max_tokens, reinterpret_cast<const float*>(c->d_queries_enc),
+                                reinterpret_cast<const uint32_t*>(d + lay.qoff_at), nv, max_qv, n_queries, reinterpret_cast<const float*>(d + lay.lambdas_at),
+                                reinterpret_cast<const qb_scored_point*>(d + lay.cand_at), reinterpret_cast<const uint32_t*>(d + lay.counts_at), max_candidates,
+                                n_max, limit, reinterpret_cast<qb_scored_point*>(d + lay.out_at), out_stride, reinterpret_cast<uint32_t*>(d),
+                                reinterpret_cast<unsigned long long*>(d + lay.pairs_at), reinterpret_cast<float*>(d + lay.scratch_at), c->stream));
+    QB_CUDA(cudaMemcpyAsync(h_tail, d + lay.out_at, res_bytes, cudaMemcpyDeviceToHost, c->stream));
+    QB_CUDA(cudaMemcpyAsync(h_tail + res_bytes, d, lay.cand_at, cudaMemcpyDeviceToHost, c->stream));
+    QB_CUDA(cudaStreamSynchronize(c->stream));
+    const qb_scored_point* h_res = reinterpret_cast<const qb_scored_point*>(h_tail);
+    const uint32_t* h_cnt = reinterpret_cast<const uint32_t*>(h_tail + res_bytes);
+    for (uint32_t q = 0; q < n_queries; ++q) {
+        out_counts[q] = h_cnt[q];
+        memcpy(out + (size_t)q * limit, h_res + (size_t)q * out_stride, (size_t)h_cnt[q] * sizeof(qb_scored_point));
+        // MultiMetricQueryScorer meters dim * 4 per (query-side vector, stored vector) pair; vector_io_read: the volatile storage is never on disk
+        uint64_t pairs;
+        memcpy(&pairs, h_tail + res_bytes + lay.pairs_at + (size_t)q * 8, 8);
+        if (counters) counters->cpu += pairs * s->dim * 4;
+    }
+    return QB_OK;
+}
+
+extern "C" qb_status qb_mmr_maxsim_batch_device(qb_storage* tokens, const uint32_t* point_offsets, uint32_t n_points, const float* dev_query_vectors,
+                                                uint32_t n_query_vectors, const uint32_t* dev_query_offsets, uint32_t n_queries, uint32_t max_query_vectors,
+                                                const float* dev_lambdas, const qb_scored_point* dev_candidates, const uint32_t* dev_candidate_counts,
+                                                uint32_t max_candidates, uint32_t limit, qb_scored_point* dev_out, uint32_t* dev_out_counts) {
+    qb_storage* s = tokens;
+    QB_CHECK(s, QB_ERR_INVALID, "mmr_maxsim_batch_device: null argument");
+    QB_CHECK(n_queries == 0 || (dev_query_vectors && dev_query_offsets && dev_lambdas && dev_candidate_counts && dev_out && dev_out_counts &&
+                                (dev_candidates || max_candidates == 0)),
+             QB_ERR_INVALID, "mmr_maxsim_batch_device: null argument");
+    QB_CHECK(max_query_vectors >= 1 && max_query_vectors <= 4096, QB_ERR_INVALID, "mmr_maxsim_batch_device: max_query_vectors %u outside [1,4096]",
+             max_query_vectors);
+    uint32_t max_tokens = 0;
+    QB_TRY(mmr_maxsim_check(s, point_offsets, n_points, max_candidates, limit, "mmr_maxsim_batch_device", &max_tokens));
+    if (n_queries == 0) return QB_OK;
+    QB_TRY(use_device(s->device));
+    QbSearchCtx* c = nullptr;
+    QB_TRY(qb_ctx_device(s, &c));
+    QB_TRY(encode_device_queries(s, c, dev_query_vectors, n_query_vectors));
+    // c->d_mmr = [pairs nq (u64) | point offsets n_points + 1 | Cosine scratch]; the pair counts are not read back.  The offsets are copied
+    // from the caller's memory before this returns (a pageable copy is staged at once), in stream order.
+    const size_t tok_at = round_up_u64((size_t)n_queries * 8, 256), scratch_at = round_up_u64(tok_at + ((size_t)n_points + 1) * 4, 256);
+    QB_TRY(qb_ensure_device(&c->d_mmr, &c->mmr_bytes, scratch_at + qb_mmr_maxsim_scratch_bytes(s, n_queries, max_candidates, max_tokens)));
+    uint8_t* d = reinterpret_cast<uint8_t*>(c->d_mmr);
+    QB_CUDA(cudaMemcpyAsync(d + tok_at, point_offsets, ((size_t)n_points + 1) * 4, cudaMemcpyHostToDevice, c->stream));
+    return qb_mmr_maxsim_launch(s, reinterpret_cast<const uint32_t*>(d + tok_at), n_points, max_tokens, reinterpret_cast<const float*>(c->d_queries_enc),
+                                dev_query_offsets, n_query_vectors, max_query_vectors, n_queries, dev_lambdas, dev_candidates, dev_candidate_counts,
+                                max_candidates, max_candidates, limit, dev_out, limit, dev_out_counts, reinterpret_cast<unsigned long long*>(d),
+                                reinterpret_cast<float*>(d + scratch_at), c->stream);
+}
+
 // ------------------------------------------------------------------------------------------------ RawScorer
 static qb_status scorer_alloc(qb_storage* s, qb_scorer** out) {
     qb_scorer* sc = new qb_scorer();

@@ -288,6 +288,15 @@ size_t qb_mmr_scratch_bytes(const qb_storage* s, uint32_t nq, uint32_t max_cand)
 qb_status qb_mmr_launch(const qb_storage* s, const float* d_q_pre, uint32_t nq, const float* d_lambdas, const qb_scored_point* d_cand,
                         const uint32_t* d_cand_counts, uint32_t max_cand, uint32_t n_max, uint32_t limit, qb_scored_point* d_out, uint32_t out_stride,
                         uint32_t* d_out_counts, uint32_t* d_n_unique, float* d_scratch, cudaStream_t stream);
+// MMR reranking over multivector candidates (qb_mmr_maxsim.cu): point p = token rows [d_tok[p], d_tok[p + 1]) of s (max_tokens bounds a
+// point's rows), query q = preprocessed vectors [d_q_off[q], d_q_off[q + 1]) of d_q_pre clamped to n_qv (max_qv bounds a query's count);
+// candidates, selections and counts as qb_mmr_launch; d_pairs[q] = the query's token-weighted pair count.  d_scratch:
+// qb_mmr_maxsim_scratch_bytes (Cosine: preprocessed candidate token rows, the batch in chunks of a fixed budget)
+size_t qb_mmr_maxsim_scratch_bytes(const qb_storage* s, uint32_t nq, uint32_t max_cand, uint32_t max_tokens);
+qb_status qb_mmr_maxsim_launch(const qb_storage* s, const uint32_t* d_tok, uint32_t n_points, uint32_t max_tokens, const float* d_q_pre,
+                               const uint32_t* d_q_off, uint32_t n_qv, uint32_t max_qv, uint32_t nq, const float* d_lambdas, const qb_scored_point* d_cand,
+                               const uint32_t* d_cand_counts, uint32_t max_cand, uint32_t n_max, uint32_t limit, qb_scored_point* d_out,
+                               uint32_t out_stride, uint32_t* d_out_counts, unsigned long long* d_pairs, float* d_scratch, cudaStream_t stream);
 
 // dense preprocess of rows in place (qb_dense.cu)
 qb_status qb_launch_preprocess_rows(qb_distance distance, uint32_t dim, uint64_t n, const float* in, uint64_t in_stride_f,

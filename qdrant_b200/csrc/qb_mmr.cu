@@ -18,24 +18,14 @@
 // applies the same swap_remove.  The scores are the f32 chains of qb_score.cuh that qb_score_points runs (score_avx_group8 for
 // dim >= 32, score_small below), with the candidate's preprocessed row as the query side.  For Cosine, preprocess(v_c) is
 // materialised by a gather + qb_launch_preprocess_rows into scratch; for the other distances it is the stored row itself.
-#include <cooperative_groups.h>
+#include "qb_mmr.cuh"
 
-#include "qb_internal.h"
-#include "qb_score.cuh"
-
-namespace cg = cooperative_groups;
-using namespace qbs;
+using namespace qb_mmr;
 
 namespace {
 
-constexpr uint32_t MMR_THREADS = 512;
-constexpr uint32_t MMR_WARPS = MMR_THREADS / 32;
 constexpr uint32_t MMR_STAGE_MAX_F = 16384;           // stored rows of up to 64 KB are staged in shared memory, longer ones read from HBM
 constexpr size_t MMR_PRE_BUDGET = 512ull << 20;       // Cosine: preprocessed candidate rows of one launch
-constexpr uint16_t MMR_GONE = 0xFFFF;                 // `where` of a candidate that is selected, a duplicate or out of range
-
-// CTAs per cluster for lists of up to n candidates
-static inline uint32_t mmr_ctas(uint32_t n) { return n <= 256 ? 1u : n <= 1024 ? 2u : n <= 4096 ? 4u : 8u; }
 
 // dynamic shared memory of one CTA: [staged row | 2 step slots + one per warp (u64) | 4 u32 | rel, maxsim, row (per owned) | rem, where]
 struct MmrSmem {
@@ -66,25 +56,6 @@ struct MmrParams {
     uint32_t* n_unique;                // [nq]: candidates left after the dedup (for the counters)
     MmrSmem sm;
 };
-
-// OrderedFloat as an unsigned key: NaN above everything and equal to NaN, -0.0 == +0.0
-__device__ __forceinline__ uint32_t ord_key(float s) { return qb_orderable(s == 0.0f ? 0.0f : s); }
-// (value, position): the larger wins, the later position on equal values (max_by_key keeps the last maximum); never 0
-__device__ __forceinline__ unsigned long long pos_key(float s, uint32_t pos) { return ((unsigned long long)ord_key(s) << 32) | pos; }
-
-__device__ __forceinline__ unsigned long long block_max(unsigned long long v, unsigned long long* wbest) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const unsigned long long w = __shfl_xor_sync(0xFFFFFFFFu, v, o);
-        v = w > v ? w : v;
-    }
-    const uint32_t warp = threadIdx.x >> 5;
-    if ((threadIdx.x & 31) == 0) wbest[warp] = v;
-    __syncthreads();
-    v = 0;
-    for (uint32_t w = 0; w < MMR_WARPS; ++w) v = wbest[w] > v ? wbest[w] : v;
-    return v;
-}
 
 // score = sim(qry, row) by the chain qb_score_points runs: lanes of an 8-lane group (AVX tier) or one thread (dim < 32)
 template <int METRIC, bool SMALL>
@@ -197,24 +168,13 @@ __global__ void __launch_bounds__(MMR_THREADS, 1) mmr_kernel(const MmrParams p) 
     uint32_t remaining = n_keep, par = 0;
     for (uint32_t k = 0;; ++k, par ^= 1u) {
         // 4. cluster argmax of this step: every CTA reads every CTA's slot after one barrier, and takes the same pick
-        best = block_max(best, wbest);
-        if (tid == 0) slot[par] = best;
-        cluster.sync();
-        for (uint32_t r = 0; r < C; ++r) {
-            const unsigned long long v = cluster.map_shared_rank(slot, r)[par];
-            best = v > best ? v : best;
-        }
+        best = mmr_cluster_best(tid, cluster, C, best, wbest, slot, par);
         const uint32_t pos = (uint32_t)(best & 0xFFFFFFFFu), sel = rem[pos];
         if (rank == 0 && tid == 0) p.out[(size_t)q * p.out_stride + k] = cand[sel];
         if (k + 1 == L) break;
         __syncthreads();   // every thread has read rem[pos]
         // 5. IndexSet::swap_remove on the replicated positions; stage the pick's stored row
-        if (tid == 0) {
-            const uint32_t moved = rem[remaining - 1];
-            rem[pos] = (uint16_t)moved;
-            where[moved] = (uint16_t)pos;
-            where[sel] = MMR_GONE;
-        }
+        if (tid == 0) mmr_swap_remove(rem, where, pos, sel, remaining);
         --remaining;
         const float* srow_g = p.rows + (size_t)(cand[sel].idx - p.id_base) * p.stride_f;
         const float* vs = srow_g;

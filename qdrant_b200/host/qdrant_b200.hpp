@@ -124,6 +124,20 @@ public:
         out.resize(count);
         return out;
     }
+    // the same over multivector candidates whose token rows are this storage's rows (point p = rows [point_offsets[p], point_offsets[p+1])):
+    // one query of n_query_vectors x dim raw f32, (point offset, score) candidates, pair scores MaxSim -> the selection, with the input scores
+    std::vector<qb_scored_point> mmr_maxsim(const std::vector<uint32_t>& point_offsets, const float* query_vectors, uint32_t n_query_vectors,
+                                            const std::vector<qb_scored_point>& candidates, float lambda, uint32_t limit,
+                                            qb_hw_counters* counters = nullptr) const {
+        std::vector<qb_scored_point> out(std::max<uint32_t>(limit, 1));
+        const uint32_t n = (uint32_t)candidates.size(), q_off[2] = {0, n_query_vectors};
+        const uint32_t n_points = point_offsets.empty() ? 0 : (uint32_t)point_offsets.size() - 1;
+        uint32_t count = 0;
+        check(qb_mmr_maxsim_batch(h_, point_offsets.data(), n_points, query_vectors, q_off, 1, &lambda, candidates.data(), &n, n, limit, out.data(), &count,
+                                  counters));
+        out.resize(count);
+        return out;
+    }
     uint64_t count() const {
         uint64_t c = 0;
         check(qb_storage_info(h_, nullptr, &c, nullptr));

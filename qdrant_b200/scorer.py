@@ -639,6 +639,33 @@ class MultiVectorView:
                                     ids.ctypes.data_as(u32p), ids.size, scores.ctypes.data_as(f32p)))
         return scores
 
+    def mmr(self, queries, candidates, lambdas, limit: int, counters: Optional[HwCounters] = None):
+        """Maximal marginal relevance over multivector candidates (mmr_from_points_with_vector, shard/src/query/mmr/mod.rs:42-125, with
+        MaxSim pair scores): queries = one [T_q, dim] array per query (raw f32); candidates = one SCORED_POINT_OFFSET array per query, ids
+        are point offsets (what the MaxSim searches return); lambdas = one per query (1 - diversity) or one for all -> list (one per
+        query) of the selected candidates with their input scores."""
+        qs = [self._query(q) for q in queries]
+        nq = len(qs)
+        if len(candidates) != nq:
+            raise ValueError(f"{len(candidates)} candidate lists for {nq} queries")
+        q_off = np.concatenate([[0], np.cumsum([q.shape[0] for q in qs], dtype=np.int64)]).astype(np.uint32)
+        qv = np.ascontiguousarray(np.concatenate(qs)) if nq else np.zeros((1, self.storage.dim), np.float32)
+        lam = np.ascontiguousarray(np.broadcast_to(np.asarray(lambdas, np.float32), (nq,)))
+        max_c = max((len(c) for c in candidates), default=0)
+        cand = np.zeros((nq, max(max_c, 1)), dtype=SCORED_POINT_OFFSET)
+        counts = np.zeros(nq, dtype=np.uint32)
+        for i, c in enumerate(candidates):
+            c = np.asarray(c, dtype=SCORED_POINT_OFFSET)
+            cand[i, : c.size] = c
+            counts[i] = c.size
+        out = np.zeros((nq, max(int(limit), 1)), dtype=SCORED_POINT_OFFSET)
+        out_counts = np.zeros(nq, dtype=np.uint32)
+        check(lib().qb_mmr_maxsim_batch(self.storage._h, self.offsets.ctypes.data_as(u32p), self.n_points, qv.ctypes.data_as(f32p), q_off.ctypes.data_as(u32p),
+                                        nq, lam.ctypes.data_as(f32p), cand.ctypes.data_as(C.POINTER(ScoredPoint)), counts.ctypes.data_as(u32p),
+                                        cand.shape[1] if max_c else 0, int(limit), out.ctypes.data_as(C.POINTER(ScoredPoint)), out_counts.ctypes.data_as(u32p),
+                                        None if counters is None else C.byref(counters)))
+        return [out[i, : out_counts[i]].copy() for i in range(nq)]
+
     # ---- custom queries whose examples are multivectors (MultiCustomQueryScorer, multi_custom_query_scorer.rs:88-104).  `query` is one of the
     # query classes above with 2-D arrays (vectors x dim) in place of vectors.
     def _flat_multi(self, query):
