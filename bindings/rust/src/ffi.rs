@@ -20,6 +20,8 @@ pub const QB_DT_F32: i32 = 0; pub const QB_DT_F16: i32 = 1; pub const QB_DT_U8: 
 pub const QB_QD_COSINE: i32 = 0; pub const QB_QD_DOT: i32 = 1; pub const QB_QD_L1: i32 = 2; pub const QB_QD_L2: i32 = 3;
 // qb_hnsw_algorithm (SearchAlgorithm, graph_layers.rs:80-84)
 pub const QB_HNSW_ALGO_HNSW: i32 = 0; pub const QB_HNSW_ALGO_ACORN: i32 = 1;
+// qb_sparse_kind: InvertedIndexRam (may prune), the compressed indexes with f32 / f16 / u8 weights
+pub const QB_SPARSE_RAM: i32 = 0; pub const QB_SPARSE_COMPRESSED: i32 = 1; pub const QB_SPARSE_COMPRESSED_F16: i32 = 2; pub const QB_SPARSE_COMPRESSED_U8: i32 = 3;
 
 #[repr(C)]
 pub struct qb_storage { _private: [u8; 0] }
@@ -29,6 +31,8 @@ pub struct qb_scorer { _private: [u8; 0] }
 pub struct qb_hnsw { _private: [u8; 0] }
 #[repr(C)]
 pub struct qb_comm { _private: [u8; 0] }
+#[repr(C)]
+pub struct qb_sparse_index { _private: [u8; 0] }
 
 /// Same layout as `common::types::ScoredPointOffset` (`#[repr(C)] { idx: u32, score: f32 }`).
 #[repr(C)]
@@ -129,6 +133,13 @@ extern "C" {
     pub fn qb_mmr_batch_device(s: *mut qb_storage, dev_queries: *const f32, n_queries: u32, dev_lambdas: *const f32, dev_candidates: *const qb_scored_point, dev_candidate_counts: *const u32, max_candidates: u32, limit: u32, dev_out: *mut qb_scored_point, dev_out_counts: *mut u32) -> qb_status;
     pub fn qb_mmr_maxsim_batch(tokens: *mut qb_storage, point_offsets: *const u32, n_points: u32, query_vectors: *const f32, query_offsets: *const u32, n_queries: u32, lambdas: *const f32, candidates: *const qb_scored_point, candidate_counts: *const u32, max_candidates: u32, limit: u32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters) -> qb_status;
     pub fn qb_mmr_maxsim_batch_device(tokens: *mut qb_storage, point_offsets: *const u32, n_points: u32, dev_query_vectors: *const f32, n_query_vectors: u32, dev_query_offsets: *const u32, n_queries: u32, max_query_vectors: u32, dev_lambdas: *const f32, dev_candidates: *const qb_scored_point, dev_candidate_counts: *const u32, max_candidates: u32, limit: u32, dev_out: *mut qb_scored_point, dev_out_counts: *mut u32) -> qb_status;
+    pub fn qb_sparse_index_create(device: i32, kind: i32, n_points: u32, n_dims: u32, indptr: *const u64, dims: *const u32, weights: *const f32, out: *mut *mut qb_sparse_index) -> qb_status;
+    pub fn qb_sparse_index_destroy(idx: *mut qb_sparse_index);
+    pub fn qb_sparse_index_info(idx: *const qb_sparse_index, n_points: *mut u32, n_dims: *mut u32, n_elements: *mut u64, hbm_bytes: *mut u64) -> qb_status;
+    pub fn qb_sparse_index_stream(idx: *mut qb_sparse_index) -> *mut c_void;
+    pub fn qb_sparse_search_batch(idx: *mut qb_sparse_index, q_indptr: *const u64, q_dims: *const u32, q_weights: *const f32, n_queries: u32, top: u32, deleted_bitmap: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters) -> qb_status;
+    pub fn qb_sparse_search_batch_device(idx: *mut qb_sparse_index, dev_q_indptr: *const u64, dev_q_dims: *const u32, dev_q_weights: *const f32, n_queries: u32, max_query_nnz: u32, top: u32, dev_deleted_bitmap: *const u64, dev_out: *mut qb_scored_point, dev_out_counts: *mut u32) -> qb_status;
+    pub fn qb_sparse_search_plain_batch(idx: *mut qb_sparse_index, q_indptr: *const u64, q_dims: *const u32, q_weights: *const f32, n_queries: u32, id_indptr: *const u64, ids: *const u32, top: u32, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters) -> qb_status;
     pub fn qb_search_stats(s: *mut qb_storage, searches: *mut u64, reruns: *mut u64, reset: i32) -> qb_status;
     pub fn qb_profile_enable(s: *mut qb_storage, on: i32) -> qb_status;
     pub fn qb_profile_read(s: *mut qb_storage, launches: *mut u64, total_ms: *mut f64, reset: i32) -> qb_status;

@@ -723,6 +723,66 @@ QB_API qb_status qb_mmr_maxsim_batch_device(qb_storage* tokens, const uint32_t* 
                                             const float* dev_lambdas, const qb_scored_point* dev_candidates, const uint32_t* dev_candidate_counts,
                                             uint32_t max_candidates, uint32_t limit, qb_scored_point* dev_out, uint32_t* dev_out_counts);
 
+/* ---------------------------------------------------------------- sparse vectors -------------------- */
+/* An inverted index over sparse vectors (SPLADE, BM25 and the like) and the reference's SearchContext over it
+ * (lib/sparse/src/index/search_context.rs).  Dims are internal dims: the caller remaps its user dims as the segment's IndicesTracker
+ * does (indices_tracker.rs:53-72) and keeps that map on the host.
+ *   kind   QB_SPARSE_RAM: the mutable InvertedIndexRam, whose lists report reliable max_next_weight, so search may prune
+ *          (posting_list.rs:228).  QB_SPARSE_COMPRESSED: the immutable / mmap compressed indexes with f32 weights, which never prune
+ *          (compressed_posting_list.rs:661).  Compressed lists with f16 or u8 weights: QB_ERR_UNSUPPORTED. */
+typedef enum { QB_SPARSE_RAM = 0, QB_SPARSE_COMPRESSED = 1, QB_SPARSE_COMPRESSED_F16 = 2, QB_SPARSE_COMPRESSED_U8 = 3 } qb_sparse_kind;
+typedef struct qb_sparse_index qb_sparse_index;
+/* n_points rows in CSR form: row r = dims / weights [indptr[r], indptr[r + 1]), indptr[0] = 0.  Each row is sorted by dim on creation;
+ * one posting list per dim holds (id, weight, max_next_weight) sorted by id, max_next_weight = the largest weight after the element
+ * (-inf for the last; PostingBuilder::build, posting_list.rs:140-170).  QB_ERR_INVALID for a null argument, an unknown kind, offsets that
+ * descend or do not start at 0, a dim >= n_dims, a dim repeated within a row or a weight that is not finite.  2^32 - 1 or more elements:
+ * QB_ERR_UNSUPPORTED.  HBM: 20 bytes per element, 8 per point and 8 per dim.  Synchronous. */
+QB_API qb_status qb_sparse_index_create(int32_t device, qb_sparse_kind kind, uint32_t n_points, uint32_t n_dims, const uint64_t* indptr,
+                                        const uint32_t* dims, const float* weights, qb_sparse_index** out);
+QB_API void qb_sparse_index_destroy(qb_sparse_index* idx);
+QB_API qb_status qb_sparse_index_info(const qb_sparse_index* idx, uint32_t* n_points, uint32_t* n_dims, uint64_t* n_elements, uint64_t* hbm_bytes);
+/* the cudaStream_t the index's searches run on (qb_sparse_search_batch_device enqueues there) */
+QB_API void* qb_sparse_index_stream(qb_sparse_index* idx);
+/* SearchContext::new + search (:42-87, :263-414) per query: query q = q_dims / q_weights [q_indptr[q], q_indptr[q + 1]).
+ *   The query is sorted by dim and its dims >= n_dims are dropped, as remap_vector drops the dims the tracker does not know; a dim
+ *   repeated in a query is QB_ERR_INVALID (SparseVector validation).  An empty query, or one whose lists are all empty, gives an empty list.
+ *   Batches of ids [min_id, min(min_id + 10000, max_record_id)]: every list in its current order adds weight * query_weight into a zeroed f32
+ *   score (0 + p1 + p2 + ...); a score is pushed when it is non-zero, greater than the running threshold and not deleted.  After each
+ *   batch the exhausted lists are removed in order; one list left pushes all its remaining undeleted elements (weight * query_weight, no
+ *   non-zero test); otherwise, with pruning on and a full TopK whose threshold changed, the longest list (the last of equal lengths) is
+ *   swapped to the front and skipped ahead when max(weight, max_next_weight) * query_weight <= threshold.  Pruning is on for
+ *   QB_SPARSE_RAM when every kept query weight is >= 0.
+ *   TopK (common/src/top_k.rs:22-64): the threshold starts at f32::MIN, a push needs score > threshold, at 2k entries the threshold
+ *   becomes the k-th largest score and k entries stay.  The entries kept order by (score desc, id asc), so among equal scores at the
+ *   boundary the smaller ids stay, where the reference keeps an unspecified subset; scores, the threshold history and so pruning are
+ *   the reference's bit for bit.
+ *   deleted_bitmap  optional, ceil(n_points / 64) words, bit = 1 deleted (the filter)
+ *   is_stopped      optional, polled before the launch (QB_ERR_CANCELLED)
+ *   out             n_queries x top in (score desc, id asc) order; out_counts[q] valid entries
+ * top in 1..4096 (0: QB_ERR_INVALID, above: QB_ERR_UNSUPPORTED); more than 4096 kept dims in a query: QB_ERR_UNSUPPORTED.
+ * Counters: cpu += 4 * the total length of the query's posting lists (:272-283); vector_io_read += 0.  Every check runs before any device
+ * work.  The choice between this and qb_sparse_search_plain_batch stays with the caller, as in the reference
+ * (read_view/search.rs:258-300): plain search when the filter's estimated cardinality is below full_scan_threshold (default 5000).
+ * Synchronous. */
+QB_API qb_status qb_sparse_search_batch(qb_sparse_index* idx, const uint64_t* q_indptr, const uint32_t* q_dims, const float* q_weights, uint32_t n_queries,
+                                        uint32_t top, const uint64_t* deleted_bitmap, const volatile int32_t* is_stopped, qb_scored_point* out,
+                                        uint32_t* out_counts, qb_hw_counters* counters /* optional */);
+/* same with the queries, the optional bitmap and the outputs resident in HBM, enqueued on qb_sparse_index_stream(idx) with no host
+ * synchronisation.  The queries are sorted and their dims >= n_dims dropped on the device; they are not checked: a query's entries past
+ * max_query_nnz (<= 4096, else QB_ERR_UNSUPPORTED) are ignored, and a repeated dim counts as two lists.  No counters. */
+QB_API qb_status qb_sparse_search_batch_device(qb_sparse_index* idx, const uint64_t* dev_q_indptr, const uint32_t* dev_q_dims, const float* dev_q_weights,
+                                               uint32_t n_queries, uint32_t max_query_nnz, uint32_t top, const uint64_t* dev_deleted_bitmap,
+                                               qb_scored_point* dev_out, uint32_t* dev_out_counts);
+/* SearchContext::plain_search (:92-143) per query over its own ids [id_indptr[q], id_indptr[q + 1]) — already filtered by the caller, as
+ * the reference's prefiltered_points are.  For each id, the dims the point shares with the query score 0 + sum of stored * query in
+ * ascending dim order (score_vectors, sparse_vector.rs:66-90); an id with no shared dim is skipped; any other score above f32::MIN,
+ * zero included, is pushed.  Queries as qb_sparse_search_batch; out in (score desc, id asc) order.  An id >= n_points or repeated within
+ * a query: QB_ERR_INVALID.  Counters: cpu += kept query dims + 4 * shared dims per scored id; vector_io_read += 0.  Synchronous. */
+QB_API qb_status qb_sparse_search_plain_batch(qb_sparse_index* idx, const uint64_t* q_indptr, const uint32_t* q_dims, const float* q_weights,
+                                              uint32_t n_queries, const uint64_t* id_indptr, const uint32_t* ids, uint32_t top,
+                                              const volatile int32_t* is_stopped, qb_scored_point* out, uint32_t* out_counts,
+                                              qb_hw_counters* counters /* optional */);
+
 /* ---------------------------------------------------------------- profiling hooks ------------------- */
 /* Fused searches run a fast path first and rerun without it when the device reports that one of its assumptions did not
  * hold (candidate buffer overflow, a dot product outside the f32-exact window, a survivor segment full).  searches =

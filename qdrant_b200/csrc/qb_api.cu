@@ -138,6 +138,8 @@ static qb_status use_device(int device) {
     return QB_OK;
 }
 
+qb_status qb_use_device(int device) { return use_device(device); }
+
 // Point ids crossing the C ABI are the ids searches on this storage report: local row + id_base (qb_storage_set_id_base).
 // Every id-taking entry point validates the range and works on local rows.
 static qb_status localize_ids(const qb_storage* s, const uint32_t* ids, uint64_t n, uint32_t* dst, const char* who) {

@@ -236,6 +236,7 @@ qb_status qb_ensure_pinned(void** p, size_t* have, size_t need_bytes);
 qb_status qb_ctx_acquire(qb_storage* s, QbSearchCtx** out);
 void qb_ctx_release(qb_storage* s, QbSearchCtx* c);
 qb_status qb_ctx_device(qb_storage* s, QbSearchCtx** out);
+qb_status qb_use_device(int device);   // checks the device ordinal and makes it current
 
 // ---------------------------------------------------------------- kernels' host launchers
 // All launchers enqueue on `stream` and never synchronise.

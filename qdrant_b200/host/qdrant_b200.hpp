@@ -405,4 +405,71 @@ private:
     qb_comm* c_ = nullptr;
 };
 
+// A sparse vector: internal dims (the segment's IndicesTracker remapping) and their weights
+struct SparseVector {
+    std::vector<uint32_t> indices;
+    std::vector<float> values;
+};
+
+// The inverted index of a sparse named vector and SearchContext over it (sparse/src/index/search_context.rs): search() is
+// SearchContext::search, plain_search() is SearchContext::plain_search over already-filtered ids.  Ram may prune (InvertedIndexRam),
+// Compressed never does (the compressed indexes with f32 weights).
+class SparseVectorIndex {
+public:
+    enum class Kind : int { Ram = QB_SPARSE_RAM, Compressed = QB_SPARSE_COMPRESSED };
+    SparseVectorIndex(const std::vector<SparseVector>& points, uint32_t n_dims, Kind kind = Kind::Ram, int device = 0) {
+        std::vector<uint64_t> indptr(1, 0);
+        std::vector<uint32_t> dims;
+        std::vector<float> w;
+        flatten(points, indptr, dims, w);
+        check(qb_sparse_index_create(device, (qb_sparse_kind)kind, (uint32_t)points.size(), n_dims, indptr.data(), dims.data(), w.data(), &h_));
+    }
+    ~SparseVectorIndex() { qb_sparse_index_destroy(h_); }
+    SparseVectorIndex(const SparseVectorIndex&) = delete;
+    SparseVectorIndex& operator=(const SparseVectorIndex&) = delete;
+
+    std::vector<std::vector<ScoredPointOffset>> search(const std::vector<SparseVector>& queries, uint32_t top, const uint64_t* deleted_bitmap = nullptr,
+                                                       qb_hw_counters* counters = nullptr) const {
+        std::vector<uint64_t> qp(1, 0);
+        std::vector<uint32_t> qd;
+        std::vector<float> qw;
+        flatten(queries, qp, qd, qw);
+        std::vector<ScoredPointOffset> flat(queries.size() * (size_t)top);
+        std::vector<uint32_t> counts(queries.size());
+        check(qb_sparse_search_batch(h_, qp.data(), qd.data(), qw.data(), (uint32_t)queries.size(), top, deleted_bitmap, nullptr, flat.data(), counts.data(),
+                                     counters));
+        return split(flat, counts, top);
+    }
+    std::vector<std::vector<ScoredPointOffset>> plain_search(const std::vector<SparseVector>& queries, const std::vector<std::vector<PointOffsetType>>& ids,
+                                                             uint32_t top, qb_hw_counters* counters = nullptr) const {
+        std::vector<uint64_t> qp(1, 0), ip(1, 0);
+        std::vector<uint32_t> qd, flat_ids;
+        std::vector<float> qw;
+        flatten(queries, qp, qd, qw);
+        for (const auto& l : ids) { flat_ids.insert(flat_ids.end(), l.begin(), l.end()); ip.push_back(flat_ids.size()); }
+        if (ids.size() != queries.size()) throw OperationError(QB_ERR_INVALID, "plain_search: one id list per query");
+        std::vector<ScoredPointOffset> flat(queries.size() * (size_t)top);
+        std::vector<uint32_t> counts(queries.size());
+        check(qb_sparse_search_plain_batch(h_, qp.data(), qd.data(), qw.data(), (uint32_t)queries.size(), ip.data(), flat_ids.data(), top, nullptr,
+                                           flat.data(), counts.data(), counters));
+        return split(flat, counts, top);
+    }
+
+private:
+    static void flatten(const std::vector<SparseVector>& v, std::vector<uint64_t>& ptr, std::vector<uint32_t>& dims, std::vector<float>& w) {
+        for (const auto& x : v) {
+            if (x.indices.size() != x.values.size()) throw OperationError(QB_ERR_INVALID, "sparse vector: indices and values differ in length");
+            dims.insert(dims.end(), x.indices.begin(), x.indices.end());
+            w.insert(w.end(), x.values.begin(), x.values.end());
+            ptr.push_back(dims.size());
+        }
+    }
+    static std::vector<std::vector<ScoredPointOffset>> split(const std::vector<ScoredPointOffset>& flat, const std::vector<uint32_t>& counts, uint32_t top) {
+        std::vector<std::vector<ScoredPointOffset>> out(counts.size());
+        for (size_t q = 0; q < counts.size(); ++q) out[q].assign(flat.begin() + q * top, flat.begin() + q * top + counts[q]);
+        return out;
+    }
+    qb_sparse_index* h_ = nullptr;
+};
+
 }  // namespace qdrant_b200

@@ -764,6 +764,103 @@ def load_quantized(meta_json, data, metric: Distance, count: int = 0, device: in
     return _LoadedStorage(h, device, metric)
 
 
+class SparseIndexKind(enum.IntEnum):  # qb_sparse_kind
+    Ram = 0           # InvertedIndexRam: search may prune
+    Compressed = 1    # the immutable / mmap compressed indexes with f32 weights: never prunes
+    CompressedF16 = 2
+    CompressedU8 = 3
+
+
+def _csr(vectors):
+    """(indptr, dims, weights) as given, or a list of (dims, weights) pairs -> u64 offsets, u32 dims, f32 weights"""
+    if isinstance(vectors, tuple) and len(vectors) == 3:
+        indptr, dims, weights = vectors
+    else:
+        vectors = list(vectors)
+        indptr = np.zeros(len(vectors) + 1, np.uint64)
+        indptr[1:] = np.cumsum([len(d) for d, _ in vectors])
+        dims = np.concatenate([np.asarray(d, np.uint32) for d, _ in vectors]) if vectors else np.zeros(0, np.uint32)
+        weights = np.concatenate([np.asarray(w, np.float32) for _, w in vectors]) if vectors else np.zeros(0, np.float32)
+    indptr = np.ascontiguousarray(indptr, np.uint64)
+    dims = np.ascontiguousarray(dims, np.uint32)
+    weights = np.ascontiguousarray(weights, np.float32)
+    if dims.size != weights.size or indptr.size == 0:
+        raise ValueError("sparse vectors: dims and weights differ in length, or no offsets")
+    return indptr, dims, weights
+
+
+class SparseVectorIndex:
+    """An inverted index over sparse vectors in HBM and the reference's SearchContext over it (qb_sparse_*).  Points and queries are
+    CSR triples (indptr, dims, weights) or lists of (dims, weights) pairs, with internal dims (the caller's IndicesTracker remapping)."""
+
+    def __init__(self, vectors, n_dims: int, kind: SparseIndexKind = SparseIndexKind.Ram, device: int = 0):
+        indptr, dims, weights = _csr(vectors)
+        self._h = vp()
+        h = vp()
+        check(lib().qb_sparse_index_create(int(device), int(kind), indptr.size - 1, int(n_dims), indptr.ctypes.data_as(u64p), dims.ctypes.data_as(u32p),
+                                           weights.ctypes.data_as(f32p), C.byref(h)))
+        self._h = h
+        self.count, self.n_dims = indptr.size - 1, int(n_dims)
+
+    def info(self) -> tuple[int, int, int, int]:
+        """(points, dims, posting elements, HBM bytes)"""
+        n, d, e, b = C.c_uint32(), C.c_uint32(), C.c_uint64(), C.c_uint64()
+        check(lib().qb_sparse_index_info(self._h, C.byref(n), C.byref(d), C.byref(e), C.byref(b)))
+        return n.value, d.value, e.value, b.value
+
+    @staticmethod
+    def _stop(is_stopped):
+        if is_stopped is None:
+            return None
+        return is_stopped if isinstance(is_stopped, C.c_int32) else C.c_int32(int(bool(is_stopped)))
+
+    def search(self, queries, top: int, point_deleted=None, is_stopped=None, counters: Optional[HwCounters] = None):
+        """SearchContext::search per query -> list of SCORED_POINT_OFFSET arrays, (score desc, id asc)"""
+        qp, qd, qw = _csr(queries)
+        nq = qp.size - 1
+        out = np.zeros((nq, max(int(top), 1)), dtype=SCORED_POINT_OFFSET)
+        counts = np.zeros(nq, dtype=np.uint32)
+        bm = _bitmap(point_deleted, self.count)
+        stop = self._stop(is_stopped)
+        check(lib().qb_sparse_search_batch(self._h, qp.ctypes.data_as(u64p), qd.ctypes.data_as(u32p), qw.ctypes.data_as(f32p), nq, int(top),
+                                           None if bm is None else bm.ctypes.data_as(u64p), None if stop is None else C.byref(stop),
+                                           out.ctypes.data_as(C.POINTER(ScoredPoint)), counts.ctypes.data_as(u32p),
+                                           None if counters is None else C.byref(counters)))
+        return [out[i, : counts[i]].copy() for i in range(nq)]
+
+    def search_plain(self, queries, id_lists, top: int, is_stopped=None, counters: Optional[HwCounters] = None):
+        """SearchContext::plain_search per query over its own (already filtered) ids -> list of SCORED_POINT_OFFSET arrays"""
+        qp, qd, qw = _csr(queries)
+        nq = qp.size - 1
+        lists = [np.asarray(x, np.uint32) for x in id_lists]
+        if len(lists) != nq:
+            raise ValueError(f"{len(lists)} id lists for {nq} queries")
+        ip = np.zeros(nq + 1, np.uint64)
+        ip[1:] = np.cumsum([x.size for x in lists])
+        ids = np.ascontiguousarray(np.concatenate(lists) if lists else np.zeros(0, np.uint32), np.uint32)
+        out = np.zeros((nq, max(int(top), 1)), dtype=SCORED_POINT_OFFSET)
+        counts = np.zeros(nq, dtype=np.uint32)
+        stop = self._stop(is_stopped)
+        check(lib().qb_sparse_search_plain_batch(self._h, qp.ctypes.data_as(u64p), qd.ctypes.data_as(u32p), qw.ctypes.data_as(f32p), nq,
+                                                 ip.ctypes.data_as(u64p), ids.ctypes.data_as(u32p), int(top), None if stop is None else C.byref(stop),
+                                                 out.ctypes.data_as(C.POINTER(ScoredPoint)), counts.ctypes.data_as(u32p),
+                                                 None if counters is None else C.byref(counters)))
+        return [out[i, : counts[i]].copy() for i in range(nq)]
+
+    def close(self):
+        if self._h:
+            lib().qb_sparse_index_destroy(self._h)
+            self._h = vp()
+
+    def __del__(self):
+        try:
+            if sys is None or sys.is_finalizing():
+                return
+            self.close()
+        except Exception:
+            pass
+
+
 def set_option(name: str, value: int) -> None:
     """Debugging / experiment switches of the library (qb_set_option)."""
     check(lib().qb_set_option(name.encode(), int(value)))

@@ -11,8 +11,8 @@ OUT = os.path.join(ROOT, "bindings", "rust", "src", "ffi.rs")
 
 SCALARS = {"int32_t": "i32", "uint32_t": "u32", "uint64_t": "u64", "int64_t": "i64", "uint8_t": "u8", "size_t": "usize", "float": "f32", "double": "f64",
            "int": "i32", "qb_status": "qb_status", "char": "c_char", "void": "c_void"}
-ENUMS = ("qb_distance", "qb_dtype", "qb_qdistance", "qb_bq_encoding", "qb_bq_query_encoding", "qb_query_kind", "qb_hnsw_algorithm")
-OPAQUE = ("qb_storage", "qb_scorer", "qb_hnsw", "qb_comm")
+ENUMS = ("qb_distance", "qb_dtype", "qb_qdistance", "qb_bq_encoding", "qb_bq_query_encoding", "qb_query_kind", "qb_hnsw_algorithm", "qb_sparse_kind")
+OPAQUE = ("qb_storage", "qb_scorer", "qb_hnsw", "qb_comm", "qb_sparse_index")
 STRUCTS = ("qb_scored_point", "qb_hw_counters")
 
 
@@ -71,7 +71,9 @@ def main():
           "pub const QB_DT_F32: i32 = 0; pub const QB_DT_F16: i32 = 1; pub const QB_DT_U8: i32 = 2;",
           "pub const QB_QD_COSINE: i32 = 0; pub const QB_QD_DOT: i32 = 1; pub const QB_QD_L1: i32 = 2; pub const QB_QD_L2: i32 = 3;",
           "// qb_hnsw_algorithm (SearchAlgorithm, graph_layers.rs:80-84)",
-          "pub const QB_HNSW_ALGO_HNSW: i32 = 0; pub const QB_HNSW_ALGO_ACORN: i32 = 1;", ""]
+          "pub const QB_HNSW_ALGO_HNSW: i32 = 0; pub const QB_HNSW_ALGO_ACORN: i32 = 1;",
+          "// qb_sparse_kind: InvertedIndexRam (may prune), the compressed indexes with f32 / f16 / u8 weights",
+          "pub const QB_SPARSE_RAM: i32 = 0; pub const QB_SPARSE_COMPRESSED: i32 = 1; pub const QB_SPARSE_COMPRESSED_F16: i32 = 2; pub const QB_SPARSE_COMPRESSED_U8: i32 = 3;", ""]
     for name in OPAQUE:
         o += ["#[repr(C)]", f"pub struct {name} {{ _private: [u8; 0] }}"]
     o += ["", "/// Same layout as `common::types::ScoredPointOffset` (`#[repr(C)] { idx: u32, score: f32 }`).", "#[repr(C)]", "#[derive(Copy, Clone, Default, Debug, PartialEq)]",
