@@ -33,6 +33,8 @@ pub struct qb_hnsw { _private: [u8; 0] }
 pub struct qb_comm { _private: [u8; 0] }
 #[repr(C)]
 pub struct qb_sparse_index { _private: [u8; 0] }
+#[repr(C)]
+pub struct qb_sparse_storage { _private: [u8; 0] }
 
 /// Same layout as `common::types::ScoredPointOffset` (`#[repr(C)] { idx: u32, score: f32 }`).
 #[repr(C)]
@@ -140,6 +142,11 @@ extern "C" {
     pub fn qb_sparse_search_batch(idx: *mut qb_sparse_index, q_indptr: *const u64, q_dims: *const u32, q_weights: *const f32, n_queries: u32, top: u32, deleted_bitmap: *const u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters) -> qb_status;
     pub fn qb_sparse_search_batch_device(idx: *mut qb_sparse_index, dev_q_indptr: *const u64, dev_q_dims: *const u32, dev_q_weights: *const f32, n_queries: u32, max_query_nnz: u32, top: u32, dev_deleted_bitmap: *const u64, dev_out: *mut qb_scored_point, dev_out_counts: *mut u32) -> qb_status;
     pub fn qb_sparse_search_plain_batch(idx: *mut qb_sparse_index, q_indptr: *const u64, q_dims: *const u32, q_weights: *const f32, n_queries: u32, id_indptr: *const u64, ids: *const u32, top: u32, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters) -> qb_status;
+    pub fn qb_sparse_storage_create(device: i32, n_points: u32, indptr: *const u64, dims: *const u32, weights: *const f32, on_disk: i32, out: *mut *mut qb_sparse_storage) -> qb_status;
+    pub fn qb_sparse_storage_destroy(s: *mut qb_sparse_storage);
+    pub fn qb_sparse_storage_info(s: *const qb_sparse_storage, n_points: *mut u32, n_elements: *mut u64, hbm_bytes: *mut u64) -> qb_status;
+    pub fn qb_sparse_search_custom_batch(s: *mut qb_sparse_storage, kind: i32, n_a: u32, n_b: u32, ex_indptr: *const u64, ex_dims: *const u32, ex_weights: *const f32, coef: *const f32, n_queries: u32, top: u32, deleted_bitmap: *const u64, id_list: *const u32, n_ids: u64, is_stopped: *const i32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters) -> qb_status;
+    pub fn qb_sparse_score_custom(s: *mut qb_sparse_storage, kind: i32, n_a: u32, n_b: u32, ex_indptr: *const u64, ex_dims: *const u32, ex_weights: *const f32, coef: *const f32, ids: *const u32, n: u64, scores: *mut f32, counters: *mut qb_hw_counters) -> qb_status;
     pub fn qb_search_stats(s: *mut qb_storage, searches: *mut u64, reruns: *mut u64, reset: i32) -> qb_status;
     pub fn qb_profile_enable(s: *mut qb_storage, on: i32) -> qb_status;
     pub fn qb_profile_read(s: *mut qb_storage, launches: *mut u64, total_ms: *mut f64, reset: i32) -> qb_status;

@@ -5,4 +5,4 @@ pub mod batch_searcher;  // BatchFilteredSearcher::peek_top_* + oversample / res
 pub mod hnsw;            // GraphLayers::search, batched, traversal on the device
 pub mod sharded;         // per-GPU segments + device-side BatchResultAggregator
 pub mod mmr;             // maximal marginal relevance reranking
-pub mod sparse;          // sparse vectors: inverted index, SearchContext::search / plain_search
+pub mod sparse;          // sparse vectors: inverted index, SearchContext::search / plain_search; the storage's custom-query scan

@@ -783,6 +783,49 @@ QB_API qb_status qb_sparse_search_plain_batch(qb_sparse_index* idx, const uint64
                                               const volatile int32_t* is_stopped, qb_scored_point* out, uint32_t* out_counts,
                                               qb_hw_counters* counters /* optional */);
 
+/* The segment's sparse vector storage (SparseVectorStorage) and the custom queries over it: every sparse query that is not Nearest
+ * (recommend, discover, context, feedback) skips the inverted index and scans the storage (sparse_vector_index/read_view/search.rs:99-151,
+ * 302-341) with SparseCustomQueryScorer (query_scorer/sparse_custom_query_scorer.rs).  Dims here are USER dims (any u32): the scorer
+ * merges the stored vectors with the examples in user-dim order, which the index's internal dims do not keep. */
+typedef struct qb_sparse_storage qb_sparse_storage;
+/* n_points rows in CSR form as qb_sparse_index_create takes them, in user dims; each row is sorted by dim on creation.  QB_ERR_INVALID for a
+ * null argument, offsets that descend or do not start at 0, a dim repeated within a row or a weight that is not finite.  2^32 - 1 or more
+ * elements: QB_ERR_UNSUPPORTED.  on_disk != 0: an mmap storage, whose reads count vector_io_read (multiplier 4, size_of::<DimId>()); 0: an
+ * in-memory storage (multiplier 0).  HBM: 8 bytes per element and 8 per point.  Synchronous. */
+QB_API qb_status qb_sparse_storage_create(int32_t device, uint32_t n_points, const uint64_t* indptr, const uint32_t* dims, const float* weights,
+                                          int32_t on_disk, qb_sparse_storage** out);
+QB_API void qb_sparse_storage_destroy(qb_sparse_storage* s);
+QB_API qb_status qb_sparse_storage_info(const qb_sparse_storage* s, uint32_t* n_points, uint64_t* n_elements, uint64_t* hbm_bytes);
+/* search_scored per query: peek_top_iter over the scored points with a SparseCustomQueryScorer.
+ *   kind, n_a, n_b  one kind and one shape per call, as qb_hnsw_search_custom_batch takes them; query q has E = qb_custom_examples(kind,
+ *                   n_a, n_b) examples in the qb_scorer_create_custom order (feedback: the target, then n_a pairs).  E above 256:
+ *                   QB_ERR_UNSUPPORTED
+ *   ex_indptr, ex_dims, ex_weights   example j of query q is CSR entry q * E + j (n_queries * E + 1 offsets from 0), user dims, any order;
+ *                   more than 4096 non-zeros over one query's examples: QB_ERR_UNSUPPORTED.  Weights are not checked
+ *   coef            QB_QUERY_FEEDBACK_NAIVE: n_queries x (1 + n_a) values [a, partial_computation of pair 0, ...]; NULL otherwise
+ *   deleted_bitmap  optional, ceil(n_points / 64) words, bit = 1 deleted
+ *   id_list         optional, n_ids distinct ids < n_points shared by the whole batch (the reference's prefiltered_points); the scored points
+ *                   are the listed ids that are not deleted, or every point that is not deleted when id_list is NULL
+ *   is_stopped      optional, polled before the launch (QB_ERR_CANCELLED)
+ *   out             n_queries x top in (score desc, id asc) order, out_counts[q] valid entries; NaN ranks above everything (OrderedFloat)
+ * A point's similarity to an example is score_vectors (sparse_vector.rs:66-90): both sides sorted by dim, 0 + sum of example weight x stored
+ * weight over the shared dims in ascending dim order, every product and sum rounded, +0.0 when no dim is shared; the E similarities are
+ * folded by Query::score_by as in qb_scorer_create_custom.  top in 1..4096 (0: QB_ERR_INVALID, above: QB_ERR_UNSUPPORTED).
+ * Counters, summed over the batch: per scored point of |v| stored elements, cpu += 4 x the sum over the examples of (|v| + |example|), every
+ * given example element counted; vector_io_read += 2 |v| x (4 on disk, else 0).  QB_ERR_INVALID, checked before any device work: a null
+ * argument, an unknown kind or a shape qb_scorer_create_custom rejects, example offsets that descend or do not start at 0, a dim repeated
+ * within an example, feedback without coef, top 0, an id >= n_points or repeated in id_list.  Synchronous. */
+QB_API qb_status qb_sparse_search_custom_batch(qb_sparse_storage* s, qb_query_kind kind, uint32_t n_a, uint32_t n_b, const uint64_t* ex_indptr,
+                                               const uint32_t* ex_dims, const float* ex_weights, const float* coef, uint32_t n_queries, uint32_t top,
+                                               const uint64_t* deleted_bitmap, const uint32_t* id_list, uint64_t n_ids, const volatile int32_t* is_stopped,
+                                               qb_scored_point* out, uint32_t* out_counts, qb_hw_counters* counters /* optional */);
+/* score_stored_batch of ONE query (E examples, CSR entries 0 .. E - 1; coef = 1 + n_a values for feedback) over n given ids: scores[k] of
+ * ids[k], equal bit for bit to the scores qb_sparse_search_custom_batch ranks.  No filter.  Counters and errors as the batch entry (ids
+ * distinct and < n_points).  Synchronous. */
+QB_API qb_status qb_sparse_score_custom(qb_sparse_storage* s, qb_query_kind kind, uint32_t n_a, uint32_t n_b, const uint64_t* ex_indptr, const uint32_t* ex_dims,
+                                        const float* ex_weights, const float* coef, const uint32_t* ids, uint64_t n, float* scores,
+                                        qb_hw_counters* counters /* optional */);
+
 /* ---------------------------------------------------------------- profiling hooks ------------------- */
 /* Fused searches run a fast path first and rerun without it when the device reports that one of its assumptions did not
  * hold (candidate buffer overflow, a dot product outside the f32-exact window, a survivor segment full).  searches =

@@ -140,6 +140,12 @@ SIGNATURES = {
     "qb_sparse_search_batch_device": (C.c_int32, [vp, vp, vp, vp, C.c_uint32, C.c_uint32, C.c_uint32, vp, vp, vp]),
     "qb_sparse_search_plain_batch": (C.c_int32, [vp, u64p, u32p, f32p, C.c_uint32, u64p, u32p, C.c_uint32, i32p, C.POINTER(ScoredPoint), u32p,
                                                  C.POINTER(HwCounters)]),
+    "qb_sparse_storage_create": (C.c_int32, [C.c_int32, C.c_uint32, u64p, u32p, f32p, C.c_int32, C.POINTER(vp)]),
+    "qb_sparse_storage_destroy": (None, [vp]),
+    "qb_sparse_storage_info": (C.c_int32, [vp, u32p, u64p, u64p]),
+    "qb_sparse_search_custom_batch": (C.c_int32, [vp, C.c_int, C.c_uint32, C.c_uint32, u64p, u32p, f32p, f32p, C.c_uint32, C.c_uint32, u64p, u32p,
+                                                  C.c_uint64, i32p, C.POINTER(ScoredPoint), u32p, C.POINTER(HwCounters)]),
+    "qb_sparse_score_custom": (C.c_int32, [vp, C.c_int, C.c_uint32, C.c_uint32, u64p, u32p, f32p, f32p, u32p, C.c_uint64, f32p, C.POINTER(HwCounters)]),
     "qb_profile_enable": (C.c_int32, [vp, C.c_int32]),
     "qb_profile_read": (C.c_int32, [vp, u64p, C.POINTER(C.c_double), C.c_int32]),
 }

@@ -282,6 +282,14 @@ qb_status qb_launch_select(const unsigned long long* d_cand, const unsigned int*
                            cudaStream_t stream);
 qb_status qb_launch_fill_u32(unsigned int* p, unsigned int v, size_t n, cudaStream_t stream);
 
+// sparse rows (qb_sparse.cu): CSR rows sorted by (row, dim) into d_rdims / d_rw, the (dim, id) keys of the sorted elements into
+// d_post_keys; *h_flags: bit 0 a dim >= dim_bound (never with any_dim), bit 1 a non-finite weight, bit 2 a dim repeated within a row.
+// Synchronous on st
+qb_status qb_sparse_sort_rows(cudaStream_t st, uint32_t n_points, uint64_t n, const uint64_t* d_rptr, const uint32_t* dims, const float* weights,
+                              uint32_t dim_bound, bool any_dim, uint32_t* d_rdims, float* d_rw, unsigned long long* d_post_keys, unsigned int* h_flags);
+// QueryVector kinds beyond Nearest: examples per query (qb_custom.cu)
+uint32_t qb_custom_examples(int kind, uint32_t n_a, uint32_t n_b);
+
 // MMR reranking (qb_mmr.cu): nq lists of up to max_cand candidates (n_max bounds the counts), queries preprocessed ([nq][row_stride / 4]);
 // selections to d_out[q * out_stride ..), their number to d_out_counts, the candidates left after the dedup to d_n_unique.  d_scratch:
 // qb_mmr_scratch_bytes (Cosine: preprocessed candidate rows, the batch in chunks of a fixed budget)

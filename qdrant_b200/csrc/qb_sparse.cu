@@ -394,6 +394,58 @@ static qb_status sp_alloc(qb_sparse_index* x, T** p, size_t elems) {
     return QB_OK;
 }
 
+// The CSR rows (offsets already in d_rptr) sorted by (row, dim) into d_rdims / d_rw, with the checks of every element: bit 0 of
+// *h_flags a dim >= dim_bound (any_dim: no bound, every u32 is a dim), bit 1 a non-finite weight, bit 2 a dim repeated within a row.
+// d_post_keys (n entries) receives the (dim, id) keys of the sorted elements.  The index and the sparse vector storage (qb_sparse_custom.cu)
+// both build their rows here.  Synchronous.
+qb_status qb_sparse_sort_rows(cudaStream_t st, uint32_t n_points, uint64_t n, const uint64_t* d_rptr, const uint32_t* dims, const float* weights,
+                              uint32_t dim_bound, bool any_dim, uint32_t* d_rdims, float* d_rw, unsigned long long* d_post_keys, unsigned int* h_flags) {
+    unsigned long long *k0 = nullptr, *k1 = nullptr;
+    uint32_t* in_dims = nullptr; float* in_w = nullptr; unsigned int* flags = nullptr; void* tmp = nullptr;
+    size_t tmp_bytes = 0;
+    const int row_bits = 32 + std::max(1, 32 - __builtin_clz(std::max(n_points, 1u)));
+    // any_dim: the bound 0xFFFFFFFF flags only dim 0xFFFFFFFF, a valid dim; bit 0 is dropped
+    const unsigned int keep = any_dim ? ~1u : ~0u;
+    if (any_dim) dim_bound = 0xFFFFFFFFu;
+    if (n) QB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, k0, k1, in_w, d_rw, (int64_t)n, 0, row_bits, st));
+    *h_flags = 0;
+    auto run = [&]() -> qb_status {
+        QB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&flags), 16, st));
+        QB_CUDA(cudaMemsetAsync(flags, 0, 4, st));
+        if (n) {
+            QB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&k0), n * 8, st));
+            QB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&k1), n * 8, st));
+            QB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&in_dims), n * 4, st));
+            QB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&in_w), n * 4, st));
+            QB_CUDA(cudaMallocAsync(&tmp, std::max<size_t>(tmp_bytes, 16), st));
+            QB_CUDA(cudaMemcpyAsync(in_dims, dims, n * 4, cudaMemcpyHostToDevice, st));
+            QB_CUDA(cudaMemcpyAsync(in_w, weights, n * 4, cudaMemcpyHostToDevice, st));
+            if (n_points) {
+                sparse_row_keys_kernel<<<(n_points + 255) / 256, 256, 0, st>>>(d_rptr, n_points, in_dims, in_w, dim_bound, k0, flags);
+                QB_LAUNCHED();
+            }
+            // the index lays its lists out by dim: stop here when a dim is out of range
+            QB_CUDA(cudaMemcpyAsync(h_flags, flags, 4, cudaMemcpyDeviceToHost, st));
+            QB_CUDA(cudaStreamSynchronize(st));
+            if (*h_flags & keep) return QB_OK;
+            size_t b = tmp_bytes;
+            QB_CUDA(cub::DeviceRadixSort::SortPairs(tmp, b, k0, k1, in_w, d_rw, (int64_t)n, 0, row_bits, st));
+            sparse_posting_keys_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(k1, n, d_rdims, d_post_keys, flags);
+            QB_LAUNCHED();
+            QB_CUDA(cudaGetLastError());
+        }
+        QB_CUDA(cudaMemcpyAsync(h_flags, flags, 4, cudaMemcpyDeviceToHost, st));
+        return QB_OK;
+    };
+    const qb_status rc = run();
+    cudaFreeAsync(k0, st); cudaFreeAsync(k1, st); cudaFreeAsync(in_dims, st); cudaFreeAsync(in_w, st); cudaFreeAsync(tmp, st); cudaFreeAsync(flags, st);
+    const cudaError_t e = cudaStreamSynchronize(st);
+    QB_TRY(rc);
+    QB_CHECK(e == cudaSuccess, QB_ERR_CUDA, "sparse rows: %s", cudaGetErrorString(e));
+    *h_flags &= keep;
+    return QB_OK;
+}
+
 static qb_status sparse_build(qb_sparse_index* x, const uint64_t* indptr, const uint32_t* dims, const float* weights) {
     const uint64_t n = x->nnz;
     cudaStream_t st = x->stream;
@@ -406,58 +458,32 @@ static qb_status sparse_build(qb_sparse_index* x, const uint64_t* indptr, const 
     QB_TRY(sp_alloc(x, &x->d_dptr, (size_t)x->n_dims + 1));
     QB_CUDA(cudaMemcpyAsync(x->d_rptr, indptr, ((size_t)x->n_points + 1) * 8, cudaMemcpyHostToDevice, st));
     QB_CUDA(cudaMemsetAsync(x->d_dptr, 0, ((size_t)x->n_dims + 1) * 8, st));
-    // temporaries: the input dims / weights, two key arrays, the CUB scratch and the flags word
+    // the rows, then the posting lists: the (dim, id) keys sorted with the weights, split into ids and dim offsets
     unsigned long long *k0 = nullptr, *k1 = nullptr;
-    uint32_t* in_dims = nullptr; float* in_w = nullptr; unsigned int* flags = nullptr; void* tmp = nullptr;
-    size_t tmp_bytes = 0, t2 = 0;
-    const int row_bits = 32 + std::max(1, 32 - __builtin_clz(std::max(x->n_points, 1u)));
+    void* tmp = nullptr;
+    size_t tmp_bytes = 0;
     const int dim_bits = 32 + std::max(1, 32 - __builtin_clz(std::max(x->n_dims, 1u)));
-    if (n) {
-        QB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, k0, k1, in_w, x->d_rw, (int64_t)n, 0, row_bits, st));
-        QB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t2, k0, k1, x->d_rw, x->d_w, (int64_t)n, 0, dim_bits, st));
-    }
-    tmp_bytes = std::max(tmp_bytes, t2);
-    qb_status rc = QB_OK;
+    if (n) QB_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, k0, k1, x->d_rw, x->d_w, (int64_t)n, 0, dim_bits, st));
     unsigned int h_flags = 0;
     auto run = [&]() -> qb_status {
-        QB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&flags), 16, st));
-        QB_CUDA(cudaMemsetAsync(flags, 0, 4, st));
-        if (n) {
-            QB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&k0), n * 8, st));
-            QB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&k1), n * 8, st));
-            QB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&in_dims), n * 4, st));
-            QB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&in_w), n * 4, st));
-            QB_CUDA(cudaMallocAsync(&tmp, std::max<size_t>(tmp_bytes, 16), st));
-            QB_CUDA(cudaMemcpyAsync(in_dims, dims, n * 4, cudaMemcpyHostToDevice, st));
-            QB_CUDA(cudaMemcpyAsync(in_w, weights, n * 4, cudaMemcpyHostToDevice, st));
-            if (x->n_points) {
-                sparse_row_keys_kernel<<<(x->n_points + 255) / 256, 256, 0, st>>>(x->d_rptr, x->n_points, in_dims, in_w, x->n_dims, k0, flags);
-                QB_LAUNCHED();
-            }
-            // the lists are laid out by dim: stop here when a dim is out of range
-            QB_CUDA(cudaMemcpyAsync(&h_flags, flags, 4, cudaMemcpyDeviceToHost, st));
-            QB_CUDA(cudaStreamSynchronize(st));
-            if (h_flags) return QB_OK;
-            size_t b = tmp_bytes;
-            QB_CUDA(cub::DeviceRadixSort::SortPairs(tmp, b, k0, k1, in_w, x->d_rw, (int64_t)n, 0, row_bits, st));
-            const unsigned g = (unsigned)((n + 255) / 256);
-            sparse_posting_keys_kernel<<<g, 256, 0, st>>>(k1, n, x->d_rdims, k0, flags);
+        if (n) QB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&k0), n * 8, st));
+        QB_TRY(qb_sparse_sort_rows(st, x->n_points, n, x->d_rptr, dims, weights, x->n_dims, false, x->d_rdims, x->d_rw, k0, &h_flags));
+        if (!n || h_flags) return QB_OK;
+        QB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&k1), n * 8, st));
+        QB_CUDA(cudaMallocAsync(&tmp, std::max<size_t>(tmp_bytes, 16), st));
+        size_t b = tmp_bytes;
+        QB_CUDA(cub::DeviceRadixSort::SortPairs(tmp, b, k0, k1, x->d_rw, x->d_w, (int64_t)n, 0, dim_bits, st));
+        sparse_split_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(k1, n, x->n_dims, x->d_ids, x->d_dptr);
+        QB_LAUNCHED();
+        if (x->n_dims) {
+            sparse_max_next_kernel<<<(unsigned)(((uint64_t)x->n_dims * 32 + 255) / 256), 256, 0, st>>>(x->d_dptr, x->n_dims, x->d_w, x->d_mnw);
             QB_LAUNCHED();
-            b = tmp_bytes;
-            QB_CUDA(cub::DeviceRadixSort::SortPairs(tmp, b, k0, k1, x->d_rw, x->d_w, (int64_t)n, 0, dim_bits, st));
-            sparse_split_kernel<<<g, 256, 0, st>>>(k1, n, x->n_dims, x->d_ids, x->d_dptr);
-            QB_LAUNCHED();
-            if (x->n_dims) {
-                sparse_max_next_kernel<<<(unsigned)(((uint64_t)x->n_dims * 32 + 255) / 256), 256, 0, st>>>(x->d_dptr, x->n_dims, x->d_w, x->d_mnw);
-                QB_LAUNCHED();
-            }
-            QB_CUDA(cudaGetLastError());
         }
-        QB_CUDA(cudaMemcpyAsync(&h_flags, flags, 4, cudaMemcpyDeviceToHost, st));
+        QB_CUDA(cudaGetLastError());
         return QB_OK;
     };
-    rc = run();
-    cudaFreeAsync(k0, st); cudaFreeAsync(k1, st); cudaFreeAsync(in_dims, st); cudaFreeAsync(in_w, st); cudaFreeAsync(tmp, st); cudaFreeAsync(flags, st);
+    const qb_status rc = run();
+    cudaFreeAsync(k0, st); cudaFreeAsync(k1, st); cudaFreeAsync(tmp, st);
     const cudaError_t e = cudaStreamSynchronize(st);
     QB_TRY(rc);
     QB_CHECK(e == cudaSuccess, QB_ERR_CUDA, "sparse_index_create: %s", cudaGetErrorString(e));

@@ -405,7 +405,7 @@ private:
     qb_comm* c_ = nullptr;
 };
 
-// A sparse vector: internal dims (the segment's IndicesTracker remapping) and their weights
+// A sparse vector: internal dims (the segment's IndicesTracker remapping) for SparseVectorIndex, user dims for SparseVectorStorage
 struct SparseVector {
     std::vector<uint32_t> indices;
     std::vector<float> values;
@@ -456,6 +456,7 @@ public:
     }
 
 private:
+    friend class SparseVectorStorage;
     static void flatten(const std::vector<SparseVector>& v, std::vector<uint64_t>& ptr, std::vector<uint32_t>& dims, std::vector<float>& w) {
         for (const auto& x : v) {
             if (x.indices.size() != x.values.size()) throw OperationError(QB_ERR_INVALID, "sparse vector: indices and values differ in length");
@@ -470,6 +471,54 @@ private:
         return out;
     }
     qb_sparse_index* h_ = nullptr;
+};
+
+// The sparse vector storage of a named vector, in user dims, and search_scored over it: the recommend / discover / context / feedback
+// queries, which skip the inverted index (peek_top_iter with a SparseCustomQueryScorer).  One kind and shape per call: `examples` holds
+// E = qb_custom_examples(kind, n_a, n_b) examples per query in the qb_scorer_create_custom order; `coef` [a, partial...] per query for
+// feedback.  `id_list` (optional) is shared by the batch.
+class SparseVectorStorage {
+public:
+    SparseVectorStorage(const std::vector<SparseVector>& points, bool on_disk = false, int device = 0) {
+        std::vector<uint64_t> indptr(1, 0);
+        std::vector<uint32_t> dims;
+        std::vector<float> w;
+        SparseVectorIndex::flatten(points, indptr, dims, w);
+        check(qb_sparse_storage_create(device, (uint32_t)points.size(), indptr.data(), dims.data(), w.data(), on_disk ? 1 : 0, &h_));
+    }
+    ~SparseVectorStorage() { qb_sparse_storage_destroy(h_); }
+    SparseVectorStorage(const SparseVectorStorage&) = delete;
+    SparseVectorStorage& operator=(const SparseVectorStorage&) = delete;
+
+    std::vector<std::vector<ScoredPointOffset>> search_custom(qb_query_kind kind, const std::vector<SparseVector>& examples, uint32_t n_a, uint32_t n_b,
+                                                              const std::vector<float>* coef, uint32_t top, const uint64_t* deleted_bitmap = nullptr,
+                                                              const std::vector<PointOffsetType>* id_list = nullptr, qb_hw_counters* counters = nullptr) const {
+        std::vector<uint64_t> ep(1, 0);
+        std::vector<uint32_t> ed;
+        std::vector<float> ew;
+        SparseVectorIndex::flatten(examples, ep, ed, ew);
+        const uint32_t e = kind == QB_QUERY_RECO_BEST_SCORE || kind == QB_QUERY_RECO_SUM_SCORES ? n_a + n_b : kind == QB_QUERY_CONTEXT ? 2 * n_a : 1 + 2 * n_a;
+        const size_t nq = e ? examples.size() / e : 0;
+        std::vector<ScoredPointOffset> flat(nq * (size_t)top);
+        std::vector<uint32_t> counts(nq);
+        check(qb_sparse_search_custom_batch(h_, kind, n_a, n_b, ep.data(), ed.data(), ew.data(), coef ? coef->data() : nullptr, (uint32_t)nq, top, deleted_bitmap,
+                                            id_list ? id_list->data() : nullptr, id_list ? id_list->size() : 0, nullptr, flat.data(), counts.data(), counters));
+        return SparseVectorIndex::split(flat, counts, top);
+    }
+    std::vector<float> score_custom(qb_query_kind kind, const std::vector<SparseVector>& examples, uint32_t n_a, uint32_t n_b, const std::vector<float>* coef,
+                                    const std::vector<PointOffsetType>& ids, qb_hw_counters* counters = nullptr) const {
+        std::vector<uint64_t> ep(1, 0);
+        std::vector<uint32_t> ed;
+        std::vector<float> ew;
+        SparseVectorIndex::flatten(examples, ep, ed, ew);
+        std::vector<float> scores(ids.size());
+        check(qb_sparse_score_custom(h_, kind, n_a, n_b, ep.data(), ed.data(), ew.data(), coef ? coef->data() : nullptr, ids.data(), ids.size(), scores.data(),
+                                     counters));
+        return scores;
+    }
+
+private:
+    qb_sparse_storage* h_ = nullptr;
 };
 
 }  // namespace qdrant_b200

@@ -861,6 +861,84 @@ class SparseVectorIndex:
             pass
 
 
+class SparseVectorStorage:
+    """The sparse vector storage of a named vector in HBM, in user dims, and search_scored over it (qb_sparse_storage_*): the
+    recommend / discover / context / feedback queries, which skip the inverted index.  Points are a CSR triple (indptr, dims, weights) or
+    a list of (dims, weights) pairs; on_disk=True counts vector_io_read as an mmap storage does."""
+
+    def __init__(self, vectors, on_disk: bool = False, device: int = 0):
+        indptr, dims, weights = _csr(vectors)
+        self._h = vp()
+        h = vp()
+        check(lib().qb_sparse_storage_create(int(device), indptr.size - 1, indptr.ctypes.data_as(u64p), dims.ctypes.data_as(u32p),
+                                             weights.ctypes.data_as(f32p), int(bool(on_disk)), C.byref(h)))
+        self._h = h
+        self.count = indptr.size - 1
+
+    def info(self) -> tuple[int, int, int]:
+        """(points, elements, HBM bytes)"""
+        n, e, b = C.c_uint32(), C.c_uint64(), C.c_uint64()
+        check(lib().qb_sparse_storage_info(self._h, C.byref(n), C.byref(e), C.byref(b)))
+        return n.value, e.value, b.value
+
+    @staticmethod
+    def _examples(examples, kind: int, n_a: int, n_b: int):
+        """a CSR triple over queries x E examples, or one list of E (dims, weights) pairs per query -> (CSR, queries)"""
+        n_ex = {1: n_a + n_b, 2: n_a + n_b, 3: 1 + 2 * n_a, 4: 2 * n_a, 5: 1 + 2 * n_a}.get(kind, 0)
+        if isinstance(examples, tuple) and len(examples) == 3:
+            csr = _csr(examples)
+        else:
+            flat = [e for q in examples for e in q]
+            if any(len(q) != n_ex for q in examples):
+                raise ValueError(f"every query needs {n_ex} examples")
+            csr = _csr(flat) if flat else (np.zeros(1, np.uint64), np.zeros(0, np.uint32), np.zeros(0, np.float32))
+        return csr, ((csr[0].size - 1) // n_ex if n_ex else 0)
+
+    def search_custom(self, kind: QueryKind, examples, n_a: int, n_b: int = 0, coef=None, top: int = 10, point_deleted=None, id_list=None,
+                      is_stopped=None, counters: Optional[HwCounters] = None):
+        """search_scored per query (qb_sparse_search_custom_batch), one kind and shape per call: examples = one list of E (dims, weights)
+        pairs per query in the qb_scorer_create_custom order, or a CSR triple over queries x E; coef: [queries, 1 + n_a] for feedback;
+        id_list: the ids to score, shared by the batch -> list of SCORED_POINT_OFFSET arrays, (score desc, id asc)"""
+        (ep, ed, ew), nq = self._examples(examples, int(kind), n_a, n_b)
+        cf = None if coef is None else np.ascontiguousarray(_f32(coef).reshape(-1))
+        ids = None if id_list is None else _ids(id_list)
+        out = np.zeros((max(nq, 1), max(int(top), 1)), dtype=SCORED_POINT_OFFSET)
+        counts = np.zeros(max(nq, 1), dtype=np.uint32)
+        bm = _bitmap(point_deleted, self.count)
+        stop = SparseVectorIndex._stop(is_stopped)
+        check(lib().qb_sparse_search_custom_batch(self._h, int(kind), int(n_a), int(n_b), ep.ctypes.data_as(u64p), ed.ctypes.data_as(u32p),
+                                                  ew.ctypes.data_as(f32p), None if cf is None else cf.ctypes.data_as(f32p), nq, int(top),
+                                                  None if bm is None else bm.ctypes.data_as(u64p), None if ids is None else ids.ctypes.data_as(u32p),
+                                                  0 if ids is None else ids.size, None if stop is None else C.byref(stop),
+                                                  out.ctypes.data_as(C.POINTER(ScoredPoint)), counts.ctypes.data_as(u32p),
+                                                  None if counters is None else C.byref(counters)))
+        return [out[i, : counts[i]].copy() for i in range(nq)]
+
+    def score_points_custom(self, kind: QueryKind, examples, n_a: int, n_b: int, ids, coef=None, counters: Optional[HwCounters] = None) -> np.ndarray:
+        """score_stored_batch of ONE query (examples: its E (dims, weights) pairs) over ids (qb_sparse_score_custom) -> f32 scores"""
+        (ep, ed, ew), _ = self._examples([list(examples)] if not (isinstance(examples, tuple) and len(examples) == 3) else examples, int(kind), n_a, n_b)
+        cf = None if coef is None else np.ascontiguousarray(_f32(coef).reshape(-1))
+        ids = _ids(ids)
+        scores = np.zeros(ids.size, np.float32)
+        check(lib().qb_sparse_score_custom(self._h, int(kind), int(n_a), int(n_b), ep.ctypes.data_as(u64p), ed.ctypes.data_as(u32p), ew.ctypes.data_as(f32p),
+                                           None if cf is None else cf.ctypes.data_as(f32p), ids.ctypes.data_as(u32p), ids.size, scores.ctypes.data_as(f32p),
+                                           None if counters is None else C.byref(counters)))
+        return scores
+
+    def close(self):
+        if self._h:
+            lib().qb_sparse_storage_destroy(self._h)
+            self._h = vp()
+
+    def __del__(self):
+        try:
+            if sys is None or sys.is_finalizing():
+                return
+            self.close()
+        except Exception:
+            pass
+
+
 def set_option(name: str, value: int) -> None:
     """Debugging / experiment switches of the library (qb_set_option)."""
     check(lib().qb_set_option(name.encode(), int(value)))

@@ -12,7 +12,7 @@ OUT = os.path.join(ROOT, "bindings", "rust", "src", "ffi.rs")
 SCALARS = {"int32_t": "i32", "uint32_t": "u32", "uint64_t": "u64", "int64_t": "i64", "uint8_t": "u8", "size_t": "usize", "float": "f32", "double": "f64",
            "int": "i32", "qb_status": "qb_status", "char": "c_char", "void": "c_void"}
 ENUMS = ("qb_distance", "qb_dtype", "qb_qdistance", "qb_bq_encoding", "qb_bq_query_encoding", "qb_query_kind", "qb_hnsw_algorithm", "qb_sparse_kind")
-OPAQUE = ("qb_storage", "qb_scorer", "qb_hnsw", "qb_comm", "qb_sparse_index")
+OPAQUE = ("qb_storage", "qb_scorer", "qb_hnsw", "qb_comm", "qb_sparse_index", "qb_sparse_storage")
 STRUCTS = ("qb_scored_point", "qb_hw_counters")
 
 
