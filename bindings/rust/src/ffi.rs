@@ -135,6 +135,7 @@ extern "C" {
     pub fn qb_mmr_batch_device(s: *mut qb_storage, dev_queries: *const f32, n_queries: u32, dev_lambdas: *const f32, dev_candidates: *const qb_scored_point, dev_candidate_counts: *const u32, max_candidates: u32, limit: u32, dev_out: *mut qb_scored_point, dev_out_counts: *mut u32) -> qb_status;
     pub fn qb_mmr_maxsim_batch(tokens: *mut qb_storage, point_offsets: *const u32, n_points: u32, query_vectors: *const f32, query_offsets: *const u32, n_queries: u32, lambdas: *const f32, candidates: *const qb_scored_point, candidate_counts: *const u32, max_candidates: u32, limit: u32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters) -> qb_status;
     pub fn qb_mmr_maxsim_batch_device(tokens: *mut qb_storage, point_offsets: *const u32, n_points: u32, dev_query_vectors: *const f32, n_query_vectors: u32, dev_query_offsets: *const u32, n_queries: u32, max_query_vectors: u32, dev_lambdas: *const f32, dev_candidates: *const qb_scored_point, dev_candidate_counts: *const u32, max_candidates: u32, limit: u32, dev_out: *mut qb_scored_point, dev_out_counts: *mut u32) -> qb_status;
+    pub fn qb_mmr_sparse_batch(s: *mut qb_sparse_storage, q_indptr: *const u64, q_dims: *const u32, q_weights: *const f32, n_queries: u32, lambdas: *const f32, candidates: *const qb_scored_point, candidate_counts: *const u32, max_candidates: u32, limit: u32, out: *mut qb_scored_point, out_counts: *mut u32, counters: *mut qb_hw_counters) -> qb_status;
     pub fn qb_sparse_index_create(device: i32, kind: i32, n_points: u32, n_dims: u32, indptr: *const u64, dims: *const u32, weights: *const f32, out: *mut *mut qb_sparse_index) -> qb_status;
     pub fn qb_sparse_index_destroy(idx: *mut qb_sparse_index);
     pub fn qb_sparse_index_info(idx: *const qb_sparse_index, n_points: *mut u32, n_dims: *mut u32, n_elements: *mut u64, hbm_bytes: *mut u64) -> qb_status;

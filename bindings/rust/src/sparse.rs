@@ -3,7 +3,8 @@
 //! passes internal dims; `search` replaces `SearchContext::search`, `plain_search` replaces `SearchContext::plain_search` over the
 //! prefiltered points.  `Ram` may prune like `InvertedIndexRam`; `Compressed` never prunes, like the compressed indexes with f32 weights.
 //! `B200SparseStorage` holds the segment's sparse vector storage in user dims and replaces `search_scored` for the queries that are not
-//! Nearest (recommend, discover, context, feedback), which skip the inverted index.
+//! Nearest (recommend, discover, context, feedback), which skip the inverted index, and the MMR rerank of sparse candidates (`mmr`), which
+//! replaces `mmr_from_points_with_vector` for a sparse named vector.
 use common::counter::hardware_counter::HardwareCounterCell;
 use common::types::{PointOffsetType, ScoredPointOffset};
 
@@ -154,6 +155,33 @@ impl B200SparseStorage {
         hc.cpu_counter().incr_delta(counters.cpu as usize);
         hc.vector_io_read().incr_delta(counters.vector_io_read as usize);
         Ok(scores)
+    }
+
+    /// MMR over sparse candidates whose vectors are this storage's points: `queries[q]` in user dims (any order), `candidates[q]` are
+    /// (point id, score) pairs (at most 16 384), `lambdas[q]` = 1 - diversity.  Returns each query's selection, in selection order, with
+    /// the candidates' own scores.
+    pub fn mmr(&self, queries: &[&SparseVector], candidates: &[&[ScoredPointOffset]], lambdas: &[f32], limit: usize,
+               hc: &HardwareCounterCell) -> OperationResult<Vec<Vec<ScoredPointOffset>>> {
+        let nq = queries.len();
+        let (ptr, dims, w) = flatten_user(queries);
+        let max_c = candidates.iter().map(|c| c.len()).max().unwrap_or(0);
+        let mut cand = vec![qb_scored_point { idx: 0, score: 0.0 }; nq * max_c.max(1)];
+        let mut counts = Vec::with_capacity(nq);
+        for (q, c) in candidates.iter().enumerate() {
+            for (i, p) in c.iter().enumerate() { cand[q * max_c + i] = qb_scored_point { idx: p.idx as PointOffsetType, score: p.score }; }
+            counts.push(c.len() as u32);
+        }
+        let mut out = vec![qb_scored_point { idx: 0, score: 0.0 }; nq * limit.max(1)];
+        let mut out_counts = vec![0u32; nq];
+        let mut counters = qb_hw_counters::default();
+        let st = unsafe {
+            qb_mmr_sparse_batch(self.raw, ptr.as_ptr(), dims.as_ptr(), w.as_ptr(), nq as u32, lambdas.as_ptr(), cand.as_ptr(), counts.as_ptr(), max_c as u32,
+                                limit as u32, out.as_mut_ptr(), out_counts.as_mut_ptr(), &mut counters)
+        };
+        if st != QB_OK { return Err(OperationError::service_error(last_error())); }
+        hc.cpu_counter().incr_delta(counters.cpu as usize);
+        hc.vector_io_read().incr_delta(counters.vector_io_read as usize);
+        Ok(B200SparseIndex::lists(&out, &out_counts, limit))
     }
 }
 

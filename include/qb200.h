@@ -69,6 +69,7 @@ typedef struct { uint64_t cpu; uint64_t vector_io_read; } qb_hw_counters;
 
 typedef struct qb_storage qb_storage;  /* one segment's vectors (dense or quantized) resident in HBM */
 typedef struct qb_scorer qb_scorer;    /* Box<dyn RawScorer>: a preprocessed/encoded query bound to a storage */
+typedef struct qb_sparse_storage qb_sparse_storage;   /* a sparse vector storage in user dims (qb_sparse_storage_create) */
 
 /* ---------------------------------------------------------------- library / device ------------------ */
 QB_API const char* qb_last_error(void);
@@ -723,6 +724,36 @@ QB_API qb_status qb_mmr_maxsim_batch_device(qb_storage* tokens, const uint32_t* 
                                             const float* dev_lambdas, const qb_scored_point* dev_candidates, const uint32_t* dev_candidate_counts,
                                             uint32_t max_candidates, uint32_t limit, qb_scored_point* dev_out, uint32_t* dev_out_counts);
 
+/* The same rerank over a sparse named vector: mmr_from_points_with_vector (mod.rs:42-157) puts the candidates' sparse vectors into a
+ * VolatileSparseVectorStorage (mod.rs:130), each sorted by dim on insertion (volatile_sparse_vector_storage.rs:214-226), and its
+ * LazyMatrix scores pairs with SparseMetricQueryScorer (query_scorer/sparse_metric_query_scorer.rs).
+ *   s           the qb_sparse_storage (below) holding the candidates' vectors; candidate ids are its point ids (< n_points)
+ *   query q     CSR entry [q_indptr[q], q_indptr[q+1]) of q_dims / q_weights in user dims, any order (offsets from 0, ascending).  It is
+ *               sorted by dim here, as VectorInternal::preprocess sorts it (vectors.rs:68-80) before NearestWithMmr becomes MmrInternal
+ *               (collection_query.rs:430, 472-480); its weights are not checked
+ *   lambdas, candidates, candidate_counts, max_candidates (<= 16384, else QB_ERR_UNSUPPORTED), limit, out, out_counts   as qb_mmr_batch
+ * Per query (mod.rs:42-279):
+ *   1. unique_by(id) keeps the first occurrence.  A candidate with an empty row is a vector: it stays and scores +0.0 against everything
+ *   2. fewer than two candidates are returned as they are; nothing is scored or counted (mod.rs:77-80)
+ *   3. rel[i] = score_vectors(q, v_i) (raw_scorer.rs:142-160, sparse_vector.rs:66-90): both sides sorted by dim, a sum from 0.0 of
+ *      q_w * v_w over the shared dims in ascending dim order, every product and sum rounded; no shared dim gives +0.0 (unwrap_or_default)
+ *   4. pair(c, s) = score_vectors(v_c, v_s), computed the first time (c, s) is needed (lazy_matrix.rs:45-67); symmetric bit for bit
+ *   5. the selection is qb_mmr_batch's: the first pick is the argmax of rel, each later pick the argmax of lambda * rel - (1 - lambda) *
+ *      max_sim in four rounded f32 operations, max_sim the max over the picks so far in pick order; every max / argmax keeps the last
+ *      maximum under OrderedFloat (NaN above everything, -0.0 == +0.0); the remaining candidates in IndexSet order, a pick swap_remove-d;
+ *      the output is the picks in order with their ORIGINAL scores
+ *   6. counters (SparseMetricQueryScorer: cpu multiplier 1, min(|a|, |b|) per scored pair): per query of n >= 2 unique candidates and L
+ *      picks, cpu += sum_i min(|q|, |v_i|) + sum over picks k = 1 .. L-1 of the sum over the candidates c remaining after pick k of
+ *      min(|v_c|, |v_pick_k|); vector_io_read += 0, since the volatile storage is in memory, also when s was created on_disk.
+ * Zero scores are common with sparse data (two rows without a shared dim), so plateaus of equal mmr values are frequent and the
+ * swap_remove position order decides them.
+ * Errors, checked before any device work: a null argument, limit = 0, a lambda NaN or outside [0, 1], query offsets that descend or do not
+ * start at 0, a dim repeated within a query, a count above max_candidates or an id >= n_points: QB_ERR_INVALID.  Synchronous. */
+QB_API qb_status qb_mmr_sparse_batch(qb_sparse_storage* s, const uint64_t* q_indptr, const uint32_t* q_dims, const float* q_weights,
+                                     uint32_t n_queries, const float* lambdas, const qb_scored_point* candidates,
+                                     const uint32_t* candidate_counts, uint32_t max_candidates, uint32_t limit,
+                                     qb_scored_point* out, uint32_t* out_counts, qb_hw_counters* counters /* optional */);
+
 /* ---------------------------------------------------------------- sparse vectors -------------------- */
 /* An inverted index over sparse vectors (SPLADE, BM25 and the like) and the reference's SearchContext over it
  * (lib/sparse/src/index/search_context.rs).  Dims are internal dims: the caller remaps its user dims as the segment's IndicesTracker
@@ -787,7 +818,6 @@ QB_API qb_status qb_sparse_search_plain_batch(qb_sparse_index* idx, const uint64
  * (recommend, discover, context, feedback) skips the inverted index and scans the storage (sparse_vector_index/read_view/search.rs:99-151,
  * 302-341) with SparseCustomQueryScorer (query_scorer/sparse_custom_query_scorer.rs).  Dims here are USER dims (any u32): the scorer
  * merges the stored vectors with the examples in user-dim order, which the index's internal dims do not keep. */
-typedef struct qb_sparse_storage qb_sparse_storage;
 /* n_points rows in CSR form as qb_sparse_index_create takes them, in user dims; each row is sorted by dim on creation.  QB_ERR_INVALID for a
  * null argument, offsets that descend or do not start at 0, a dim repeated within a row or a weight that is not finite.  2^32 - 1 or more
  * elements: QB_ERR_UNSUPPORTED.  on_disk != 0: an mmap storage, whose reads count vector_io_read (multiplier 4, size_of::<DimId>()); 0: an

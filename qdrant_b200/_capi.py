@@ -132,6 +132,8 @@ SIGNATURES = {
                                         C.POINTER(ScoredPoint), u32p, C.POINTER(HwCounters)]),
     "qb_mmr_maxsim_batch_device": (C.c_int32, [vp, u32p, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, vp, vp, vp, C.c_uint32, C.c_uint32, vp,
                                                vp]),
+    "qb_mmr_sparse_batch": (C.c_int32, [vp, u64p, u32p, f32p, C.c_uint32, f32p, C.POINTER(ScoredPoint), u32p, C.c_uint32, C.c_uint32,
+                                        C.POINTER(ScoredPoint), u32p, C.POINTER(HwCounters)]),
     "qb_sparse_index_create": (C.c_int32, [C.c_int32, C.c_int, C.c_uint32, C.c_uint32, u64p, u32p, f32p, C.POINTER(vp)]),
     "qb_sparse_index_destroy": (None, [vp]),
     "qb_sparse_index_info": (C.c_int32, [vp, u32p, u32p, u64p, u64p]),

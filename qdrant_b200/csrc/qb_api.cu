@@ -990,8 +990,6 @@ extern "C" qb_status qb_search_batch_device(qb_storage* s, const float* dev_quer
 }
 
 // ------------------------------------------------------------------------------------------------ MMR reranking
-constexpr uint32_t QB_MMR_MAX_CANDIDATES = 16384;   // candidates_limit's cap (api/src/rest/schema.rs:771); positions are u16 on the device
-
 // the checks both MMR entries make on the host before any device work
 static qb_status mmr_check(const qb_storage* s, uint32_t max_candidates, uint32_t limit, const char* who) {
     QB_CHECK(s->kind == QB_KIND_DENSE && s->dtype == QB_DT_F32, QB_ERR_UNSUPPORTED, "%s: the storage must be dense f32 (the reference scores MMR on a volatile f32 storage)", who);

@@ -206,6 +206,21 @@ qb_status qb_hnsw_inline_launch(qb_hnsw* g, const float* d_q_pre, uint32_t pre_s
 // adds the device counters to g->hops / g->evals / g->base_evals / g->mv_rows / g->mv_qrows and clears them; evals_by_slot (optional, [2]) receives each regular slot's scored points
 qb_status qb_hnsw_read_stats(qb_hnsw* g, cudaStream_t stream, uint64_t* evals_by_slot = nullptr);
 
+// A sparse vector storage (qb_sparse_custom.cu): CSR rows in user dims, read by the custom queries there and by the sparse MMR rerank
+// (qb_mmr_sparse.cu).  mu serialises the calls, which share the stream and the scratch.
+struct qb_sparse_storage {
+    int device = 0;
+    uint32_t n_points = 0;
+    uint64_t nnz = 0, hbm_bytes = 0;
+    int on_disk = 0;
+    cudaStream_t stream = nullptr;
+    uint64_t* d_rptr = nullptr; uint32_t* d_rdims = nullptr; float* d_rw = nullptr;   // rows in user dims, sorted by dim
+    std::vector<uint64_t> h_rptr;                                                      // the row offsets, for the counters
+    std::mutex mu;
+    void* d_scratch = nullptr; size_t scratch_bytes = 0;
+    int sm_count = 132;
+};
+
 // One rank of a sharded search (qb_comm.cu): an exchange buffer every peer maps + the peers' buffers
 constexpr uint32_t QB_MAX_WORLD = 16;
 constexpr uint32_t QB_XCHG_SLOTS = 4;     // ring of exchange slots (window of 2 pipelined steps, see qb_comm.cu)
@@ -289,6 +304,8 @@ qb_status qb_sparse_sort_rows(cudaStream_t st, uint32_t n_points, uint64_t n, co
                               uint32_t dim_bound, bool any_dim, uint32_t* d_rdims, float* d_rw, unsigned long long* d_post_keys, unsigned int* h_flags);
 // QueryVector kinds beyond Nearest: examples per query (qb_custom.cu)
 uint32_t qb_custom_examples(int kind, uint32_t n_a, uint32_t n_b);
+
+constexpr uint32_t QB_MMR_MAX_CANDIDATES = 16384;   // candidates_limit's cap (api/src/rest/schema.rs:771); positions are u16 on the device
 
 // MMR reranking (qb_mmr.cu): nq lists of up to max_cand candidates (n_max bounds the counts), queries preprocessed ([nq][row_stride / 4]);
 // selections to d_out[q * out_stride ..), their number to d_out_counts, the candidates left after the dedup to d_n_unique.  d_scratch:

@@ -134,20 +134,7 @@ __global__ void __launch_bounds__(SC_THREADS) sparse_custom_kernel(const ScParam
 
 }  // namespace
 
-// ------------------------------------------------------------------------------------------------ the handle
-struct qb_sparse_storage {
-    int device = 0;
-    uint32_t n_points = 0;
-    uint64_t nnz = 0, hbm_bytes = 0;
-    int on_disk = 0;
-    cudaStream_t stream = nullptr;
-    uint64_t* d_rptr = nullptr; uint32_t* d_rdims = nullptr; float* d_rw = nullptr;   // rows in user dims, sorted by dim
-    std::vector<uint64_t> h_rptr;                                                      // the row offsets, for the counters
-    std::mutex mu;
-    void* d_scratch = nullptr; size_t scratch_bytes = 0;
-    int sm_count = 132;
-};
-
+// ------------------------------------------------------------------------------------------------ the handle (qb_internal.h)
 static void sc_free(qb_sparse_storage* x) {
     if (!x) return;
     cudaSetDevice(x->device);

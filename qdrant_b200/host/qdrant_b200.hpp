@@ -516,6 +516,21 @@ public:
                                      counters));
         return scores;
     }
+    // maximal marginal relevance over candidates whose sparse vectors are this storage's points: one query in user dims (any order),
+    // (point id, score) candidates, pair scores score_vectors -> the selection, with the input scores
+    std::vector<ScoredPointOffset> mmr(const SparseVector& query, const std::vector<ScoredPointOffset>& candidates, float lambda, uint32_t limit,
+                                       qb_hw_counters* counters = nullptr) const {
+        std::vector<uint64_t> qp(1, 0);
+        std::vector<uint32_t> qd;
+        std::vector<float> qw;
+        SparseVectorIndex::flatten({query}, qp, qd, qw);
+        std::vector<ScoredPointOffset> out(std::max<uint32_t>(limit, 1));
+        const uint32_t n = (uint32_t)candidates.size();
+        uint32_t count = 0;
+        check(qb_mmr_sparse_batch(h_, qp.data(), qd.data(), qw.data(), 1, &lambda, candidates.data(), &n, n, limit, out.data(), &count, counters));
+        out.resize(count);
+        return out;
+    }
 
 private:
     qb_sparse_storage* h_ = nullptr;

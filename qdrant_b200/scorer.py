@@ -925,6 +925,31 @@ class SparseVectorStorage:
                                            None if counters is None else C.byref(counters)))
         return scores
 
+    def mmr(self, queries, candidates, lambdas, limit: int, counters: Optional[HwCounters] = None):
+        """Maximal marginal relevance (mmr_from_points_with_vector, shard/src/query/mmr/mod.rs:42-279) over candidates whose sparse vectors
+        are this storage's points (qb_mmr_sparse_batch): queries = a CSR triple or one (dims, weights) pair per query, user dims in any
+        order; candidates = one SCORED_POINT_OFFSET array per query; lambdas = one per query (1 - diversity) or one for all -> list (one
+        per query) of the selected candidates with their input scores."""
+        qp, qd, qw = _csr(queries)
+        nq = qp.size - 1
+        if len(candidates) != nq:
+            raise ValueError(f"{len(candidates)} candidate lists for {nq} queries")
+        lam = np.ascontiguousarray(np.broadcast_to(np.asarray(lambdas, np.float32), (nq,)))
+        max_c = max((len(c) for c in candidates), default=0)
+        cand = np.zeros((max(nq, 1), max(max_c, 1)), dtype=SCORED_POINT_OFFSET)
+        counts = np.zeros(max(nq, 1), dtype=np.uint32)
+        for i, c in enumerate(candidates):
+            c = np.asarray(c, dtype=SCORED_POINT_OFFSET)
+            cand[i, : c.size] = c
+            counts[i] = c.size
+        out = np.zeros((max(nq, 1), max(int(limit), 1)), dtype=SCORED_POINT_OFFSET)
+        out_counts = np.zeros(max(nq, 1), dtype=np.uint32)
+        check(lib().qb_mmr_sparse_batch(self._h, qp.ctypes.data_as(u64p), qd.ctypes.data_as(u32p), qw.ctypes.data_as(f32p), nq, lam.ctypes.data_as(f32p),
+                                        cand.ctypes.data_as(C.POINTER(ScoredPoint)), counts.ctypes.data_as(u32p), cand.shape[1] if max_c else 0, int(limit),
+                                        out.ctypes.data_as(C.POINTER(ScoredPoint)), out_counts.ctypes.data_as(u32p),
+                                        None if counters is None else C.byref(counters)))
+        return [out[i, : out_counts[i]].copy() for i in range(nq)]
+
     def close(self):
         if self._h:
             lib().qb_sparse_storage_destroy(self._h)
